@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — clips/sec of the MERTools hot path on B200 (contract in the task statement).
+"""bench.py — clips/sec of the MERTools hot path on one or more H100s.
 
 One "step" = one pass of the hot path over one batch of synthetic clips per GPU:
   tri-modal feature extraction (ViT-B/16 on 8 frames 224x224, HuBERT-base on a 5 s 16 kHz waveform,
@@ -9,7 +9,9 @@ One "step" = one pass of the hot path over one batch of synthetic clips per GPU:
 `e2e`    : same metric through the public host-buffer API (pinned host inputs -> H2D -> extract ->
            features D2H -> fusion step with H2D of features/labels -> loss D2H), copies timed.
 `--impl reference` times the reference's algorithm on the host CPU cores (the oracle port: the
-reference is pure Python over torch/transformers and /root/reference is absent on the GPU box).
+reference is pure Python over torch/transformers).
+`--dump-outputs DIR` writes what the last timed step computed (the loss and the three clip-feature arrays) as
+DIR/<name>.npy; the inputs and weights are seeded, so two builds can be compared output for output.
 
 Weak scaling: every rank processes its own CLIPS clips per step; the only collective is the fusion
 gradient all-reduce (1.9 MB).  Random-init weights (no network), synthetic inputs.
@@ -40,7 +42,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"],
                     src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense fp16 / bf16 989 TFLOP/s; not reached figures
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -111,7 +114,15 @@ def device_step(models, dev_in, clips, world):
     tfeat, _ = bert.forward_packed(ids, TOKENS)
     loss, _, _ = fus.train_step(afeat, tfeat, vfeat, emo, val, lr=1e-3, weight_decay=1e-5,
                                 world_size=world)
-    return loss
+    return loss, dict(visual_features=vfeat, audio_features=afeat, text_features=tfeat)
+
+
+def dump_outputs(out_dir, loss, feats):
+    """The last timed step's results as float32 .npy files (3 x clips x 768 features + the loss vector)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = dict(feats, loss=loss)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def _log(msg):
@@ -204,9 +215,11 @@ def run_ours(args):
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     ev[0].record()
     for _ in range(args.steps):
-        loss = device_step(models, dev_in, clips, world)
+        loss, feats = device_step(models, dev_in, clips, world)
     ev[1].record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, feats)
     ms = ev[0].elapsed_time(ev[1])
     launches = int(L.lib().mer_launch_count() - l0 + models[3].graph_launches - g0)
     prof = {}
@@ -283,19 +296,15 @@ def run_ours(args):
         pk = peaks()
         total_clips = clips * world * args.steps
         # dominant kernel: the ViT stack's linear layers, fp16 operands by default (MER_VIT_PRECISION=tf32
-        # selects the TF32 variant).  Denominator (B200_PROFILING.md rule): the kernel is timed inside a long
-        # step -> the SUSTAINED bf16 figure of MEASURED_PEAKS (fp16 and bf16 share the tensor-pipe rate; tf32
-        # runs at half of it); the fraction of the burst figure is given beside it.
+        # selects the TF32 variant).  Denominator: the kernel is timed inside a long step -> the SUSTAINED bf16
+        # figure of MEASURED_PEAKS when present (fp16 and bf16 share the tensor-pipe rate; tf32 runs at half of it);
+        # the fraction of the burst figure is given beside it.
         use_f16 = prof["f16"][2] > 0
         t_ms, t_fl, t_n = prof["f16"] if use_f16 else prof["tf32"]
         div = 1.0 if use_f16 else 2.0
         tf32_peak = pk["bf16_sustained"] / div
         burst_peak = pk["bf16"] / div
         ach = t_fl / (t_ms * 1e-3) / 1e12 if t_ms > 0 else 0.0
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get("dram_bytes_per_launch")
         # every other kernel class of the encoders, event-timed the same way over the same timed region
         def entry(key, kernel, bound, peak, unit, scale):
             k_ms, k_work, k_n = prof[key]
@@ -308,18 +317,17 @@ def run_ours(args):
         other = [e for e in (
             entry("bf16x3", "gemm_kernel<*, BF16X3> (3 bf16 MMAs per product; HuBERT conv3-6 + feature projection)", "tensor",
                   sus / 3.0, "TFLOP/s (useful)", 1e12),
-            entry("conv_f16", "gemm_kernel<256, F16, CTA pair> as HuBERT conv1 / conv2 (implicit GEMM over time-major fp16 "
+            entry("conv_f16", "gemm_kernel<256, F16> as HuBERT conv1 / conv2 (implicit GEMM over time-major fp16 "
                   "rows, k = 3, stride 2)", "tensor", sus, "TFLOP/s", 1e12),
             entry("f16_small", "gemm_kernel<*, F16> on the HuBERT (63,744 rows) and BERT (8,192 rows) layers: 10 / 1.3 waves of "
                   "tiles at N = 768", "tensor", sus, "TFLOP/s", 1e12),
-            entry("att_f16", "attention_f16_kernel (tcgen05 kind::f16; ViT 197, HuBERT 249, BERT 32 tokens)", "tensor", sus,
+            entry("att_f16", "attention_vt_kernel<f16> (mma.sync f16; ViT 197, HuBERT 249, BERT 32 tokens)", "tensor", sus,
                   "TFLOP/s", 1e12),
-            entry("att_tc", "attention_tc_kernel (tcgen05 kind::tf32; HuBERT 249 tokens, BERT)", "tensor", sus / 2.0,
+            entry("att_tc", "attention_vt_kernel<tf32> (mma.sync tf32; HuBERT 249 tokens, BERT)", "tensor", sus / 2.0,
                   "TFLOP/s", 1e12),
             entry("ln", "layernorm_kernel (warp per row, 128-bit I/O)", "hbm", pk["hbm"], "GB/s", 1e9),
             entry("conv0", "conv0 moments + coefficients + apply (HuBERT conv0 + GroupNorm + GELU; statistics from the "
-                  "waveform's tap moments, one pass over the output, fp16 rows out: 4.2 GB; fp32-pipe bound, 70 % "
-                  "FMA-pipe active in ncu)", "hbm", pk["hbm"],
+                  "waveform's tap moments, one pass over the output, fp16 rows out: 4.2 GB)", "hbm", pk["hbm"],
                   "GB/s", 1e9),
             entry("posconv", "HuBERT positional conv (grouped k=128) as a windowed block-diagonal F16 GEMM; algorithmic FLOPs "
                   "(the GEMM executes 6.67x as many)", "tensor", sus, "TFLOP/s", 1e12),
@@ -337,19 +345,18 @@ def run_ours(args):
             "config": {"workload": f"tri-modal extract (ViT-B/16 {FRAMES}x224x224 frames + HuBERT-base 5 s @16 kHz + "
                                    f"BERT-base {TOKENS} tokens) + Attention-fusion train step (hidden 128, dropout 0.3), "
                                    f"{clips} clips per GPU per step",
-                       "clips_per_gpu_per_step": clips, "l2": "step inputs + activations (>10 GB) exceed the 126 MB L2",
+                       "clips_per_gpu_per_step": clips, "l2": "step inputs + activations (>10 GB) exceed the 50 MB L2",
                        "text_inputs": "pre-tokenised ids (the HF tokenizer is host code on both arms)",
                        "parallelism": f"clip-sharded x{world}, one NCCL all-reduce of the fusion gradient per step"},
             "e2e": {"value": total_clips / (e2e_ms * 1e-3), "unit": "clips/s",
                     "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h)},
             "gpu_launches": launches,
             "clocks": clocks,
-            "roofline": {"kernel": ("gemm_kernel<256, F16, CTA pair, cta_group::2> (tcgen05 kind::f16; the 48 linear layers "
-                                    "of the ViT stack, 403,456 rows)"
+            "roofline": {"kernel": ("gemm_kernel<256, F16> (wgmma f16; the 48 linear layers of the ViT stack, 403,456 rows)"
                                     if use_f16 else
-                                    "gemm_kernel<256, TF32, CTA pair, cta_group::2> (tcgen05 kind::tf32; ViT linear layers)"),
+                                    "gemm_kernel<256, TF32> (wgmma tf32; ViT linear layers)"),
                          "bound": "tensor", "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s",
-                         "frac": ach / tf32_peak if tf32_peak else None, "traffic": traffic,
+                         "frac": ach / tf32_peak if tf32_peak else None,
                          "frac_vs_burst": ach / burst_peak if burst_peak else None,
                          "launches_timed": t_n, "share_of_step": t_ms / ms_dev if ms_dev else None,
                          "peak_source": (f"{pk['src']} MEASURED_PEAKS bf16_tflops_sustained (kernel timed inside a long "
@@ -502,8 +509,8 @@ def run_reference(args):
     total = sum(secs)
     value = procs * n * args.steps / total
     sample = (f"{procs} processes x {threads} torch threads = {procs * threads} of {ncpu} host cores; {n} clips per process "
-              f"and step x {args.steps} steps; oracle port of the reference path (pure-Python reference; /root/reference is "
-              f"absent on the GPU box); one process alone: {1.0 / sec1:.2f} clips/s")
+              f"and step x {args.steps} steps; oracle port of the reference path (the reference is pure Python); one process "
+              f"alone: {1.0 / sec1:.2f} clips/s")
     line = {
         "impl": "reference", "metric": METRIC, "value": value, "unit": "clips/s", "n_gpus": args.gpus,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": total / args.steps * 1e3,
@@ -528,6 +535,8 @@ if __name__ == "__main__":
     ap.add_argument("--cpu-clips", type=int, default=48, help="upper bound of clips in the bounded CPU sample")
     ap.add_argument("--no-extras", action="store_true", help="skip the side measurements (fusion latency, mixed-length "
                     "audio, TF32 ViT, whole-host CPU figure)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write the last timed step's loss and clip features to DIR/<name>.npy (float32)")
     ap.add_argument("--cpu-worker", type=int, default=0, help=argparse.SUPPRESS)
     ap.add_argument("--cpu-threads", type=int, default=16, help=argparse.SUPPRESS)
     ap.add_argument("--cpu-steps", type=int, default=1, help=argparse.SUPPRESS)

@@ -1,4 +1,4 @@
-/* mer_b200.h — C ABI of libmer_b200.so (B200 / sm_100a only).
+/* mer_b200.h — C ABI of libmer_b200.so (H100 / sm_90a only; the b200 in the names is the project's original tag).
  *
  * Drop-in boundary for the MERTools hot path (SURVEY.md §8b): the reference has no FFI; the
  * seam a maintainer would bind is the model-object call
@@ -37,13 +37,14 @@ MER_API int mer_check_device(void);
 /* cumulative number of CUDA kernels this library has launched in this process (bench.py's
  * gpu_launches); CUDA-graph replays are not seen here and are counted by their owner */
 MER_API long long mer_launch_count(void);
-/* launches so far of the instantiation gemm_kernel<block_n (128 | 256), mode (MER_GEMM_*), cluster (1 | 2), twosm
- * (0 | 1: tcgen05.mma.cta_group::2)>; -1 for a combination that does not exist. */
+/* launches so far of the instantiation gemm_kernel<block_n (128 | 256), mode (MER_GEMM_*)>; cluster (1 | 2) and twosm
+ * (0 | 1) name CTA-pair forms, which this build does not have (0 launches for cluster 2 or twosm 1); -1 for arguments
+ * outside those ranges. */
 MER_API long long mer_gemm_variant_launches(int block_n, int mode, int cluster, int twosm);
 /* per-launch CUDA-event timing (roofline in bench.py): enable(1) starts a fresh recording, enable(0)
  * stops; collect sums duration / algorithmic work / launches of one kernel class since the last
  * enable(1).  Classes: MER_GEMM_* (work = 2*M*N*K flop; MER_GEMM_F16 launches of fewer than 2^17 rows are
- * class 3; 4 = HuBERT conv1 / conv2 as fp16 implicit GEMMs), 10 = fp16 tcgen05 attention (15 = its long-key form), 11 = TF32 tcgen05
+ * class 3; 4 = HuBERT conv1 / conv2 as fp16 implicit GEMMs), 10 = fp16 V^T attention, 11 = TF32 V^T
  * attention (work = 4*S^2*64 flop per (sequence, head), S = tokens / n_seq), 12 = LayerNorm, 14 = HuBERT
  * conv0 (work = algorithmic HBM bytes), 13 = HuBERT positional conv (flop). */
 MER_API int mer_profile_enable(int on);
@@ -58,9 +59,8 @@ enum { MER_EPI_GELU = 1, MER_EPI_ROUND_TF32 = 2, MER_EPI_SPLIT_BF16 = 4,
        MER_EPI_OUT_F16 = 16,  /* out (and vt, if given) are IEEE fp16 arrays (round-to-nearest, saturating);
                                  ld_out / vt_ld in elements */
        MER_ATT_QKV_F16 = 32   /* mer_attention only: qkv and vt are fp16 arrays (needs vt, vt_ld % 8 == 0, max_seqlen <=
-                                 505).  With MER_EPI_OUT_F16: attention_f16.cu up to 249 tokens, attention_f16_long.cu
-                                 beyond; with another ctx format (fp32, MER_EPI_ROUND_TF32, MER_EPI_SPLIT_BF16):
-                                 attention_f16_long.cu */ };
+                                 505); ctx in the format the other flags name (fp16, fp32, MER_EPI_ROUND_TF32,
+                                 MER_EPI_SPLIT_BF16): attention_f16.cu */ };
 /* Arithmetic mode of a GEMM.  TF32: operands are fp32 arrays (pre-rounded to tf32).  BF16X3: every
  * operand value x is stored as a bf16 pair (hi, lo), x = hi + lo to 2^-17; a row of K values (K % 32
  * == 0) occupies the bytes K fp32 values would, as 128-byte groups [32 x hi | 32 x lo]; three bf16
@@ -84,8 +84,8 @@ typedef struct MerGemmEpilogue {
   int flags;     /* MER_EPI_* */
   int split_off; /* reserved (0) */
   /* optional transposed side output: columns n >= vt_col0 are written as vt[(n - vt_col0) * vt_ld +
-   * out_row] INSTEAD of out[out_row, n] (the QKV GEMM hands V^T, keys contiguous, to the tcgen05
-   * attention kernel as a K-major operand) */
+   * out_row] INSTEAD of out[out_row, n] (the QKV GEMM hands V^T, keys contiguous, to the V^T
+   * attention kernel) */
   float* vt;
   long long vt_ld;
   int vt_col0;
@@ -112,8 +112,7 @@ typedef struct MerGemmDesc {
   int force_block_n; /* 0 = auto, 128 or 256 */
   int mode;          /* MER_GEMM_TF32 | MER_GEMM_BF16X3 (A strides in 4-byte slots) | MER_GEMM_F16 (A strides in
                         2-byte elements) */
-  int cluster;       /* 0 = auto, 1 = single CTAs, 2 = CTA pairs sharing a multicast weight tile,
-                        3 = CTA pairs issuing one 256-row tcgen05.mma.cta_group::2 per K step */
+  int cluster;       /* reserved: CTA-pair tiles; every value runs single-CTA tiles on sm_90a */
   /* grouped-convolution support (the HuBERT positional conv runs as a block-diagonal GEMM):
    * a_row0     : added to every A row index (may be negative); rows outside [0, a_rows_dim) of a batch
    *              entry read as zero -- the conv's zero padding.
@@ -127,7 +126,7 @@ typedef struct MerGemmDesc {
   MerGemmEpilogue ep;
 } MerGemmDesc;
 
-/* tcgen05 GEMM with fused epilogue.  Replaces torch nn.Linear / nn.Conv1d calls inside
+/* wgmma GEMM with fused epilogue.  Replaces torch nn.Linear / nn.Conv1d calls inside
  * HF ViTLayer / HubertEncoderLayer / BertLayer reached from the reference extractors. */
 MER_API int mer_gemm(const MerGemmDesc* desc, void* stream);
 /* fp32 [rows, K] -> split rows (same byte size, K % 32 == 0); used on weights at load time */
@@ -155,14 +154,13 @@ MER_API int mer_round_tf32(float* x, long long n, void* stream);
 /* softmax(Q K^T / 8) V per (sequence, head); head_dim 64.  qkv is [tokens, 3*heads*64] with
  * Q | K | V column blocks, sequences packed back to back, cu_seqlens[n_seq+1] (device, int32),
  * tokens = cu_seqlens[n_seq] (host copy, sizes the TMA descriptors).  vt (optional): V^T, [heads*64,
- * vt_ld] with vt[d, token] = V[token, d] (vt_ld >= tokens, multiple of 4), as written by mer_gemm's
- * transposed side output.  With vt and max_seqlen <= 256 the tcgen05 kernel runs (S in TMEM, P staged
- * through smem, both MMAs on K-major operands) and the V columns of qkv are not read; otherwise the
- * flash-style kernel.
+ * vt_ld] with vt[d, token] = V[token, d] (vt_ld >= tokens, multiple of 4; of 8 for fp16), as written by mer_gemm's
+ * transposed side output.  With vt and max_seqlen <= 253 the V^T kernel runs and the V columns of qkv are not
+ * read; otherwise the kernel that reads V from qkv.
  * ctx is [tokens, heads*64].  flags: MER_EPI_ROUND_TF32 rounds ctx for a TF32 out-proj GEMM,
  * MER_EPI_SPLIT_BF16 writes ctx as bf16 hi|lo rows for a BF16X3 out-proj GEMM, MER_EPI_OUT_F16 writes
- * ctx as fp16 for an F16 out-proj GEMM (tcgen05 kernels only); with MER_ATT_QKV_F16 the inputs are
- * fp16 as well (attention_f16.cu: kind::f16 MMAs, half the traffic).
+ * ctx as fp16 for an F16 out-proj GEMM (V^T kernels only); with MER_ATT_QKV_F16 the inputs are
+ * fp16 as well (attention_f16.cu: fp16 MMAs, half the traffic; up to 505 tokens).
  * Replaces HF eager/sdpa attention (modeling_vit.py:171-196, modeling_hubert.py:262-345). */
 MER_API int mer_attention(const float* qkv, const float* vt, long long vt_ld, float* ctx,
                           const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,

@@ -2,7 +2,7 @@
 
 PyTorch is used by callers for device memory and streams only; tensors cross this boundary as
 raw device pointers.  There is NO fallback: if the shared library is missing or the device is
-not sm_100, the first call raises.
+not sm_90a (H100), the first call raises.
 """
 from __future__ import annotations
 
@@ -189,10 +189,9 @@ def round_tf32_(x):
 
 
 def attention(qkv, ctx, cu_seqlens, max_seqlen, heads, round_out=False, vt=None, f16_out=False, split_out=False):
-    """vt: optional V^T [heads*64, ld] (enables the tcgen05 kernel for max_seqlen <= 253).  fp16 qkv / vt select the
-    fp16-operand kernels (max_seqlen <= 505): an fp16 ctx tensor gives attention_f16.cu (<= 249 tokens) or
-    attention_f16_long.cu; an fp32 ctx tensor (plain, round_out = tf32-rounded, split_out = bf16 hi | lo rows) the
-    long-key kernel with that output format."""
+    """vt: optional V^T [heads*64, ld] (enables the tf32 V^T kernel of attention_f16.cu for max_seqlen <= 253).  fp16
+    qkv / vt select the fp16-operand V^T kernel (max_seqlen <= 505); its ctx is fp16 for an fp16 ctx tensor, else fp32
+    (plain, round_out = tf32-rounded, split_out = bf16 hi | lo rows)."""
     import torch
     if qkv.dtype == torch.float16:
         assert vt is not None and vt.dtype == torch.float16

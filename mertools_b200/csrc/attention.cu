@@ -12,7 +12,7 @@
 // accumulator fragment is re-used directly as the A fragment of P V by permuting the key order
 // inside each 8-key group (keys 2t / 2t+1 <-> k-columns t / t+4), with V rows fetched under the
 // same permutation, so no shuffles or smem round-trip are needed.
-// [round 1: legacy tensor path; the tcgen05 version is the follow-up named in DESIGN.md]
+// Used when the QKV GEMM wrote V into qkv (no V^T): CLIP L/14 rows in the fp16 stacks, MER_ATTENTION_LEGACY.
 #include <stdlib.h>
 
 #include "mer_common.cuh"
@@ -240,30 +240,27 @@ bool mer_attention_legacy() {
 }
 
 bool mer_attention_uses_tc(int max_seqlen) {
-  return !mer_attention_legacy() && max_seqlen <= 253;  // + up to 3 alignment keys must fit the 256-key S tile
+  return !mer_attention_legacy() && max_seqlen <= 253;
 }
 
 int mer_attention_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx,
                          const int* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
                          int flags, cudaStream_t stream) {
   MER_REQUIRE(qkv && ctx && cu_seqlens, "mer_attention: null operand");
+  const int out_mode = (flags & MER_EPI_OUT_F16) ? 3 : (flags & MER_EPI_SPLIT_BF16) ? 2 : ((flags & MER_EPI_ROUND_TF32) ? 1 : 0);
   if (flags & MER_ATT_QKV_F16) {
-    // fp16 q | k rows and V^T: attention_f16.cu (<= 249 tokens, fp16 ctx) or attention_f16_long.cu (<= 505 tokens, ctx in
-    // any operand format: the TF32 / BF16X3 stacks send their 254 .. 505-token rows here)
+    // fp16 q | k rows and V^T (attention_f16.cu), ctx in any operand format: the fp16 stacks, and the TF32 / BF16X3
+    // stacks for rows of 254 .. 505 tokens
     MER_REQUIRE(vt && mer_attention_f16_supported(max_seqlen),
                 "mer_attention: fp16 inputs need V^T and sequences <= 505 tokens (max_seqlen %d)", max_seqlen);
-    if (tokens <= 0) return 0;
-    const int out_mode = (flags & MER_EPI_OUT_F16) ? 3 : (flags & MER_EPI_SPLIT_BF16) ? 2 : ((flags & MER_EPI_ROUND_TF32) ? 1 : 0);
-    if (out_mode == 3)
-      return mer_attention_f16_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, stream, max_seqlen);
-    return mer_attention_f16_long_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, stream, max_seqlen, out_mode);
+    return mer_attention_f16_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream);
   }
-  // sequences of up to 256 tokens (ViT 197, HuBERT 5 s = 249, most sentences): tcgen05 kernel,
-  // which reads V^T (written by the QKV GEMM epilogue) instead of the V columns of qkv
-  if (vt && mer_attention_uses_tc(max_seqlen) && tokens > 0)
-    return mer_attention_tc_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, flags, stream);
+  // sequences of up to 253 tokens (ViT 197, HuBERT 5 s = 249, most sentences) with V^T written by the QKV GEMM
+  // (which then leaves the V columns of qkv unwritten): the tf32 form of the V^T kernel
+  if (vt && mer_attention_uses_tc(max_seqlen))
+    return mer_attention_tc_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream);
   MER_REQUIRE(!(flags & MER_EPI_OUT_F16),
-              "mer_attention: fp16 ctx needs the tcgen05 kernel (V^T given, sequences <= 253 tokens)");
+              "mer_attention: fp16 ctx needs V^T (sequences <= 253 tokens)");
   MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535, "mer_attention: bad grid (%d heads, %d seqs)",
               heads, n_seq);
   if (n_seq <= 0 || max_seqlen <= 0) return 0;

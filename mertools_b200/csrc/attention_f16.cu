@@ -1,25 +1,22 @@
-// attention_f16.cu — tcgen05 attention on fp16 operands (sequences of up to 249 tokens, head_dim 64).
+// attention_f16.cu — softmax(Q K^T / 8) V for packed variable-length sequences (head_dim 64) that reads V
+// transposed: the form the QKV GEMM epilogue writes (V^T [heads*64, vt_ld], vt[d, token], keys contiguous).
 //
-// softmax(Q K^T / 8) V per (sequence, head) for the ViT stack when it runs in MER_GEMM_F16 mode: the
-// QKV GEMM writes q | k (fp16 rows) and V^T (fp16, keys contiguous), this kernel writes ctx as fp16,
-// the operand of the out-proj GEMM.  fp16 carries the 10 mantissa bits the TF32 kernel
-// (attention_tc.cu) rounds to, so the products are the same; the tensor-pipe rate doubles and every
-// tile is half as large.  Replaces the same reference op (HF eager/sdpa attention,
-// modeling_vit.py:171-196).
+// Two operand formats share one flash-style kernel:
+//   fp16 : q | k fp16 rows of qkv16, fp16 V^T; S = Q K^T and O += P V on mma.sync.m16n8k16 (fp16 in, fp32
+//          accumulate), P rounded to fp16.  The ViT / HuBERT / BERT stacks in MER_GEMM_F16 mode and the
+//          250 .. 505-token rows of the TF32 / BF16X3 stacks (fp16 carries the same 10 mantissa bits as tf32).
+//   tf32 : tf32-rounded fp32 q | k rows and V^T; mma.sync.m16n8k8 tf32, P rounded to tf32.  The TF32 / BF16X3
+//          stacks for sequences of up to 253 tokens.
+// Replaces the same reference op as attention.cu (HF eager/sdpa attention, modeling_vit.py:171-196,
+// modeling_hubert.py:262-345).
 //
-// Persistent, one CTA per SM, work item = (sequence, head); roles and barrier scheme as in
-// attention_tc.cu:
-//   warp 0      TMA producer: K [keys][64 d] (one 128-byte swizzle row per key), V^T [64 d][keys] in
-//               64-key chunks, the 128-row Q tiles
-//   warp 1      tcgen05 issuer: S_t = Q_t K^T (UMMA 128 x NK x 16, kind::f16) into TMEM columns
-//               [256 t, 256 t + NK); per 64-key chunk of P: O_t += P_chunk V_chunk (UMMA 128 x 64 x 16)
-//               into the first 64 columns of S_t's range
-//   warps 2..9  two softmax + epilogue groups (one per query tile): S rows TMEM -> registers (thread =
-//               query row), max, exp2, sum, fp16 P chunks -> swizzled smem (the tile's dead Q buffer);
-//               O / sum -> fp16 -> swizzled smem (the dead V^T region) -> 512-byte coalesced stores
-// TMA boxes start on 16-byte boundaries: the key axis of an item begins at the sequence start rounded
-// down to a multiple of 8 tokens; the (up to 7) leading foreign keys are masked.
-// Algorithmic HBM traffic per token and layer: 4.5 KB of q|k|v^T in, 1.5 KB of ctx out.
+// One CTA = (64-query block, head, sequence); 4 warps x 16 query rows; K [64 keys][64 d] and V^T [64 d][64 keys]
+// tiles double-buffered in shared memory by cp.async; online softmax in fp32 registers.  The S accumulator
+// fragment is the A fragment of P V (fp16: two 8-key n-tiles form one 16-key k-step; tf32: keys 2t / 2t+1 of an
+// 8-key group are k-columns t / t+4, and the V^T columns are read under the same permutation).
+// 16-byte copies need 16-byte aligned starts: the key axis of a sequence begins at its start rounded down to a
+// multiple of 8 tokens, and the (up to 7) leading foreign keys are masked.  Keys beyond the last token are
+// zero-filled, so that masked probabilities (exactly 0) never meet uninitialised V^T padding.
 #include <stdlib.h>
 
 #include "mer_common.cuh"
@@ -30,1025 +27,311 @@ namespace {
 using namespace mer;
 
 constexpr int HD = 64;
-constexpr int F16_THREADS = 320;          // producer, MMA issuer, 2 x 4 softmax/epilogue warps (VER 1..3)
-constexpr int F16_THREADS_V4 = 576;       // VER 4: 2 x 8 softmax/epilogue warps
-constexpr int F16_THREADS_V6 = 608;       // VER 6 / 7: + a second MMA issuer warp
-constexpr int K_BYTES = 256 * 128;        // K: up to 256 keys x 128 B
-constexpr int VT_CHUNK = HD * 128;        // V^T chunk: 64 d-rows x 64 keys (128 B)
-constexpr int QTILE_BYTES = 128 * 128;    // one 128-row Q tile; later the P-chunk buffer of the tile
-// two operand sets (items alternate between them, so the next item's K / V^T / Q are in flight while the
-// current one computes); inside a set:
-constexpr int SMEM_K = 0;
-constexpr int SMEM_V = K_BYTES;           // 4 V^T chunks = 32 KB; later the output staging (2 x 16 KB)
-constexpr int SMEM_Q = SMEM_V + 4 * VT_CHUNK;
-constexpr int SET_BYTES = SMEM_Q + 2 * QTILE_BYTES;  // 96 KB
-constexpr int SMEM_BAR = 2 * SET_BYTES;
-constexpr int SMEM_XCHG = SMEM_BAR + 256;   // VER 4: partial row max / row sum of the two warps sharing a row: [2 tiles][128][2] x 2
-constexpr int F16_SMEM = SMEM_XCHG + 4096 + 1024;
-constexpr uint32_t TILE_COLS = 256, TMEM_COLS = 512;
-constexpr uint32_t V6_O_COL = 192;  // VER 6: O_t lives in columns [192, 256) of its slot (see the softmax block)
+constexpr int BQ = 64;
+constexpr int BKV = 64;
+constexpr int THREADS = 128;
+constexpr int MAX_SEQ = 505;  // longest sequence the stacks send here (10 s audio rows, CLIP L/14)
 
-__device__ __forceinline__ float fast_ex2(float x) {  // MUFU.EX2, flush-to-zero
+template <bool F16>
+struct AttCfg {
+  static constexpr int kElem = F16 ? 2 : 4;
+  static constexpr int kPerChunk = 16 / kElem;  // elements per 16-byte copy
+  // padded row pitch in elements: conflict-free fragment loads (fp16: 36 words, tf32: 68 words per row)
+  static constexpr int kLds = F16 ? 72 : 68;
+  static constexpr int kTile = BKV * kLds;  // elements of one K (or V^T) tile
+  static constexpr int kSmem = 2 * 2 * kTile * kElem;
+};
+
+__device__ __forceinline__ void mma_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(src_bytes)
+               : "memory");
+}
+__device__ __forceinline__ float fast_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t addr) {  // SW128, SBO 1024
-  return static_cast<uint64_t>((addr & 0x3FFFF) >> 4) | (1ull << 16) | (uint64_t(1024 >> 4) << 32) |
-         (1ull << 46) | (2ull << 61);
-}
+// out_mode: 0 fp32, 1 tf32-rounded fp32, 2 bf16 hi | lo split rows, 3 fp16
+template <bool F16>
+__global__ void __launch_bounds__(THREADS, 3)
+attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_, long long vt_ld, void* __restrict__ ctx,
+                    const int* __restrict__ cu_seqlens, long long tokens, int heads, int out_mode) {
+  using Cfg = AttCfg<F16>;
+  using T = typename std::conditional<F16, uint16_t, float>::type;
+  constexpr int LDS = Cfg::kLds;
+  extern __shared__ __align__(16) uint8_t smem_att[];
+  T* Ks = reinterpret_cast<T*>(smem_att);  // [2][BKV][LDS]
+  T* Vs = Ks + 2 * Cfg::kTile;             // [2][HD][LDS]: V^T, keys along the row
 
-// VER 7's shared-memory plan (bytes), sized on the host from the longest sequence of the launch: K and the second Q
-// tile are loaded with boxes of exactly the rows they need (197 tokens: 208 + 80 rows instead of 256 + 128)
-struct AttLay {
-  int off_k, off_v, off_q0, off_q1, set_bytes;  // inside an operand set
-  int off_stage;                                // 2 x 16 KB output staging, outside the sets
-  int off_bar, off_xchg;
-  int k_rows, q1_rows;
-};
+  const int seq = blockIdx.z, h = blockIdx.y;
+  const int start = cu_seqlens[seq];
+  const int len = cu_seqlens[seq + 1] - start;
+  const int q0 = blockIdx.x * BQ;
+  if (q0 >= len) return;
+  const int kstart = start & ~7, shift = start - kstart;
 
-// VER 1: every score is compared against the valid key range [shift, Lk) (3 integer instructions per element
-//        in both passes: 35 % of the kernel's issued instructions in the round-1 ncu capture).
-// VER 3: VER 2 with 3 of every 8 exponential pairs of the unmasked granules computed by ex2_poly2 on the FMA / ALU
-//        pipes (the MUFU floor of this kernel is 2.75x its MMA time at head_dim 64).
-// VER 2: the key axis is handled in 16-column granules; granules that lie inside [shift, Lk) — all but the
-//        first (leading foreign keys) and the last — run unmasked with FMNMX3 / FFMA2 / FADD2, and granules
-//        beyond the UMMA key count NK are skipped (the P V MMA never reads them).
-// VER 4: 16 softmax warps.  Measured on B200 (scripts/micro/tmem_mufu_bench.cu): one warp gets a 32-column
-//        tcgen05.ld every ~100 cycles whatever it has in flight (41 B/clk), the SM 317 B/clk from 8 warps and 435
-//        from 16; MUFU.EX2 runs at exactly 16 per clock and SM.  With one thread per query row a tile costs 17
-//        serialised loads and 208 exponentials per thread, and the kernel sat at ~10k cycles per (sequence, head)
-//        against a MUFU floor of 3.3k.  Here TWO warps share each 32-row quarter of a tile: warp `half` takes
-//        columns [32 half, 32 half + 32) of every 64-key chunk in both passes (9 loads, ~104 exponentials per
-//        thread), the partial row maxima / sums meet through shared memory under a 64-thread named barrier, both
-//        halves store their 64 bytes of each P row and of each output row.  Softmax body as VER 3.
-// VER 7: VER 6 with the operand loads taken off the critical path.  The trace of VER 6 showed every tile waiting ~2.7k
-//        cycles for K / Q of the next item: an operand set was reloaded only when BOTH tiles had finished their
-//        epilogues, and 96 KB of 128-byte rows take ~8k cycles to arrive (scripts/micro/tma_bench.cu: ~400 cycles per
-//        box plus ~2 per row from L2, 23 B/clk/SM from HBM with all SMs streaming).  Here the producer refills K and the
-//        Q tiles of a set as soon as the S = Q K^T products that read them are complete (a whole item earlier), V^T as
-//        soon as the P V products are; the output is staged in its own 2 x 16 KB buffers instead of a dead operand
-//        tile, and K / the second Q tile come in boxes of exactly the rows the launch needs.
-// POLY: pairs (of the 8 per 16-key granule) whose exponentials run on the FMA pipe (VER >= 6): the kernel is issue-
-//        bound with POLY = 3 and XU-bound with POLY = 0.
-template <int VER, int POLY = 3>
-__global__ void __launch_bounds__(VER >= 6 ? F16_THREADS_V6 : VER >= 4 ? F16_THREADS_V4 : F16_THREADS, 1)
-attention_f16_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
-                     const __grid_constant__ CUtensorMap tmap_vt, const __grid_constant__ CUtensorMap tmap_k,
-                     const __grid_constant__ CUtensorMap tmap_q1, const __grid_constant__ AttLay lay,
-                     uint16_t* __restrict__ ctx, const int* __restrict__ cu_seqlens, int n_seq, int heads,
-                     long long* __restrict__ trace) {
-  // trace (debug, normally null): clock64() stamps of block 0's first 16 items, 32 slots per item (scripts/att_trace.py)
-#define ATT_TR(slot)                                                                           \
-  do {                                                                                         \
-    if (trace != nullptr && blockIdx.x == 0 && item_n < 16 && lane == 0) trace[item_n * 32 + (slot)] = clock64(); \
-  } while (0)
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (VER == 7 ? lay.off_bar : SMEM_BAR));
-  uint64_t* bar_k = bars + 0;       // [2 sets] producer -> MMA: K tile of the item
-  uint64_t* bar_q = bars + 2;       // [2 sets] producer -> MMA: Q tiles
-  uint64_t* bar_v = bars + 4;       // [2 sets] producer -> MMA: V^T chunks
-  uint64_t* bar_sfull = bars + 6;   // [2 tiles] MMA -> softmax group t: S_t complete
-  uint64_t* bar_pready = bars + 8;  // [2] softmax group t -> MMA: a P chunk of tile t sits in smem
-  uint64_t* bar_pfree = bars + 10;  // [2] MMA -> softmax group t: that chunk has been consumed
-  uint64_t* bar_ofull = bars + 12;  // [2] MMA -> softmax group t: O_t complete
-  uint64_t* bar_ofree = bars + 14;  // [2] softmax group t -> producer: output staging (V^T region) consumed
-  uint64_t* bar_otfree = bars + 16; // [2] softmax group t -> MMA: O_t has been read out of TMEM
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
-  uint64_t* bar_kfree = bars + 22;  // [2 sets] VER 7, MMA -> producer: both tile slots are done with the set's K / Q tiles
-  uint64_t* bar_vfree = bars + 24;  // [2 sets] VER 7, MMA -> producer: ... and with its V^T (a slot that skips the item arrives too)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const long long ld = 3ll * heads * HD;
+  const T* qkv = static_cast<const T*>(qkv_);
+  const T* qbase = qkv + (long long)start * ld + h * HD;
+  const T* kbase = qkv + heads * HD + h * HD;  // row = absolute token index
+  const T* vtbase = static_cast<const T*>(vt_) + (long long)h * HD * vt_ld;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_items = n_seq * heads;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_qkv);
-    tma_prefetch_desc(&tmap_vt);
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&bar_k[t], 1);
-      mbar_init(&bar_q[t], 1);
-      mbar_init(&bar_v[t], 1);
-      mbar_init(&bar_sfull[t], 1);
-      mbar_init(&bar_pready[t], VER >= 4 ? 8 : 4);
-      mbar_init(&bar_pfree[t], 1);
-      mbar_init(&bar_ofull[t], 1);
-      mbar_init(&bar_ofree[t], VER >= 4 ? 8 : 4);
-      mbar_init(&bar_otfree[t], VER >= 4 ? 8 : 4);
-      mbar_init(&bar_kfree[t], 2);
-      mbar_init(&bar_vfree[t], 2);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0 && VER == 7) {
-    // ===================== TMA producer, VER 7: refill as soon as the readers are done =====================
-    uint32_t uses[2] = {0, 0};
-    int h_nmt[2] = {0, 0};
-    uint32_t h_use[2][2] = {{0, 0}, {0, 0}};
-    uint32_t item_n = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      const int set = item_n & 1;
-      uint8_t* sm = smem + set * lay.set_bytes;
-      const int seq = it / heads, h = it % heads;
-      const int start = cu_seqlens[seq];
-      const int len = cu_seqlens[seq + 1] - start;
-      const int n_mt = (len + 127) >> 7;
-      const int a_start = start & ~7;
-      const int Lk = (start - a_start) + len;
-      const int n_vc = (Lk + 63) >> 6;
-      // K and the Q tiles of this set were last read by the S products of item n - 2.  Own barriers (not sfull /
-      // ofull, whose phases the free-running tile pipelines may advance twice before this warp looks): kfree / vfree
-      // complete exactly once per item of the set, and the next completion needs the loads issued below
-      if (item_n >= 2) mbar_wait(&bar_kfree[set], ((item_n >> 1) - 1) & 1);
-      if (elect_one()) {
-        mbar_expect_tx(&bar_k[set], (uint32_t)(lay.k_rows * 128));
-        tma_load_2d(sm + lay.off_k, &tmap_k, &bar_k[set], heads * HD + h * HD, a_start);
-        mbar_expect_tx(&bar_q[set], (uint32_t)(QTILE_BYTES + (n_mt > 1 ? lay.q1_rows * 128 : 0)));
-        tma_load_2d(sm + lay.off_q0, &tmap_qkv, &bar_q[set], h * HD, start);
-        if (n_mt > 1) tma_load_2d(sm + lay.off_q1, &tmap_q1, &bar_q[set], h * HD, start + 128);
-      }
-      __syncwarp();
-      // V^T of this set was last read by the P V products of item n - 2
-      if (item_n >= 2) mbar_wait(&bar_vfree[set], ((item_n >> 1) - 1) & 1);
-      if (elect_one()) {
-        mbar_expect_tx(&bar_v[set], (uint32_t)(n_vc * VT_CHUNK));
-        for (int c = 0; c < n_vc; ++c)
-          tma_load_2d(sm + lay.off_v + c * VT_CHUNK, &tmap_vt, &bar_v[set], a_start + c * 64, h * HD);
-      }
-      __syncwarp();
-      ATT_TR(0);
-      h_nmt[set] = n_mt;
-      for (int t = 0; t < n_mt; ++t) h_use[set][t] = uses[t]++;
-    }
-  } else if (warp == 0) {
-    // ===================== TMA producer (warp-uniform; one elected lane issues) =====================
-    // Item n uses operand set n & 1: its K, Q tiles and V^T are requested as soon as item n - 2 has left
-    // that set (its epilogues, the last users, are done), i.e. while item n - 1 is still computing.
-    uint32_t uses[2] = {0, 0};      // how often tile slot t has been used so far
-    int h_nmt[2] = {0, 0};          // per set: tiles of the item that used it last ...
-    uint32_t h_use[2][2] = {{0, 0}, {0, 0}};  // ... and the use index of each tile slot at that item
-    uint32_t item_n = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      const int set = item_n & 1;
-      uint8_t* sm = smem + set * SET_BYTES;
-      const int seq = it / heads, h = it % heads;
-      const int start = cu_seqlens[seq];
-      const int len = cu_seqlens[seq + 1] - start;
-      const int n_mt = (len + 127) >> 7;
-      const int a_start = start & ~7, shift = start - a_start;  // 16-byte aligned V^T column start
-      const int Lk = shift + len;
-      const int nb = (Lk + 127) >> 7;
-      const int n_vc = (Lk + 63) >> 6;
-      if (item_n >= 2)
-        for (int t = 0; t < h_nmt[set]; ++t) mbar_wait(&bar_ofree[t], h_use[set][t] & 1);
-      if (elect_one()) {
-        mbar_expect_tx(&bar_k[set], (uint32_t)(nb * 16384));
-        for (int b = 0; b < nb; ++b)
-          tma_load_2d(sm + SMEM_K + b * 16384, &tmap_qkv, &bar_k[set], heads * HD + h * HD, a_start + b * 128);
-        mbar_expect_tx(&bar_q[set], (uint32_t)(n_mt * QTILE_BYTES));
-        for (int t = 0; t < n_mt; ++t)
-          tma_load_2d(sm + SMEM_Q + t * QTILE_BYTES, &tmap_qkv, &bar_q[set], h * HD, start + t * 128);
-        mbar_expect_tx(&bar_v[set], (uint32_t)(n_vc * VT_CHUNK));
-        for (int c = 0; c < n_vc; ++c)
-          tma_load_2d(sm + SMEM_V + c * VT_CHUNK, &tmap_vt, &bar_v[set], a_start + c * 64, h * HD);
-      }
-      __syncwarp();
-      ATT_TR(0);
-      h_nmt[set] = n_mt;
-      for (int t = 0; t < n_mt; ++t) h_use[set][t] = uses[t]++;
-    }
-  } else if (VER >= 6 && (warp == 1 || warp == 18)) {
-    // ===================== MMA issuers, VER 6 / 7: one warp per tile slot (warp 1: slot 0, warp 18: slot 1) ============
-    // The phase trace of VER 4 (profiles/r2_attention_f16_v4_trace.txt) showed the two tiles of an item marching in
-    // lock-step behind one issuing warp that served them in program order; a single warp polling both slots (VER 5,
-    // dropped) reacted ~1.3k cycles late because the elected lane's issue loop competes for issue slots with four
-    // busy softmax warps of its scheduler.  Two warps on two schedulers, each walking through the items for its own
-    // slot with plain blocking waits: slot 0 may be in item n + 1 (operand set B) while slot 1 finishes item n (set A).
-    // The sequence bounds of the next item are loaded one item ahead (two independent loads, first touched later).
-    const int t = warp == 1 ? 0 : 1;
-    // these two warps have nothing else to do: spin on non-blocking probes (a try_wait that has gone to sleep reacted
-    // ~1k cycles late in the traces).  A nanosleep back-off of 20 .. 160 ns between probes (to hand the issue slots to
-    // the softmax warps of the same scheduler) measured 0 .. -2 % (profiles/r2_ab_microbench.json): not kept.
-    auto spin = [&](uint64_t* bar, uint32_t parity) {
-      while (!mbar_test_wait(bar, parity)) {
-      }
-    };
-    const int set_bytes = VER == 7 ? lay.set_bytes : SET_BYTES;
-    const uint64_t desc_q = desc_kmajor(smem_u32(smem + (VER == 7 ? (t ? lay.off_q1 : lay.off_q0) : SMEM_Q + t * QTILE_BYTES)));
-    const uint64_t desc_k = desc_kmajor(smem_u32(smem + (VER == 7 ? lay.off_k : SMEM_K)));
-    const uint64_t desc_v = desc_kmajor(smem_u32(smem + (VER == 7 ? lay.off_v : SMEM_V)));
-    const uint32_t slot = tmem_base + t * TILE_COLS;
-    const uint32_t idesc_o = umma_idesc(0, 128, HD);
-    uint32_t uses = 0, item_n = 0;
-    int nx_start = 0, nx_end = 0;
-    if ((int)blockIdx.x < n_items) {
-      nx_start = cu_seqlens[blockIdx.x / heads];
-      nx_end = cu_seqlens[blockIdx.x / heads + 1];
-    }
-    // The two slots run chains of equal length: started together they stay in phase -- both softmax groups fight for
-    // the XU / issue slots at the same time and the tensor pipe idles meanwhile (trace of the first two-warp build).
-    // Slot 1 therefore starts half a chain late; the hand-shakes keep the offset.
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      const int start = nx_start, len = nx_end - nx_start;
-      if (it + (int)gridDim.x < n_items) {
-        const int nseq = (it + (int)gridDim.x) / heads;
-        nx_start = cu_seqlens[nseq];
-        nx_end = cu_seqlens[nseq + 1];
-      }
-      const int set = item_n & 1;
-      const uint32_t set_par = (item_n >> 1) & 1;
-      const int n_mt = (len + 127) >> 7;
-      if (t >= n_mt) {  // this item has no second tile: the slot still releases the operand set (VER 7)
-        if (VER == 7 && elect_one()) {
-          mbar_arrive(&bar_kfree[set]);
-          mbar_arrive(&bar_vfree[set]);
-        }
-        __syncwarp();
-        continue;
-      }
-      const int NK = ((start & 7) + len + 15) & ~15;
-      const int nks = NK >> 4, ks0 = (nks + 1) >> 1;
-      const uint64_t set_off = (uint64_t)((set * set_bytes) >> 4);
-      const uint64_t da = desc_q + set_off, db = desc_k + set_off, dv = desc_v + set_off;
-      const uint32_t idesc_s = umma_idesc(0, 128, NK);
-      spin(&bar_k[set], set_par);
-      spin(&bar_q[set], set_par);
-      if (uses > 0) spin(&bar_otfree[t], (uses - 1) & 1);  // O_t of the previous item has been read out
-      if (uses == 0 && t == 1) __nanosleep(2400);  // (after the first operands have landed: their latency would swallow it)
-      tc_fence_after();
-      if (elect_one()) {
+  // ---- Q fragments ----
+  constexpr int QK_STEPS = F16 ? 4 : 8;  // k-steps over head_dim
+  uint32_t qa[QK_STEPS][4];
+  {
+    const T* q_lo = qbase + (long long)min(q0 + warp * 16 + g, len - 1) * ld;
+    const T* q_hi = qbase + (long long)min(q0 + warp * 16 + g + 8, len - 1) * ld;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc_mma_bf16(slot, da + 2 * k, db + 2 * k, idesc_s, k != 0);
-        tc_commit(&bar_sfull[t]);
-        if (VER == 7) tc_commit(&bar_kfree[set]);
-      }
-      __syncwarp();
-      if (t == 0) ATT_TR(2);
-      if (t == 1) ATT_TR(3);
-      spin(&bar_v[set], set_par);
-      spin(&bar_pready[t], uses & 1);  // all eight softmax warps of the tile have written their P columns
-      tc_fence_after();
-      if (elect_one()) {
-        // K step ks: A = the 8 P columns of keys 16 ks .. 16 ks + 15 (the two key ranges of the softmax warps start at
-        // columns 0 and 16 ks0), B = 16 rows of V^T chunk ks / 4
-        uint32_t a_col = slot;
-        uint64_t b = dv;
-        for (int ks = 0; ks < nks; ++ks) {
-          if (ks == ks0) a_col = slot + 16 * ks0;
-          tc_mma_f16_ts(slot + V6_O_COL, a_col, b, idesc_o, ks != 0);
-          a_col += 8;
-          b += ((ks & 3) == 3) ? (uint64_t)((VT_CHUNK >> 4) - 6) : 2;
-        }
-        tc_commit(&bar_ofull[t]);
-        if (VER == 7) tc_commit(&bar_vfree[set]);
-      }
-      __syncwarp();
-      if (t == 0) ATT_TR(5);
-      if (t == 1) ATT_TR(6);
-      ++uses;
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp-uniform; one elected lane issues and commits) =========
-    uint32_t uses[2] = {0, 0};
-    uint32_t g[2] = {0, 0};  // P chunks consumed per tile slot
-    uint32_t item_n = 0;
-    const uint64_t desc_q0 = desc_kmajor(smem_u32(smem + SMEM_Q));
-    const uint64_t desc_k0 = desc_kmajor(smem_u32(smem + SMEM_K));
-    const uint64_t desc_v0 = desc_kmajor(smem_u32(smem + SMEM_V));
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      const int set = item_n & 1;
-      const uint32_t set_par = (item_n >> 1) & 1;
-      const uint64_t set_off = (uint64_t)((set * SET_BYTES) >> 4);
-      const uint64_t desc_q = desc_q0 + set_off, desc_k = desc_k0 + set_off, desc_v = desc_v0 + set_off;
-      const int seq = it / heads;
-      const int start = cu_seqlens[seq];
-      const int len = cu_seqlens[seq + 1] - start;
-      const int n_mt = (len + 127) >> 7;
-      const int NK = ((start & 7) + len + 15) & ~15;  // shifted key axis, padded to the UMMA N / K step
-      const int n_pc = (NK + 63) >> 6;
-      const uint32_t idesc_s = umma_idesc(0, 128, NK);
-      const uint32_t idesc_o = umma_idesc(0, 128, HD);
-      mbar_wait(&bar_k[set], set_par);
-      mbar_wait(&bar_q[set], set_par);
-      ATT_TR(1);
-      // ---- S_t = Q_t K^T for both tiles ----
-      for (int t = 0; t < n_mt; ++t) {
-        if (uses[t] > 0) mbar_wait(&bar_otfree[t], (uses[t] - 1) & 1);  // S_t / O_t columns free again
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t da = desc_q + (uint64_t)((t * QTILE_BYTES) >> 4);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)  // 4 x 16 of the 64 head dims
-            tc_mma_bf16(tmem_base + t * TILE_COLS, da + 2 * k, desc_k + 2 * k, idesc_s, k != 0);
-          tc_commit(&bar_sfull[t]);
-        }
-        __syncwarp();
-        ATT_TR(2 + t);
-      }
-      // ---- O_t += P_t chunk * V chunk, the two tiles interleaved ----
-      mbar_wait(&bar_v[set], set_par);
-      ATT_TR(4);
-      for (int pc = 0; pc < n_pc; ++pc) {
-        const int keys = min(64, NK - pc * 64);
-        for (int t = 0; t < n_mt; ++t) {
-          mbar_wait(&bar_pready[t], g[t] & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t da = desc_q + (uint64_t)((t * QTILE_BYTES) >> 4);
-            const uint64_t db = desc_v + (uint64_t)((pc * VT_CHUNK) >> 4);
-            for (int k = 0; k < keys / 16; ++k)
-              tc_mma_bf16(tmem_base + t * TILE_COLS, da + 2 * k, db + 2 * k, idesc_o, (pc | k) != 0);
-            tc_commit(&bar_pfree[t]);
-            if (pc == n_pc - 1) tc_commit(&bar_ofull[t]);
-          }
-          __syncwarp();
-          ATT_TR(5 + 2 * pc + t);
-          ++g[t];
-        }
-      }
-      for (int t = 0; t < n_mt; ++t) ++uses[t];
-    }
-  } else if constexpr (VER == 4) {
-    // ===================== softmax + epilogue, 16 warps: tile = (warp - 2) / 8, column half = ((warp - 2) / 4) & 1 ====
-    const int sw = warp - 2;
-    const int grp = sw >> 3, half = (sw >> 2) & 1;
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const uint32_t t_lane = tmem_base + (uint32_t(q * 32) << 16) + grp * TILE_COLS;
-    constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
-    const int ldc = heads * HD;
-    const int r_tile = q * 32 + lane;  // row inside the 128-row tile
-    float* xmax = reinterpret_cast<float*>(smem + (VER == 7 ? lay.off_xchg : SMEM_XCHG)) + (grp * 128 + r_tile) * 2;
-    float* xsum = xmax + 512;
-    const uint32_t pair_bar = 1 + grp * 4 + q;  // named barrier of the two warps that share these 32 rows
-    uint32_t uses = 0, G = 0, item_n = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      uint8_t* sm = smem + (item_n & 1) * SET_BYTES;
-      uint8_t* p_row = sm + SMEM_Q + grp * QTILE_BYTES + r_tile * 128;
-      uint8_t* o_row = sm + SMEM_V + grp * QTILE_BYTES + r_tile * 128;
-      const uint8_t* stg = sm + SMEM_V + grp * QTILE_BYTES + q * 32 * 128;
-      const int seq = it / heads, h = it % heads;
-      const int start = cu_seqlens[seq];
-      const int len = cu_seqlens[seq + 1] - start;
-      const int n_mt = (len + 127) >> 7;
-      if (grp >= n_mt) continue;
-      const int shift = start & 7;
-      const int Lk = shift + len;
-      const int NK = (Lk + 15) & ~15;
-      const int n_pc = (NK + 63) >> 6;
-      mbar_wait(&bar_sfull[grp], uses & 1);
-      tc_fence_after();
-      const bool tr = (q == 0 && half == 0);  // one warp per tile stamps: slots 13.. (tile 0), 22.. (tile 1)
-      if (tr) ATT_TR(13 + 9 * grp);
-      float mb = 0.f, sum = 1.f;
-      if (grp * 128 + q * 32 >= len) {
-        // all 32 rows beyond the sequence (both warps of the pair take this branch): only the chunk hand-shake
-        for (int pc = 0; pc < n_pc; ++pc, ++G) {
-          mbar_wait(&bar_pfree[grp], (G & 1) ^ 1);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar_pready[grp]);
-        }
+    for (int ks = 0; ks < QK_STEPS; ++ks) {
+      if (F16) {
+        const uint32_t* lo = reinterpret_cast<const uint32_t*>(q_lo + ks * 16);
+        const uint32_t* hi = reinterpret_cast<const uint32_t*>(q_hi + ks * 16);
+        qa[ks][0] = lo[t]; qa[ks][1] = hi[t]; qa[ks][2] = lo[t + 4]; qa[ks][3] = hi[t + 4];
       } else {
-        // pass 1: maximum of this half's columns, then the row maximum through shared memory
-        float mx0 = -INFINITY, mx1 = -INFINITY;
-        for (int pc = 0; pc < n_pc; ++pc) {
-          const int cb = pc * 64 + half * 32;
-          if (cb >= Lk) break;
-          uint32_t r[32];
-          tmem_ld_32x32(t_lane + cb, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int gi = 0; gi < 2; ++gi) {
-            const int c0 = cb + gi * 16;
-            if (c0 >= shift && c0 + 16 <= Lk) {
-#pragma unroll
-              for (int j = 0; j < 16; j += 4) {
-                mx0 = max3(mx0, __uint_as_float(r[gi * 16 + j]), __uint_as_float(r[gi * 16 + j + 1]));
-                mx1 = max3(mx1, __uint_as_float(r[gi * 16 + j + 2]), __uint_as_float(r[gi * 16 + j + 3]));
-              }
-            } else if (c0 < Lk) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (c0 + j >= shift && c0 + j < Lk) mx0 = fmaxf(mx0, __uint_as_float(r[gi * 16 + j]));
-            }
-          }
-        }
-        xmax[half] = fmaxf(mx0, mx1);
-        asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-        mb = fmaxf(xmax[0], xmax[1]) * SCALE_LOG2;
-        if (tr) ATT_TR(14 + 9 * grp);
-        // pass 2: this half's 32 columns of every 64-key chunk
-        const uint64_t scale2 = pack2(SCALE_LOG2, SCALE_LOG2), nmb2 = pack2(-mb, -mb);
-        uint64_t acc2 = pack2(0.f, 0.f);
-        sum = 0.f;
-        for (int pc = 0; pc < n_pc; ++pc, ++G) {
-          const int cb = pc * 64 + half * 32;
-          uint32_t pk[16];  // 32 fp16 values of this row; granules >= NK stay unwritten and unstored
-          if (cb < NK) {
-            uint32_t r[32];
-            tmem_ld_32x32(t_lane + cb, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int gi = 0; gi < 2; ++gi) {
-              const uint32_t* rr = r + gi * 16;
-              const int c0 = cb + gi * 16;
-              if (c0 >= shift && c0 + 16 <= Lk) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 2) {
-                  float a, b;
-                  const uint64_t x2 = fma2(pack2(__uint_as_float(rr[j]), __uint_as_float(rr[j + 1])), scale2, nmb2);
-                  if (j == 2 || j == 8 || j == 12) {  // 3 of the 8 pairs: polynomial, off the XU pipe
-                    ex2_poly2(x2, a, b);
-                  } else {
-                    unpack2(x2, a, b);
-                    a = fast_ex2(a);
-                    b = fast_ex2(b);
-                  }
-                  acc2 = add2(acc2, pack2(a, b));
-                  pk[gi * 8 + (j >> 1)] = pack_f16x2(a, b);
-                }
-              } else if (c0 < NK) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 2) {
-                  float a = 0.f, b = 0.f;
-                  if (c0 + j >= shift && c0 + j < Lk) a = fast_ex2(fmaf(__uint_as_float(rr[j]), SCALE_LOG2, -mb));
-                  if (c0 + j + 1 >= shift && c0 + j + 1 < Lk)
-                    b = fast_ex2(fmaf(__uint_as_float(rr[j + 1]), SCALE_LOG2, -mb));
-                  sum += a + b;
-                  pk[gi * 8 + (j >> 1)] = pack_f16x2(a, b);
-                }
-              }
-            }
-          }
-          const int n_slots = min(64, NK - pc * 64) >> 3;  // 16-byte slots the P V MMAs of this chunk read
-          mbar_wait(&bar_pfree[grp], (G & 1) ^ 1);  // the previous chunk's MMAs have read the buffer
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {  // this half's slots 4 half .. 4 half + 3 (keys 8 slot .. 8 slot + 7)
-            const int j = 4 * half + jj;
-            if (j < n_slots)
-              *reinterpret_cast<uint4*>(p_row + ((j ^ (r_tile & 7)) << 4)) =
-                  make_uint4(pk[4 * jj], pk[4 * jj + 1], pk[4 * jj + 2], pk[4 * jj + 3]);
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar_pready[grp]);
-          if (tr && pc < 4) ATT_TR(15 + 9 * grp + pc);
-        }
-        float s_lo, s_hi;
-        unpack2(acc2, s_lo, s_hi);
-        xsum[half] = sum + (s_lo + s_hi);
-        asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-        sum = xsum[0] + xsum[1];
+        const float* lo = reinterpret_cast<const float*>(q_lo) + ks * 8;
+        const float* hi = reinterpret_cast<const float*>(q_hi) + ks * 8;
+        qa[ks][0] = __float_as_uint(lo[t]); qa[ks][1] = __float_as_uint(hi[t]);
+        qa[ks][2] = __float_as_uint(lo[t + 4]); qa[ks][3] = __float_as_uint(hi[t + 4]);
       }
-      const float inv = 1.0f / sum;
-      // epilogue: this half's 32 head dims of O / sum -> fp16 -> swizzled staging -> 64-byte row segments of ctx
-      mbar_wait(&bar_ofull[grp], uses & 1);
-      tc_fence_after();
-      if (tr) ATT_TR(19 + 9 * grp);
-      uint32_t o[32];
-      tmem_ld_32x32(t_lane + half * 32, o);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_otfree[grp]);
-      if (tr) ATT_TR(20 + 9 * grp);
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int j = 4 * half + jj;  // 16-byte slot = head dims 8j .. 8j+7
-        const uint32_t* ov = o + 8 * jj;
-        *reinterpret_cast<uint4*>(o_row + ((j ^ (r_tile & 7)) << 4)) =
-            make_uint4(pack_f16x2(__uint_as_float(ov[0]) * inv, __uint_as_float(ov[1]) * inv),
-                       pack_f16x2(__uint_as_float(ov[2]) * inv, __uint_as_float(ov[3]) * inv),
-                       pack_f16x2(__uint_as_float(ov[4]) * inv, __uint_as_float(ov[5]) * inv),
-                       pack_f16x2(__uint_as_float(ov[6]) * inv, __uint_as_float(ov[7]) * inv));
-      }
-      __syncwarp();
-      const int row0 = grp * 128 + q * 32;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {  // 8 rows x 64 bytes per instruction
-        const int rr = 8 * i + (lane >> 2);
-        const int rt = q * 32 + rr;
-        const int j = 4 * half + (lane & 3);
-        const uint4 d = *reinterpret_cast<const uint4*>(stg + rr * 128 + ((j ^ (rt & 7)) << 4));
-        if (row0 + rr < len)
-          *reinterpret_cast<uint4*>(ctx + (long long)(start + row0 + rr) * ldc + h * HD + j * 8) = d;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_ofree[grp]);
-      if (tr) ATT_TR(21 + 9 * grp);
-      ++uses;
     }
-  } else if constexpr (VER >= 6) {
-    // (warp 18, the second MMA issuer, took the branch above)
-    // ===================== softmax + epilogue, VER 6 / 7: P never leaves tensor memory =====================
-    // VER 4 / 5 pass P through shared memory in 64-key chunks: four store -> fence.proxy.async -> mbarrier -> MMA ->
-    // commit round trips per tile (the trace: ~1.3k cycles each).  Here the two warps of a row split the KEY AXIS in
-    // two contiguous ranges ([0, 16 ks0) and [16 ks0, NK), ks0 = ceil(NK / 32)); each turns its scores into fp16
-    // probabilities 16 keys at a time and writes them back with tcgen05.st over the START of its own range -- step j
-    // of a range that begins at column c lands in columns [c + 8 j, c + 8 j + 8), which that same thread has already
-    // read (8 j + 8 <= 16 j + 16), so no ordering between threads is needed.  When all eight warps of the tile have
-    // arrived ONCE, the MMA warp issues every K step of O_t = P V with the A operand in tensor memory; O_t accumulates
-    // in columns [192, 256) (S is dead by then).  Granule-pipelined loads and the per-tile pipelines as VER 5.
-    const int sw = warp - 2;
-    const int grp = sw >> 3, half = (sw >> 2) & 1;
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const uint32_t t_lane = tmem_base + (uint32_t(q * 32) << 16) + grp * TILE_COLS;
-    constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
-    const int ldc = heads * HD;
-    const int r_tile = q * 32 + lane;  // row inside the 128-row tile
-    float* xmax = reinterpret_cast<float*>(smem + (VER == 7 ? lay.off_xchg : SMEM_XCHG)) + (grp * 128 + r_tile) * 2;
-    float* xsum = xmax + 512;
-    const uint32_t pair_bar = 1 + grp * 4 + q;  // named barrier of the two warps that share these 32 rows
-    uint32_t uses = 0, G = 0, item_n = 0;
-    int nx_start = 0, nx_end = 0;  // raw loads of the next item's bounds: first touched when that item begins
-    if ((int)blockIdx.x < n_items) {
-      nx_start = cu_seqlens[blockIdx.x / heads];
-      nx_end = cu_seqlens[blockIdx.x / heads + 1];
+  }
+
+  float o[8][4];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
+  const int n_kv = (shift + len + BKV - 1) / BKV;
+
+  auto load_tile = [&](int j, int buf) {
+    const int p0 = kstart + j * BKV;  // first key position (absolute token index) of the tile
+    T* kd = Ks + buf * Cfg::kTile;
+    T* vd = Vs + buf * Cfg::kTile;
+    constexpr int CPR = HD / Cfg::kPerChunk;  // 16-byte chunks per 64-element row
+#pragma unroll
+    for (int i = 0; i < BKV * CPR / THREADS; ++i) {
+      const int idx = tid + i * THREADS;
+      const int r = idx / CPR, c = (idx % CPR) * Cfg::kPerChunk;
+      // K row r = key p0 + r (zero outside the sequence); V^T row r = head dim r, keys p0 + c ..
+      const int key = p0 + r;
+      const bool kin = key >= start && key < start + len;
+      cp_async16(kd + r * LDS + c, kbase + (long long)(kin ? key : start) * ld + c, kin ? 16 : 0);
+      const long long vk = p0 + c;
+      const int vbytes = vk >= tokens ? 0 : (int)min(16ll, (tokens - vk) * Cfg::kElem);
+      cp_async16(vd + r * LDS + c, vtbase + (long long)r * vt_ld + (vbytes ? vk : 0), vbytes);
     }
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      // output staging: VER 6: the tile's own Q buffer of this item's set (dead once S_t is complete; not the V^T
-      // region VER 1..4 use: the other tile slot runs on its own clock and may still need every V^T chunk);
-      // VER 7: a buffer of its own -- the Q tiles are being refilled for the item after next by then
-      uint8_t* stage_t = VER == 7 ? smem + lay.off_stage + grp * QTILE_BYTES
-                                  : smem + (item_n & 1) * SET_BYTES + SMEM_Q + grp * QTILE_BYTES;
-      uint8_t* o_row = stage_t + r_tile * 128;
-      const uint8_t* stg = stage_t + q * 32 * 128;
-      const int h = it % heads;
-      const int start = nx_start, len = nx_end - nx_start;
-      if (it + (int)gridDim.x < n_items) {  // the next item's bounds: in flight while this item is processed
-        const int nseq = (it + (int)gridDim.x) / heads;
-        nx_start = cu_seqlens[nseq];
-        nx_end = cu_seqlens[nseq + 1];
-      }
-      const int n_mt = (len + 127) >> 7;
-      if (grp >= n_mt) continue;
-      const int shift = start & 7;
-      const int Lk = shift + len;
-      const int NK = (Lk + 15) & ~15;
-      const int n_pc = (NK + 63) >> 6;
-      mbar_wait(&bar_sfull[grp], uses & 1);
-      tc_fence_after();
-      const bool tr = (q == 0 && half == 0);  // one warp per tile stamps: slots 13.. (tile 0), 22.. (tile 1)
-      if (tr) ATT_TR(13 + 9 * grp);
-      float mb = 0.f, sum = 1.f;
-      if (grp * 128 + q * 32 >= len) {
-        // all 32 rows beyond the sequence (both warps of the pair take this branch): only the tile's hand-shake (their
-        // P columns keep whatever bits S left there: rows of a product are independent and these are never stored)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_pready[grp]);
-        ++G;
-      } else {
-        // pass 1: maximum of this warp's key range, 32 columns per load (few, large loads: this pass is all latency)
-        float mx0 = -INFINITY, mx1 = -INFINITY;
-        const int nks = NK >> 4, ks0 = (nks + 1) >> 1;
-        const int k_first = half ? ks0 : 0, nq = half ? nks - ks0 : ks0;  // this warp's 16-key steps
-        const int cb0 = 16 * k_first;
-        auto col = [&](int g) { return cb0 + 16 * g; };
-        {
-          uint32_t w[32];
-          const int n32 = (nq + 1) >> 1;  // loads of 32 columns (the last one may reach 16 columns past the range)
-          for (int g = 0; g < n32; ++g) {
-            tmem_ld_32x32(t_lane + cb0 + 32 * g, w);
-            tmem_ld_wait();
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {  // the two 16-key steps of this load (the second may lie past the range)
-              const int c0 = cb0 + 32 * g + 16 * hh;
-              if (2 * g + hh < nq) {
-                if (c0 >= shift && c0 + 16 <= Lk) {
-#pragma unroll
-                  for (int j = 0; j < 16; j += 4) {
-                    mx0 = max3(mx0, __uint_as_float(w[16 * hh + j]), __uint_as_float(w[16 * hh + j + 1]));
-                    mx1 = max3(mx1, __uint_as_float(w[16 * hh + j + 2]), __uint_as_float(w[16 * hh + j + 3]));
-                  }
-                } else if (c0 < Lk) {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j)
-                    if (c0 + j >= shift && c0 + j < Lk) mx0 = fmaxf(mx0, __uint_as_float(w[16 * hh + j]));
-                }
-              }
-            }
-          }
-        }
-        uint32_t r[2][16];
-        if (nq > 0) tmem_ld_32x16(t_lane + cb0, r[0]);  // pass 2's first granule: under way during the exchange below
-        xmax[half] = fmaxf(mx0, mx1);
-        asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-        mb = fmaxf(xmax[0], xmax[1]) * SCALE_LOG2;
-        if (tr) ATT_TR(14 + 9 * grp);
-        // pass 2: the same granules; each becomes 8 columns of fp16 P written over this warp's own consumed range
-        const uint64_t scale2 = pack2(SCALE_LOG2, SCALE_LOG2), nmb2 = pack2(-mb, -mb);
-        uint64_t acc2 = pack2(0.f, 0.f);
-        sum = 0.f;
-        for (int q0 = 0; q0 < nq; q0 += 2) {
-#pragma unroll
-          for (int b = 0; b < 2; ++b) {
-            const int q = q0 + b, c0 = col(q);
-            if (q < nq) {
-              tmem_ld_wait();
-              if (q + 1 < nq) tmem_ld_32x16(t_lane + col(q + 1), r[b ^ 1]);
-              uint32_t pk[8];
-              if (c0 >= shift && c0 + 16 <= Lk) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 2) {
-                  float x0, x1;
-                  const uint64_t x2 = fma2(pack2(__uint_as_float(r[b][j]), __uint_as_float(r[b][j + 1])), scale2, nmb2);
-                  if ((POLY >= 1 && j == 8) || (POLY >= 2 && j == 2) || (POLY >= 3 && j == 12)) {  // FMA-pipe exponentials
-                    ex2_poly2(x2, x0, x1);
-                  } else {
-                    unpack2(x2, x0, x1);
-                    x0 = fast_ex2(x0);
-                    x1 = fast_ex2(x1);
-                  }
-                  acc2 = add2(acc2, pack2(x0, x1));
-                  pk[j >> 1] = pack_f16x2(x0, x1);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; j += 2) {
-                  float x0 = 0.f, x1 = 0.f;
-                  if (c0 + j >= shift && c0 + j < Lk) x0 = fast_ex2(fmaf(__uint_as_float(r[b][j]), SCALE_LOG2, -mb));
-                  if (c0 + j + 1 >= shift && c0 + j + 1 < Lk)
-                    x1 = fast_ex2(fmaf(__uint_as_float(r[b][j + 1]), SCALE_LOG2, -mb));
-                  sum += x0 + x1;
-                  pk[j >> 1] = pack_f16x2(x0, x1);
-                }
-              }
-              tmem_st_32x8(t_lane + cb0 + 8 * q, pk);
-            }
-          }
-        }
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_pready[grp]);
-        if (tr) ATT_TR(15 + 9 * grp);
-        ++G;
-        float s_lo, s_hi;
-        unpack2(acc2, s_lo, s_hi);
-        xsum[half] = sum + (s_lo + s_hi);
-        asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-        sum = xsum[0] + xsum[1];
-      }
-      const float inv = 1.0f / sum;
-      // epilogue: this half's 32 head dims of O / sum -> fp16 -> swizzled staging -> 64-byte row segments of ctx
-      mbar_wait(&bar_ofull[grp], uses & 1);
-      tc_fence_after();
-      if (tr) ATT_TR(19 + 9 * grp);
-      uint32_t o[32];
-      tmem_ld_32x32(t_lane + V6_O_COL + half * 32, o);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_otfree[grp]);
-      if (tr) ATT_TR(20 + 9 * grp);
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int j = 4 * half + jj;  // 16-byte slot = head dims 8j .. 8j+7
-        const uint32_t* ov = o + 8 * jj;
-        *reinterpret_cast<uint4*>(o_row + ((j ^ (r_tile & 7)) << 4)) =
-            make_uint4(pack_f16x2(__uint_as_float(ov[0]) * inv, __uint_as_float(ov[1]) * inv),
-                       pack_f16x2(__uint_as_float(ov[2]) * inv, __uint_as_float(ov[3]) * inv),
-                       pack_f16x2(__uint_as_float(ov[4]) * inv, __uint_as_float(ov[5]) * inv),
-                       pack_f16x2(__uint_as_float(ov[6]) * inv, __uint_as_float(ov[7]) * inv));
-      }
-      __syncwarp();
-      const int row0 = grp * 128 + q * 32;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {  // 8 rows x 64 bytes per instruction
-        const int rr = 8 * i + (lane >> 2);
-        const int rt = q * 32 + rr;
-        const int j = 4 * half + (lane & 3);
-        const uint4 d = *reinterpret_cast<const uint4*>(stg + rr * 128 + ((j ^ (rt & 7)) << 4));
-        if (row0 + rr < len)
-          *reinterpret_cast<uint4*>(ctx + (long long)(start + row0 + rr) * ldc + h * HD + j * 8) = d;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_ofree[grp]);
-      if (tr) ATT_TR(21 + 9 * grp);
-      ++uses;
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+
+  load_tile(0, 0);
+  constexpr float SL2 = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+
+  for (int j = 0; j < n_kv; ++j) {
+    const int buf = j & 1;
+    if (j + 1 < n_kv) {
+      load_tile(j + 1, buf ^ 1);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
-  } else {
-    // ===================== softmax + epilogue: group 0 = warps 2..5 (tile 0), group 1 = warps 6..9 =====
-    const int grp = (warp - 2) >> 2;
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const uint32_t t_lane = tmem_base + (uint32_t(q * 32) << 16) + grp * TILE_COLS;
-    constexpr float SCALE_LOG2 = 0.125f * 1.4426950408889634f;
-    const int ldc = heads * HD;
-    const int r_tile = q * 32 + lane;  // row inside the 128-row tile
-    const int sub_r = lane >> 3, sub_c = lane & 7;
-    uint32_t uses = 0, G = 0, item_n = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++item_n) {
-      uint8_t* sm = smem + (item_n & 1) * SET_BYTES;  // this item's operand set
-      // P chunk buffer of this tile: [128 rows][128 B] (the tile's Q buffer, dead after S_t); this thread's row
-      uint8_t* p_row = sm + SMEM_Q + grp * QTILE_BYTES + r_tile * 128;
-      // output staging: 16 KB of the V^T region per tile (V^T is dead once O_t is complete)
-      uint8_t* o_row = sm + SMEM_V + grp * QTILE_BYTES + r_tile * 128;
-      const uint8_t* stg = sm + SMEM_V + grp * QTILE_BYTES + q * 32 * 128;  // this warp's 32 rows
-      const int seq = it / heads, h = it % heads;
-      const int start = cu_seqlens[seq];
-      const int len = cu_seqlens[seq + 1] - start;
-      const int n_mt = (len + 127) >> 7;
-      if (grp >= n_mt) continue;  // single-tile item: group 1 has nothing to do
-      const int shift = start & 7;  // keys live at columns [shift, shift + len) of S
-      const int Lk = shift + len;
-      const int n_chunks = (Lk + 31) >> 5;
-      const int n_pc = (((Lk + 15) & ~15) + 63) >> 6;
-      mbar_wait(&bar_sfull[grp], uses & 1);
-      tc_fence_after();
-      float mb, sum = 0.f;
-      if constexpr (VER >= 2) {
-        if (grp * 128 + q * 32 >= len) {
-          // all 32 query rows of this warp lie beyond the sequence (rows 224..255 at 197 tokens): nothing to
-          // compute -- the P rows it would write feed output rows that are never stored -- but the chunk
-          // hand-shake with the MMA warp still counts four arrivals per tile
-          mb = 0.f;
-          sum = 1.f;
-          for (int pc = 0; pc < n_pc; ++pc, ++G) {
-            mbar_wait(&bar_pfree[grp], (G & 1) ^ 1);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bar_pready[grp]);
-          }
+    __syncthreads();
+    const T* kt = Ks + buf * Cfg::kTile;
+    const T* vt = Vs + buf * Cfg::kTile;
+
+    // ---- S = Q K^T: 16 x 64 per warp ----
+    float s[8][4];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+      const T* kr = kt + (nt * 8 + g) * LDS;
+#pragma unroll
+      for (int ks = 0; ks < QK_STEPS; ++ks) {
+        if (F16) {
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(kr + ks * 16);
+          mma_f16(s[nt], qa[ks], w[t], w[t + 4]);
         } else {
-          const int NK = (Lk + 15) & ~15;  // the UMMA key count of this item (MMA warp: same expression)
-          // pass 1: row maximum over the valid keys
-          float mx0 = -INFINITY, mx1 = -INFINITY;
-          for (int c = 0; c < n_chunks; ++c) {
-            uint32_t r[32];
-            tmem_ld_32x32(t_lane + c * 32, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int gi = 0; gi < 2; ++gi) {
-              const int c0 = c * 32 + gi * 16;
-              if (c0 >= shift && c0 + 16 <= Lk) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) {
-                  mx0 = max3(mx0, __uint_as_float(r[gi * 16 + j]), __uint_as_float(r[gi * 16 + j + 1]));
-                  mx1 = max3(mx1, __uint_as_float(r[gi * 16 + j + 2]), __uint_as_float(r[gi * 16 + j + 3]));
-                }
-              } else if (c0 < Lk) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                  if (c0 + j >= shift && c0 + j < Lk) mx0 = fmaxf(mx0, __uint_as_float(r[gi * 16 + j]));
-              }
-            }
-          }
-          mb = fmaxf(mx0, mx1) * SCALE_LOG2;
-          // pass 2, per 64-key chunk (see VER 1 below), in 16-key granules
-          const uint64_t scale2 = pack2(SCALE_LOG2, SCALE_LOG2), nmb2 = pack2(-mb, -mb);
-          uint64_t acc2 = pack2(0.f, 0.f);
-          for (int pc = 0; pc < n_pc; ++pc, ++G) {
-            uint32_t r0[32], r1[32];
-            tmem_ld_32x32(t_lane + pc * 64, r0);
-            tmem_ld_32x32(t_lane + pc * 64 + 32, r1);
-            tmem_ld_wait();
-            uint32_t pk[32];  // 64 fp16 values of this row; words of granules >= NK stay unwritten and unstored
-#pragma unroll
-            for (int gi = 0; gi < 4; ++gi) {
-              const uint32_t* rr = gi < 2 ? r0 + gi * 16 : r1 + (gi - 2) * 16;
-              const int c0 = pc * 64 + gi * 16;
-              if (c0 >= shift && c0 + 16 <= Lk) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 2) {
-                  float a, b;
-                  const uint64_t x2 = fma2(pack2(__uint_as_float(rr[j]), __uint_as_float(rr[j + 1])), scale2, nmb2);
-                  if (VER == 3 && (j == 2 || j == 8 || j == 12)) {  // 3 of the 8 pairs: polynomial, off the XU pipe
-                    ex2_poly2(x2, a, b);
-                  } else {
-                    unpack2(x2, a, b);
-                    a = fast_ex2(a);
-                    b = fast_ex2(b);
-                  }
-                  acc2 = add2(acc2, pack2(a, b));
-                  pk[gi * 8 + (j >> 1)] = pack_f16x2(a, b);
-                }
-              } else if (c0 < NK) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 2) {
-                  float a = 0.f, b = 0.f;
-                  if (c0 + j >= shift && c0 + j < Lk) a = fast_ex2(fmaf(__uint_as_float(rr[j]), SCALE_LOG2, -mb));
-                  if (c0 + j + 1 >= shift && c0 + j + 1 < Lk)
-                    b = fast_ex2(fmaf(__uint_as_float(rr[j + 1]), SCALE_LOG2, -mb));
-                  sum += a + b;
-                  pk[gi * 8 + (j >> 1)] = pack_f16x2(a, b);
-                }
-              }
-            }
-            const int n_slots = min(64, NK - pc * 64) >> 3;  // 16-byte slots the P V MMAs of this chunk read
-            mbar_wait(&bar_pfree[grp], (G & 1) ^ 1);  // the previous chunk's MMAs have read the buffer
-#pragma unroll
-            for (int j = 0; j < 8; ++j)  // 16-byte slot j = keys 8j .. 8j+7
-              if (j < n_slots)
-                *reinterpret_cast<uint4*>(p_row + ((j ^ (r_tile & 7)) << 4)) =
-                    make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bar_pready[grp]);
-          }
-          float s_lo, s_hi;
-          unpack2(acc2, s_lo, s_hi);
-          sum += s_lo + s_hi;
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(kr) + ks * 8;
+          mma_tf32(s[nt], qa[ks], w[t], w[t + 4]);
         }
-      } else {
-      // pass 1: row maximum over the valid keys
-      float mx = -INFINITY;
-      for (int c = 0; c < n_chunks; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_lane + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (c * 32 + j >= shift && c * 32 + j < Lk) mx = fmaxf(mx, __uint_as_float(r[j]));
       }
-      mb = mx * SCALE_LOG2;
-      // pass 2, per 64-key chunk: p = exp2((s - max) / 8 * log2 e) -> row sum, fp16 P into the swizzled
-      // smem chunk (A operand of the P V MMA)
-      for (int pc = 0; pc < n_pc; ++pc, ++G) {
-        uint32_t r0[32], r1[32];
-        tmem_ld_32x32(t_lane + pc * 64, r0);
-        tmem_ld_32x32(t_lane + pc * 64 + 32, r1);
-        tmem_ld_wait();
-        uint32_t pk[32];  // 64 fp16 values of this row
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
-          const int k0 = pc * 64 + j, k1 = k0 + 32;
-          if (k0 >= shift && k0 < Lk) a0 = fast_ex2(fmaf(__uint_as_float(r0[j]), SCALE_LOG2, -mb));
-          if (k0 + 1 >= shift && k0 + 1 < Lk) a1 = fast_ex2(fmaf(__uint_as_float(r0[j + 1]), SCALE_LOG2, -mb));
-          if (k1 >= shift && k1 < Lk) b0 = fast_ex2(fmaf(__uint_as_float(r1[j]), SCALE_LOG2, -mb));
-          if (k1 + 1 >= shift && k1 + 1 < Lk) b1 = fast_ex2(fmaf(__uint_as_float(r1[j + 1]), SCALE_LOG2, -mb));
-          sum += (a0 + a1) + (b0 + b1);
-          pk[j >> 1] = pack_f16x2(a0, a1);
-          pk[16 + (j >> 1)] = pack_f16x2(b0, b1);
-        }
-        mbar_wait(&bar_pfree[grp], (G & 1) ^ 1);  // the previous chunk's MMAs have read the buffer
-#pragma unroll
-        for (int j = 0; j < 8; ++j)  // 16-byte slot j = keys 8j .. 8j+7
-          *reinterpret_cast<uint4*>(p_row + ((j ^ (r_tile & 7)) << 4)) =
-              make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-        fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_pready[grp]);
-      }
-      }
-      const float inv = 1.0f / sum;
-      // epilogue: O / sum -> fp16 -> (swizzled smem transpose) -> 512-byte coalesced stores into ctx
-      mbar_wait(&bar_ofull[grp], uses & 1);
-      tc_fence_after();
-      uint32_t o0[32], o1[32];
-      tmem_ld_32x32(t_lane, o0);
-      tmem_ld_32x32(t_lane + 32, o1);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_otfree[grp]);  // the MMA warp may start the next item's S_t
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {  // 16-byte slot j = head dims 8j .. 8j+7
-        const uint32_t* o = (j < 4) ? (o0 + 8 * j) : (o1 + 8 * (j - 4));
-        *reinterpret_cast<uint4*>(o_row + ((j ^ (r_tile & 7)) << 4)) =
-            make_uint4(pack_f16x2(__uint_as_float(o[0]) * inv, __uint_as_float(o[1]) * inv),
-                       pack_f16x2(__uint_as_float(o[2]) * inv, __uint_as_float(o[3]) * inv),
-                       pack_f16x2(__uint_as_float(o[4]) * inv, __uint_as_float(o[5]) * inv),
-                       pack_f16x2(__uint_as_float(o[6]) * inv, __uint_as_float(o[7]) * inv));
-      }
-      __syncwarp();
-      const int row0 = grp * 128 + q * 32;  // first sequence row of this warp's 32
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int rr = 4 * i + sub_r;
-        const int rt = q * 32 + rr;  // row inside the tile (swizzle key)
-        const uint4 d = *reinterpret_cast<const uint4*>(stg + rr * 128 + ((sub_c ^ (rt & 7)) << 4));
-        if (row0 + rr < len)
-          *reinterpret_cast<uint4*>(ctx + (long long)(start + row0 + rr) * ldc + h * HD + sub_c * 8) = d;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_ofree[grp]);
-      ++uses;
     }
+    // ---- mask keys outside [start, start + len) (first and last tiles only) ----
+    const int rel0 = j * BKV - shift;  // key index inside the sequence of tile column 0
+    if (rel0 < 0 || rel0 + BKV > len) {
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const int k0 = rel0 + nt * 8 + 2 * t;
+        if (k0 < 0 || k0 >= len) { s[nt][0] = -INFINITY; s[nt][2] = -INFINITY; }
+        if (k0 + 1 < 0 || k0 + 1 >= len) { s[nt][1] = -INFINITY; s[nt][3] = -INFINITY; }
+      }
+    }
+    // ---- online softmax (base 2, scale folded in) ----
+    float mx_lo = -INFINITY, mx_hi = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      mx_lo = fmaxf(mx_lo, fmaxf(s[nt][0], s[nt][1]));
+      mx_hi = fmaxf(mx_hi, fmaxf(s[nt][2], s[nt][3]));
+    }
+    mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 1));
+    mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 2));
+    mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 1));
+    mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 2));
+    const float mn_lo = fmaxf(m_lo, mx_lo), mn_hi = fmaxf(m_hi, mx_hi);
+    // every row has a valid key in its first tile, so mn is finite from there on
+    const float sc_lo = fast_ex2((m_lo - mn_lo) * SL2), sc_hi = fast_ex2((m_hi - mn_hi) * SL2);
+    m_lo = mn_lo;
+    m_hi = mn_hi;
+    const float b_lo = mn_lo * SL2, b_hi = mn_hi * SL2;
+    float ps_lo = 0.f, ps_hi = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      s[nt][0] = fast_ex2(fmaf(s[nt][0], SL2, -b_lo));
+      s[nt][1] = fast_ex2(fmaf(s[nt][1], SL2, -b_lo));
+      s[nt][2] = fast_ex2(fmaf(s[nt][2], SL2, -b_hi));
+      s[nt][3] = fast_ex2(fmaf(s[nt][3], SL2, -b_hi));
+      ps_lo += s[nt][0] + s[nt][1];
+      ps_hi += s[nt][2] + s[nt][3];
+    }
+    l_lo = l_lo * sc_lo + ps_lo;
+    l_hi = l_hi * sc_hi + ps_hi;
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt) {
+      o[dt][0] *= sc_lo; o[dt][1] *= sc_lo; o[dt][2] *= sc_hi; o[dt][3] *= sc_hi;
+    }
+    // ---- O += P V ----
+    if (F16) {
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {  // 16 keys per step: n-tiles 2 ks and 2 ks + 1 of S
+        uint32_t pa[4];
+        pa[0] = pack_f16x2(s[2 * ks][0], s[2 * ks][1]);
+        pa[1] = pack_f16x2(s[2 * ks][2], s[2 * ks][3]);
+        pa[2] = pack_f16x2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
+        pa[3] = pack_f16x2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
+#pragma unroll
+        for (int dt = 0; dt < 8; ++dt) {
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(vt + (dt * 8 + g) * LDS + ks * 16);
+          mma_f16(o[dt], pa, w[t], w[t + 4]);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) {  // keys 2t / 2t+1 of the group <-> k-columns t / t+4
+        uint32_t pa[4];
+        pa[0] = __float_as_uint(round_tf32(s[ks][0]));
+        pa[1] = __float_as_uint(round_tf32(s[ks][2]));
+        pa[2] = __float_as_uint(round_tf32(s[ks][1]));
+        pa[3] = __float_as_uint(round_tf32(s[ks][3]));
+#pragma unroll
+        for (int dt = 0; dt < 8; ++dt) {
+          const float2 w = *reinterpret_cast<const float2*>(
+              reinterpret_cast<const float*>(vt) + (dt * 8 + g) * LDS + ks * 8 + 2 * t);
+          mma_tf32(o[dt], pa, __float_as_uint(w.x), __float_as_uint(w.y));
+        }
+      }
+    }
+    __syncthreads();  // everyone is done with buf before the next prefetch overwrites it
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // ---- finalize ----
+  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
+  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
+  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
+  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
+  const float inv_lo = 1.0f / l_lo, inv_hi = 1.0f / l_hi;
+  const int row_lo = q0 + warp * 16 + g, row_hi = row_lo + 8;
+  const long long ldc = (long long)heads * HD;
+#pragma unroll
+  for (int dt = 0; dt < 8; ++dt) {
+    const int col = h * HD + dt * 8 + 2 * t;
+    float2 a = make_float2(o[dt][0] * inv_lo, o[dt][1] * inv_lo);
+    float2 b = make_float2(o[dt][2] * inv_hi, o[dt][3] * inv_hi);
+    const long long r_lo = (long long)(start + row_lo) * ldc, r_hi = (long long)(start + row_hi) * ldc;
+    if (out_mode == 3) {
+      uint16_t* c16 = static_cast<uint16_t*>(ctx);
+      if (row_lo < len) *reinterpret_cast<uint32_t*>(c16 + r_lo + col) = pack_f16x2(a.x, a.y);
+      if (row_hi < len) *reinterpret_cast<uint32_t*>(c16 + r_hi + col) = pack_f16x2(b.x, b.y);
+      continue;
+    }
+    float* c32 = static_cast<float*>(ctx);
+    if (out_mode == 2) {  // split bf16 rows for a BF16X3 out-proj GEMM
+      if (row_lo < len) store_split2(c32 + r_lo, col, a.x, a.y);
+      if (row_hi < len) store_split2(c32 + r_hi, col, b.x, b.y);
+      continue;
+    }
+    if (out_mode == 1) {
+      a.x = round_tf32(a.x); a.y = round_tf32(a.y); b.x = round_tf32(b.x); b.y = round_tf32(b.y);
+    }
+    if (row_lo < len) *reinterpret_cast<float2*>(c32 + r_lo + col) = a;
+    if (row_hi < len) *reinterpret_cast<float2*>(c32 + r_hi + col) = b;
   }
 }
 
-}  // namespace
-
-static long long* g_att_trace = nullptr;  // debug hook: device buffer of 16 x 32 stamps (scripts/att_trace.py)
-extern "C" __attribute__((visibility("default"))) void mer_debug_attention_trace(long long* device_buffer) {
-  g_att_trace = device_buffer;
-}
-
-// <= 249 tokens: this file; 250 .. 505: attention_f16_long.cu (MER_ATT_F16_LONG=0 sends those back to the fp32-operand
-// kernels, for A/B runs)
-bool mer_attention_f16_supported(int max_seqlen) {
-  if (max_seqlen <= 0 || mer_attention_legacy()) return false;
-  if (max_seqlen <= 249) return true;
-  const char* e = getenv("MER_ATT_F16_LONG");
-  return (e == nullptr || atoi(e) != 0) && mer_attention_f16_long_supported(max_seqlen);
-}
-
-// qkv16: fp16 [tokens, 3*heads*64] (V columns unused), vt16: fp16 [heads*64, vt_ld] with vt[d, token],
-// ctx16: fp16 [tokens, heads*64]
-int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
-                             const int* cu_seqlens, int n_seq, long long tokens, int heads,
-                             cudaStream_t stream, int max_seqlen) {
-  MER_REQUIRE(qkv16 && vt16 && ctx16 && cu_seqlens, "mer_attention_f16: null operand");
-  MER_REQUIRE(vt_ld >= tokens && vt_ld % 8 == 0, "mer_attention_f16: V^T pitch %lld must be a multiple of 8 >= tokens",
-              vt_ld);
-  if (max_seqlen > 249)
-    return mer_attention_f16_long_launch(qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens, heads, stream, max_seqlen, 3);
-  if (max_seqlen <= 0) max_seqlen = 249;
-  // MER_ATT_F16_VER selects the kernel generation (see the header comments); read at every launch so that a test can
-  // run all of them in one process.  VER 7 needs its shared-memory plan to fit (sequences up to ~230 tokens), else 6.
-  const char* ver_env = getenv("MER_ATT_F16_VER");
-  int ver = ver_env ? atoi(ver_env) : 6;  // measured (profiles/r2_attention_f16_versions.json): 6 ~ 7 > 4 ~ 3 > 2 > 1
-  if (ver == 5) ver = 6;  // VER 5 (one polling MMA warp, P through shared memory) was measured slower than VER 3 and dropped
-  const char* poly_env = getenv("MER_ATT_F16_POLY");
-  const int poly = poly_env ? atoi(poly_env) : 1;
-  // VER 7 plan: exact-size boxes for K (all keys of the longest sequence, shifted by up to 7) and the second Q tile
-  AttLay lay;
-  memset(&lay, 0, sizeof(lay));
-  lay.k_rows = (max_seqlen + 7 + 15) & ~15;
-  if (lay.k_rows > 256) lay.k_rows = 256;
-  lay.q1_rows = max_seqlen > 128 ? ((max_seqlen - 128 + 7) & ~7) : 0;
-  auto up = [](int x) { return (x + 1023) & ~1023; };
-  lay.off_k = 0;
-  lay.off_v = up(lay.k_rows * 128);
-  lay.off_q0 = lay.off_v + ((lay.k_rows + 63) / 64) * VT_CHUNK;
-  lay.off_q1 = lay.off_q0 + QTILE_BYTES;
-  lay.set_bytes = lay.off_q1 + up(lay.q1_rows * 128);
-  lay.off_stage = 2 * lay.set_bytes;
-  lay.off_bar = lay.off_stage + 2 * QTILE_BYTES;
-  lay.off_xchg = lay.off_bar + 256;
-  const int smem7 = lay.off_xchg + 4096 + 1024;
-  if (ver == 7 && smem7 > 227 * 1024) ver = 6;
-  CUtensorMap tm, tv, tk, tq1;
-  const uint64_t qdims[2] = {(uint64_t)(3 * heads * HD), (uint64_t)tokens};
-  const uint64_t qstrides[1] = {(uint64_t)(3 * heads * HD) * 2ull};
-  {
-    const uint32_t box[2] = {64, 128};
-    if (int rc = mer_make_tmap(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv16, qdims, qstrides, box,
-                               CU_TENSOR_MAP_SWIZZLE_128B))
-      return rc;
-  }
-  {
-    const uint32_t box[2] = {64, (uint32_t)lay.k_rows};
-    if (int rc = mer_make_tmap(&tk, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv16, qdims, qstrides, box,
-                               CU_TENSOR_MAP_SWIZZLE_128B))
-      return rc;
-  }
-  {
-    const uint32_t box[2] = {64, (uint32_t)(lay.q1_rows > 0 ? lay.q1_rows : 8)};
-    if (int rc = mer_make_tmap(&tq1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qkv16, qdims, qstrides, box,
-                               CU_TENSOR_MAP_SWIZZLE_128B))
-      return rc;
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)tokens, (uint64_t)(heads * HD)};
-    const uint64_t strides[1] = {(uint64_t)vt_ld * 2ull};
-    const uint32_t box[2] = {64, HD};
-    if (int rc = mer_make_tmap(&tv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, vt16, dims, strides, box,
-                               CU_TENSOR_MAP_SWIZZLE_128B))
-      return rc;
-  }
-  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttLay, uint16_t*,
-                        const int*, int, int, long long*);
-  Kern kern = ver == 7 ? (poly == 0 ? attention_f16_kernel<7, 0> : poly == 1 ? attention_f16_kernel<7, 1>
-                                   : poly == 2 ? attention_f16_kernel<7, 2> : attention_f16_kernel<7, 3>)
-            : ver == 6 ? (poly == 1 ? attention_f16_kernel<6, 1> : attention_f16_kernel<6, 3>)
-            : ver == 4 ? attention_f16_kernel<4>
-            : ver == 3 ? attention_f16_kernel<3> : ver == 2 ? attention_f16_kernel<2> : attention_f16_kernel<1>;
+template <bool F16>
+int launch_vt(const void* qkv, const void* vt, long long vt_ld, void* ctx, const int* cu_seqlens, int n_seq,
+              long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream) {
+  MER_REQUIRE(qkv && vt && ctx && cu_seqlens, "mer_attention (V^T): null operand");
+  MER_REQUIRE(out_mode >= 0 && out_mode <= 3, "mer_attention (V^T): out_mode %d", out_mode);
+  using Cfg = AttCfg<F16>;
+  MER_REQUIRE(vt_ld >= tokens && vt_ld % Cfg::kPerChunk == 0,
+              "mer_attention (V^T): V^T pitch %lld must be a multiple of %d >= tokens", vt_ld, Cfg::kPerChunk);
+  MER_REQUIRE(max_seqlen > 0 && max_seqlen <= MAX_SEQ, "mer_attention (V^T): max_seqlen %d (1 .. %d)", max_seqlen,
+              MAX_SEQ);
+  MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535, "mer_attention (V^T): bad grid (%d heads, %d seqs)",
+              heads, n_seq);
+  if (n_seq <= 0 || tokens <= 0) return 0;
   static MerPerDevice attr_set;
   if (attr_set.needs_setup()) {
-    const Kern all[] = {attention_f16_kernel<1>, attention_f16_kernel<2>, attention_f16_kernel<3>, attention_f16_kernel<4>,
-                        attention_f16_kernel<6, 1>, attention_f16_kernel<6, 3>,
-                        attention_f16_kernel<7, 0>, attention_f16_kernel<7, 1>, attention_f16_kernel<7, 2>,
-                        attention_f16_kernel<7, 3>};
-    for (Kern k : all) MER_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    MER_CUDA_CHECK(cudaFuncSetAttribute(attention_vt_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        Cfg::kSmem));
     attr_set.mark();
   }
-  const long long items = (long long)n_seq * heads;
-  if (items <= 0) return 0;
-  int grid = mer_num_sms();
-  if (items < grid) grid = (int)items;
   const double s_avg = (double)tokens / n_seq;  // exact for equal-length batches (ViT frames)
-  const int prof = mer_prof_begin(MER_PROF_ATT_F16, 4.0 * s_avg * s_avg * HD * (double)items, stream);
-  kern<<<grid, ver >= 6 ? F16_THREADS_V6 : ver >= 4 ? F16_THREADS_V4 : F16_THREADS, ver == 7 ? smem7 : F16_SMEM, stream>>>(
-      tm, tv, tk, tq1, lay, static_cast<uint16_t*>(ctx16), cu_seqlens, n_seq, heads, g_att_trace);
+  const int prof = mer_prof_begin(F16 ? MER_PROF_ATT_F16 : MER_PROF_ATT_TC,
+                                  4.0 * s_avg * s_avg * HD * (double)n_seq * heads, stream);
+  dim3 grid((max_seqlen + BQ - 1) / BQ, heads, n_seq);
+  attention_vt_kernel<F16><<<grid, THREADS, Cfg::kSmem, stream>>>(qkv, vt, vt_ld, ctx, cu_seqlens, tokens, heads,
+                                                                   out_mode);
   mer_prof_end(prof, stream);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
   return 0;
+}
+
+}  // namespace
+
+// fp16 q | k | V^T for every sequence of up to 505 tokens; MER_ATT_F16_LONG=0 sends rows of 250 .. 505 tokens of the
+// TF32 / BF16X3 stacks to the fp32-operand kernel of attention.cu instead (A/B runs)
+bool mer_attention_f16_supported(int max_seqlen) {
+  if (max_seqlen <= 0 || mer_attention_legacy()) return false;
+  if (max_seqlen <= 249) return true;
+  const char* e = getenv("MER_ATT_F16_LONG");
+  return (e == nullptr || atoi(e) != 0) && max_seqlen <= MAX_SEQ;
+}
+
+// qkv16: fp16 [tokens, 3*heads*64] (V columns unused), vt16: fp16 [heads*64, vt_ld] with vt[d, token];
+// ctx [tokens, heads*64] in the format `out_mode` names (3 fp16, 2 bf16 hi | lo split rows, 1 tf32-rounded fp32, 0 fp32)
+int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
+                             int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream) {
+  return launch_vt<true>(qkv16, vt16, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream);
+}
+
+// tf32-rounded fp32 q | k rows and V^T (the V columns of qkv are not written when V^T is)
+int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
+                            int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream) {
+  return launch_vt<false>(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream);
 }

@@ -77,9 +77,9 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
     const int first_acc = a.n_layers - a.acc_last;  // hidden state index l+1 > first_acc is summed
     // operand format of the tensor-core inputs in this stack: tf32-rounded fp32, or split bf16
     const bool split = a.mode == MER_GEMM_BF16X3;
-    // tcgen05 attention (sequences <= 256): the QKV GEMM writes V transposed into a.vt instead of
+    // V^T attention (sequences <= 253): the QKV GEMM writes V transposed into a.vt instead of
     // the V columns of qkv
-    // (254 .. 505 tokens: attention_f16_long.cu, which takes fp16 q | k | V^T whatever the stack's operand format)
+    // (254 .. 505 tokens: the fp16 V^T kernel, which takes fp16 q | k | V^T whatever the stack's operand format)
     const bool long_att = a.vt && !mer_attention_uses_tc(a.max_seqlen) && mer_attention_f16_supported(a.max_seqlen);
     float* vt = (a.vt && (long_att || mer_attention_uses_tc(a.max_seqlen))) ? a.vt : nullptr;
     // the TF32 / BF16X3 stacks: QKV epilogue and attention flags (q | k | v tf32-rounded fp32, or fp16 = the same 10-bit
@@ -129,7 +129,7 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
       MER_TRY(linear(a.mode, a.xn, w.w_fc1, w.b_fc1, nullptr, a.h, M, DFF, D, ACT | opnd, stream));
       MER_TRY(linear(a.mode, a.h, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
     } else if (a.mode == MER_GEMM_F16) {
-      // post-LN on fp16 operands (round 2; profiles/r2_precision_table.json): x stays the exact fp32 LayerNorm output
+      // post-LN on fp16 operands (scripts/precision_table.py): x stays the exact fp32 LayerNorm output
       // (residual stream, hidden state), xs carries its fp16 copy (GEMM operand, written by the same LayerNorm
       // pass); ctx and the FC1 output are fp16; the pre-LN sums are fp32.
       float* x16 = a.xs;
@@ -748,7 +748,7 @@ static int hubert_forward_impl(const MerHubertModel* m, const float* wave, int B
   if (!m->stable_layer_norm) {
     // encoder.layer_norm -> x ; post-LN layers; readout = sum of the last four LayerNorm outputs
     // layers_f16 given: the 12 layers run on fp16 operands (the conv feature encoder above stays BF16X3: it has no
-    // normalisation between its layers and is where the operand precision matters, profiles/r2_precision_table.json)
+    // normalisation between its layers and is where the operand precision matters, scripts/precision_table.py)
     const bool f16 = m->layers_f16 != nullptr;
     MER_TRY(mer_layernorm_launch(xn, m->enc_ln_g, m->enc_ln_b, x, xs, nullptr, M, D, m->ln_eps,
                                  f16 ? MER_LN_SPLIT_F16 : 0, stream));

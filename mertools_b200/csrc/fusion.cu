@@ -246,14 +246,10 @@ fus_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __res
   const float bc2_sqrt = sqrtf(1.f - powf(beta2, t));
   float grad = g[i] * gscale;
   if (clip > 0.f) grad = fminf(fmaxf(grad, -clip), clip);
-  const float pi = p[i];
-  grad = fmaf(wd, pi, grad);
-  const float mi = m[i] + (grad - m[i]) * (1.f - beta1);       // lerp, as torch
-  const float vi = v[i] * beta2 + (1.f - beta2) * grad * grad; // mul + addcmul
+  float mi = m[i], vi = v[i];
+  p[i] = mer::adam_param(p[i], grad, mi, vi, lr, beta1, beta2, eps, wd, bc1, bc2_sqrt);
   m[i] = mi;
   v[i] = vi;
-  const float denom = sqrtf(vi) / bc2_sqrt + eps;
-  p[i] = pi - (lr / bc1) * (mi / denom);
 }
 __global__ void fus_step_inc_kernel(int* step) { if (threadIdx.x == 0 && blockIdx.x == 0) ++(*step); }
 

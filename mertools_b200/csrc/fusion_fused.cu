@@ -629,7 +629,7 @@ __global__ void __launch_bounds__(NT, 1) fus_rows_kernel(const __grid_constant__
 
 // ---------------------------------------------------------------------------------------------------------------
 // fus_rows_fast_kernel — the same row-parallel pass for the common shapes (hidden <= 128, feature widths that are
-// multiples of 4 and fit the plan below), rebuilt around what the first version measured on B200: 96 us per step at
+// multiples of 4 and fit the plan below), rebuilt around what the first version measured: per step at
 // B = 32, almost all of it exposed L2 latency (every layer began with a dependent weight load) -- not arithmetic.
 //   * Weights come in through the bulk-copy engine (cp.async.bulk + mbarrier), never through a load a warp waits on:
 //     this CTA's row slices W[n0:n1, :] of the five hidden-layer matrices (88 KB at hidden 128) are requested at kernel
@@ -1087,14 +1087,10 @@ struct WArgs {
 // corrections 1 - beta1^t and sqrt(1 - beta2^t) of this step (computed once per thread)
 __device__ __forceinline__ void adam_update(const WArgs& a, long long i, float grad, float bc1, float bc2_sqrt) {
   if (a.clip > 0.f) grad = fminf(fmaxf(grad, -a.clip), a.clip);
-  const float pi = a.P[i];
-  grad = fmaf(a.wd, pi, grad);
-  const float mi = a.M[i] + (grad - a.M[i]) * (1.f - a.beta1);
-  const float vi = a.V[i] * a.beta2 + (1.f - a.beta2) * grad * grad;
+  float mi = a.M[i], vi = a.V[i];
+  a.P[i] = mer::adam_param(a.P[i], grad, mi, vi, a.lr, a.beta1, a.beta2, a.eps, a.wd, bc1, bc2_sqrt);
   a.M[i] = mi;
   a.V[i] = vi;
-  const float denom = sqrtf(vi) / bc2_sqrt + a.eps;
-  a.P[i] = pi - (a.lr / bc1) * (mi / denom);
 }
 
 // VW outputs dW[n, k .. k + VW) per thread (VW = 4 when every K is a multiple of 4 and the activations are 16-byte

@@ -12,24 +12,22 @@
 // see DESIGN.md kernel table).
 // W is the nn.Linear weight as stored: [N, K] row-major == K-major B operand.
 //
-// Structure (persistent, warp-specialised, one CTA per SM):
-//   warp 0      TMA producer: A/B tiles -> swizzled smem ring (mbarrier full/empty)
-//   warp 1      MMA issuer  : tcgen05.mma, UMMA 128 x BLOCK_N x (32 bytes of K), fp32 accum in TMEM
-//   warp 2      TMEM allocator
-//   warps 4..19 epilogue    : tcgen05.ld TMEM -> registers -> swizzled smem transpose -> bias / activation /
-//                             residual / output format on the coalesced side -> 8 rows x 64 B per
-//                             st.global (four warps per TMEM lane quarter, a quarter of the columns
-//                             each; compile-time specialised variants, see epi_tile)
-// TMEM holds two accumulator stages so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Structure (persistent, warp-specialised, one CTA per SM, 128 x BLOCK_N output tiles):
+//   warpgroup 0 (warp 0)  TMA producer: A/B tiles -> 128B-swizzled smem ring (mbarrier full/empty)
+//   warpgroups 1, 2       consumers: rows [0, 64) / [64, 128) of the tile; wgmma.mma_async 64 x 128 x (32 bytes
+//                         of K) per instruction (two per K step for BLOCK_N = 256), fp32 accumulators in
+//                         registers; then the epilogue straight from the accumulator fragment (bias / activation /
+//                         residual / output format, 8 rows x 32 contiguous bytes per store instruction)
+// The producer runs ahead across tile boundaries, so the next tile's operands stream in during the epilogue.
 //
 // Three arithmetic modes share the pipeline (128 bytes of K per smem row and stage in each):
-//   MER_GEMM_F16    : IEEE fp16 operands (64 K elements per stage), kind::f16.  Same 10-bit mantissa as
+//   MER_GEMM_F16    : IEEE fp16 operands (64 K elements per stage), wgmma f16.  Same 10-bit mantissa as
 //                     tf32, twice the MMA rate, half the operand bytes: the ViT stack's default.
-//   MER_GEMM_TF32   : fp32 operands (pre-rounded to tf32 by their producers), kind::tf32, 128B swizzle.
+//   MER_GEMM_TF32   : fp32 operands (pre-rounded to tf32 by their producers), wgmma tf32, 128B swizzle.
 //                     ~2.4e-4 relative error per GEMM: enough for the pre-LN ViT at 1e-3.
 //   MER_GEMM_BF16X3 : every operand stored as bf16 (hi, lo) pairs, x = hi + lo to 2^-17, in 128-byte
 //                     groups [32 hi | 32 lo] so that tiles move exactly like TF32 tiles; three
-//                     kind::f16 MMAs per 16-wide K step (hi*hi + lo*hi + hi*lo), fp32 accumulate.
+//                     bf16 MMAs per 16-wide K step (hi*hi + lo*hi + hi*lo), fp32 accumulate.
 //                     ~2e-5 relative error per GEMM: what the post-LN HuBERT/BERT stacks need to stay
 //                     inside 1e-3 after 12 layers (measured: single-pass TF32 reaches 1.0e-3 after 4).
 #include <stdlib.h>
@@ -43,57 +41,27 @@ using namespace mer;
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 32;  // K elements per stage in TF32 / BF16X3 mode (128 B of tf32 / 64 B of bf16 per part)
-constexpr int EPI_WARP0 = 4;
-constexpr int EPI_WARPS = 16;     // four per TMEM lane quarter, each taking a quarter of the tile's columns
-constexpr int NUM_THREADS = 32 * (EPI_WARP0 + EPI_WARPS);  // 4 control warps + 16 epilogue warps
+constexpr int CONSUMERS = 2;  // consumer warpgroups, 64 tile rows each
+constexpr int NUM_THREADS = 128 * (1 + CONSUMERS);
 
-template <int BLOCK_N, int MODE, bool TWOSM = false>
+template <int BLOCK_N, int MODE>
 struct GemmCfg {
   static constexpr bool kSplit = MODE == MER_GEMM_BF16X3;
   static constexpr bool kF16 = MODE == MER_GEMM_F16;
   static constexpr int kBlockK = kF16 ? 64 : BLOCK_K;  // K elements per stage
   static constexpr int kRowBytes = 128;                 // bytes of K per smem row = swizzle span
-  static constexpr int kSBO = 8 * kRowBytes;            // byte stride between 8-row core groups
-  static constexpr int kLayout = 2;                     // UMMA LayoutType SWIZZLE_128B
-  static constexpr int kFmt = kSplit ? 1 : (kF16 ? 0 : 2);  // instr-desc operand format: bf16 / f16 / tf32
-  // TWOSM (cta_group::2): each CTA of the pair keeps only ITS half of the weight tile in smem
-  // stage count: what fits beside the epilogue's 32 KB of staging (227 KB usable per CTA)
-  static constexpr int kStages = TWOSM ? 6 : (BLOCK_N == 256 ? 4 : 6);
+  static constexpr int kKind = kSplit ? 1 : (kF16 ? 0 : 2);  // wgmma operand type: f16 / bf16 / tf32
   static constexpr int kABytes = BLOCK_M * kRowBytes;
-  static constexpr int kBBytes = (TWOSM ? BLOCK_N / 2 : BLOCK_N) * kRowBytes;
+  static constexpr int kBBytes = BLOCK_N * kRowBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = 2 * BLOCK_N;
+  static constexpr int kStages = BLOCK_N == 256 ? 4 : 6;  // 192 KB of operands either way (227 KB usable)
   static constexpr int kBarBytes = 256;
-  // per epilogue warp: a 32 x 64 B transpose tile
-  static constexpr int kStagingBytes = EPI_WARPS * 2048;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBarBytes + 1024;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
 
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, int sbo_bytes, int layout) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
-  return d;
-}
-
-// tcgen05.wait::ld that also names the destination registers, so no use of them can be scheduled above it
-__device__ __forceinline__ void tmem_ld_wait_regs(uint32_t* r) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]),
-                 "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]),
-                 "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]),
-                 "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]),
-                 "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
 // internal epilogue flag (set by mer_gemm_launch when MER_GELU_PACKED=1): erf-GELU on value pairs through the
-// packed fp32 pipe (GELU kind 5; fp16 and split-bf16 outputs, no residual).  Off by default until measured.
+// paired polynomial (GELU kind 5; fp16 and split-bf16 outputs, no residual).  Off by default.
 constexpr int EPI_GELU_PACKED = 1 << 16;
 
 template <int GELU>
@@ -101,9 +69,9 @@ __device__ __forceinline__ float epi_act(float v) {
   if (GELU == 1) return gelu_erf_fast(v);
   if (GELU == 2) return gelu_erf(v);
   if (GELU == 3) return quick_gelu_fast(v);
-  return v;  // GELU == 4 (ReLU) is applied after the residual add, in the write-out phase
+  return v;  // GELU == 4 (ReLU) is applied after the residual add
 }
-// two adjacent values at once (GELU == 5: the packed polynomial; otherwise the scalar form twice)
+// two adjacent values at once (GELU == 5: the paired polynomial; otherwise the scalar form twice)
 template <int GELU>
 __device__ __forceinline__ void epi_act2(float a, float b, float& ga, float& gb) {
   if (GELU == 5) {
@@ -114,243 +82,128 @@ __device__ __forceinline__ void epi_act2(float a, float b, float& ga, float& gb)
   }
 }
 
-// What one epilogue warp needs to know about its share of the current output tile.
-struct EpiTile {
-  uint32_t t_addr;        // TMEM address: this warp's lane quarter, accumulator stage, first column
-  int n0;                 // first global output column of the warp's slice
-  int rows_left;          // rows r < rows_left of the warp's 32 are real
-  long long out_off;      // element index of out[row0 + lane / 4][n0]  (write-out phase)
-  const float* res_lane;  // same position in the residual, or nullptr
-  long long vt_idx;       // column (= output row) of this lane in the transposed side output
-  long long ld_out8, ld_res8;  // 8 rows of out / res, in floats
-};
-
-// Epilogue of one warp for one tile: CH chunks of 32 accumulator columns, each handled as two
-// 16-column halves through a 32 x 64 B staging tile (XOR-swizzled 16-byte slots, conflict-free both
-// ways):
-//   phase 1 (thread = accumulator row): tcgen05.ld registers -> smem, raw
-//   phase 2 (lane = (row % 8, 16-byte slot); one warp instruction = 8 rows x 64 contiguous bytes):
-//           smem -> + bias -> GELU -> + residual -> TF32 round / bf16 split -> st.global.
-// All arithmetic sits in phase 2, where bias values are per-lane constants and the residual is read in
-// the shape it is written (its lines were prefetched into L2 at tile start, under the MMAs).
-// The TMEM stage is handed back to the MMA warp as soon as the LAST chunk has been read into
-// registers, i.e. before that chunk's math and stores.
-// GELU: 0 none, 1 polynomial erf, 2 libdevice erff.  OUT: 0 fp32, 1 TF32-rounded fp32, 2 bf16 (hi|lo),
-// 3 fp16.
-// RES: add the residual after the activation (OUT 0 or 1).  The transposed side output exists for
-// GELU == 0 without residual.
-template <int CH, int GELU, int OUT, bool RES, typename ReleaseFn>
-__device__ __forceinline__ void epi_tile(const EpiTile& tl, const MerGemmEpilogue& ep, float* stg,
-                                         int lane, ReleaseFn release_tmem) {
+// Epilogue of one consumer warpgroup for its 64 x BLOCK_N share of a tile, straight from the wgmma accumulator
+// fragment: acc[h][4 j + 2 i + c] holds row 16 warp + g + 8 i, column 128 h + 8 j + 2 t + c (g = lane / 4,
+// t = lane % 4).  Each thread handles column pairs; one store instruction covers 8 rows x 32 contiguous bytes.
+// GELU: 0 none, 1 polynomial erf, 2 libdevice erff, 3 quick-GELU, 4 ReLU (after the residual), 5 paired erf.
+// OUT: 0 fp32, 1 TF32-rounded fp32, 2 bf16 (hi|lo), 3 fp16.  RES: add the residual after the activation.
+// The transposed side output (V^T of the QKV GEMM) exists for GELU == 0 without residual: columns >= vt_col0 go
+// to vt[n - vt_col0, out_row] INSTEAD of out.
+template <int NH, int GELU, int OUT, bool RES>
+__device__ __forceinline__ void epi_tile(float (&acc)[NH][64], const MerGemmEpilogue& ep, int n_base, int m_base,
+                                         int rows_per_batch, long long out_row_b, long long res_row_b, int wg_row0) {
   constexpr bool kVt = GELU == 0 && !RES;
-  const int p_row = lane >> 2, p_slot = lane & 3;  // phase-2 coordinates
-  auto slot = [&](int row, int j) -> float4* {       // 16-byte slot j (0..3) of staging row `row`
-    return reinterpret_cast<float4*>(stg + row * 16 + ((j ^ ((row >> 1) & 3)) << 2));
-  };
-  uint32_t r[32];
-  tmem_ld_32x32(tl.t_addr, r);
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int g = lane >> 2, t = lane & 3;
 #pragma unroll
-  for (int ci = 0; ci < CH; ++ci) {
-    const int n0 = tl.n0 + ci * 32;
-    tmem_ld_wait_regs(r);
-    if (ci == CH - 1) release_tmem();
-    if (kVt && ep.vt != nullptr && n0 >= ep.vt_col0) {
-      // transposed side output (V^T of the QKV GEMM): lanes = consecutive rows, so each scalar store
-      // instruction is one contiguous 128-byte run of vt
-      const long long vt_off = (long long)(n0 - ep.vt_col0) * ep.vt_ld;
+  for (int i = 0; i < 2; ++i) {
+    const int m = m_base + wg_row0 + 16 * w + g + 8 * i;  // row inside the batch entry
+    if (m >= rows_per_batch) continue;
+    const long long orow = out_row_b + m;
+    const float* rrow = RES ? ep.res + (res_row_b + m) * (long long)ep.ld_res : nullptr;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (ep.bias) q = __ldg(reinterpret_cast<const float4*>(ep.bias + n0) + j);  // warp-uniform address
-        float4 v = make_float4(__uint_as_float(r[4 * j + 0]) + q.x, __uint_as_float(r[4 * j + 1]) + q.y,
-                               __uint_as_float(r[4 * j + 2]) + q.z, __uint_as_float(r[4 * j + 3]) + q.w);
-        if (OUT == 1) {
-          v.x = round_tf32(v.x); v.y = round_tf32(v.y); v.z = round_tf32(v.z); v.w = round_tf32(v.w);
+    for (int hh = 0; hh < NH; ++hh) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int n = n_base + 128 * hh + 8 * j + 2 * t;
+        float v0 = acc[hh][4 * j + 2 * i], v1 = acc[hh][4 * j + 2 * i + 1];
+        if (ep.bias) {
+          const float2 q = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+          v0 += q.x;
+          v1 += q.y;
         }
-        if (lane < tl.rows_left) {
-          if (OUT == 3) {  // fp16 V^T: 64-byte runs per store instruction
-            uint16_t* vt16 = reinterpret_cast<uint16_t*>(ep.vt) + tl.vt_idx + vt_off;
-            const uint32_t xy = pack_f16x2(v.x, v.y), zw = pack_f16x2(v.z, v.w);
-            vt16[(long long)(4 * j + 0) * ep.vt_ld] = (uint16_t)(xy & 0xffffu);
-            vt16[(long long)(4 * j + 1) * ep.vt_ld] = (uint16_t)(xy >> 16);
-            vt16[(long long)(4 * j + 2) * ep.vt_ld] = (uint16_t)(zw & 0xffffu);
-            vt16[(long long)(4 * j + 3) * ep.vt_ld] = (uint16_t)(zw >> 16);
+        if (kVt && ep.vt != nullptr && n >= ep.vt_col0) {
+          const long long vo = (long long)(n - ep.vt_col0) * ep.vt_ld + orow;
+          if (OUT == 3) {
+            uint16_t* vt16 = reinterpret_cast<uint16_t*>(ep.vt) + vo;
+            const uint32_t p = pack_f16x2(v0, v1);
+            vt16[0] = (uint16_t)(p & 0xffffu);
+            vt16[ep.vt_ld] = (uint16_t)(p >> 16);
           } else {
-            float* vt_col = ep.vt + tl.vt_idx + vt_off;
-            vt_col[(long long)(4 * j + 0) * ep.vt_ld] = v.x;
-            vt_col[(long long)(4 * j + 1) * ep.vt_ld] = v.y;
-            vt_col[(long long)(4 * j + 2) * ep.vt_ld] = v.z;
-            vt_col[(long long)(4 * j + 3) * ep.vt_ld] = v.w;
+            if (OUT == 1) {
+              v0 = round_tf32(v0);
+              v1 = round_tf32(v1);
+            }
+            ep.vt[vo] = v0;
+            ep.vt[vo + ep.vt_ld] = v1;
           }
+          continue;
         }
-      }
-      if (ci + 1 < CH) tmem_ld_32x32(tl.t_addr + (ci + 1) * 32, r);
-      continue;
-    }
-    if (OUT == 3) {
-      // fp16 output: the arithmetic runs here, on the accumulator-row thread (bias values come as
-      // warp-uniform L1 loads), so that the staging tile already holds fp16 -- one 32 x 64 B pass per
-      // chunk and 16-byte stores (8 rows x 64 B per instruction) instead of two passes of 8-byte stores
-      uint32_t pk[16];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (ep.bias) q = __ldg(reinterpret_cast<const float4*>(ep.bias + n0) + j);
-        float g0, g1, g2, g3;
-        epi_act2<GELU>(__uint_as_float(r[4 * j + 0]) + q.x, __uint_as_float(r[4 * j + 1]) + q.y, g0, g1);
-        epi_act2<GELU>(__uint_as_float(r[4 * j + 2]) + q.z, __uint_as_float(r[4 * j + 3]) + q.w, g2, g3);
-        pk[2 * j] = pack_f16x2(g0, g1);
-        pk[2 * j + 1] = pack_f16x2(g2, g3);
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j)  // 16-byte slot j = columns 8j .. 8j+7 of the chunk
-        *reinterpret_cast<uint4*>(slot(lane, j)) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-      if (ci + 1 < CH) tmem_ld_32x32(tl.t_addr + (ci + 1) * 32, r);  // flies during the write-out
-      __syncwarp();
-      uint16_t* o16 = reinterpret_cast<uint16_t*>(ep.out) + tl.out_off + ci * 32 + 8 * p_slot;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int row = 8 * i + p_row;
-        const uint4 d = *reinterpret_cast<const uint4*>(slot(row, p_slot));
-        if (row < tl.rows_left) *reinterpret_cast<uint4*>(o16 + i * tl.ld_out8) = d;
-      }
-      __syncwarp();
-    }
-#pragma unroll
-    for (int sub = 0; sub < (OUT == 3 ? 0 : 2); ++sub) {
-      const int col = ci * 32 + sub * 16 + 4 * p_slot;  // this lane's 4 columns, relative to tl.n0
-      float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (ep.bias) q = __ldg(reinterpret_cast<const float4*>(ep.bias + tl.n0 + col));
-      float4 rr[4];
-      if (RES) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          rr[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (8 * i + p_row < tl.rows_left)
-            rr[i] = __ldg(reinterpret_cast<const float4*>(tl.res_lane + i * tl.ld_res8 + col));
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *slot(lane, j) = make_float4(__uint_as_float(r[16 * sub + 4 * j + 0]), __uint_as_float(r[16 * sub + 4 * j + 1]),
-                                     __uint_as_float(r[16 * sub + 4 * j + 2]), __uint_as_float(r[16 * sub + 4 * j + 3]));
-      if (sub == 1 && ci + 1 < CH) tmem_ld_32x32(tl.t_addr + (ci + 1) * 32, r);  // flies during the write-out
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int row = 8 * i + p_row;
-        float4 v = *slot(row, p_slot);
-        epi_act2<GELU>(v.x + q.x, v.y + q.y, v.x, v.y);
-        epi_act2<GELU>(v.z + q.z, v.w + q.w, v.z, v.w);
+        epi_act2<GELU>(v0, v1, v0, v1);
         if (RES) {
-          v.x += rr[i].x; v.y += rr[i].y; v.z += rr[i].z; v.w += rr[i].w;
+          const float2 r = __ldg(reinterpret_cast<const float2*>(rrow + n));
+          v0 += r.x;
+          v1 += r.y;
         }
         if (GELU == 4) {
-          v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
         }
-        if (OUT == 2) {
-          // the 32-column group's 128 bytes are [32 x bf16 hi | 32 x bf16 lo]
-          const float hx = bf16_round(v.x), hy = bf16_round(v.y), hz = bf16_round(v.z), hw = bf16_round(v.w);
-          if (row < tl.rows_left) {
-            uint16_t* grp = reinterpret_cast<uint16_t*>(ep.out + tl.out_off + i * tl.ld_out8 + ci * 32);
-            const int c = sub * 16 + 4 * p_slot;
-            *reinterpret_cast<uint2*>(grp + c) = make_uint2(pack_bf16x2(hx, hy), pack_bf16x2(hz, hw));
-            *reinterpret_cast<uint2*>(grp + 32 + c) =
-                make_uint2(pack_bf16x2(v.x - hx, v.y - hy), pack_bf16x2(v.z - hz, v.w - hw));
-          }
+        if (OUT == 3) {
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(ep.out) + orow * ep.ld_out + n) = pack_f16x2(v0, v1);
+        } else if (OUT == 2) {
+          store_split2(ep.out + orow * ep.ld_out, n, v0, v1);
         } else {
           if (OUT == 1) {
-            v.x = round_tf32(v.x); v.y = round_tf32(v.y); v.z = round_tf32(v.z); v.w = round_tf32(v.w);
+            v0 = round_tf32(v0);
+            v1 = round_tf32(v1);
           }
-          if (row < tl.rows_left) *reinterpret_cast<float4*>(ep.out + tl.out_off + i * tl.ld_out8 + col) = v;
+          *reinterpret_cast<float2*>(ep.out + orow * ep.ld_out + n) = make_float2(v0, v1);
         }
       }
-      __syncwarp();
     }
   }
 }
 
-// CLUSTER == 2: a pair of CTAs works on two vertically adjacent 128-row tiles of the same BLOCK_N
-// column block; each loads its own A tile and HALF of the shared B tile, multicast into both CTAs'
-// shared memory (L2 -> SM traffic per CTA drops from 128+BLOCK_N to 128+BLOCK_N/2 rows per stage).
-// TWOSM (requires CLUSTER == 2): the pair issues ONE tcgen05.mma.cta_group::2 of shape 256 x BLOCK_N
-// per K step from the even ("leader") CTA.  Each CTA loads its own 128 A rows and its own half of the
-// weight tile into its own smem (TMA .cta_group::2, completing on the leader's barrier), so per SM
-// and stage the TMA writes 32 KB instead of 48 KB and the tensor core reads 8 KB instead of 12 KB per
-// MMA: the single-CTA form is shared-memory-bandwidth bound at ~2/3 of the tensor peak (measured).
-template <int BLOCK_N, int MODE, int CLUSTER, bool TWOSM>
+template <int BLOCK_N, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
             const __grid_constant__ CUtensorMap tmap_b, const MerGemmEpilogue ep,
             int rows_per_batch, int batches, int N, int K, int K_inner, int P, int a_row0, int a_col_group) {
-  using Cfg = GemmCfg<BLOCK_N, MODE, TWOSM>;
-  static_assert(!TWOSM || CLUSTER == 2, "the 2-SM MMA needs CTA pairs");
+  using Cfg = GemmCfg<BLOCK_N, MODE>;
+  constexpr int NH = BLOCK_N / 128;  // 64 x 128 accumulator blocks per consumer thread
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by OFFSET (not through an integer round trip) so the compiler keeps the
-  // shared address space of everything derived from it (st.shared / ld.shared, not generic ST / LD)
+  // shared address space of everything derived from it
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
-  uint8_t* staging = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tfull_bar = bars + 2 * Cfg::kStages;
-  uint64_t* tempty_bar = bars + 2 * Cfg::kStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::kStages + 4);
 
+  const int wg = threadIdx.x >> 7;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   const int m_tiles = (rows_per_batch + BLOCK_M - 1) / BLOCK_M;
   const int n_tiles = N / BLOCK_N;
   const int num_kb = K / Cfg::kBlockK;
-  // work items: (row-tile group, column block); a group is CLUSTER consecutive (batch, m-tile) tiles
-  const int total_m = batches * m_tiles;
-  const int num_tiles = ((total_m + CLUSTER - 1) / CLUSTER) * n_tiles;
-  const int cta_rank = CLUSTER > 1 ? (int)cluster_ctarank() : 0;
-  const int first_tile = blockIdx.x / CLUSTER;
-  const int tile_step = gridDim.x / CLUSTER;
+  const int num_tiles = batches * m_tiles * n_tiles;  // work item t: column block t % n_tiles, row tile t / n_tiles
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < Cfg::kStages; ++i) {
-      mbar_init(&full_bar[i], TWOSM ? 2 : 1);       // 2-SM: one expect-tx arrival per CTA, on the leader
-      mbar_init(&empty_bar[i], TWOSM ? 1 : CLUSTER);  // commit arrivals (2-SM: one multicast commit)
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EPI_WARPS * (TWOSM ? 2 : 1));  // one arrive per epilogue warp (of the pair)
+      mbar_init(&full_bar[i], 1);                // the producer's expect-tx arrival
+      mbar_init(&empty_bar[i], 4 * CONSUMERS);   // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (TWOSM) {
-      tmem_alloc_2sm(tmem_slot, Cfg::kTmemCols);
-      tmem_relinquish_2sm();
-    } else {
-      tmem_alloc(tmem_slot, Cfg::kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (CLUSTER > 1) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp != 0) return;
     // The whole warp runs the loop (so addresses and coordinates stay in uniform registers); one
     // elected lane issues the copies.  No division inside the K loop.
     int stage = 0;
     uint32_t phase = 0;
     constexpr int kEl = Cfg::kSplit ? 2 : 1;  // tensor-map elements per operand value
-    for (int t = first_tile; t < num_tiles; t += tile_step) {
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const int n_blk = t % n_tiles;
-      const int mb = (t / n_tiles) * CLUSTER + cta_rank;  // >= total_m: padding tile (TMA zero-fills)
+      const int mb = t / n_tiles;
       const int b = mb / m_tiles;
       const int mt = mb % m_tiles;
       int c0 = 0, tap_phase = 0, tap_row = 0;  // K offset inside the tap; tap % P; tap / P
@@ -358,29 +211,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
       const int c_win = a_col_group > 0 ? ((n_blk * BLOCK_N) / a_col_group) * a_col_group : 0;
       const int row_base = mt * BLOCK_M + a_row0;
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
         if (elect_one()) {
-          if (TWOSM) {
-            const uint32_t lbar = leader_addr(&full_bar[stage]);
-            mbar_expect_tx_cluster(lbar, Cfg::kStageBytes);
-            tma_load_4d_2sm(smem_a + stage * Cfg::kABytes, &tmap_a, lbar, (c_win + c0) * kEl, tap_phase,
-                            row_base + tap_row, b);
-            tma_load_2d_2sm(smem_b + stage * Cfg::kBBytes, &tmap_b, lbar, kb * Cfg::kBlockK * kEl,
-                            n_blk * BLOCK_N + cta_rank * (BLOCK_N / 2));
-          } else {
-            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-            tma_load_4d(smem_a + stage * Cfg::kABytes, &tmap_a, &full_bar[stage], (c_win + c0) * kEl, tap_phase,
-                        row_base + tap_row, b);
-            if (CLUSTER == 1) {
-              tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, &full_bar[stage], kb * Cfg::kBlockK * kEl,
-                          n_blk * BLOCK_N);
-            } else {
-              tma_load_2d_mc(smem_b + stage * Cfg::kBBytes + cta_rank * (Cfg::kBBytes / CLUSTER), &tmap_b,
-                             &full_bar[stage], kb * Cfg::kBlockK * kEl,
-                             n_blk * BLOCK_N + cta_rank * (BLOCK_N / CLUSTER),
-                             (uint16_t)((1u << CLUSTER) - 1));
-            }
-          }
+          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          tma_load_4d(smem_a + stage * Cfg::kABytes, &tmap_a, &full_bar[stage], (c_win + c0) * kEl, tap_phase,
+                      row_base + tap_row, b);
+          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, &full_bar[stage], kb * Cfg::kBlockK * kEl,
+                      n_blk * BLOCK_N);
         }
         __syncwarp();
         c0 += Cfg::kBlockK;
@@ -397,184 +234,112 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // Warp-uniform loop; one elected lane issues the MMAs and their commits (a commit tracks the
-    // MMAs of the thread that executes it).
-    if (!TWOSM || cta_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc(Cfg::kFmt, TWOSM ? 2 * BLOCK_M : BLOCK_M, BLOCK_N);
-      const uint64_t desc_a0 = umma_desc(smem_u32(smem_a), Cfg::kSBO, Cfg::kLayout);
-      const uint64_t desc_b0 = umma_desc(smem_u32(smem_b), Cfg::kSBO, Cfg::kLayout);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int t = first_tile; t < num_tiles; t += tile_step) {
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (elect_one()) {
-            // descriptors: start address field counts 16-byte units; a stage is kABytes / kBBytes further
-            const uint64_t da = desc_a0 + (uint64_t)(stage * (Cfg::kABytes >> 4));
-            const uint64_t db = desc_b0 + (uint64_t)(stage * (Cfg::kBBytes >> 4));
-            // advance the start address by 32-byte K steps inside the 128B swizzle row (>>4 => +2)
-            if (Cfg::kF16) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {  // 4 x 16 fp16
-                if (TWOSM) tc_mma_bf16_2sm(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                else tc_mma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-              }
-            } else if (!Cfg::kSplit) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {  // 4 x 8 tf32
-                if (TWOSM) tc_mma_tf32_2sm(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                else tc_mma_tf32(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-              }
-            } else {
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {  // 2 x 16 bf16; hi at bytes [0,64), lo at [64,128) of the row
-                if (TWOSM) {
-                  tc_mma_bf16_2sm(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                  tc_mma_bf16_2sm(d_tmem, da + 4 + 2 * k, db + 2 * k, idesc, 1);
-                  tc_mma_bf16_2sm(d_tmem, da + 2 * k, db + 4 + 2 * k, idesc, 1);
-                } else {
-                  tc_mma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);  // hi * hi
-                  tc_mma_bf16(d_tmem, da + 4 + 2 * k, db + 2 * k, idesc, 1);          // lo * hi
-                  tc_mma_bf16(d_tmem, da + 2 * k, db + 4 + 2 * k, idesc, 1);          // hi * lo
-                }
-              }
-            }
-            // free the smem slot when these MMAs retire (in every CTA that writes into it / owns a copy)
-            if (TWOSM) tc_commit_2sm(&empty_bar[stage]);
-            else if (CLUSTER == 1) tc_commit(&empty_bar[stage]);
-            else tc_commit_mc(&empty_bar[stage], (uint16_t)((1u << CLUSTER) - 1));
-            if (kb == num_kb - 1) {
-              if (TWOSM) tc_commit_2sm(&tfull_bar[as]);  // accumulator complete -> both CTAs' epilogues
-              else tc_commit(&tfull_bar[as]);           // accumulator complete -> epilogue
-            }
-          }
-          __syncwarp();
-          if (++stage == Cfg::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= EPI_WARP0) {
-    // ===================== epilogue =====================
-    // 16 warps: warp % 4 = the TMEM lane quarter it may read (32 accumulator rows), (warp - 4) / 4 = the
-    // quarter of the tile's columns it handles.  See epi_tile for the per-chunk data path.
-    const int ew = (warp - EPI_WARP0) & 3;
-    const int cq = (warp - EPI_WARP0) >> 2;
-    constexpr int CH = BLOCK_N / 128;           // 32-column chunks per warp and tile
-    float* stg = reinterpret_cast<float*>(staging) + (warp - EPI_WARP0) * 512;
-    const int p_row = lane >> 2;
-    int as = 0;
-    uint32_t aphase = 0;
-    const int gelu_kind = (ep.flags & MER_EPI_RELU) ? 4 : (ep.flags & MER_EPI_QUICK_GELU) ? 3
-                          : (ep.flags & MER_EPI_GELU)
-                              ? ((ep.flags & MER_EPI_GELU_LIBM) ? 2 : ((ep.flags & EPI_GELU_PACKED) ? 5 : 1)) : 0;
-    const int out_kind = (ep.flags & MER_EPI_OUT_F16) ? 3 : (ep.flags & MER_EPI_SPLIT_BF16) ? 2 :
-                         ((ep.flags & MER_EPI_ROUND_TF32) ? 1 : 0);
-    const int kind = gelu_kind * 4 + out_kind;
-    for (int t = first_tile; t < num_tiles; t += tile_step) {
-      const int n_blk = t % n_tiles;
-      const int mb = (t / n_tiles) * CLUSTER + cta_rank;
-      const int b = mb / m_tiles;
-      const int mt = mb % m_tiles;
-      const int m0 = mt * BLOCK_M + ew * 32;  // first row (inside the batch entry) of this warp's 32
-      EpiTile tl;
-      tl.n0 = n_blk * BLOCK_N + cq * (BLOCK_N / 4);
-      tl.rows_left = (mb < total_m) ? rows_per_batch - m0 : 0;
-      const long long out_row = (long long)b * ep.out_bstride + ep.out_row0 + m0;
-      tl.out_off = (out_row + p_row) * (long long)ep.ld_out + tl.n0;
-      tl.res_lane = ep.res ? ep.res + ((long long)b * ep.res_bstride + ep.res_row0 + m0 + p_row) *
-                                          (long long)ep.ld_res + tl.n0
-                           : nullptr;
-      tl.vt_idx = out_row + lane;
-      tl.ld_out8 = 8ll * ep.ld_out;
-      tl.ld_res8 = 8ll * ep.ld_res;
-      if (ep.res && lane < tl.rows_left) {
-        // this warp's 32 x (BLOCK_N / 4) residual block: pull its lines into L2 while the MMAs run
-        const float* rrow = ep.res + ((long long)b * ep.res_bstride + ep.res_row0 + m0 + lane) *
-                                         (long long)ep.ld_res + tl.n0;
-#pragma unroll
-        for (int i = 0; i < BLOCK_N / 128; ++i)
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(rrow + 32 * i));
-      }
-      __syncwarp();
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      tl.t_addr = tmem_base + (uint32_t(ew * 32) << 16) + as * BLOCK_N + cq * (BLOCK_N / 4);
-      // all of this warp's TMEM reads of the stage are complete -> hand it back to the MMA warp
-      auto release = [&]() {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (TWOSM) mbar_arrive_cluster(leader_addr(&tempty_bar[as]));  // the leader's MMA warp waits for both CTAs
-          else mbar_arrive(&tempty_bar[as]);
-        }
-      };
-      if (tl.res_lane != nullptr) {  // warp-uniform; each variant is straight-line code
-        if (gelu_kind == 4) epi_tile<CH, 4, 0, true>(tl, ep, stg, lane, release);   // relu(acc + bias + res)
-        else if (gelu_kind != 0) epi_tile<CH, 1, 0, true>(tl, ep, stg, lane, release);  // res + GELU(acc + bias), erf form
-        else if (out_kind == 1) epi_tile<CH, 0, 1, true>(tl, ep, stg, lane, release);
-        else epi_tile<CH, 0, 0, true>(tl, ep, stg, lane, release);
-      } else {
-        switch (kind) {
-          case 0: epi_tile<CH, 0, 0, false>(tl, ep, stg, lane, release); break;
-          case 1: epi_tile<CH, 0, 1, false>(tl, ep, stg, lane, release); break;
-          case 2: epi_tile<CH, 0, 2, false>(tl, ep, stg, lane, release); break;
-          case 3: epi_tile<CH, 0, 3, false>(tl, ep, stg, lane, release); break;
-          case 4: epi_tile<CH, 1, 0, false>(tl, ep, stg, lane, release); break;
-          case 5: epi_tile<CH, 1, 1, false>(tl, ep, stg, lane, release); break;
-          case 6: epi_tile<CH, 1, 2, false>(tl, ep, stg, lane, release); break;
-          case 7: epi_tile<CH, 1, 3, false>(tl, ep, stg, lane, release); break;
-          case 8: epi_tile<CH, 2, 0, false>(tl, ep, stg, lane, release); break;
-          case 9: epi_tile<CH, 2, 1, false>(tl, ep, stg, lane, release); break;
-          case 10: epi_tile<CH, 2, 2, false>(tl, ep, stg, lane, release); break;
-          case 11: epi_tile<CH, 2, 3, false>(tl, ep, stg, lane, release); break;
-          case 13: epi_tile<CH, 3, 1, false>(tl, ep, stg, lane, release); break;   // quick-GELU: the operand
-          case 15: epi_tile<CH, 3, 3, false>(tl, ep, stg, lane, release); break;   // formats FC1 can feed
-          case 16: epi_tile<CH, 4, 0, false>(tl, ep, stg, lane, release); break;   // relu(acc + bias)
-          case 22: epi_tile<CH, 5, 2, false>(tl, ep, stg, lane, release); break;   // packed erf-GELU (opt-in)
-          case 23: epi_tile<CH, 5, 3, false>(tl, ep, stg, lane, release); break;
-          default: epi_tile<CH, 3, 0, false>(tl, ep, stg, lane, release); break;
-        }
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  // nobody leaves while a peer may still multicast into this CTA's smem / arrive on its barriers
-  if (CLUSTER > 1) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if (TWOSM) tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
-    else tmem_dealloc(tmem_base, Cfg::kTmemCols);
+  // ===================== consumers =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const int wg_row0 = (wg - 1) * 64;  // this warpgroup's rows of the tile
+  const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(smem_a + wg_row0 * Cfg::kRowBytes));
+  const uint64_t desc_b0 = wgmma_desc_sw128(smem_u32(smem_b));
+  const int gelu_kind = (ep.flags & MER_EPI_RELU) ? 4 : (ep.flags & MER_EPI_QUICK_GELU) ? 3
+                        : (ep.flags & MER_EPI_GELU)
+                            ? ((ep.flags & MER_EPI_GELU_LIBM) ? 2 : ((ep.flags & EPI_GELU_PACKED) ? 5 : 1)) : 0;
+  const int out_kind = (ep.flags & MER_EPI_OUT_F16) ? 3 : (ep.flags & MER_EPI_SPLIT_BF16) ? 2 :
+                       ((ep.flags & MER_EPI_ROUND_TF32) ? 1 : 0);
+  const int kind = gelu_kind * 4 + out_kind;
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[NH][64];
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    const int n_blk = t % n_tiles;
+    const int mb = t / n_tiles;
+    const int b = mb / m_tiles;
+    const int mt = mb % m_tiles;
+    int prev_stage = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait_nocall(&full_bar[stage], phase);
+      // descriptors: start address field counts 16-byte units; a stage is kABytes / kBBytes further
+      const uint64_t da = desc_a0 + (uint64_t)(stage * (Cfg::kABytes >> 4));
+      const uint64_t db = desc_b0 + (uint64_t)(stage * (Cfg::kBBytes >> 4));
+      constexpr uint64_t kHalfB = (128 * Cfg::kRowBytes) >> 4;  // B rows [128, 256) of the stage
+      wgmma_fence();
+      // advance the start address by 32-byte K steps inside the 128B swizzle row (>>4 => +2)
+#pragma unroll
+      for (int k = 0; k < (Cfg::kSplit ? 2 : 4); ++k) {
+#pragma unroll
+        for (int hh = 0; hh < NH; ++hh) {
+          const uint64_t dbh = db + hh * kHalfB;
+          if (!Cfg::kSplit) {
+            wgmma_m64n128<Cfg::kKind>(acc[hh], da + 2 * k, dbh + 2 * k, (kb | k) != 0);
+          } else {  // 2 x 16 bf16; hi at bytes [0,64), lo at [64,128) of the row
+            wgmma_m64n128<1>(acc[hh], da + 2 * k, dbh + 2 * k, (kb | k) != 0);  // hi * hi
+            wgmma_m64n128<1>(acc[hh], da + 4 + 2 * k, dbh + 2 * k, 1);          // lo * hi
+            wgmma_m64n128<1>(acc[hh], da + 2 * k, dbh + 4 + 2 * k, 1);          // hi * lo
+          }
+        }
+      }
+      wgmma_commit();
+      // the previous stage's MMAs have retired once at most this stage's group is in flight: free its slot
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int hh = 0; hh < NH; ++hh)
+#pragma unroll
+      for (int r = 0; r < 64; ++r) wgmma_fence_operand(acc[hh][r]);
+    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    const int n_base = n_blk * BLOCK_N;
+    const int m_base = mt * BLOCK_M;
+    const long long out_row_b = (long long)b * ep.out_bstride + ep.out_row0;
+    const long long res_row_b = (long long)b * ep.res_bstride + ep.res_row0;
+#define MER_EPI(G, O, R) epi_tile<NH, G, O, R>(acc, ep, n_base, m_base, rows_per_batch, out_row_b, res_row_b, wg_row0)
+    if (ep.res != nullptr) {  // uniform across the kernel; each variant is straight-line code
+      if (gelu_kind == 4) MER_EPI(4, 0, true);        // relu(acc + bias + res)
+      else if (gelu_kind != 0) MER_EPI(1, 0, true);   // res + GELU(acc + bias), erf form
+      else if (out_kind == 1) MER_EPI(0, 1, true);
+      else MER_EPI(0, 0, true);
+    } else {
+      switch (kind) {
+        case 0: MER_EPI(0, 0, false); break;
+        case 1: MER_EPI(0, 1, false); break;
+        case 2: MER_EPI(0, 2, false); break;
+        case 3: MER_EPI(0, 3, false); break;
+        case 4: MER_EPI(1, 0, false); break;
+        case 5: MER_EPI(1, 1, false); break;
+        case 6: MER_EPI(1, 2, false); break;
+        case 7: MER_EPI(1, 3, false); break;
+        case 8: MER_EPI(2, 0, false); break;
+        case 9: MER_EPI(2, 1, false); break;
+        case 10: MER_EPI(2, 2, false); break;
+        case 11: MER_EPI(2, 3, false); break;
+        case 13: MER_EPI(3, 1, false); break;   // quick-GELU: the operand
+        case 15: MER_EPI(3, 3, false); break;   // formats FC1 can feed
+        case 16: MER_EPI(4, 0, false); break;   // relu(acc + bias)
+        case 22: MER_EPI(5, 2, false); break;   // paired erf-GELU (opt-in)
+        case 23: MER_EPI(5, 3, false); break;
+        default: MER_EPI(3, 0, false); break;
+      }
+    }
+#undef MER_EPI
   }
 }
 
 // launches per kernel instantiation (tests assert that the variant a configuration is benchmarked on is the one a
-// parity test exercised): index = mode | (BLOCK_N == 256) << 2 | (CLUSTER == 2) << 3 | TWOSM << 4
-long long g_variant_launches[32] = {};
+// parity test exercised): index = mode | (BLOCK_N == 256) << 2
+long long g_variant_launches[8] = {};
 
-template <int BLOCK_N, int MODE, int CLUSTER, bool TWOSM = false>
+template <int BLOCK_N, int MODE>
 int launch_gemm(const MerGemmDesc* g, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, MODE, TWOSM>;
-  ++g_variant_launches[(MODE & 3) | (BLOCK_N == 256 ? 4 : 0) | (CLUSTER == 2 ? 8 : 0) | (TWOSM ? 16 : 0)];
+  using Cfg = GemmCfg<BLOCK_N, MODE>;
+  ++g_variant_launches[(MODE & 3) | (BLOCK_N == 256 ? 4 : 0)];
   CUtensorMap ta, tb;
   const CUtensorMapDataType dt = Cfg::kSplit ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                  : Cfg::kF16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -597,55 +362,38 @@ int launch_gemm(const MerGemmDesc* g, cudaStream_t stream) {
     const int K = g->K_inner * g->taps;
     const uint64_t dims[2] = {(uint64_t)K * mult, (uint64_t)g->N};
     const uint64_t strides[1] = {(uint64_t)K * sbytes};
-    const uint32_t box[2] = {(uint32_t)(Cfg::kBlockK * mult), BLOCK_N / CLUSTER};  // each CTA loads its share
+    const uint32_t box[2] = {(uint32_t)(Cfg::kBlockK * mult), BLOCK_N};
     if (int rc = mer_make_tmap(&tb, dt, 2, g->W, dims, strides, box, sw)) return rc;
   }
   static MerPerDevice attr_set;
   if (attr_set.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<BLOCK_N, MODE, CLUSTER, TWOSM>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
+    MER_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<BLOCK_N, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         Cfg::kSmemBytes));
     attr_set.mark();
   }
   const int m_tiles = (g->rows_per_batch + BLOCK_M - 1) / BLOCK_M;
-  const long long groups = ((long long)g->batches * m_tiles + CLUSTER - 1) / CLUSTER;
-  const long long tiles = groups * (g->N / BLOCK_N);
-  int grid = (mer_num_sms() / CLUSTER) * CLUSTER;
-  if (tiles * CLUSTER < grid) grid = (int)tiles * CLUSTER;
-  // profile class: the GEMM mode; fp16 problems of fewer than 2^17 rows (the HuBERT / BERT layers: 63,744 / 8,192 rows
-  // at the bench shapes, against the ViT's 403,456) are kept apart as class 3 so that the dominant kernel's roofline
-  // is not an average over launches of very different sizes
+  const long long tiles = (long long)g->batches * m_tiles * (g->N / BLOCK_N);
+  MER_REQUIRE(tiles < (1ll << 31), "mer_gemm: %lld tiles", tiles);
+  int grid = mer_num_sms();
+  if (tiles < grid) grid = (int)tiles;
+  // profile class: the GEMM mode; fp16 problems of fewer than 2^17 rows (the HuBERT / BERT layers) are kept apart
+  // as class 3 so that the dominant kernel's roofline is not an average over launches of very different sizes
   const int klass = (MODE == MER_GEMM_F16 && (long long)g->rows_per_batch * g->batches < (1ll << 17)) ? MER_PROF_F16_SMALL
                                                                                                         : MODE;
   const int prof = mer_prof_begin(klass, 2.0 * (double)g->rows_per_batch * g->batches * g->N *
                                              (double)(g->K_inner * g->taps), stream);
+  MerGemmEpilogue ep = g->ep;
   {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CLUSTER;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    MerGemmEpilogue ep = g->ep;
-    {
-      const bool plain_gelu = (ep.flags & MER_EPI_GELU) && !(ep.flags & MER_EPI_GELU_LIBM) && !ep.res;
-      if (plain_gelu && (ep.flags & (MER_EPI_OUT_F16 | MER_EPI_SPLIT_BF16))) {
-        // FC1 launches only; read at every such launch so that tests can run both forms in one process
-        const char* e = getenv("MER_GELU_PACKED");
-        if (e && atoi(e) == 1) ep.flags |= EPI_GELU_PACKED;
-      }
+    const bool plain_gelu = (ep.flags & MER_EPI_GELU) && !(ep.flags & MER_EPI_GELU_LIBM) && !ep.res;
+    if (plain_gelu && (ep.flags & (MER_EPI_OUT_F16 | MER_EPI_SPLIT_BF16))) {
+      // FC1 launches only; read at every such launch so that tests can run both forms in one process
+      const char* e = getenv("MER_GELU_PACKED");
+      if (e && atoi(e) == 1) ep.flags |= EPI_GELU_PACKED;
     }
-    MER_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<BLOCK_N, MODE, CLUSTER, TWOSM>, ta, tb, ep,
-                                      g->rows_per_batch, g->batches, g->N, g->K_inner * g->taps,
-                                      g->K_inner, g->P, g->a_row0, g->a_col_group));
   }
+  gemm_kernel<BLOCK_N, MODE><<<grid, NUM_THREADS, Cfg::kSmemBytes, stream>>>(
+      ta, tb, ep, g->rows_per_batch, g->batches, g->N, g->K_inner * g->taps, g->K_inner, g->P, g->a_row0,
+      g->a_col_group);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
   mer_prof_end(prof, stream);
@@ -656,7 +404,8 @@ int launch_gemm(const MerGemmDesc* g, cudaStream_t stream) {
 
 extern "C" long long mer_gemm_variant_launches(int block_n, int mode, int cluster, int twosm) {
   if ((block_n != 128 && block_n != 256) || mode < 0 || mode > 2 || cluster < 1 || cluster > 2) return -1;
-  return g_variant_launches[(mode & 3) | (block_n == 256 ? 4 : 0) | (cluster == 2 ? 8 : 0) | (twosm ? 16 : 0)];
+  if (cluster != 1 || twosm) return 0;  // sm_90 build: single-CTA tiles only
+  return g_variant_launches[(mode & 3) | (block_n == 256 ? 4 : 0)];
 }
 
 int mer_gemm_launch(const MerGemmDesc* g, cudaStream_t stream) {
@@ -701,23 +450,9 @@ int mer_gemm_launch(const MerGemmDesc* g, cudaStream_t stream) {
   // 128 x 256 tiles whenever they fill the machine; 128 x 128 for small problems / N % 256 != 0
   const bool wide = (tiles256 >= mer_num_sms() && g->force_block_n != 128) ||
                     (g->force_block_n == 256 && tiles256 > 0);
-  // CTA pairs with a multicast B tile once there is more than a wave of 128x256 tiles
-  const bool pair = wide && g->cluster != 1 && (g->cluster >= 2 || tiles256 >= 2 * mer_num_sms());
-  // CTA pairs issue cta_group::2 MMAs by default (measured +3..9% over single-CTA MMAs with a multicast
-  // weight tile); MER_GEMM_NO_2SM=1 or cluster == 2 selects the multicast variant
-  static const bool no_twosm_env = getenv("MER_GEMM_NO_2SM") != nullptr;
-  const bool twosm = pair && (g->cluster == 3 || (g->cluster == 0 && !no_twosm_env));
-  if (g->mode == MER_GEMM_F16) {
-    if (pair) return launch_gemm<256, MER_GEMM_F16, 2, true>(g, stream);  // pairs always issue cta_group::2
-    return wide ? launch_gemm<256, MER_GEMM_F16, 1>(g, stream) : launch_gemm<128, MER_GEMM_F16, 1>(g, stream);
-  }
-  if (g->mode == MER_GEMM_BF16X3) {
-    if (twosm) return launch_gemm<256, MER_GEMM_BF16X3, 2, true>(g, stream);
-    if (pair) return launch_gemm<256, MER_GEMM_BF16X3, 2>(g, stream);
-    return wide ? launch_gemm<256, MER_GEMM_BF16X3, 1>(g, stream)
-                : launch_gemm<128, MER_GEMM_BF16X3, 1>(g, stream);
-  }
-  if (twosm) return launch_gemm<256, MER_GEMM_TF32, 2, true>(g, stream);
-  if (pair) return launch_gemm<256, MER_GEMM_TF32, 2>(g, stream);
-  return wide ? launch_gemm<256, MER_GEMM_TF32, 1>(g, stream) : launch_gemm<128, MER_GEMM_TF32, 1>(g, stream);
+  if (g->mode == MER_GEMM_F16)
+    return wide ? launch_gemm<256, MER_GEMM_F16>(g, stream) : launch_gemm<128, MER_GEMM_F16>(g, stream);
+  if (g->mode == MER_GEMM_BF16X3)
+    return wide ? launch_gemm<256, MER_GEMM_BF16X3>(g, stream) : launch_gemm<128, MER_GEMM_BF16X3>(g, stream);
+  return wide ? launch_gemm<256, MER_GEMM_TF32>(g, stream) : launch_gemm<128, MER_GEMM_TF32>(g, stream);
 }

@@ -1,6 +1,6 @@
-// mer_common.cuh — sm_100a building blocks shared by every kernel in libmer_b200.so.
+// mer_common.cuh — sm_90a building blocks shared by every kernel in libmer_b200.so.
 //
-// Thin inline-PTX wrappers (mbarrier, TMA, tcgen05/TMEM) plus the error plumbing of the
+// Thin inline-PTX wrappers (mbarrier, TMA, wgmma) plus the error plumbing of the
 // C ABI declared in include/mer_b200.h.  Nothing here has a CPU fallback: every entry point
 // of the library runs on the device or fails with a non-zero status.
 #pragma once
@@ -125,6 +125,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// same bound without the printf: a function call between wgmma instructions makes ptxas serialise them
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > MER_SPIN_LIMIT) __trap();
+  }
+}
 
 // ---- TMA -----------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -156,86 +163,57 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       : "memory");
 }
 
-// B-operand half tile, multicast to every CTA in cta_mask (same smem offset and mbarrier offset in each)
-__device__ __forceinline__ void tma_load_2d_mc(void* smem, const CUtensorMap* m, uint64_t* bar,
-                                               int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
+// ---- wgmma (sm_90a warpgroup MMA; operands in shared memory, fp32 accumulators in registers) ----------
+// Shared-memory matrix descriptor of a K-major operand tile laid out by TMA with SWIZZLE_128B: rows of 128 bytes,
+// 8-row groups 1024 bytes apart (SBO), LBO unused (1).  bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 |
+// [62,64) layout (1 = 128B swizzle).  Advancing the start address by 32 bytes steps K inside the swizzle row.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (uint64_t(1024 >> 4) << 32) |
+         (1ull << 62);
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+__device__ __forceinline__ void wgmma_fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// ---- CTA-pair (cta_group::2) forms: the pair's barriers live in the even ("leader") CTA; clearing bit
-// 24 of a shared-window address turns a CTA-local barrier address into the leader's copy of it ----
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t leader_addr(const void* p) { return smem_u32(p) & kPeerBitMask; }
-__device__ __forceinline__ void mbar_expect_tx_cluster(uint32_t bar_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem, const CUtensorMap* m, uint32_t bar_addr,
-                                                int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* smem, const CUtensorMap* m, uint32_t bar_addr,
-                                                int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// commit of the pair's MMAs, arriving on the barrier at this offset in both CTAs
-__device__ __forceinline__ void tc_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-          "r"(smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-// D[tmem of both CTAs] (+)= A[2 x 128 rows, one half per CTA] * B[N rows, one half per CTA]
-__device__ __forceinline__ void tc_mma_tf32_2sm(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b,
-                                                uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_2sm(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b,
-                                                uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+#define MER_WGMMA_D64                                                                                            \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "  \
+  "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define MER_WGMMA_OUT64(d)                                                                                        \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),      \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),       \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),      \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),      \
+      "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),      \
+      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),      \
+      "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),      \
+      "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+
+// D[64 x 128] (+)= A[64 x K-step] * B[128 x K-step]^T, both K-major in shared memory; one warpgroup issues.
+// kind: 0 = f16 (k16), 1 = bf16 (k16), 2 = tf32 (k8).  accumulate = 0 overwrites D.
+template <int KIND>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+  if (KIND == 0) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " MER_WGMMA_D64 ", %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : MER_WGMMA_OUT64(d)
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+  } else if (KIND == 1) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " MER_WGMMA_D64 ", %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : MER_WGMMA_OUT64(d)
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+  } else {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " MER_WGMMA_D64 ", %64, %65, p, 1, 1;\n}\n"
+                 : MER_WGMMA_OUT64(d)
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+  }
 }
 
 // ---- thread-block clusters ----
@@ -247,131 +225,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// ---- tcgen05 / TMEM ------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// tcgen05.commit: arrive on an mbarrier once every previously issued MMA of this thread is done
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::
-                   "r"(smem_u32(bar))
-               : "memory");
-}
-// same, arriving on the barrier at this smem offset in every CTA of cta_mask
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-          "r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], tf32 inputs, fp32 accumulate.  One thread issues.
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread (thread = TMEM lane)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 16 columns (2 KB): half the registers of the x32 form, for software-pipelined readers
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM: 32 lanes x 8 columns (thread = lane / row), and the matching wait
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (128 rows = lanes, 16 fp16 per K step packed two per column) comes
-// from tensor memory -- the P V product of the attention kernel, P written by the softmax threads with tcgen05.st
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major operand tile laid out by TMA with
-// SWIZZLE_128B: rows of 128 bytes, 8-row groups 1024 bytes apart (SBO), LBO ignored (=1).
-// bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor, kind::tf32 / kind::f16, fp32 accumulate, K-major A and B.
-// fmt: 0 = f16, 1 = bf16, 2 = tf32
-__host__ __device__ constexpr uint32_t umma_idesc(int fmt, int m, int n) {
-  return (1u << 4) | (uint32_t(fmt) << 7) | (uint32_t(fmt) << 10) | (uint32_t(n >> 3) << 17) |
-         (uint32_t(m >> 4) << 24);
 }
 
 // ---- numerics ------------------------------------------------------------------------------
@@ -456,14 +309,9 @@ __device__ __forceinline__ float quick_gelu_fast(float x) {
   return x * r;
 }
 
-// ---- packed fp32 pairs (Blackwell FFMA2 / FMUL2 / FADD2: one issue slot for two lanes' worth of fp32 math;
-//      operands are 64-bit register pairs, broadcast scalars and |x| modifiers fold into the instruction) and
-//      the three-input max (FMNMX3) ----
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+// ---- fp32 pairs (two lanes' worth of math on a 64-bit register pair, as the softmax / GELU code is written;
+//      sm_90 has no paired fp32 instructions, so each pair op is two scalar ones) and the three-input max ----
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -473,19 +321,23 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 // 2^x for two values on the FMA / ALU pipes instead of MUFU.EX2 (softmax kernels, where the 16 lanes of the XU
 // pipe are the floor): x = n + f with n = round(x) taken from the mantissa of x + 1.5 * 2^23, f in [-0.5, 0.5],
@@ -508,8 +360,7 @@ __device__ __forceinline__ void ex2_poly2(uint64_t x2, float& a, float& b) {
   a = __uint_as_float(__float_as_uint(p0) + (__float_as_uint(r0) << 23));
   b = __uint_as_float(__float_as_uint(p1) + (__float_as_uint(r1) << 23));
 }
-// gelu_erf_fast on two values at once: 7 FFMA2 + 5 FMUL2 + 4 MUFU for the pair (the scalar form spends
-// 7 FFMA + 5 FMUL + 2 MUFU per value).  Same polynomial; the constants of the first two steps are folded
+// gelu_erf_fast on two values at once.  Same polynomial; the constants of the first two steps are folded
 // (0.3275911 / sqrt 2 and -log2(e) / 2), which moves individual results by at most an ulp of the intermediate.
 __device__ __forceinline__ void gelu_erf_fast2(float x0, float x1, float& g0, float& g1) {
   const uint64_t x = pack2(x0, x1), ax = pack2(fabsf(x0), fabsf(x1));
@@ -528,6 +379,19 @@ __device__ __forceinline__ void gelu_erf_fast2(float x0, float x1, float& g0, fl
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
   const uint64_t erf_abs = fma2(mul2(p, t), pack2(e0, e1), bc(1.0f));  // erf(|x| / sqrt 2)
   unpack2(fma2(mul2(ax, bc(0.5f)), erf_abs, mul2(x, bc(0.5f))), g0, g1);
+}
+
+// torch.optim.Adam (coupled L2) on one parameter, in torch's operation order (lerp for the first moment, mul +
+// addcmul for the second).  Every rounding step is explicit so that the fused and the stand-alone Adam kernels, compiled
+// in different contexts, contract nothing differently and agree bit for bit.  bc1 = 1 - beta1^t,
+// bc2_sqrt = sqrt(1 - beta2^t).  Returns the new parameter; m / v are updated in place.
+__device__ __forceinline__ float adam_param(float pi, float grad, float& m, float& v, float lr, float beta1, float beta2,
+                                            float eps, float wd, float bc1, float bc2_sqrt) {
+  grad = __fmaf_rn(wd, pi, grad);
+  m = __fmaf_rn(__fsub_rn(grad, m), __fsub_rn(1.f, beta1), m);
+  v = __fmaf_rn(v, beta2, __fmul_rn(__fmul_rn(__fsub_rn(1.f, beta2), grad), grad));
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+  return __fsub_rn(pi, __fmul_rn(__fdiv_rn(lr, bc1), __fdiv_rn(m, denom)));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -40,23 +40,14 @@ int mer_layernorm_launch(const float* x, const float* gamma, const float* beta, 
 int mer_attention_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx,
                          const int* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
                          int flags, cudaStream_t stream);
-bool mer_attention_uses_tc(int max_seqlen);  // the tcgen05 kernel needs V^T from the QKV GEMM
-// attention_tc.cu (tcgen05; max_seqlen <= 256)
-int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx,
-                            const int* cu_seqlens, int n_seq, long long tokens, int heads, int flags,
-                            cudaStream_t stream);
-
-// attention_f16.cu (tcgen05, fp16 q | k | v^T in, fp16 ctx out; max_seqlen <= 249) and attention_f16_long.cu (250 .. 505:
-// audio rows of up to 10 s, CLIP L/14).  _supported: some fp16 kernel takes sequences of this length
-bool mer_attention_f16_supported(int max_seqlen);
-bool mer_attention_f16_long_supported(int max_seqlen);
-int mer_attention_f16_long_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
-                                  const int* cu_seqlens, int n_seq, long long tokens, int heads, cudaStream_t stream,
-                                  int max_seqlen, int out_mode);
-bool mer_attention_legacy();  // MER_ATTENTION_LEGACY set: only the mma.sync kernel of attention.cu (debug)
-int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
-                             const int* cu_seqlens, int n_seq, long long tokens, int heads,
-                             cudaStream_t stream, int max_seqlen = 0);
+bool mer_attention_uses_tc(int max_seqlen);  // the tf32 V^T kernel takes this length (needs V^T from the QKV GEMM)
+bool mer_attention_legacy();  // MER_ATTENTION_LEGACY set: only the kernel of attention.cu (debug)
+// attention_f16.cu: V^T kernels.  out_mode: 0 fp32, 1 tf32-rounded fp32, 2 bf16 hi | lo split rows, 3 fp16
+bool mer_attention_f16_supported(int max_seqlen);  // fp16 q | k | V^T, up to 505 tokens
+int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
+                             int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
+int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
+                            int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 
 // helpers.cu
 int mer_vit_patchify_launch(const uint8_t* frames_bgr, int n_frames, float* a_patches,
@@ -110,7 +101,7 @@ struct MerStackArgs {
   float* x;                  // [tokens,768] residual stream (in/out)
   float* xn;                 // [tokens,768] scratch (LN out / attention ctx / pre-LN sum)
   float* xs;                 // BF16X3 only: [tokens,768] slots holding the split copy of x
-  float* vt;                 // [768, vt_ld] V^T for the tcgen05 attention (or null: flash kernel)
+  float* vt;                 // [768, vt_ld] V^T for the V^T attention kernels (or null: attention.cu)
   long long vt_ld;           // >= tokens, multiple of 4
   float* qkv;                // [tokens,2304]
   float* h;                  // [tokens,3072]

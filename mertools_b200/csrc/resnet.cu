@@ -3,7 +3,7 @@
 // fc layer on Resize(224) / ToTensor / Normalize(ImageNet) frames -> one 512-vector per frame).
 //
 // Every convolution (BatchNorm folded into weight and bias at load time) is an im2col gather into an fp16
-// operand followed by the shared tcgen05 GEMM (MER_GEMM_F16) with its epilogue doing bias (+ identity)
+// operand followed by the shared wgmma GEMM (MER_GEMM_F16) with its epilogue doing bias (+ identity)
 // + ReLU; activations stay NHWC fp32 between layers (the GEMM's residual input is fp32).  64-channel layers
 // are stored with 128 channels (upper half zero) because the GEMM's narrowest column block is 128; the gather
 // reads only the real channels, so K is not inflated.  Max-pool and the im2col gathers are plain coalesced

@@ -88,9 +88,8 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
 }
 
 // Round-2 form (default; MER_LN_VER=1 keeps the kernel above): the same arithmetic, row for row, with gamma / beta in
-// shared memory instead of 2 x 4 VEC registers per lane.  ncu of the first form at the ViT shape (profiles/
-// r1_layernorm_kernel_hotspots.json): 96 registers -> two blocks = 16 warps per SM, each alternating between a load
-// phase (3 KB in flight) and a reduce / store phase with nothing in flight: 0.69-0.72 of the HBM peak.  Here a warp
+// shared memory instead of 2 x 4 VEC registers per lane.  The first form needs 96 registers -> two blocks = 16 warps
+// per SM, each alternating between a load phase (3 KB in flight) and a reduce / store phase with nothing in flight.  Here a warp
 // fits 64 registers at 768 columns (four blocks = 32 warps per SM) and requests its NEXT row before it reduces and stores the
 // current one, so loads stay in flight through the whole loop.
 template <int VEC>
@@ -260,7 +259,7 @@ int mer_accumulate_launch(const float* x, float* acc, long long n, int init, cud
   MER_REQUIRE(x && acc && n % 4 == 0, "mer_accumulate: bad operands");
   if (n <= 0) return 0;
   long long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > mer_num_sms() * 32) blocks = mer_num_sms() * 32;
   accumulate_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<const float4*>(x),
                                                      reinterpret_cast<float4*>(acc), n / 4, init);
   MER_CUDA_CHECK(cudaGetLastError());
@@ -272,7 +271,7 @@ int mer_cast_f16_launch(const float* in, void* out, long long n, cudaStream_t st
   MER_REQUIRE(in && out && n % 4 == 0, "mer_cast_f16: bad operands");
   if (n <= 0) return 0;
   long long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > mer_num_sms() * 32) blocks = mer_num_sms() * 32;
   cast_f16_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<const float4*>(in),
                                                    reinterpret_cast<uint2*>(out), n / 4);
   MER_CUDA_CHECK(cudaGetLastError());
@@ -283,7 +282,7 @@ int mer_cast_f16_launch(const float* in, void* out, long long n, cudaStream_t st
 extern "C" int mer_round_tf32(float* x, long long n, void* stream) {
   if (n <= 0) return 0;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > mer_num_sms() * 32) blocks = mer_num_sms() * 32;
   round_tf32_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
@@ -294,7 +293,7 @@ extern "C" int mer_split_bf16(const float* in, void* out, long long rows, int K,
   MER_REQUIRE(in && out && (const void*)in != out && K > 0 && K % 32 == 0, "mer_split_bf16: bad operands");
   if (rows <= 0) return 0;
   long long blocks = (rows * (K / 4) + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > mer_num_sms() * 32) blocks = mer_num_sms() * 32;
   split_bf16_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(in, out, rows, K);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);

@@ -183,7 +183,7 @@ int mer_num_sms() {
   const int dev = MerPerDevice::current();
   int& n = cache[dev];
   if (!n) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -204,7 +204,7 @@ int mer_check_device(void) {
   MER_CUDA_CHECK(cudaGetDevice(&dev));
   MER_CUDA_CHECK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   MER_CUDA_CHECK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  MER_REQUIRE(major == 10, "libmer_b200 needs an sm_100a device, found sm_%d%d", major, minor);
+  MER_REQUIRE(major == 9 && minor == 0, "libmer_b200 needs an sm_90a device (H100), found sm_%d%d", major, minor);
   return 0;
 }
 

@@ -340,7 +340,7 @@ class MerResnet18Model(C.Structure):
 
 class ResNet18Encoder:
     """torchvision resnet18 without its fc layer (the reference's ImageNet CNN extractor): BatchNorm folded
-    into the convolutions at load, every convolution an fp16 im2col + tcgen05 GEMM with a ReLU epilogue.
+    into the convolutions at load, every convolution an fp16 im2col + wgmma GEMM with a ReLU epilogue.
 
     Reference: MERBench/feature_extraction/visual/extract_imagenet_embedding.py:47-55."""
 
@@ -811,7 +811,7 @@ class FerplusResnet50Encoder(_CnnEncoder):
     """``resnet50_ferplus_dag`` (or ``senet50_ferplus_dag``: same skeleton + a squeeze-and-excitation gate per block,
     picked up from the state_dict) up to ``conv5_3_3x3_relu`` + AvgPool2d(7) (what the reference's FER+ extractor keeps
     with its default ``--layer_name``): 52 BatchNorm-folded convolutions through the table-driven CNN executor
-    (im2col + tcgen05 GEMMs on split-bf16 operands: fp16 operands measured 6e-4 in an fp32 emulation, too close
+    (im2col + wgmma GEMMs on split-bf16 operands: fp16 operands measured 6e-4 in an fp32 emulation, too close
     to the 1e-3 bar), caffe-style strides, ceil-mode max-pool.
 
     Reference: MERBench/feature_extraction/visual/extract_ferplus_embedding.py:62-115,
@@ -830,7 +830,7 @@ class FerplusResnet50Encoder(_CnnEncoder):
 class ManetEncoder(_CnnEncoder):
     """MA-Net (the RAF-DB checkpoint the reference extracts ``manet_<UTT|FRA>`` features with): ResNet-18 trunk, four
     14 x 14 patch branches of CBAM AttentionBlocks, a multi-scale branch of MulScaleBlocks; 1024-d embedding.
-    120 BatchNorm-folded convolutions on split-bf16 tcgen05 GEMMs + 16 fused CBAM gates.
+    120 BatchNorm-folded convolutions on split-bf16 wgmma GEMMs + 16 fused CBAM gates.
 
     Reference: MERBench/feature_extraction/visual/extract_manet_embedding.py:31-61,
     manet/model/manet.py:16-270, manet/model/attention.py:27-84."""
@@ -925,7 +925,7 @@ def vggish_tables(state_dict, pack):
 
 
 class VggishEncoder:
-    """VGGish embedding network of the reference's audio extractor: six 3x3 convolutions as im2col + tcgen05
+    """VGGish embedding network of the reference's audio extractor: six 3x3 convolutions as im2col + wgmma
     GEMMs with ReLU epilogues, 2x2 max-pools, three fully connected layers; all GEMMs on split-bf16 operands
     (MER_GEMM_BF16X3, ~fp32 accuracy: there is no normalisation between the nine layers).
 
@@ -1099,7 +1099,7 @@ class HubertEncoder:
         # Operand format of the transformer layers (the conv feature encoder always runs BF16X3):
         #  * post-LN base family (HuBERT-base, wav2vec2-base, data2vec-audio): "f16" by default since round 2 -- one
         #    MMA per product instead of three; emulated readout error at 12 layers 3.3e-4 against 4e-5
-        #    (profiles/r2_precision_table.json), measured in tests/test_bench_config_gpu.py; MER_AUDIO_PRECISION=bf16x3
+        #    (scripts/precision_table.py), measured in tests/test_bench_config_gpu.py; MER_AUDIO_PRECISION=bf16x3
         #    (or stack_precision="bf16x3") keeps the split operands.
         #  * large (pre-LN) family: BF16X3 by default, "f16" opt-in (MER_HUBERT_LARGE_PRECISION=f16; clips of <= 249
         #    frames then run the stack on fp16 operands like the ViT, longer ones keep BF16X3).
@@ -1116,7 +1116,7 @@ class HubertEncoder:
         # "f16" (default there) runs them as ONE fp16 MMA per product, conv3..6 and the feature projection stay BF16X3.
         # Emulated readout error at 12 layers (4 checkpoints x clips): 3.5e-4 mean / 4.2e-4 max against 3.2e-4 / 3.7e-4
         # with every conv on split operands; conv1..6 in fp16 would be 4.4e-4 / 5.1e-4
-        # (profiles/r2_precision_conv_layers.json).  MER_AUDIO_CONV_PRECISION=bf16x3 / conv_precision="bf16x3" opts out.
+        # (scripts/precision_conv_layers.py).  MER_AUDIO_CONV_PRECISION=bf16x3 / conv_precision="bf16x3" opts out.
         default_conv = "f16" if (self.stack_precision == "f16" and not ln_convs and not m.stable_layer_norm and
                                  self.hidden == 768 and self.n_layers <= 12) else "bf16x3"  # the emulated configuration
         self.conv_precision = conv_precision or _os.environ.get("MER_AUDIO_CONV_PRECISION", default_conv)
@@ -1204,7 +1204,7 @@ class BertEncoder:
         """precision: operand format of the layers' linear products.  "f16" (default for the 12-layer base models since
         round 2; env MER_TEXT_PRECISION): one fp16 MMA per product, readout error 2.9e-4 at 12 layers; "bf16x3"
         (default for the 24-layer -large models): three bf16 MMAs on (hi, lo) pairs, 3.5e-5
-        (profiles/r2_precision_table.json)."""
+        (scripts/precision_table.py)."""
         L.check(L.lib().mer_check_device())
         sd = W._np(state_dict)
         self.device = torch.device(device)
@@ -1212,7 +1212,7 @@ class BertEncoder:
         self.position_offset = position_offset  # 0 = BERT, 2 = RoBERTa (pad_token_id + 1)
         self.n_layers = W.count_layers(sd, "encoder.layer.{i}.output.LayerNorm.weight")
         assert "embeddings_project.weight" not in sd, \
-            "ELECTRA-small style checkpoints (embedding_size != hidden_size) are not on the B200 path"
+            "ELECTRA-small style checkpoints (embedding_size != hidden_size) are not on the H100 path"
         m = MerBertModel()
         m.n_layers, m.ln_eps = self.n_layers, ln_eps
         self.word = pk.keep(sd["embeddings.word_embeddings.weight"])

@@ -1,4 +1,4 @@
-"""Acoustic feature extraction — B200 mirror of
+"""Acoustic feature extraction — H100 mirror of
 MERBench/feature_extraction/audio/extract_audio_huggingface.py (HuBERT / wav2vec2-base branch).
 
 Keeps ``extract(model_name, audio_files, save_dir, feature_level, gpu)`` (:52) and
@@ -60,8 +60,8 @@ class AudioExtractor:
             self.enc = HubertEncoder(state_dict, device=device)
         self.device = self.enc.device
         self.max_rows = max_rows_per_launch
-        # measured on B200 (round 2): 979 clips/s ragged against 101 with one pass per distinct length, on 128 clips
-        # of U(2 s, 10 s); results agree to 9e-6
+        # ragged batches: one launch chain for clips of any length instead of one pass per distinct length; results
+        # agree with the per-length passes to float rounding
         self.ragged = (os.environ.get("MER_AUDIO_RAGGED", "1") != "0") if ragged is None else bool(ragged)
         self.max_samples = max_samples_per_launch
         # Wav2Vec2FeatureExtractor.do_normalize of the checkpoint (common.read_do_normalize): zero-mean / unit-variance or not

@@ -2,12 +2,12 @@
 graph; MERBench/feature_extraction/visual/extract_vision_huggingface.py:124-133: every frame -> processor ->
 ``hidden_states[-1].sum(dim=1)``).
 
-BEiT layers add a per-layer relative position bias to the attention scores, which the tcgen05 attention kernels do not
+BEiT layers add a per-layer relative position bias to the attention scores, which the tensor-core attention kernels do not
 take; the embeddings run through ``mer_clip_vision_forward`` (MER_VISION_EMBED_ONLY: patch gather + GEMM + class row)
 and the layers are orchestrated over kernel-level entry points through an ``ops`` backend (TF32 linears,
 ``mer_layernorm``, ``mer_biased_attention``), so that the orchestration runs against the oracle with a torch backend on
 CPU (tests/test_host_logic.py).  LayerScale is folded into each branch's last linear layer at load.
-GPU parity test: tests/test_variants_gpu.py (green on a B200 since round 2).
+GPU parity test: tests/test_variants_gpu.py.
 """
 from __future__ import annotations
 

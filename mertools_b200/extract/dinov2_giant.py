@@ -6,7 +6,7 @@ dinov2-large runs on the fused CLIP L/14 tower (``encoders.Dinov2Encoder``); the
 tower, so its layers are orchestrated over kernel-level entry points through an ``ops`` backend (TF32 linears,
 ``mer_layernorm`` at 1536 columns, the flash attention kernel over 257 tokens, ``mer_swiglu``), embeddings through
 ``PatchEmbedder`` (MER_VISION_EMBED_ONLY).  LayerScale is folded into each branch's last linear layer at load.
-GPU parity test: tests/test_variants_gpu.py (green on a B200 since round 2).
+GPU parity test: tests/test_variants_gpu.py.
 """
 from __future__ import annotations
 

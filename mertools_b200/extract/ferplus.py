@@ -39,7 +39,7 @@ def main(params, config=None, state_dict=None):
     if config is None:
         from .. import config as config  # noqa: PLW0127
     assert params.model_name in SUPPORTED and params.layer_name == SUPPORTED[params.model_name], \
-        f"the B200 path covers {SUPPORTED} (other hook layers: use the reference script)"
+        f"the H100 path covers {SUPPORTED} (other hook layers: use the reference script)"
     print("==> Extracting ferplus embedding...")
     face_dir = config.PATH_TO_RAW_FACE[params.dataset]
     save_name = f"{params.model_name.split('_')[0]}face_{params.feature_level[:3]}"

@@ -1,4 +1,4 @@
-"""Lexical feature extraction — B200 mirror of
+"""Lexical feature extraction — H100 mirror of
 MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa-base branch).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
@@ -110,7 +110,7 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
     assert cfg.model_type in ("bert", "roberta", "xlm-roberta"), \
-        f"only BERT/RoBERTa-base encoders are on the B200 path, got {cfg.model_type}"
+        f"only BERT/RoBERTa-base encoders are on the H100 path, got {cfg.model_type}"
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     roberta = cfg.model_type != "bert"
     ext = TextExtractor(common.load_hf_state_dict(model_dir), tokenizer, device=f"cuda:{gpu}",

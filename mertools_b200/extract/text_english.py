@@ -1,4 +1,4 @@
-"""English word-aligned lexical features — B200 mirror of
+"""English word-aligned lexical features — H100 mirror of
 MER2023/feature_extraction/text/extract_text_embedding_LZ.py:extract_bert_embedding_english (:168-311).
 
 The host side is the reference's: split the transcript into words and sentences (:205-224), tokenise each
@@ -6,7 +6,7 @@ sentence as pre-split words (:232), and, after the encoder, merge sub-word embed
 word (:254-291, ``combine_type`` mean | sum | last), then the FRAME / UTTERANCE save rules (:296-309).  The
 encoder pass (sum of the last four hidden states of every real token, :236-238) runs in libmer_b200.so over
 all sentences of a transcript as one packed batch.  BERT / RoBERTa-base style checkpoints only (the
-reference's list also names ALBERT, XLNet, GPT, T5, DeBERTa, which are outside the B200 path).
+reference's list also names ALBERT, XLNet, GPT, T5, DeBERTa, which are outside the H100 path).
 """
 from __future__ import annotations
 
@@ -124,7 +124,7 @@ def extract_bert_embedding_english(model_name, trans_dir, save_dir, feature_leve
         from .. import config as config  # noqa: PLW0127
     print("=" * 30 + f' Extracting "{model_name}" ' + "=" * 30)
     start_time = time.time()
-    assert layer_ids is None or list(layer_ids) == [-4, -3, -2, -1], "only the last-four readout is on the B200 path"
+    assert layer_ids is None or list(layer_ids) == [-4, -3, -2, -1], "only the last-four readout is on the H100 path"
     dir_name = f"{model_name}-4"
     save_dir = os.path.join(save_dir, dir_name + ("-FRA" if feature_level == "FRAME" else "-UTT"))
     if not os.path.exists(save_dir):
@@ -135,7 +135,7 @@ def extract_bert_embedding_english(model_name, trans_dir, save_dir, feature_leve
         raise Exception(f'==> Error: csv out dir "{dir_name}" already exists, set overwrite=TRUE if needed!')
     model_dir = os.path.join(config.PATH_TO_PRETRAINED_MODELS, f"transformers/{model_name}")
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta"), f"only BERT/RoBERTa-base encoders are on the B200 path, got {cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta"), f"only BERT/RoBERTa-base encoders are on the H100 path, got {cfg.model_type}"
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = BertEncoder(common.load_hf_state_dict(model_dir), device=f"cuda:{gpu}", ln_eps=cfg.layer_norm_eps,
                       position_offset=(cfg.pad_token_id + 1) if cfg.model_type != "bert" else 0)

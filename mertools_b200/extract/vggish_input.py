@@ -4,7 +4,7 @@ Mirrors MERBench/feature_extraction/audio/vggish/vggish_input.py (``waveform_to_
 ``wavfile_to_examples`` :85-105) on top of ``mer_logmel`` (mel_features.log_mel_spectrogram with the
 constants of vggish_params.py).  Input audio must already be 16 kHz (the reference resamples other rates
 with resampy; every MER corpus is extracted at 16 kHz, extract_vggish_embedding.py).  The VGGish network
-that consumes these examples is outside the B200 path (SURVEY.md §8f N3/N4).
+that consumes these examples is outside the H100 path (SURVEY.md §8f N3/N4).
 """
 from __future__ import annotations
 

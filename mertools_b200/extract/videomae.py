@@ -5,7 +5,7 @@
 The encoder is orchestrated over kernel-level entry points of libmer_b200.so through the same ``ops`` backend as the
 Whisper branch (``mer_videomae_patchify`` + the patch-embedding GEMM, TF32 linears, ``mer_layernorm``, ``mer_attention``
 over 1568 tokens), so that the orchestration runs against the oracle with a torch backend on CPU
-(tests/test_host_logic.py).  GPU parity test: tests/test_variants_gpu.py (green on a B200 since round 2).
+(tests/test_host_logic.py).  GPU parity test: tests/test_variants_gpu.py.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Frame-level visual feature extraction — B200 mirror of
+"""Frame-level visual feature extraction — H100 mirror of
 MERBench/feature_extraction/visual/extract_vision_huggingface.py.
 
 Same CLI flags (:67-72), same ``config.py`` keys, same output naming

@@ -7,7 +7,7 @@ different attention: a bucketed relative position bias, computed once from layer
 head and query by a small projection of the layer input (HF modeling_wavlm.py WavLMAttention).  The layers are
 orchestrated over kernel-level entry points through an ``ops`` backend (TF32 GEMMs, ``mer_layernorm``,
 ``mer_wavlm_gate``, ``mer_biased_attention``), so that the orchestration runs against the oracle with a torch backend on
-CPU (tests/test_host_logic.py).  GPU parity test: tests/test_variants_gpu.py (green on a B200 since round 2).
+CPU (tests/test_host_logic.py).  GPU parity test: tests/test_variants_gpu.py.
 """
 from __future__ import annotations
 

@@ -7,7 +7,7 @@ for ``whisper-base`` (d_model 512, 8 heads) and ``whisper-large-v2`` (1280, 20 h
 ``mer_layernorm``, ``mer_attention`` (encoder, 1500 frames), ``mer_small_attention`` (decoder) — through a small
 ``ops`` backend, so that the orchestration (weight packing, layer order, residuals, position tables) can be run against
 the reference golden with a torch backend on CPU (tests/test_host_logic.py); ``CudaOps`` is the product backend.
-GPU parity test: tests/test_variants_gpu.py (green on a B200 since round 2).
+GPU parity test: tests/test_variants_gpu.py.
 """
 from __future__ import annotations
 

@@ -596,7 +596,7 @@ class get_models(torch.nn.Module):  # noqa: N801 -- the reference's name (toolki
                                 device=getattr(args, "device", "cuda"))
             object.__setattr__(self, "model", net)
             return
-        assert args.model == "attention", "only the Attention / Attention_TOPN fusion nets are on the B200 path"
+        assert args.model == "attention", "only the Attention / Attention_TOPN fusion nets are on the H100 path"
         self.model = Attention(args)
 
     def forward(self, batch):

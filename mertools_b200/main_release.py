@@ -1,4 +1,4 @@
-"""Attention-fusion training CLI — B200 mirror of MERBench/main-release.py for
+"""Attention-fusion training CLI — H100 mirror of MERBench/main-release.py for
 ``--model attention --feat_type utt --dataset MER2023`` (the configuration of SURVEY.md §8 rows
 a9-a12).  Same flags (:93-124), same hyper-parameter handling (model-tune.yaml ``attention`` grid or
 ``--hyper_path``, :159-165), same label / feature file formats (toolkit/dataloader/mer2023.py:82-104,
@@ -259,7 +259,7 @@ def main(args, config=None, log=None):
     if config is None:
         from . import config as config  # noqa: PLW0127
     assert args.model == "attention" and args.dataset == "MER2023", \
-        "the B200 path covers --model attention --dataset MER2023 (SURVEY.md §8)"
+        "the H100 path covers --model attention --dataset MER2023 (SURVEY.md §8)"
     rank, world = _init_distributed(args)
     torch.cuda.set_device(args.gpu)
     device = torch.device("cuda", args.gpu)

@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# A/B of the opt-in kernel variants (DESIGN.md §8, "prepared ... not yet run on a GPU") on one B200:
+# A/B of the opt-in kernel variants (DESIGN.md §8, "prepared ... not yet run on a GPU") on one GPU:
 #   1. the kernel-level tests of the variants (tests/test_zz_unverified_gpu.py),
 #   2. bench.py once per switch setting; one JSON line per run in gpurun_out/ab_<name>.json.
 # Usage (from the repo root, on the GPU box):  bash scripts/ab_switches.sh [steps] [warmup]

@@ -158,31 +158,6 @@ def sec_gemm_x3():
     return ok
 
 
-def sec_gemm_2sm():
-    """cta_group::2 variant: correctness, then speed against the single-CTA-MMA pair kernel."""
-    ok = True
-    ok &= check_gemm("2sm_int", 256, 256, 64, ints=True, force=256, cluster=3)
-    ok &= check_gemm("2sm_odd_tiles", 128 * 5 + 7, 768, 768, bias=True, res=True, force=256, cluster=3)
-    ok &= check_gemm("2sm_big", 40000, 2304, 768, bias=True, rnd=True, cluster=3)
-    ok &= check_gemm("2sm_fc2", 40000, 768, 3072, bias=True, res=True, cluster=3)
-    for (name, M, N, K, kw) in [("qkv", 100864, 2304, 768, dict(rnd=True)), ("outproj", 100864, 768, 768, dict(res=True)),
-                                ("fc1", 100864, 3072, 768, dict(gelu=True, rnd=True)), ("fc2", 100864, 768, 3072, dict(res=True)),
-                                ("fc1_full", 403456, 3072, 768, dict(gelu=True, rnd=True))]:
-        A = tf32(torch.randn(M, K, device="cuda"))
-        W = tf32(torch.randn(N, K, device="cuda") * 0.02)
-        b = torch.randn(N, device="cuda")
-        R = torch.randn(M, N, device="cuda") if kw.get("res") else None
-        out = torch.empty(M, N, device="cuda")
-        res = {}
-        for cl in (2, 3):
-            ms = time_cuda(lambda: L.gemm(A, W, out, bias=b, res=R, gelu=kw.get("gelu", False),
-                                          round_out=kw.get("rnd", False), cluster=cl), iters=10)
-            res[cl] = 2.0 * M * N * K / ms / 1e9
-        emit(perf=name, tflops_pair=res[2], tflops_2sm=res[3])
-        del A, W, out, R
-    return ok
-
-
 def sec_gelu_ab():
     """A/B in one process: polynomial vs libdevice erf in the FC1 epilogue, interleaved repeats."""
     M, N, K = 403456, 3072, 768
@@ -233,7 +208,7 @@ def sec_conv():
 
 
 def sec_gemm_perf():
-    """ViT-B/16 linear shapes at the bench's M (2,048 frames x 197 tokens); default dispatch (cta_group::2)."""
+    """ViT-B/16 linear shapes at the bench's M (2,048 frames x 197 tokens); default dispatch."""
     M = 403456
     for (name, N, K, kw) in [
         ("qkv", 2304, 768, dict(bias=True, rnd=True)),
@@ -396,7 +371,7 @@ def sec_attn():
 
 
 def sec_attn_f16():
-    """All-fp16 tcgen05 attention (fp16 q | k | v^T in, fp16 ctx out) against fp64 softmax attention."""
+    """All-fp16 V^T attention (fp16 q | k | v^T in, fp16 ctx out) against fp64 softmax attention."""
     ok = True
     heads = 12
     for lens in [[197] * 5, [249] * 3, [7, 64, 65, 1, 130, 240], [7, 64, 65, 1, 130, 200, 128, 129, 3], [16] * 40]:
@@ -443,7 +418,7 @@ def sec_vit():
     return True
 
 
-SECTIONS = dict(attn_f16=sec_attn_f16, one=sec_one, gemm_f16=sec_gemm_f16, vit=sec_vit, gemm_x3=sec_gemm_x3, gemm_2sm=sec_gemm_2sm, gelu_ab=sec_gelu_ab, gemm=sec_gemm, conv=sec_conv, gemm_perf=sec_gemm_perf, ln=sec_ln, attn=sec_attn)
+SECTIONS = dict(attn_f16=sec_attn_f16, one=sec_one, gemm_f16=sec_gemm_f16, vit=sec_vit, gemm_x3=sec_gemm_x3, gelu_ab=sec_gelu_ab, gemm=sec_gemm, conv=sec_conv, gemm_perf=sec_gemm_perf, ln=sec_ln, attn=sec_attn)
 
 if __name__ == "__main__":
     os.makedirs("gpurun_out", exist_ok=True)

@@ -15,7 +15,7 @@ scheme's tensor-core instruction would (accumulation stays fp32, as on the devic
                convolutional feature encoder and the feature projection                                  (1 | 3 MMAs)
   f16-conv     the converse: 11-bit operands in conv1-6 only                                             (1 | 3 MMAs)
 
-Attention operands (q, k, v, p) are rounded to 11 bits in every scheme except fp32, as the tcgen05 attention kernels do.
+Attention operands (q, k, v, p) are rounded to 11 bits in every scheme except fp32, as the tensor-core attention kernels do.
 Metric: the test metric of tests/ (max |feature - fp32 feature| / max |fp32 feature| on the UTTERANCE readout).
 Writes profiles/r2_precision_table.json.  CPU only; ~2 minutes."""
 import json

@@ -1,5 +1,5 @@
 """Small launches of every hand-synchronised kernel family, for compute-sanitizer (scripts/sanitize.sh):
-the tcgen05 GEMM in its three operand modes and both tile widths, both tcgen05 attention kernels (all softmax versions)
+the wgmma GEMM in its three operand modes and both tile widths, both V^T attention kernels
 on ragged batches, LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
 fused fusion step (cluster kernel with DSMEM exchange + weight-gradient kernel).  Sizes are tiny: racecheck is slow."""
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """SASS-level diff of the kernels in mertools_b200/csrc/*.cu between a git revision and the working tree (no GPU
-needed: nvcc cross-compiles sm_100a cubins, cuobjdump lists them).  Used at the end of round 1 to show that the default
+needed: nvcc cross-compiles sm_90a cubins, cuobjdump lists them).  Used at the end of round 1 to show that the default
 kernels were untouched by the work done after the last GPU run:
 
     python scripts/sass_diff.py a914b7b attention_f16 attention_tc hubert_frontend helpers rowwise gemm
@@ -16,7 +16,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SCRATCH = os.path.join(ROOT, "gpurun_out", "sasscmp")
-NVCC = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "--expt-relaxed-constexpr", "-DMER_BUILD=1"]
+NVCC = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr", "-DMER_BUILD=1"]
 
 
 def kernels(cubin):

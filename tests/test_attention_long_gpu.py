@@ -1,4 +1,4 @@
-"""GPU parity of attention_f16_long.cu: the tcgen05 kernel for sequences of 250 .. 505 tokens (audio rows of up to
+"""GPU parity of the fp16 V^T attention kernel (attention_f16.cu) on sequences of 250 .. 505 tokens (audio rows of up to
 10 s = 499 HuBERT frames, extract_audio_huggingface.py:40-50; CLIP L/14's 257 tokens).
 
 Kernel level: ragged batches against a float64 softmax(Q K^T / 8) V of the same fp16 operand values (HF eager

@@ -6,9 +6,8 @@ test_parity_at_the_benchmarked_configuration builds exactly what bench.py times 
 (VitEncoder.clip_features on 256 x 8 frames, HubertEncoder.forward on 256 x 80,000 samples,
 BertEncoder.forward_packed on 256 x 32 ids) plus TriModalPipeline.step_host.  Eight sampled clips per modality are
 compared with the oracle (1e-3 relative, north_star), the fusion loss of the step with the oracle trainer on the
-device-extracted features, and the GEMM instantiations the bench runs on (gemm_kernel<256, F16, pair, cta_group::2>
-for the ViT / HuBERT / BERT layers, gemm_kernel<256, BF16X3, pair, cta_group::2> for the HuBERT conv stack) are
-asserted to have launched.
+device-extracted features, and the GEMM instantiations the bench runs on (gemm_kernel<256, F16> for the ViT / HuBERT /
+BERT layers, gemm_kernel<256, BF16X3> for the HuBERT conv stack) are asserted to have launched.
 """
 import ctypes as C
 
@@ -42,16 +41,16 @@ def test_parity_at_the_benchmarked_configuration(cuda):
     vit, hub, bert, fus = models = bench.build_models(cuda)
     host_in = bench.make_inputs(0, clips)
     frames, wave, ids, emo, val = dev_in = [x.to(cuda) for x in host_in]
-    n_f16, n_x3 = variant(256, 2, 2, 1), variant(256, 1, 2, 1)
+    n_f16, n_x3 = variant(256, 2, 1, 0), variant(256, 1, 1, 0)
     vfeat = vit.clip_features(frames, bench.FRAMES).clone()
-    assert variant(256, 2, 2, 1) - n_f16 >= 48, "the ViT linears did not run on gemm_kernel<256, F16, 2, 2SM>"
-    n_f16 = variant(256, 2, 2, 1)
+    assert variant(256, 2, 1, 0) - n_f16 >= 48, "the ViT linears did not run on gemm_kernel<256, F16>"
+    n_f16 = variant(256, 2, 1, 0)
     afeat = hub.forward(wave, normalize=True)[0].clone()
     tfeat = bert.forward_packed(ids, bench.TOKENS)[0].clone()
     assert hub.stack_precision == "f16" and hub.conv_precision == "f16" and bert.precision == "f16"
     # conv3..6 + the feature projection on split operands; conv1 / conv2 and the 12 layers on fp16 operands
-    assert variant(256, 1, 2, 1) - n_x3 >= 5, "HuBERT conv3..6 / projection did not run on gemm_kernel<256, BF16X3, 2, 2SM>"
-    assert variant(256, 2, 2, 1) - n_f16 >= 50, "HuBERT conv1 / conv2 / layers did not run on gemm_kernel<256, F16, 2, 2SM>"
+    assert variant(256, 1, 1, 0) - n_x3 >= 5, "HuBERT conv3..6 / projection did not run on gemm_kernel<256, BF16X3>"
+    assert variant(256, 2, 1, 0) - n_f16 >= 50, "HuBERT conv1 / conv2 / layers did not run on gemm_kernel<256, F16>"
     torch.cuda.synchronize()
     assert vfeat.shape == afeat.shape == tfeat.shape == (clips, 768)
     for t in (vfeat, afeat, tfeat):

@@ -1,7 +1,6 @@
 """GPU parity of the kernel variants and of the wider extractor families (SURVEY.md §8f rows N2-N4).
 
-First run on a B200 at the start of round 2 (all 33 green, `profiles/r2_ab_switches.json`), since then part of the
-always-on `-m gpu` suite.  Kernel level: the two tcgen05 attention kernels on their own (fp16 operands: ViT; TF32
+Part of the always-on `-m gpu` suite.  Kernel level: the two V^T attention kernels on their own (fp16 operands: ViT; TF32
 operands: HuBERT / BERT) on ragged batches in every softmax version (MER_ATT_F16_VER 1 .. 4, 6, 7 = default,
 MER_ATT_TC_VER 1 | 2 = default) against a float64 softmax(Q K^T / 8) V of the same operand values (HF eager
 attention, modeling_vit.py:171-196); packed GELU / conv0 forms against the scalar ones.  Extractor level: ragged
@@ -174,7 +173,7 @@ def test_gemm_packed_gelu_epilogue(cuda):
 
 
 def test_vggish_embeddings_match_oracle(cuda):
-    """VGGish network (vggish_slim.py:37-100) on split-bf16 tcgen05 GEMMs against the fp32 restatement."""
+    """VGGish network (vggish_slim.py:37-100) on split-bf16 wgmma GEMMs against the fp32 restatement."""
     import numpy as np
 
     from mertools_b200 import synthetic as S

@@ -66,7 +66,7 @@ def test_vit_batch_invariance(cuda):
     enc = VitEncoder(sd, device=cuda)
     a = enc.frame_features(frames).clone()
     b = torch.cat([enc.frame_features(frames[:2]).clone(), enc.frame_features(frames[2:]).clone()])
-    # not bit-identical: the tcgen05 attention aligns each sequence's key axis to a 16-byte boundary of
+    # not bit-identical: the V^T attention aligns each sequence's key axis to a 16-byte boundary of
     # the packed token buffer, so the fp32 summation order depends on where a frame sits in the batch;
     # a 1e-7 difference that crosses a tf32 rounding boundary of a GEMM operand becomes 5e-4 on that
     # element, hence ~1e-5 on the output
