@@ -48,6 +48,10 @@ int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_l
                              int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
                             int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
+// attention_short.cu: the fp16 V^T operands of rows of <= 249 tokens, one CTA per (sequence, head)
+bool mer_attention_short_enabled(int max_seqlen);  // max_seqlen <= 249 and MER_ATT_SHORT is not 0
+int mer_attention_short_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
+                               int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 
 // helpers.cu
 int mer_vit_patchify_launch(const uint8_t* frames_bgr, int n_frames, float* a_patches,

@@ -38,13 +38,11 @@ except Exception as e:  # noqa: BLE001
 PY
 }
 run default MER_NOP=1
-run att_f16_v2 MER_ATT_F16_VER=2
-run att_f16_v3 MER_ATT_F16_VER=3
-run att_tc_v2 MER_ATT_TC_VER=2
+run att_short_off MER_ATT_SHORT=0
+run att_short_all MER_ATT_SHORT=1
 run gelu_packed MER_GELU_PACKED=1
 run conv0_packed MER_CONV0_PACKED=1
-run all_v2 MER_ATT_F16_VER=2 MER_ATT_TC_VER=2 MER_GELU_PACKED=1 MER_CONV0_PACKED=1
-run all_v3 MER_ATT_F16_VER=3 MER_ATT_TC_VER=2 MER_GELU_PACKED=1 MER_CONV0_PACKED=1
+run all_on MER_ATT_SHORT=1 MER_GELU_PACKED=1 MER_CONV0_PACKED=1
 run default_again MER_NOP=1
 # mixed-length audio: one pass per clip (default) against ragged batches
 python scripts/bench_ragged_audio.py --clips 128 > "$out/ab_ragged_audio.jsonl" 2> "$out/ab_ragged_audio.err"
