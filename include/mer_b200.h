@@ -503,6 +503,33 @@ MER_API int mer_videomae_patchify(const uint8_t* frames_bgr, int n_clips, const 
  * = weights_in(x); out [rows, hidden] = silu(in[:, :hidden]) * in[:, hidden:], TF32-rounded when round_tf32_out. */
 MER_API int mer_swiglu(const float* in, float* out, long long rows, int hidden, int round_tf32_out, void* stream);
 
+/* ---- LLaMA decoder layers (LlamaModel of the text extractor's LLM branch, extract_text_huggingface.py:170-196): the
+ * pieces the GEMM does not cover; the layers are orchestrated from the host over these and mer_gemm
+ * (mertools_b200/extract/llama_text.py).  Head dim 128, no grouped-query attention. ---- */
+/* SwiGLU of HF LlamaMLP: in fp32 [rows, 2 * hidden] = the fused gate | up GEMM output; out16 fp16 [rows, hidden] =
+ * silu(in[:, :hidden]) * in[:, hidden:], the MER_GEMM_F16 operand of down_proj. */
+MER_API int mer_swiglu_f16(const float* in, void* out16, long long rows, int hidden, void* stream);
+/* HF LlamaRMSNorm over fp32 rows x [rows, dim] (dim % 256 == 0, <= 8192): y = w * (x * rsqrt(mean(x^2) + eps)) with
+ * mean(x^2) in fp32.  y16 (optional): fp16 [rows, dim], the operand of the next GEMM.  acc (optional): fp32 [rows, dim]
+ * accumulator, acc += y (the final `norm` term of the last-four readout).  At least one of them. */
+MER_API int mer_rmsnorm(const float* x, const float* w, void* y16, float* acc, long long rows, int dim, float eps,
+                        void* stream);
+/* Rotate-half rotary embedding (HF apply_rotary_pos_emb), in place on the q | k columns [0, 2 * heads * 128) of fp16
+ * rows qkv16 [tokens, ld]: for every head and j < 64, (x_j, x_j+64) -> (x_j c - x_j+64 s, x_j+64 c + x_j s), c / s =
+ * cos_t / sin_t [max_pos, 64] fp32 at the token's position, computed in fp32 and rounded once.  Positions: positions
+ * (device int32 [tokens]) when given, else the index inside the packed sequence (cu_seqlens, device [n_seq + 1]).
+ * A position outside [0, max_pos) turns the token's q | k into NaN. */
+MER_API int mer_rope_f16(void* qkv16, long long ld, long long tokens, int heads, const int32_t* cu_seqlens, int n_seq,
+                         const int32_t* positions, const float* cos_t, const float* sin_t, int max_pos, void* stream);
+/* Causal softmax(Q K^T / sqrt(128)) V per (sequence, head), head_dim 128 (HF LlamaAttention).  qkv16: fp16 [tokens,
+ * 3 * heads * 128] with Q | K column blocks (V columns not read), sequences packed back to back, cu_seqlens [n_seq + 1]
+ * (device int32); vt16: fp16 V^T [heads * 128, vt_ld] (vt_ld >= tokens, multiple of 8) as written by mer_gemm's
+ * transposed side output; ctx16: fp16 [tokens, heads * 128].  Query i of a sequence attends to its keys 0 .. i; no
+ * length cap (max_seqlen sizes the grid).  fp16 P, fp32 softmax statistics: attention_causal.cu. */
+MER_API int mer_causal_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
+                                     const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
+                                     void* stream);
+
 /* ---- Whisper branch of the audio extractor (extract_audio_huggingface.py:83-91): the two kernels the shared GEMM /
  * LayerNorm / attention entry points do not cover; the encoder / decoder are orchestrated from the host over those
  * (mertools_b200/extract/whisper.py). ---- */

@@ -1,5 +1,6 @@
 """Lexical feature extraction — H100 mirror of
-MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa-base branch).
+MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; LLaMA-family decoders through
+extract/llama_text.py, saved as float16 like the reference's fp16 GPU run).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
 model_dir)`` (:139), ``find_start_end_pos`` (:90-114) and the save-dir naming (:148-157).  Token ids
@@ -44,11 +45,15 @@ def find_start_end_pos(tokenizer):
 
 class TextExtractor:
     def __init__(self, state_dict, tokenizer, device="cuda", ln_eps=1e-12, position_offset=0,
-                 max_tokens_per_launch=16384):
-        self.enc = BertEncoder(state_dict, device=device, ln_eps=ln_eps, position_offset=position_offset)
+                 max_tokens_per_launch=16384, encoder=None, out_dtype=None):
+        """encoder: an already built encoder with the BertEncoder ``forward`` contract (the LLaMA branch) instead of a
+        BertEncoder over state_dict; out_dtype: dtype of the saved features (None: as computed, fp32)."""
+        self.enc = encoder if encoder is not None else BertEncoder(state_dict, device=device, ln_eps=ln_eps,
+                                                                   position_offset=position_offset)
         self.tokenizer = tokenizer
         self.start, self.end = find_start_end_pos(tokenizer)
         self.max_tokens = max_tokens_per_launch
+        self.out_dtype = out_dtype
 
     def tokenize(self, sentence):
         return self.tokenizer(sentence, return_tensors="pt")["input_ids"][0].tolist()
@@ -72,6 +77,9 @@ class TextExtractor:
                                          want_tokens=(feature_level == "FRAME"))
             utt = utt.cpu().numpy()
             toks = toks.cpu().numpy() if toks is not None else None
+            if self.out_dtype is not None:
+                utt = utt.astype(self.out_dtype)
+                toks = toks.astype(self.out_dtype) if toks is not None else None
             o = 0
             for j in range(b, e):
                 n = len(ids[j])
@@ -82,6 +90,22 @@ class TextExtractor:
             b = e
         return [common.save_feature(save_files[i] if save_files is not None else None, r,
                                     feature_level, self.enc.hidden) for i, r in enumerate(res)]
+
+
+def _llama_extractor(model_name, model_dir, cfg, device):
+    """The reference's LLM branch (:170-175, 193-196): LlamaModel + AutoTokenizer(use_fast=False), fp16 features.
+    Tokens per launch: what half of the device memory left after the weights holds at the model's activation size."""
+    import torch
+    from transformers import AutoTokenizer
+
+    from .llama_text import LlamaTextEncoder, check_llama_config, load_llama_weights
+    check_llama_config(cfg)  # before any weight is read
+    tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
+    enc = LlamaTextEncoder(load_llama_weights(model_dir, device, prefer_bin=(model_name == "Llama-2-13b-hf")), cfg,
+                           device=device)
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    tokens = int(min(16384, max(cfg.max_position_embeddings, free // 2 // enc.bytes_per_token)))
+    return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
 
 
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
@@ -109,13 +133,16 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     from .. import shard
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta", "xlm-roberta"), \
-        f"only BERT/RoBERTa-base encoders are on the H100 path, got {cfg.model_type}"
-    tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
-    roberta = cfg.model_type != "bert"
-    ext = TextExtractor(common.load_hf_state_dict(model_dir), tokenizer, device=f"cuda:{gpu}",
-                        ln_eps=cfg.layer_norm_eps,
-                        position_offset=(cfg.pad_token_id + 1) if roberta else 0)
+    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "llama"), \
+        f"only BERT/RoBERTa encoders and LLaMA decoders are on the H100 path, got {cfg.model_type}"
+    if cfg.model_type == "llama":
+        ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
+    else:
+        tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
+        roberta = cfg.model_type != "bert"
+        ext = TextExtractor(common.load_hf_state_dict(model_dir), tokenizer, device=f"cuda:{gpu}",
+                            ln_eps=cfg.layer_norm_eps,
+                            position_offset=(cfg.pad_token_id + 1) if roberta else 0)
     df = pd.read_csv(trans_dir)
     col = "chinese" if language == "chinese" else "english"
     by_name = dict(zip(df["name"], df[col]))

@@ -501,6 +501,29 @@ def bert_state_dict(vocab_size, seed=2, layers=12, scale=1.0, max_pos=None, type
     return g.sd
 
 
+LLAMA_SMALL_CFG = dict(vocab=4000, hidden=512, heads=4, ffn=1408, layers=6, max_pos=2048)
+
+
+def llama_state_dict(seed=21, vocab=4000, hidden=512, ffn=1408, layers=6, scale=1.0):
+    """Keys of ``transformers.LlamaModel`` (head_dim 128: hidden / 128 heads).  Every value is rounded to fp16 and
+    stored as fp32, like the fp16 checkpoints the LLaMA family ships: the fp16 device copy is then exact and the parity
+    bar measures the computation alone.  ``scale`` multiplies every layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    g.normal("embed_tokens.weight", (vocab, hidden), 0.5)
+    std = 0.03 * scale
+    for i in range(layers):
+        p = f"layers.{i}."
+        for n in ("q_proj", "k_proj", "v_proj", "o_proj"):
+            g.normal(p + f"self_attn.{n}.weight", (hidden, hidden), std)
+        g.normal(p + "mlp.gate_proj.weight", (ffn, hidden), std)
+        g.normal(p + "mlp.up_proj.weight", (ffn, hidden), std)
+        g.normal(p + "mlp.down_proj.weight", (hidden, ffn), std)
+        for n in ("input_layernorm", "post_attention_layernorm"):
+            g.sd[p + n + ".weight"] = (1.0 + 0.1 * g.rng.standard_normal(hidden)).astype(np.float32)
+    g.sd["norm.weight"] = (1.0 + 0.1 * g.rng.standard_normal(hidden)).astype(np.float32)
+    return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
+
+
 def fusion_state_dict(seed=3, audio_dim=768, text_dim=768, video_dim=768, hidden=128,
                       out1=6, out2=1, feat_type="utt"):
     """Keys of toolkit/models/attention.py:Attention, nn.Linear / nn.LSTM-style

@@ -1,6 +1,6 @@
 """Small launches of every hand-synchronised kernel family, for compute-sanitizer (scripts/sanitize.sh):
 the wgmma GEMM in its three operand modes and both tile widths, both V^T attention kernels
-on ragged batches, LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
+on ragged batches, the LLaMA kernels (causal head-dim-128 attention, RoPE, RMSNorm, SwiGLU), LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
 fused fusion step (cluster kernel with DSMEM exchange + weight-gradient kernel).  Sizes are tiny: racecheck is slow."""
 import os
 import sys
@@ -51,6 +51,39 @@ def attention():
     print("attention ok")
 
 
+def llama():
+    """The LLaMA kernels: causal head-dim-128 attention on ragged rows with unaligned starts, RoPE (both position
+    sources), RMSNorm in both output modes, the fp16 SwiGLU, then a 3-layer LlamaNet forward."""
+    from mertools_b200.extract import llama_text as LT
+    heads, lens = 2, [5, 70, 1, 129, 17]
+    tokens, D = sum(lens), heads * 128
+    qkv = torch.randn(tokens, 3 * D, device=dev).half()
+    vt = torch.zeros(D, (tokens + 7) // 8 * 8, dtype=torch.float16, device=dev)
+    vt[:, :tokens] = qkv[:, 2 * D:].T
+    cu = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int32, device=dev)
+    ops = LT.CudaOps(dev)
+    cos, sin = (t.to(dev) for t in LT.rope_tables(256, 10000.0))
+    b = ops.batch(lens)
+    L.check(ops._rope(L.ptr(qkv), 3 * D, tokens, heads, L.ptr(cu), len(lens), None, L.ptr(cos), L.ptr(sin), 256,
+                      L.stream_ptr()))
+    pos = torch.cat([torch.arange(n) for n in lens]).to(torch.int32).to(dev)
+    L.check(ops._rope(L.ptr(qkv), 3 * D, tokens, heads, None, 0, L.ptr(pos), L.ptr(cos), L.ptr(sin), 256, L.stream_ptr()))
+    ctx = torch.empty(tokens, D, dtype=torch.float16, device=dev)
+    L.check(ops._att(L.ptr(qkv), L.ptr(vt), vt.shape[1], L.ptr(ctx), L.ptr(cu), len(lens), tokens, max(lens), heads,
+                     L.stream_ptr()))
+    x = torch.randn(tokens, 512, device=dev)
+    w = torch.ones(512, device=dev)
+    ops.rmsnorm(x, w, 1e-6)
+    ops.rmsnorm(x, w, 1e-6, acc=torch.zeros_like(x))
+    L.check(ops._swiglu(L.ptr(torch.randn(tokens, 2 * 512, device=dev)), L.ptr(torch.empty(tokens, 512, dtype=torch.float16,
+                                                                                            device=dev)), tokens, 512,
+                        L.stream_ptr()))
+    sd = {k: torch.from_numpy(v) for k, v in S.llama_state_dict(seed=21, vocab=300, layers=3).items()}
+    LT.LlamaNet(sd, ops, 3, 4, 1e-6, 10000.0, 256).forward(np.arange(3, 3 + tokens) % 300, lens)
+    torch.cuda.synchronize()
+    print("llama ok")
+
+
 def encoders():
     from mertools_b200.encoders import BertEncoder, HubertEncoder, VitEncoder
     sd = S.hubert_state_dict(seed=1, layers=4)
@@ -77,6 +110,6 @@ def fusion():
 
 
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["gemms", "attention", "encoders", "fusion"]
+    which = sys.argv[1:] or ["gemms", "attention", "llama", "encoders", "fusion"]
     for w in which:
         globals()[w]()
