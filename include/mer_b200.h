@@ -55,7 +55,10 @@ enum { MER_EPI_GELU = 1, MER_EPI_ROUND_TF32 = 2, MER_EPI_SPLIT_BF16 = 4,
        MER_EPI_GELU_LIBM = 8, /* with MER_EPI_GELU: libdevice erff instead of the 12-op polynomial */
        MER_EPI_QUICK_GELU = 64, /* x * sigmoid(1.702 x) (CLIP's hidden_act) instead of GELU; excludes MER_EPI_GELU */
        MER_EPI_RELU = 128,    /* max(x, 0), applied AFTER the residual add when there is one (ResNet BasicBlock);
-                                 fp32 output only, excludes the GELU flags */
+                                 fp32 output, or fp16 output without a residual (OPT's fc1); excludes the GELU flags */
+       MER_EPI_GELU_TANH = 256, /* 0.5 x (1 + tanh(0.79788456 x (1 + 0.044715 x^2))) (BLOOM's bloom_gelu_forward),
+                                   |error| <= 1e-6; fp32 or fp16 output, optional bias; no residual / split / tf32 /
+                                   V^T, excludes the other activations */
        MER_EPI_OUT_F16 = 16,  /* out (and vt, if given) are IEEE fp16 arrays (round-to-nearest, saturating);
                                  ld_out / vt_ld in elements */
        MER_ATT_QKV_F16 = 32   /* mer_attention only: qkv and vt are fp16 arrays (needs vt, vt_ld % 8 == 0, max_seqlen <=
@@ -529,6 +532,22 @@ MER_API int mer_rope_f16(void* qkv16, long long ld, long long tokens, int heads,
 MER_API int mer_causal_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                                      const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
                                      void* stream);
+
+/* ---- pre-LayerNorm decoders with biases (BLOOM / OPT, extract_text_huggingface.py:170-196; orchestrated from the host
+ * in mertools_b200/extract/ln_decoder_text.py over these, mer_gemm (MER_EPI_GELU_TANH, MER_EPI_RELU | MER_EPI_OUT_F16)
+ * and mer_causal_attention_f16). ---- */
+/* mer_causal_attention_f16 with ALiBi (HF BloomAttention): scores q_i . k_j / sqrt(128) + slopes[h] * (j - i) in fp32,
+ * i and j counted from the sequence start; HF's slopes[h] * j differs by a per-row constant, which the softmax cancels.
+ * slopes: device fp32 [heads] (build_alibi_tensor's).  Same operands and limits otherwise. */
+MER_API int mer_causal_alibi_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
+                                           const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
+                                           int heads, const float* slopes, void* stream);
+/* HF nn.LayerNorm over fp32 rows x [rows, dim] (dim % 256 == 0, <= 8192): y = (x - mean) * rsqrt(var + eps) * gamma +
+ * beta, two-pass mean and biased variance in fp32.  Outputs, any non-empty subset: y16 fp16 [rows, dim] (the next GEMM's
+ * operand), y32 fp32 [rows, dim] (may not alias x), acc fp32 [rows, dim] with acc += y (the final-norm term of the
+ * last-four readout). */
+MER_API int mer_layernorm_f16(const float* x, const float* gamma, const float* beta, void* y16, float* y32, float* acc,
+                              long long rows, int dim, float eps, void* stream);
 
 /* ---- Whisper branch of the audio extractor (extract_audio_huggingface.py:83-91): the two kernels the shared GEMM /
  * LayerNorm / attention entry points do not cover; the encoder / decoder are orchestrated from the host over those

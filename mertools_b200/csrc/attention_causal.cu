@@ -14,6 +14,12 @@
 // issued longest-first.  The key axis begins at the sequence start rounded down to 8 tokens (16-byte copies), so the
 // up to 7 leading foreign keys are masked; keys beyond `tokens` are zero-filled, so that masked probabilities (exactly
 // 0) never meet V^T padding.  No length cap: the host bounds sequences by max_position_embeddings.
+//
+// ALiBi variant (template ALIBI = true; HF BloomAttention, mertools_b200/extract/ln_decoder_text.py): the score of query
+// i and key j of a sequence is q_i . k_j / sqrt(128) + slope_h * (j - i), formed in fp32 before the row maximum, with i
+// and j counted from the sequence start (not the packed position).  HF adds slope_h * j; the per-row constant
+// slope_h * i cancels in the softmax, and with (j - i) <= 0 the bias stays bounded however long the row is.  Masked and
+// foreign keys stay -inf.  ALIBI = false is the LLaMA kernel, unchanged.
 #include "mer_common.cuh"
 #include "mer_kernels.h"
 
@@ -48,9 +54,11 @@ __device__ __forceinline__ float fast_ex2(float x) {
   return y;
 }
 
+template <bool ALIBI>
 __global__ void __launch_bounds__(THREADS, 2)
 causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __restrict__ vt_, long long vt_ld,
-                        uint16_t* __restrict__ ctx, const int* __restrict__ cu_seqlens, long long tokens, int heads) {
+                        uint16_t* __restrict__ ctx, const int* __restrict__ cu_seqlens, long long tokens, int heads,
+                        const float* __restrict__ slopes) {
   extern __shared__ __align__(16) uint8_t smem_att[];
   uint16_t* Ks = reinterpret_cast<uint16_t*>(smem_att);  // [2][BKV][LDK]
   uint16_t* Vs = Ks + 2 * K_TILE;                         // [2][HD][LDV]: V^T, keys along the row
@@ -116,6 +124,9 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
 
   load_tile(0, 0);
   constexpr float SL2 = 0.08838834764831845f * 1.4426950408889634f;  // 1/sqrt(128) * log2(e)
+  // ALiBi bias in the units of the raw product q.k (the scale is folded into SL2): slope * sqrt(128) per key step, so
+  // that zero slopes leave s, and the output, bit-identical to the plain kernel
+  const float slope = ALIBI ? __ldg(slopes + h) * 11.313708498984761f : 0.f;
 
   for (int j = 0; j < n_kv; ++j) {
     const int buf = j & 1;
@@ -137,6 +148,16 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
         const uint32_t* w = reinterpret_cast<const uint32_t*>(kt + (nt * 8 + g) * LDK);
 #pragma unroll
         for (int ks = 0; ks < HD / 16; ++ks) mma_f16(s[nt], qa[ks], w[ks * 8 + t], w[ks * 8 + t + 4]);
+      }
+      if (ALIBI) {  // s / sqrt(128) = q.k / sqrt(128) + slope_h * (j - i)
+#pragma unroll
+        for (int nt = 0; nt < BKV / 8; ++nt) {
+          const int k0 = rel0 + nt * 8 + 2 * t;
+          s[nt][0] = fmaf(slope, (float)(k0 - row_lo), s[nt][0]);
+          s[nt][1] = fmaf(slope, (float)(k0 + 1 - row_lo), s[nt][1]);
+          s[nt][2] = fmaf(slope, (float)(k0 - row_hi), s[nt][2]);
+          s[nt][3] = fmaf(slope, (float)(k0 + 1 - row_hi), s[nt][3]);
+        }
       }
       // ---- mask foreign leading keys and keys after the row (diagonal / first tiles only) ----
       if (rel0 < 0 || rel0 + BKV - 1 > q0 + warp * 16) {
@@ -216,29 +237,44 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
   }
 }
 
+template <bool ALIBI>
+int launch_causal(const char* name, const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
+                  const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
+                  const float* slopes, cudaStream_t stream) {
+  MER_REQUIRE(qkv16 && vt16 && ctx16 && cu_seqlens, "%s: null operand", name);
+  MER_REQUIRE(vt_ld >= tokens && vt_ld % 8 == 0, "%s: V^T pitch %lld must be a multiple of 8 >= tokens", name, vt_ld);
+  MER_REQUIRE(max_seqlen > 0 && max_seqlen <= tokens, "%s: max_seqlen %d (1 .. tokens %lld)", name, max_seqlen, tokens);
+  MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq > 0 && n_seq <= 65535, "%s: bad grid (%d heads, %d seqs)", name,
+              heads, n_seq);
+  static MerPerDevice attr_set;
+  if (attr_set.needs_setup()) {
+    MER_CUDA_CHECK(cudaFuncSetAttribute(causal_attention_kernel<ALIBI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        SMEM));
+    attr_set.mark();
+  }
+  dim3 grid((max_seqlen + BQ - 1) / BQ, heads, n_seq);
+  causal_attention_kernel<ALIBI><<<grid, THREADS, SMEM, stream>>>(static_cast<const uint16_t*>(qkv16),
+                                                                  static_cast<const uint16_t*>(vt16), vt_ld,
+                                                                  static_cast<uint16_t*>(ctx16), cu_seqlens, tokens,
+                                                                  heads, slopes);
+  MER_CUDA_CHECK(cudaGetLastError());
+  mer_count_launches(1);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int mer_causal_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                                         const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
                                         int heads, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  MER_REQUIRE(qkv16 && vt16 && ctx16 && cu_seqlens, "mer_causal_attention_f16: null operand");
-  MER_REQUIRE(vt_ld >= tokens && vt_ld % 8 == 0, "mer_causal_attention_f16: V^T pitch %lld must be a multiple of 8 >= tokens",
-              vt_ld);
-  MER_REQUIRE(max_seqlen > 0 && max_seqlen <= tokens, "mer_causal_attention_f16: max_seqlen %d (1 .. tokens %lld)",
-              max_seqlen, tokens);
-  MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq > 0 && n_seq <= 65535,
-              "mer_causal_attention_f16: bad grid (%d heads, %d seqs)", heads, n_seq);
-  static MerPerDevice attr_set;
-  if (attr_set.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(causal_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attr_set.mark();
-  }
-  dim3 grid((max_seqlen + BQ - 1) / BQ, heads, n_seq);
-  causal_attention_kernel<<<grid, THREADS, SMEM, stream>>>(static_cast<const uint16_t*>(qkv16),
-                                                           static_cast<const uint16_t*>(vt16), vt_ld,
-                                                           static_cast<uint16_t*>(ctx16), cu_seqlens, tokens, heads);
-  MER_CUDA_CHECK(cudaGetLastError());
-  mer_count_launches(1);
-  return 0;
+  return launch_causal<false>("mer_causal_attention_f16", qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens,
+                              max_seqlen, heads, nullptr, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int mer_causal_alibi_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
+                                              const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
+                                              int heads, const float* slopes, void* stream_) {
+  MER_REQUIRE(slopes, "mer_causal_alibi_attention_f16: null slopes");
+  return launch_causal<true>("mer_causal_alibi_attention_f16", qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens,
+                             max_seqlen, heads, slopes, static_cast<cudaStream_t>(stream_));
 }

@@ -64,11 +64,25 @@ struct GemmCfg {
 // paired polynomial (GELU kind 5; fp16 and split-bf16 outputs, no residual).  Off by default.
 constexpr int EPI_GELU_PACKED = 1 << 16;
 
+// BLOOM's bloom_gelu_forward, 0.5 x (1 + tanh(u)) with u = 0.79788456 x (1 + 0.044715 x^2) (u formed in HF's order).
+// As x sigmoid(2u): with t = exp(-2|u|) and r = t / (1 + t) in [0, 1/2], the result is x - x r for x >= 0 and x r
+// below.  Only the small term x r carries the ex2 / rcp approximation error, so |error| stays within an ulp of the
+// result (<= 1e-6 on [-20, 20] against torch's fp32 tanh form); tanh.approx.f32 would not.
+__device__ __forceinline__ float gelu_tanh(float x) {
+  const float u = (0.79788456f * x) * (1.0f + (0.044715f * x) * x);
+  float t, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(-2.8853900817779268f * fabsf(u)));  // exp(-2|u|)
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + t));
+  r *= t;
+  return x >= 0.f ? fmaf(-x, r, x) : x * r;
+}
+
 template <int GELU>
 __device__ __forceinline__ float epi_act(float v) {
   if (GELU == 1) return gelu_erf_fast(v);
   if (GELU == 2) return gelu_erf(v);
   if (GELU == 3) return quick_gelu_fast(v);
+  if (GELU == 6) return gelu_tanh(v);
   return v;  // GELU == 4 (ReLU) is applied after the residual add
 }
 // two adjacent values at once (GELU == 5: the paired polynomial; otherwise the scalar form twice)
@@ -85,7 +99,8 @@ __device__ __forceinline__ void epi_act2(float a, float b, float& ga, float& gb)
 // Epilogue of one consumer warpgroup for its 64 x BLOCK_N share of a tile, straight from the wgmma accumulator
 // fragment: acc[h][4 j + 2 i + c] holds row 16 warp + g + 8 i, column 128 h + 8 j + 2 t + c (g = lane / 4,
 // t = lane % 4).  Each thread handles column pairs; one store instruction covers 8 rows x 32 contiguous bytes.
-// GELU: 0 none, 1 polynomial erf, 2 libdevice erff, 3 quick-GELU, 4 ReLU (after the residual), 5 paired erf.
+// GELU: 0 none, 1 polynomial erf, 2 libdevice erff, 3 quick-GELU, 4 ReLU (after the residual), 5 paired erf,
+// 6 tanh-GELU (BLOOM).
 // OUT: 0 fp32, 1 TF32-rounded fp32, 2 bf16 (hi|lo), 3 fp16.  RES: add the residual after the activation.
 // The transposed side output (V^T of the QKV GEMM) exists for GELU == 0 without residual: columns >= vt_col0 go
 // to vt[n - vt_col0, out_row] INSTEAD of out.
@@ -242,7 +257,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const int wg_row0 = (wg - 1) * 64;  // this warpgroup's rows of the tile
   const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(smem_a + wg_row0 * Cfg::kRowBytes));
   const uint64_t desc_b0 = wgmma_desc_sw128(smem_u32(smem_b));
-  const int gelu_kind = (ep.flags & MER_EPI_RELU) ? 4 : (ep.flags & MER_EPI_QUICK_GELU) ? 3
+  const int gelu_kind = (ep.flags & MER_EPI_GELU_TANH) ? 6 : (ep.flags & MER_EPI_RELU) ? 4
+                        : (ep.flags & MER_EPI_QUICK_GELU) ? 3
                         : (ep.flags & MER_EPI_GELU)
                             ? ((ep.flags & MER_EPI_GELU_LIBM) ? 2 : ((ep.flags & EPI_GELU_PACKED) ? 5 : 1)) : 0;
   const int out_kind = (ep.flags & MER_EPI_OUT_F16) ? 3 : (ep.flags & MER_EPI_SPLIT_BF16) ? 2 :
@@ -323,6 +339,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
         case 13: MER_EPI(3, 1, false); break;   // quick-GELU: the operand
         case 15: MER_EPI(3, 3, false); break;   // formats FC1 can feed
         case 16: MER_EPI(4, 0, false); break;   // relu(acc + bias)
+        case 19: MER_EPI(4, 3, false); break;   // the same as the fp16 operand of the next GEMM (OPT fc1)
+        case 24: MER_EPI(6, 0, false); break;   // tanh-GELU (BLOOM dense_h_to_4h)
+        case 27: MER_EPI(6, 3, false); break;
         case 22: MER_EPI(5, 2, false); break;   // paired erf-GELU (opt-in)
         case 23: MER_EPI(5, 3, false); break;
         default: MER_EPI(3, 0, false); break;
@@ -439,9 +458,13 @@ int mer_gemm_launch(const MerGemmDesc* g, cudaStream_t stream) {
                 ((g->ep.flags & (MER_EPI_GELU | MER_EPI_SPLIT_BF16)) || g->ep.res || g->ep.vt)),
               "mer_gemm: quick-GELU comes alone (fp32, tf32 or fp16 output; no residual / split / V^T)");
   MER_REQUIRE(!((g->ep.flags & MER_EPI_RELU) &&
-                ((g->ep.flags & (MER_EPI_GELU | MER_EPI_QUICK_GELU | MER_EPI_SPLIT_BF16 | MER_EPI_ROUND_TF32 |
-                                 MER_EPI_OUT_F16)) || g->ep.vt)),
-              "mer_gemm: ReLU goes with a plain fp32 output (optionally + residual)");
+                ((g->ep.flags & (MER_EPI_GELU | MER_EPI_QUICK_GELU | MER_EPI_SPLIT_BF16 | MER_EPI_ROUND_TF32)) ||
+                 g->ep.vt)),
+              "mer_gemm: ReLU goes with a plain fp32 output (optionally + residual) or an fp16 output");
+  MER_REQUIRE(!((g->ep.flags & MER_EPI_GELU_TANH) &&
+                ((g->ep.flags & (MER_EPI_GELU | MER_EPI_GELU_LIBM | MER_EPI_QUICK_GELU | MER_EPI_RELU |
+                                 MER_EPI_SPLIT_BF16 | MER_EPI_ROUND_TF32)) || g->ep.res || g->ep.vt)),
+              "mer_gemm: tanh-GELU comes alone (fp32 or fp16 output, optional bias; no residual / split / tf32 / V^T)");
   MER_REQUIRE(g->a_col_group == 0 || g->force_block_n == 128 || g->force_block_n == 256,
               "mer_gemm: a_col_group needs force_block_n (the weights are built for one block width)");
   MER_REQUIRE(!(g->ep.vt && (g->ep.flags & MER_EPI_GELU)), "mer_gemm: GELU + transposed side output is not supported");

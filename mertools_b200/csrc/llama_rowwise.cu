@@ -1,7 +1,8 @@
 // llama_rowwise.cu — the element- and row-wise kernels of a LLaMA decoder layer (HF modeling_llama.py) that the GEMM
 // and the causal attention kernel do not cover: RMSNorm over wide fp32 residual rows, the rotate-half rotary embedding
 // in place on the fp16 q | k columns of the QKV GEMM output, and the SwiGLU gate with an fp16 output.  Used by the
-// LLaMA text extractor (mertools_b200/extract/llama_text.py, reference extract_text_huggingface.py:170-196).
+// LLaMA text extractor (mertools_b200/extract/llama_text.py, reference extract_text_huggingface.py:170-196).  Also the
+// wide nn.LayerNorm (fp16 / fp32 / accumulate outputs) of the BLOOM / OPT decoders (extract/ln_decoder_text.py).
 #include <cuda_fp16.h>
 
 #include "mer_common.cuh"
@@ -55,6 +56,67 @@ rmsnorm_kernel(const float* __restrict__ x, const float* __restrict__ w, uint16_
       float4 s = *a;
       s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
       *a = s;
+    }
+  }
+}
+
+__device__ __forceinline__ float block_sum(float v, float* red) {  // red: RMS_THREADS / 32 floats, reusable after
+  v = warp_sum(v);
+  const int tid = threadIdx.x;
+  if ((tid & 31) == 0) red[tid >> 5] = v;
+  __syncthreads();
+  float tot = 0.f;
+#pragma unroll
+  for (int i = 0; i < RMS_THREADS / 32; ++i) tot += red[i];
+  return tot;
+}
+
+// nn.LayerNorm of the pre-LN decoders (BLOOM, OPT): y = (x - mean) * rsqrt(var + eps) * gamma + beta with the mean and
+// the biased variance as two passes over the row held in registers (x is read from HBM once).  One CTA per row.
+__global__ void __launch_bounds__(RMS_THREADS)
+layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     uint16_t* __restrict__ y16, float* __restrict__ y32, float* __restrict__ acc, int dim, float eps) {
+  __shared__ float red[2][RMS_THREADS / 32];
+  const long long row = blockIdx.x;
+  const int n4 = dim >> 2, tid = threadIdx.x;
+  const float4* xr = reinterpret_cast<const float4*>(x + row * dim);
+  float4 v[RMS_VEC];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < RMS_VEC; ++i) {
+    const int c = tid + i * RMS_THREADS;
+    v[i] = c < n4 ? __ldcs(xr + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+    s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+  }
+  const float mean = block_sum(s, red[0]) / (float)dim;
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < RMS_VEC; ++i) {
+    const int c = tid + i * RMS_THREADS;
+    if (c >= n4) break;
+    v[i].x -= mean; v[i].y -= mean; v[i].z -= mean; v[i].w -= mean;
+    ss = fmaf(v[i].x, v[i].x, ss);
+    ss = fmaf(v[i].y, v[i].y, ss);
+    ss = fmaf(v[i].z, v[i].z, ss);
+    ss = fmaf(v[i].w, v[i].w, ss);
+  }
+  const float r = rsqrtf(block_sum(ss, red[1]) / (float)dim + eps);
+  const float4* g4 = reinterpret_cast<const float4*>(gamma);
+  const float4* b4 = reinterpret_cast<const float4*>(beta);
+#pragma unroll
+  for (int i = 0; i < RMS_VEC; ++i) {
+    const int c = tid + i * RMS_THREADS;
+    if (c >= n4) break;
+    const float4 g = __ldg(g4 + c), b = __ldg(b4 + c);
+    const float4 o = make_float4(fmaf(v[i].x * r, g.x, b.x), fmaf(v[i].y * r, g.y, b.y), fmaf(v[i].z * r, g.z, b.z),
+                                 fmaf(v[i].w * r, g.w, b.w));
+    if (y16) *reinterpret_cast<uint2*>(y16 + row * dim + 4 * c) = make_uint2(pack_f16x2(o.x, o.y), pack_f16x2(o.z, o.w));
+    if (y32) reinterpret_cast<float4*>(y32 + row * dim)[c] = o;
+    if (acc) {
+      float4* a = reinterpret_cast<float4*>(acc + row * dim) + c;
+      float4 t = *a;
+      t.x += o.x; t.y += o.y; t.z += o.z; t.w += o.w;
+      *a = t;
     }
   }
 }
@@ -129,6 +191,21 @@ extern "C" int mer_rmsnorm(const float* x, const float* w, void* y16, float* acc
   MER_REQUIRE(dim > 0 && dim % 256 == 0 && dim <= RMS_MAX_DIM, "mer_rmsnorm: dim %d (a multiple of 256 up to %d)", dim,
               RMS_MAX_DIM);
   rmsnorm_kernel<<<(unsigned)rows, RMS_THREADS, 0, stream>>>(x, w, static_cast<uint16_t*>(y16), acc, dim, eps);
+  MER_CUDA_CHECK(cudaGetLastError());
+  mer_count_launches(1);
+  return 0;
+}
+
+extern "C" int mer_layernorm_f16(const float* x, const float* gamma, const float* beta, void* y16, float* y32, float* acc,
+                                 long long rows, int dim, float eps, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  MER_REQUIRE(x && gamma && beta && (y16 || y32 || acc) && rows > 0, "mer_layernorm_f16: bad arguments");
+  MER_REQUIRE(rows < (1ll << 31), "mer_layernorm_f16: %lld rows", rows);
+  MER_REQUIRE(dim > 0 && dim % 256 == 0 && dim <= RMS_MAX_DIM, "mer_layernorm_f16: dim %d (a multiple of 256 up to %d)",
+              dim, RMS_MAX_DIM);
+  MER_REQUIRE(y32 != x, "mer_layernorm_f16: y32 may not alias x");
+  layernorm_f16_kernel<<<(unsigned)rows, RMS_THREADS, 0, stream>>>(x, gamma, beta, static_cast<uint16_t*>(y16), y32, acc,
+                                                                   dim, eps);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
   return 0;

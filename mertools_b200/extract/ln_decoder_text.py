@@ -1,0 +1,395 @@
+"""BLOOM / OPT branch of the text extractor: the pre-LayerNorm decoder LLMs with biases among those the reference loads
+through plain ``AutoModel`` (MERBench/feature_extraction/text/extract_text_huggingface.py:170-172, ``bloom-7b1`` and
+``opt-13b``) and runs in fp16, one sentence per forward (:193-231).  Readout as for every text model:
+``torch.stack(hidden_states)[[-4, -3, -2, -1]].sum(0)``, where the last term is the output of the final LayerNorm
+(``ln_f`` / ``final_layer_norm``) and the other three are raw residual states.
+
+Both families are one orchestration (``LnDecoderNet``) over an ``ops`` backend, as in llama_text.py:
+- BLOOM: h[0] = word_embeddings_layernorm(E[ids]); causal attention with ALiBi (``mer_causal_alibi_attention_f16``),
+  slopes from ``alibi_slopes``; tanh-GELU MLP (``MER_EPI_GELU_TANH``).  The fused ``query_key_value`` rows, interleaved
+  per head as [head][q, k, v][128], are de-interleaved into q | k | v blocks at load time.
+- OPT: h[0] = E[ids] + P[pos + 2] (learned positions, offset 2); plain causal attention (``mer_causal_attention_f16``);
+  ReLU MLP (``MER_EPI_RELU | MER_EPI_OUT_F16``).
+``CudaOps``: fp16 weights and GEMM operands, fp32 biases, residual stream and readout, ``mer_layernorm_f16``.
+``TorchOps``: plain torch in HF's order of operations (CPU tests, tests/test_ln_decoder_text.py).
+"""
+from __future__ import annotations
+
+import math
+
+import numpy as np
+import torch
+
+from .llama_text import HEAD_DIM, _checkpoint_files, _iter_tensors
+
+OPT_POS_OFFSET = 2  # OPTLearnedPositionalEmbedding: position p reads row p + 2
+
+
+# ---- configs --------------------------------------------------------------------------------------------------------
+def _head_check(family, heads, hidden):
+    if heads * HEAD_DIM != hidden:
+        raise ValueError(f"{family} path: head_dim {hidden // heads} with {heads} heads and hidden {hidden} "
+                         f"(head_dim 128 only)")
+
+
+def check_ln_decoder_config(cfg):
+    """Reject, before any weight is read, every BLOOM / OPT config this path does not compute exactly."""
+    if cfg.model_type == "bloom":
+        if getattr(cfg, "apply_residual_connection_post_layernorm", False):
+            raise ValueError("BLOOM path: apply_residual_connection_post_layernorm is not supported")
+        if getattr(cfg, "slow_but_exact", False) and getattr(cfg, "pretraining_tp", 1) > 1:
+            raise ValueError("BLOOM path: slow_but_exact with pretraining_tp > 1 is not supported")
+        _head_check("BLOOM", cfg.num_attention_heads, cfg.hidden_size)
+    elif cfg.model_type == "opt":
+        if not getattr(cfg, "do_layer_norm_before", True):
+            raise ValueError("OPT path: do_layer_norm_before=False (post-LN OPT-350m) is not supported")
+        if getattr(cfg, "word_embed_proj_dim", cfg.hidden_size) != cfg.hidden_size:
+            raise ValueError(f"OPT path: word_embed_proj_dim {cfg.word_embed_proj_dim} != hidden_size "
+                             f"{cfg.hidden_size} (project_in / project_out) is not supported")
+        if not getattr(cfg, "enable_bias", True):
+            raise ValueError("OPT path: enable_bias=False is not supported")
+        if not getattr(cfg, "layer_norm_elementwise_affine", True):
+            raise ValueError("OPT path: a non-affine LayerNorm (layer_norm_elementwise_affine=False) is not supported")
+        if getattr(cfg, "_remove_final_layer_norm", False):
+            raise ValueError("OPT path: _remove_final_layer_norm is not supported")
+        if getattr(cfg, "activation_function", "relu") != "relu":
+            raise ValueError(f"OPT path: activation_function {cfg.activation_function!r} is not supported (relu only)")
+        _head_check("OPT", cfg.num_attention_heads, cfg.hidden_size)
+    else:
+        raise ValueError(f"not a BLOOM / OPT config: model_type {cfg.model_type!r}")
+
+
+def alibi_slopes(heads):
+    """fp32 [heads]: the per-head ALiBi slopes of HF build_alibi_tensor, bit for bit.  For a head count that is not a
+    power of two, the largest power of two below it gets the geometric sequence and the remaining heads take every
+    other term of the sequence for twice that count."""
+    p2 = 2 ** math.floor(math.log2(heads))
+    base = torch.tensor(2 ** (-(2 ** -(math.log2(p2) - 3))), dtype=torch.float32)
+    slopes = torch.pow(base, torch.arange(1, 1 + p2, dtype=torch.int32))
+    if p2 != heads:
+        extra = torch.tensor(2 ** (-(2 ** -(math.log2(2 * p2) - 3))), dtype=torch.float32)
+        n = min(p2, heads - p2)
+        slopes = torch.cat([slopes, torch.pow(extra, torch.arange(1, 1 + 2 * n, 2, dtype=torch.int32))])
+    return slopes
+
+
+# ---- streaming checkpoint loader ------------------------------------------------------------------------------------
+def _strip(k, family):
+    """Parameter name of BloomModel (``h.0...``) / of OPTModel.decoder (``layers.0...``), or None to drop."""
+    if k.startswith("lm_head."):
+        return None
+    for p in (("transformer.",) if family == "bloom" else ("model.", "decoder.")):
+        if k.startswith(p):
+            k = k[len(p):]
+    return k
+
+
+def load_ln_decoder_weights(model_dir, device, family):
+    """{name: fp16 tensor on ``device``} of a BLOOM (``family="bloom"``) or OPT (``"opt"``) checkpoint, read one
+    tensor at a time from safetensors or ``.bin`` shards (fp32 / fp16 / bf16).  Names lose the ``transformer.``
+    (BloomForCausalLM) or ``model.`` / ``decoder.`` (OPTForCausalLM / OPTModel) prefixes; ``lm_head`` is dropped.
+    A value that is not finite in fp16 is refused."""
+    out = {}
+    for path in _checkpoint_files(model_dir):
+        for k, v in _iter_tensors(path):
+            k = _strip(k, family)
+            if k is None:
+                continue
+            t = v.to(device).to(torch.float16)
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError(f"{path}: {k} is not finite in fp16")
+            out[k] = t
+    return out
+
+
+def deinterleave_qkv(t, heads):
+    """BLOOM query_key_value rows [head][q, k, v][128] (weight [3 D, D] or bias [3 D]) -> q | k | v blocks."""
+    shape = t.shape
+    return t.reshape(heads, 3, HEAD_DIM, *shape[1:]).transpose(0, 1).reshape(shape).contiguous()
+
+
+# ---- layer orchestration --------------------------------------------------------------------------------------------
+class LnDecoderNet:
+    """Backend-agnostic BloomModel / OPTModel.decoder forward over packed sentences.  ``sd``: {name: tensor} as
+    load_ln_decoder_weights names them; entries are popped as the backend takes them over.  ``family``: "bloom" or
+    "opt".  ``ops``: weight, vector, embedding, embed, batch, layernorm, attention, linear_res, mlp, zeros_like, add_."""
+
+    def __init__(self, sd, ops, family, n_layers, heads, eps, max_pos=None):
+        assert family in ("bloom", "opt") and n_layers >= 3, (family, n_layers)
+        self.ops, self.family, self.n_layers, self.heads, self.eps, self.max_pos = ops, family, n_layers, heads, eps, max_pos
+        self.layers = []
+        if family == "bloom":
+            self.embed = ops.embedding(sd.pop("word_embeddings.weight"))
+            self.emb_ln = (ops.vector(sd.pop("word_embeddings_layernorm.weight")),
+                           ops.vector(sd.pop("word_embeddings_layernorm.bias")))
+            self.pos = None
+            self.slopes = ops.vector(alibi_slopes(heads))
+            for i in range(n_layers):
+                p = f"h.{i}."
+                a, m = p + "self_attention.", p + "mlp."
+                self.layers.append(dict(
+                    ln1=(ops.vector(sd.pop(p + "input_layernorm.weight")), ops.vector(sd.pop(p + "input_layernorm.bias"))),
+                    qkv=ops.weight(deinterleave_qkv(sd.pop(a + "query_key_value.weight"), heads)),
+                    b_qkv=ops.vector(deinterleave_qkv(sd.pop(a + "query_key_value.bias"), heads)),
+                    o=ops.weight(sd.pop(a + "dense.weight")), b_o=ops.vector(sd.pop(a + "dense.bias")),
+                    ln2=(ops.vector(sd.pop(p + "post_attention_layernorm.weight")),
+                         ops.vector(sd.pop(p + "post_attention_layernorm.bias"))),
+                    up=ops.weight(sd.pop(m + "dense_h_to_4h.weight")), b_up=ops.vector(sd.pop(m + "dense_h_to_4h.bias")),
+                    down=ops.weight(sd.pop(m + "dense_4h_to_h.weight")),
+                    b_down=ops.vector(sd.pop(m + "dense_4h_to_h.bias"))))
+            self.ln_f = (ops.vector(sd.pop("ln_f.weight")), ops.vector(sd.pop("ln_f.bias")))
+            self.act = "gelu_tanh"
+        else:
+            self.embed = ops.embedding(sd.pop("embed_tokens.weight"))
+            self.emb_ln = None
+            self.pos = ops.embedding(sd.pop("embed_positions.weight"))
+            self.slopes = None
+            for i in range(n_layers):
+                p = f"layers.{i}."
+                a = p + "self_attn."
+                self.layers.append(dict(
+                    ln1=(ops.vector(sd.pop(p + "self_attn_layer_norm.weight")),
+                         ops.vector(sd.pop(p + "self_attn_layer_norm.bias"))),
+                    qkv=ops.weight(torch.cat([sd.pop(a + f"{n}_proj.weight") for n in "qkv"], 0)),
+                    b_qkv=ops.vector(torch.cat([sd.pop(a + f"{n}_proj.bias") for n in "qkv"], 0)),
+                    o=ops.weight(sd.pop(a + "out_proj.weight")), b_o=ops.vector(sd.pop(a + "out_proj.bias")),
+                    ln2=(ops.vector(sd.pop(p + "final_layer_norm.weight")), ops.vector(sd.pop(p + "final_layer_norm.bias"))),
+                    up=ops.weight(sd.pop(p + "fc1.weight")), b_up=ops.vector(sd.pop(p + "fc1.bias")),
+                    down=ops.weight(sd.pop(p + "fc2.weight")), b_down=ops.vector(sd.pop(p + "fc2.bias"))))
+            self.ln_f = (ops.vector(sd.pop("final_layer_norm.weight")), ops.vector(sd.pop("final_layer_norm.bias")))
+            self.act = "relu"
+        self.hidden = self.embed.shape[1]
+        assert not any(k.startswith(("h.", "layers.")) for k in sd), f"unused layer weights: {sorted(sd)[:4]}"
+
+    def forward(self, ids, lens, return_hidden=False):
+        """ids: int64 [tokens] of packed sentences with lengths ``lens``.  Returns the readout
+        h[L-3] + h[L-2] + h[L-1] + ln_f(h[L]) [tokens, hidden] (fp32 on the CUDA backend) and, with return_hidden, the HF
+        hidden_states tuple as a list."""
+        ops, n = self.ops, self.n_layers
+        if self.max_pos is not None and max(lens) > self.max_pos:
+            raise ValueError(f"a sentence of {max(lens)} tokens exceeds max_position_embeddings {self.max_pos}")
+        b = ops.batch(lens)
+        if self.family == "bloom":
+            x = ops.layernorm(ops.embed(self.embed, ids), *self.emb_ln, self.eps, out="f32")
+        else:
+            pos = np.concatenate([np.arange(m) for m in lens]) + OPT_POS_OFFSET
+            x = ops.embed(self.embed, ids) + ops.embed(self.pos, pos)
+        hs = [x.clone()] if return_hidden else None
+        acc = ops.zeros_like(x)
+        for i, L in enumerate(self.layers):
+            if i == n - 3:            # h[0] (the embedding) when n == 3
+                ops.add_(acc, x)
+            y = ops.layernorm(x, *L["ln1"], self.eps)
+            ctx = ops.attention(y, L["qkv"], L["b_qkv"], b, self.heads, self.slopes)
+            x = ops.linear_res(ctx, L["o"], L["b_o"], x)
+            y = ops.layernorm(x, *L["ln2"], self.eps)
+            x = ops.linear_res(ops.mlp(y, L["up"], L["b_up"], self.act), L["down"], L["b_down"], x)
+            if n - 3 <= i < n - 1:
+                ops.add_(acc, x)
+            if return_hidden and i < n - 1:
+                hs.append(x.clone())
+        ops.layernorm(x, *self.ln_f, self.eps, acc=acc)
+        if return_hidden:
+            hs.append(ops.layernorm(x, *self.ln_f, self.eps, acc=ops.zeros_like(x)))
+        return (acc, hs) if return_hidden else acc
+
+
+class TorchOps:
+    """Plain torch backend (CPU tests, fp32 by default): the same orchestration on torch operators, HF's order of
+    operations (BloomAttention: baddbmm of alibi and q k^T / sqrt(128); OPTAttention: q scaled before the product)."""
+
+    def __init__(self, device="cpu", dtype=torch.float32):
+        self.device, self.dtype = torch.device(device), dtype
+
+    def weight(self, t):
+        return t.to(self.device, self.dtype)
+
+    vector = embedding = weight
+
+    def embed(self, table, ids):
+        return table[torch.as_tensor(ids, device=self.device)]
+
+    def zeros_like(self, x):
+        return torch.zeros_like(x)
+
+    def add_(self, acc, x):
+        acc += x
+
+    def batch(self, lens):
+        return list(lens)
+
+    def layernorm(self, x, g, b, eps, out="f16", acc=None):
+        y = torch.nn.functional.layer_norm(x, (x.shape[-1],), g, b, eps)
+        if acc is not None:
+            acc += y
+            return acc
+        return y
+
+    def attention(self, y, w_qkv, b_qkv, lens, heads, slopes):
+        D = heads * HEAD_DIM
+        qkv = y @ w_qkv.T + b_qkv
+        ctx = torch.empty(y.shape[0], D, dtype=y.dtype, device=y.device)
+        o = 0
+        for n in lens:
+            q, k, v = (qkv[o:o + n, i * D:(i + 1) * D].view(n, heads, HEAD_DIM).transpose(0, 1) for i in range(3))
+            if slopes is not None:   # BLOOM: alibi.baddbmm(q, k^T, beta=1, alpha=1/sqrt(128)), alibi = slope * j
+                alibi = slopes[:, None, None] * torch.arange(n, device=y.device, dtype=slopes.dtype)[None, None, :]
+                sc = alibi.to(y.dtype) + (q @ k.transpose(1, 2)) * HEAD_DIM ** -0.5
+            else:                    # OPT: (q * 1/sqrt(128)) k^T
+                sc = (q * HEAD_DIM ** -0.5) @ k.transpose(1, 2)
+            sc = sc.masked_fill(torch.ones(n, n, dtype=torch.bool, device=y.device).triu(1), float("-inf"))
+            p = torch.softmax(sc.to(torch.promote_types(sc.dtype, torch.float32)), dim=-1).to(y.dtype)
+            ctx[o:o + n] = (p @ v).transpose(0, 1).reshape(n, D)
+            o += n
+        return ctx
+
+    def linear_res(self, a, w, b, x):
+        return x + (a @ w.T + b)
+
+    def mlp(self, y, w, b, act):
+        h = y @ w.T + b
+        if act == "relu":
+            return torch.relu(h)
+        return h * 0.5 * (1.0 + torch.tanh(0.79788456 * h * (1 + 0.044715 * h * h)))
+
+
+class CudaOps:
+    """Product backend: fp16 weights and GEMM operands (MER_GEMM_F16) with fp32 biases, fp32 residual stream; every op
+    is one or two libmer_b200.so launches.  ``timing``: as llama_text.CudaOps (kernel class, start, end events)."""
+
+    def __init__(self, device="cuda"):
+        import ctypes as C
+
+        from .. import _lib as L
+        L.check(L.lib().mer_check_device())
+        self.L, self.device, self.timing = L, torch.device(device), None
+        vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_longlong, C.c_float
+        self._ln = L.declare("mer_layernorm_f16", [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp])
+        self._att = L.declare("mer_causal_attention_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, vp])
+        self._att_alibi = L.declare("mer_causal_alibi_attention_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, vp, vp])
+
+    def _run(self, klass, fn):
+        if self.timing is None:
+            return fn()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        r = fn()
+        b.record()
+        self.timing.append((klass, a, b))
+        return r
+
+    def weight(self, t):
+        return t.to(self.device, torch.float16).contiguous()
+
+    embedding = weight
+
+    def vector(self, t):
+        return t.to(self.device, torch.float32).contiguous()
+
+    def embed(self, table, ids):
+        return table[torch.as_tensor(ids, device=self.device)].float()
+
+    def zeros_like(self, x):
+        return torch.zeros_like(x)
+
+    def add_(self, acc, x):
+        acc += x
+
+    def batch(self, lens):
+        cu = np.zeros(len(lens) + 1, np.int32)
+        cu[1:] = np.cumsum(lens)
+        return dict(cu=torch.from_numpy(cu).to(self.device), n=len(lens), max_len=int(max(lens)))
+
+    def layernorm(self, x, g, b, eps, out="f16", acc=None):
+        """out "f16": a new fp16 operand; "f32": a new fp32 row block; with acc: acc += y, returns acc."""
+        L = self.L
+        y16 = y32 = None
+        if acc is None:
+            if out == "f16":
+                y16 = torch.empty(x.shape, dtype=torch.float16, device=self.device)
+            else:
+                y32 = torch.empty(x.shape, dtype=torch.float32, device=self.device)
+        self._run("layernorm", lambda: L.check(self._ln(L.ptr(x), L.ptr(g), L.ptr(b), L.ptr(y16), L.ptr(y32), L.ptr(acc),
+                                                        x.shape[0], x.shape[1], eps, L.stream_ptr())))
+        return acc if acc is not None else (y16 if y16 is not None else y32)
+
+    def attention(self, y, w_qkv, b_qkv, b, heads, slopes):
+        L, T, D = self.L, y.shape[0], heads * HEAD_DIM
+        qkv = torch.empty(T, 3 * D, dtype=torch.float16, device=self.device)     # q | k rows (V columns unused)
+        vt = torch.empty(D, (T + 7) // 8 * 8, dtype=torch.float16, device=self.device)
+        self._run("gemm", lambda: L.gemm(y, w_qkv, qkv, bias=b_qkv, mode=L.MER_GEMM_F16, f16_out=True, vt=vt,
+                                         vt_col0=2 * D))
+        ctx = torch.empty(T, D, dtype=torch.float16, device=self.device)
+        args = (L.ptr(qkv), L.ptr(vt), vt.shape[1], L.ptr(ctx), L.ptr(b["cu"]), b["n"], T, b["max_len"], heads)
+        if slopes is not None:
+            self._run("attention", lambda: L.check(self._att_alibi(*args, L.ptr(slopes), L.stream_ptr())))
+        else:  # OPT scales q by 1/sqrt(128) before q k^T; the kernel scales the product: a rounding difference only
+            self._run("attention", lambda: L.check(self._att(*args, L.stream_ptr())))
+        return ctx
+
+    def linear_res(self, a, w, bias, x):
+        self._run("gemm", lambda: self.L.gemm(a, w, x, bias=bias, res=x, mode=self.L.MER_GEMM_F16))
+        return x
+
+    def mlp(self, y, w, bias, act):
+        L, T = self.L, y.shape[0]
+        h = torch.empty(T, w.shape[0], dtype=torch.float16, device=self.device)
+        self._run("gemm", lambda: L.gemm(y, w, h, bias=bias, mode=L.MER_GEMM_F16, f16_out=True,
+                                         relu=(act == "relu"), gelu_tanh=(act == "gelu_tanh")))
+        return h
+
+
+def activation_bytes_per_token(hidden, ffn):
+    """Device bytes one token of a packed pass holds at the peak of a layer: fp32 residual, readout and embedding
+    gather, fp16 operands, q | k | v rows and V^T, ctx, and the fp16 FFN activation."""
+    return hidden * (4 + 4 + 4 + 2 + 3 * 2 + 2 + 2) + ffn * 2
+
+
+def net_dims(cfg):
+    """(family, layers, heads, hidden, ffn, eps, max_pos) of a BLOOM / OPT config."""
+    if cfg.model_type == "bloom":
+        return ("bloom", cfg.num_hidden_layers, cfg.num_attention_heads, cfg.hidden_size, 4 * cfg.hidden_size,
+                float(cfg.layer_norm_epsilon), None)
+    return ("opt", cfg.num_hidden_layers, cfg.num_attention_heads, cfg.hidden_size, cfg.ffn_dim, 1e-5,
+            int(cfg.max_position_embeddings))
+
+
+class LnDecoderTextEncoder:
+    """``forward(id_lists, start, end, want_tokens)`` (the contract TextExtractor drives) over ``LnDecoderNet`` with
+    the CUDA backend.  ``cfg``: the checkpoint's BloomConfig / OPTConfig; ``sd``: {name: tensor}
+    (load_ln_decoder_weights)."""
+
+    def __init__(self, sd, cfg, device="cuda"):
+        import ctypes as C
+
+        from .. import _lib as L
+        check_ln_decoder_config(cfg)
+        family, layers, heads, hidden, ffn, eps, self.max_pos = net_dims(cfg)
+        self.ops = CudaOps(device)
+        self.device = self.ops.device
+        self.net = LnDecoderNet(sd, self.ops, family, layers, heads, eps, self.max_pos)
+        self.hidden, self.vocab_size = self.net.hidden, self.net.embed.shape[0]
+        self.bytes_per_token = activation_bytes_per_token(hidden, ffn)
+        self._L = L
+        self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                     C.c_void_p, C.c_void_p])
+
+    def forward(self, id_lists, start=0, end=None, want_tokens=False):
+        """id_lists: non-empty token id sequences.  Returns (utt [n, hidden] = mean over each sentence's kept range
+        [start : len + end], tokens [sum len, hidden] | None), fp32."""
+        L = self._L
+        lens = [len(x) for x in id_lists]
+        assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
+        if self.max_pos is not None and max(lens) > self.max_pos:
+            raise ValueError(f"a sentence of {max(lens)} tokens exceeds max_position_embeddings {self.max_pos}")
+        ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
+        assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
+        acc = self.net.forward(ids, lens)
+        cu = np.zeros(len(lens) + 1, np.int64)
+        cu[1:] = np.cumsum(lens)
+        seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)
+        seg = torch.from_numpy(np.maximum(seg, seg[:1])).to(self.device)   # empty kept range -> zeros (caller skips it)
+        utt = torch.empty(len(lens), self.hidden, dtype=torch.float32, device=self.device)
+        L.check(self._seg(L.ptr(acc), L.ptr(seg[0]), L.ptr(seg[1]), len(lens), self.hidden, 1, L.ptr(utt),
+                          L.stream_ptr()))
+        return utt, (acc if want_tokens else None)

@@ -1,6 +1,7 @@
 """Lexical feature extraction — H100 mirror of
 MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; LLaMA-family decoders through
-extract/llama_text.py, saved as float16 like the reference's fp16 GPU run).
+extract/llama_text.py and BLOOM / OPT through extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU
+run).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
 model_dir)`` (:139), ``find_start_end_pos`` (:90-114) and the save-dir naming (:148-157).  Token ids
@@ -108,6 +109,21 @@ def _llama_extractor(model_name, model_dir, cfg, device):
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
 
 
+def _ln_decoder_extractor(model_dir, cfg, device):
+    """The same LLM branch for BLOOM / OPT (:170-172, 193-196): BloomModel / OPTModel + AutoTokenizer(use_fast=False),
+    fp16 features; tokens per launch as in _llama_extractor."""
+    import torch
+    from transformers import AutoTokenizer
+
+    from .ln_decoder_text import LnDecoderTextEncoder, check_ln_decoder_config, load_ln_decoder_weights
+    check_ln_decoder_config(cfg)  # before any weight is read
+    tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
+    enc = LnDecoderTextEncoder(load_ln_decoder_weights(model_dir, device, cfg.model_type), cfg, device=device)
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    tokens = int(min(16384, max(enc.max_pos or 2048, free // 2 // enc.bytes_per_token)))
+    return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
+
+
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
                       language="chinese", model_dir=None, config=None, sentences_per_launch=256):
     """Same signature, naming and outputs as the reference (:139-252)."""
@@ -133,10 +149,12 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     from .. import shard
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "llama"), \
-        f"only BERT/RoBERTa encoders and LLaMA decoders are on the H100 path, got {cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "llama", "bloom", "opt"), \
+        f"only BERT/RoBERTa encoders and LLaMA / BLOOM / OPT decoders are on the H100 path, got {cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
+    elif cfg.model_type in ("bloom", "opt"):
+        ext = _ln_decoder_extractor(model_dir, cfg, f"cuda:{gpu}")
     else:
         tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
         roberta = cfg.model_type != "bert"

@@ -524,6 +524,49 @@ def llama_state_dict(seed=21, vocab=4000, hidden=512, ffn=1408, layers=6, scale=
     return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
 
 
+LN_DECODER_SMALL_CFG = dict(vocab=4000, hidden=512, heads=4, ffn=2048, layers=6, max_pos=2048)
+
+
+def bloom_state_dict(seed=23, vocab=4000, hidden=512, layers=6, scale=1.0):
+    """Keys of ``transformers.BloomModel`` (head_dim 128: hidden / 128 heads, FFN 4 x hidden), fused
+    ``query_key_value`` in HF's per-head interleaved row order.  Values rounded to fp16 and stored as fp32 (as
+    llama_state_dict); ``scale`` multiplies every layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    g.normal("word_embeddings.weight", (vocab, hidden), 0.5)
+    g.ln("word_embeddings_layernorm", hidden)
+    std = 0.03 * scale
+    for i in range(layers):
+        p = f"h.{i}."
+        g.ln(p + "input_layernorm", hidden)
+        g.linear(p + "self_attention.query_key_value", 3 * hidden, hidden, std)
+        g.linear(p + "self_attention.dense", hidden, hidden, std)
+        g.ln(p + "post_attention_layernorm", hidden)
+        g.linear(p + "mlp.dense_h_to_4h", 4 * hidden, hidden, std)
+        g.linear(p + "mlp.dense_4h_to_h", hidden, 4 * hidden, std)
+    g.ln("ln_f", hidden)
+    return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
+
+
+def opt_state_dict(seed=25, vocab=4000, hidden=512, ffn=2048, layers=6, max_pos=2048, scale=1.0):
+    """Keys of ``transformers.OPTModel`` (``decoder.*``; position table of max_pos + 2 rows, pre-LN layers with biases,
+    head_dim 128).  Values rounded to fp16 and stored as fp32; ``scale`` multiplies every layer matrix."""
+    g = _Gen(seed)
+    d = "decoder."
+    g.normal(d + "embed_tokens.weight", (vocab, hidden), 0.5)
+    g.normal(d + "embed_positions.weight", (max_pos + 2, hidden), 0.1)
+    std = 0.03 * scale
+    for i in range(layers):
+        p = f"{d}layers.{i}."
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            g.linear(p + f"self_attn.{n}", hidden, hidden, std)
+        g.ln(p + "self_attn_layer_norm", hidden)
+        g.linear(p + "fc1", ffn, hidden, std)
+        g.linear(p + "fc2", hidden, ffn, std)
+        g.ln(p + "final_layer_norm", hidden)
+    g.ln(d + "final_layer_norm", hidden)
+    return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
+
+
 def fusion_state_dict(seed=3, audio_dim=768, text_dim=768, video_dim=768, hidden=128,
                       out1=6, out2=1, feat_type="utt"):
     """Keys of toolkit/models/attention.py:Attention, nn.Linear / nn.LSTM-style

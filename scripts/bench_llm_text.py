@@ -1,4 +1,5 @@
-"""Throughput of the LLaMA text-feature path at 7 B and 13 B shapes against the reference's loop.
+"""Throughput of the decoder-LLM text-feature paths (LLaMA at 7 B and 13 B shapes; BLOOM-7B1 and OPT-13B on request)
+against the reference's loop.
 
 Packed path: LlamaNet on the CUDA backend (fp16 weights and operands, fp32 residual), sentences packed back to back,
 up to --tokens per pass.  Reference loop (extract_text_huggingface.py:193-231): batch 1, one sentence per forward, fp16,
@@ -6,9 +7,11 @@ output_hidden_states and the last-four sum; HF LlamaModel when transformers impo
 (LlamaNet + TorchOps) in fp16 on the GPU — the output says which ran.  Weights are seeded random fp16 tensors generated
 on the device (no checkpoint on disk); sentence lengths are seeded draws shaped like the MER2023 transcripts under a
 Chinese sentencepiece tokenizer (mean ~20 tokens, p99 ~53, capped at 128).  The time shares of GEMM / attention /
-RMSNorm / RoPE / SwiGLU come from CUDA events around every launch, in a separate pass.
+RMSNorm / RoPE / SwiGLU (LayerNorm for BLOOM / OPT) come from CUDA events around every launch, in a separate pass.
+``bloom-7b1`` / ``opt-13b`` run LnDecoderNet (extract/ln_decoder_text.py) against HF BloomModel / OPTModel in fp16 at
+batch 1 (a 32000-token vocabulary here: the embedding gather is not part of the timed work that matters).
 
-    python scripts/bench_llm_text.py [--shapes 7b,13b] [--sentences 1024] [--ref-sentences 64] [--steps 3]
+    python scripts/bench_llm_text.py [--shapes 7b,13b,bloom-7b1,opt-13b] [--sentences 1024] [--ref-sentences 64]
 """
 import argparse
 import json
@@ -22,9 +25,12 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from mertools_b200.extract import llama_text as LT  # noqa: E402
+from mertools_b200.extract import ln_decoder_text as LD  # noqa: E402
 
 SHAPES = {"7b": dict(hidden=4096, heads=32, ffn=11008, layers=32, eps=1e-6),
-          "13b": dict(hidden=5120, heads=40, ffn=13824, layers=40, eps=1e-5)}
+          "13b": dict(hidden=5120, heads=40, ffn=13824, layers=40, eps=1e-5),
+          "bloom-7b1": dict(family="bloom", hidden=4096, heads=32, ffn=16384, layers=30, eps=1e-5),
+          "opt-13b": dict(family="opt", hidden=5120, heads=40, ffn=20480, layers=40, eps=1e-5)}
 VOCAB = 32000
 
 
@@ -49,6 +55,8 @@ def random_weights(s, seed, dev):
 
     def w(*shape, std=0.02):
         return (torch.randn(*shape, generator=g, device=dev, dtype=torch.float16) * std)
+    if "family" in s:
+        return ln_decoder_weights(s, w)
     sd = {"embed_tokens.weight": w(VOCAB, D, std=1.0), "norm.weight": 1 + w(D, std=0.1)}
     for i in range(s["layers"]):
         p = f"layers.{i}."
@@ -57,6 +65,47 @@ def random_weights(s, seed, dev):
                    p + "mlp.down_proj.weight": w(D, I)})
         sd.update({p + n + ".weight": 1 + w(D, std=0.1) for n in ("input_layernorm", "post_attention_layernorm")})
     return sd
+
+
+def ln_decoder_weights(s, w):
+    """BloomModel / OPTModel (decoder.*) keys, biases on every linear and LayerNorm."""
+    D, F = s["hidden"], s["ffn"]
+
+    def ln(p):
+        return {p + ".weight": 1 + w(D, std=0.1), p + ".bias": w(D, std=0.1)}
+
+    def lin(p, o, i):
+        return {p + ".weight": w(o, i), p + ".bias": w(o)}
+    sd = {}
+    if s["family"] == "bloom":
+        sd.update({"word_embeddings.weight": w(VOCAB, D, std=1.0), **ln("word_embeddings_layernorm"), **ln("ln_f")})
+        for i in range(s["layers"]):
+            p = f"h.{i}."
+            sd.update({**ln(p + "input_layernorm"), **ln(p + "post_attention_layernorm"),
+                       **lin(p + "self_attention.query_key_value", 3 * D, D), **lin(p + "self_attention.dense", D, D),
+                       **lin(p + "mlp.dense_h_to_4h", F, D), **lin(p + "mlp.dense_4h_to_h", D, F)})
+    else:
+        sd.update({"decoder.embed_tokens.weight": w(VOCAB, D, std=1.0), "decoder.embed_positions.weight":
+                   w(2050, D, std=0.1), **ln("decoder.final_layer_norm")})
+        for i in range(s["layers"]):
+            p = f"decoder.layers.{i}."
+            sd.update({**ln(p + "self_attn_layer_norm"), **ln(p + "final_layer_norm"), **lin(p + "fc1", F, D),
+                       **lin(p + "fc2", D, F)})
+            for n in ("q", "k", "v", "out"):
+                sd.update(lin(p + f"self_attn.{n}_proj", D, D))
+    return sd
+
+
+def hf_config(s):
+    from transformers import BloomConfig, LlamaConfig, OPTConfig
+    if s.get("family") == "bloom":
+        return BloomConfig(vocab_size=VOCAB, hidden_size=s["hidden"], n_head=s["heads"], n_layer=s["layers"])
+    if s.get("family") == "opt":
+        return OPTConfig(vocab_size=VOCAB, hidden_size=s["hidden"], num_attention_heads=s["heads"], ffn_dim=s["ffn"],
+                         num_hidden_layers=s["layers"], max_position_embeddings=2048, word_embed_proj_dim=s["hidden"])
+    return LlamaConfig(vocab_size=VOCAB, hidden_size=s["hidden"], num_attention_heads=s["heads"],
+                       intermediate_size=s["ffn"], num_hidden_layers=s["layers"], rms_norm_eps=s["eps"],
+                       max_position_embeddings=4096)
 
 
 def packed_batches(ids, max_tokens):
@@ -78,24 +127,25 @@ def run_packed(net, ids, max_tokens):
 def reference_loop(s, sd, ids, dev):
     """Batch-1 fp16 forwards with output_hidden_states and the last-four sum, as the reference script does."""
     try:
-        from transformers import LlamaConfig, LlamaModel
-        cfg = LlamaConfig(vocab_size=VOCAB, hidden_size=s["hidden"], num_attention_heads=s["heads"],
-                          intermediate_size=s["ffn"], num_hidden_layers=s["layers"], rms_norm_eps=s["eps"],
-                          max_position_embeddings=4096)
+        from transformers import BloomModel, LlamaModel, OPTModel
+        cls = {"bloom": BloomModel, "opt": OPTModel}.get(s.get("family"), LlamaModel)
+        cfg = hf_config(s)
         dt = torch.get_default_dtype()
         torch.set_default_dtype(torch.float16)
         try:
             with torch.device(dev):
-                m = LlamaModel(cfg).eval()
+                m = cls(cfg).eval()
         finally:
             torch.set_default_dtype(dt)
         m.load_state_dict(sd, strict=True)
-        which = "HF LlamaModel fp16"
+        which = f"HF {cls.__name__} fp16"
+        start = 0 if s.get("family") == "bloom" else 1
 
         def fwd(x):
             hs = m(torch.from_numpy(x)[None].to(dev), output_hidden_states=True).hidden_states
-            return torch.stack(hs)[[-4, -3, -2, -1]].sum(0)[0, 1:].cpu().numpy()
+            return torch.stack(hs)[[-4, -3, -2, -1]].sum(0)[0, start:].cpu().numpy()
     except ImportError:
+        assert "family" not in s, "the BLOOM / OPT reference loop needs transformers"
         net = LT.LlamaNet(dict(sd), LT.TorchOps(dev, torch.float16), s["layers"], s["heads"], s["eps"], 10000.0, 4096)
         which = "torch restatement fp16 (transformers not importable)"
 
@@ -162,8 +212,15 @@ def main():
         ref_ids = ids[:a.ref_sentences]
         which, ref_dt = reference_loop(s, sd, ref_ids, dev)
         ref_tok = sum(len(x) for x in ref_ids)
-        ops = LT.CudaOps(dev)
-        net = LT.LlamaNet(sd, ops, s["layers"], s["heads"], s["eps"], 10000.0, 4096)
+        if "family" in s:
+            ops = LD.CudaOps(dev)
+            net = LD.LnDecoderNet({LD._strip(k, s["family"]): v for k, v in sd.items()}, ops, s["family"], s["layers"],
+                                  s["heads"], s["eps"], 2048 if s["family"] == "opt" else None)
+            linear_flops = 4 * s["hidden"] ** 2 + 2 * s["hidden"] * s["ffn"]
+        else:
+            ops = LT.CudaOps(dev)
+            net = LT.LlamaNet(sd, ops, s["layers"], s["heads"], s["eps"], 10000.0, 4096)
+            linear_flops = 4 * s["hidden"] ** 2 + 3 * s["hidden"] * s["ffn"]
         del sd
         with torch.no_grad():
             run_packed(net, ids, a.tokens)                      # warm-up: every shape of the timed window
@@ -187,7 +244,7 @@ def main():
                  reference=which, reference_sentences_per_s=len(ref_ids) / ref_dt,
                  reference_tokens_per_s=ref_tok / ref_dt, speedup=(len(ids) / dt) / (len(ref_ids) / ref_dt),
                  shares={k: v / tot for k, v in sorted(shares.items())},
-                 tflops=2.0 * sum(lens) * (s["layers"] * (4 * s["hidden"] ** 2 + 3 * s["hidden"] * s["ffn"])) / dt / 1e12)
+                 tflops=2.0 * sum(lens) * s["layers"] * linear_flops / dt / 1e12)
         results[shape] = r
         print(f"{shape}: packed {r['packed_sentences_per_s']:.1f} sentences/s, {r['packed_tokens_per_s']:.0f} tokens/s "
               f"({r['tflops']:.0f} TFLOP/s in the linears); reference loop ({which}) "

@@ -9,7 +9,7 @@ mkdir -p gpurun_out
 CS=/usr/local/cuda/bin/compute-sanitizer
 : > "$out"
 for tool in memcheck racecheck; do
-  for part in gemms attention llama encoders fusion; do
+  for part in gemms attention llama ln_decoders encoders fusion; do
     echo "==== $tool $part" | tee -a "$out"
     # --report-api-errors no: with it on, memcheck's one and only report is the CUDA runtime's own lazy-loading probe
     # (cuKernelGetFunction -> CUDA_ERROR_INVALID_HANDLE inside the first cudaLaunchKernel of the process, handled by the

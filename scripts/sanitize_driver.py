@@ -1,6 +1,7 @@
 """Small launches of every hand-synchronised kernel family, for compute-sanitizer (scripts/sanitize.sh):
 the wgmma GEMM in its three operand modes and both tile widths, both V^T attention kernels
-on ragged batches, the LLaMA kernels (causal head-dim-128 attention, RoPE, RMSNorm, SwiGLU), LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
+on ragged batches, the LLaMA kernels (causal head-dim-128 attention, RoPE, RMSNorm, SwiGLU), the BLOOM / OPT
+kernels (ALiBi attention, wide LayerNorm, tanh-GELU / fp16 ReLU epilogues), LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
 fused fusion step (cluster kernel with DSMEM exchange + weight-gradient kernel).  Sizes are tiny: racecheck is slow."""
 import os
 import sys
@@ -84,6 +85,40 @@ def llama():
     print("llama ok")
 
 
+def ln_decoders():
+    """The BLOOM / OPT kernels: causal attention with ALiBi on ragged rows with unaligned starts, the wide LayerNorm in
+    its three output modes, the tanh-GELU and fp16 ReLU GEMM epilogues, then a 3-layer LnDecoderNet forward per family."""
+    from mertools_b200.extract import ln_decoder_text as LD
+    heads, lens = 3, [5, 70, 1, 129, 17]
+    tokens, D = sum(lens), heads * 128
+    qkv = torch.randn(tokens, 3 * D, device=dev).half()
+    vt = torch.zeros(D, (tokens + 7) // 8 * 8, dtype=torch.float16, device=dev)
+    vt[:, :tokens] = qkv[:, 2 * D:].T
+    cu = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int32, device=dev)
+    ops = LD.CudaOps(dev)
+    ctx = torch.empty(tokens, D, dtype=torch.float16, device=dev)
+    L.check(ops._att_alibi(L.ptr(qkv), L.ptr(vt), vt.shape[1], L.ptr(ctx), L.ptr(cu), len(lens), tokens, max(lens),
+                           heads, L.ptr(LD.alibi_slopes(heads).to(dev)), L.stream_ptr()))
+    x = torch.randn(tokens, 512, device=dev)
+    g, b = torch.ones(512, device=dev), torch.zeros(512, device=dev)
+    ops.layernorm(x, g, b, 1e-5)
+    ops.layernorm(x, g, b, 1e-5, out="f32")
+    ops.layernorm(x, g, b, 1e-5, acc=torch.zeros_like(x))
+    a, w, bias = torch.randn(tokens, 256, device=dev).half(), torch.randn(384, 256, device=dev).half(), torch.randn(384, device=dev)
+    for f16 in (False, True):
+        out = torch.empty(tokens, 384, dtype=torch.float16 if f16 else torch.float32, device=dev)
+        L.gemm(a, w, out, bias=bias, mode=L.MER_GEMM_F16, f16_out=f16, gelu_tanh=True)
+    L.gemm(a, w, torch.empty(tokens, 384, dtype=torch.float16, device=dev), bias=bias, mode=L.MER_GEMM_F16,
+           f16_out=True, relu=True)
+    ids = np.arange(4, 4 + tokens) % 300
+    bsd = {LD._strip(k, "bloom"): torch.from_numpy(v) for k, v in S.bloom_state_dict(vocab=300, layers=3).items()}
+    LD.LnDecoderNet(bsd, ops, "bloom", 3, 4, 1e-5).forward(ids, lens)
+    osd = {LD._strip(k, "opt"): torch.from_numpy(v) for k, v in S.opt_state_dict(vocab=300, layers=3, max_pos=256).items()}
+    LD.LnDecoderNet(osd, ops, "opt", 3, 4, 1e-5, 256).forward(ids, lens)
+    torch.cuda.synchronize()
+    print("ln_decoders ok")
+
+
 def encoders():
     from mertools_b200.encoders import BertEncoder, HubertEncoder, VitEncoder
     sd = S.hubert_state_dict(seed=1, layers=4)
@@ -110,6 +145,6 @@ def fusion():
 
 
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["gemms", "attention", "llama", "encoders", "fusion"]
+    which = sys.argv[1:] or ["gemms", "attention", "llama", "ln_decoders", "encoders", "fusion"]
     for w in which:
         globals()[w]()
