@@ -51,8 +51,10 @@ MER_API int mer_profile_enable(int on);
 MER_API int mer_profile_collect(int mode, double* total_ms, double* total_flops, int* launches);
 
 /* ---- GEMM (nn.Linear / Conv1d-as-GEMM / patch-embed) ---------------------------------- */
-enum { MER_EPI_GELU = 1, MER_EPI_ROUND_TF32 = 2, MER_EPI_SPLIT_BF16 = 4,
-       MER_EPI_GELU_LIBM = 8, /* with MER_EPI_GELU: libdevice erff instead of the 12-op polynomial */
+enum { MER_EPI_GELU = 1,
+       MER_EPI_ROUND_TF32 = 2, /* out (and vt) rounded to tf32 (cvt.rna); excludes MER_EPI_SPLIT_BF16 */
+       MER_EPI_SPLIT_BF16 = 4,
+       MER_EPI_GELU_LIBM = 8, /* with MER_EPI_GELU (required): libdevice erff instead of the 12-op polynomial */
        MER_EPI_QUICK_GELU = 64, /* x * sigmoid(1.702 x) (CLIP's hidden_act) instead of GELU; excludes MER_EPI_GELU */
        MER_EPI_RELU = 128,    /* max(x, 0), applied AFTER the residual add when there is one (ResNet BasicBlock);
                                  fp32 output, or fp16 output without a residual (OPT's fc1); excludes the GELU flags */
@@ -75,9 +77,9 @@ enum { MER_EPI_GELU = 1, MER_EPI_ROUND_TF32 = 2, MER_EPI_SPLIT_BF16 = 4,
 enum { MER_GEMM_TF32 = 0, MER_GEMM_BF16X3 = 1, MER_GEMM_F16 = 2 };
 
 typedef struct MerGemmEpilogue {
-  const float* bias; /* [N] or NULL */
-  const float* res;  /* residual rows or NULL */
-  float* out;
+  const float* bias; /* [N] or NULL; 8-byte aligned */
+  const float* res;  /* residual rows or NULL; 8-byte aligned */
+  float* out;        /* 8-byte aligned (4-byte for an fp16 out) */
   long long out_bstride; /* out row = b*out_bstride + out_row0 + m */
   long long out_row0;
   long long res_bstride; /* res row = b*res_bstride + res_row0 + m */
@@ -88,7 +90,7 @@ typedef struct MerGemmEpilogue {
   int split_off; /* reserved (0) */
   /* optional transposed side output: columns n >= vt_col0 are written as vt[(n - vt_col0) * vt_ld +
    * out_row] INSTEAD of out[out_row, n] (the QKV GEMM hands V^T, keys contiguous, to the V^T
-   * attention kernel) */
+   * attention kernel); with vt, vt_col0 must be even and in [0, N) */
   float* vt;
   long long vt_ld;
   int vt_col0;

@@ -15,10 +15,12 @@ LIB_PATH = os.path.join(_HERE, "lib", "libmer_b200.so")
 MER_EPI_GELU = 1
 MER_EPI_ROUND_TF32 = 2
 MER_EPI_SPLIT_BF16 = 4
+MER_EPI_GELU_LIBM = 8
 MER_GEMM_TF32 = 0
 MER_GEMM_BF16X3 = 1
 MER_GEMM_F16 = 2
 MER_EPI_OUT_F16 = 16
+MER_EPI_QUICK_GELU = 64
 MER_EPI_RELU = 128
 MER_EPI_GELU_TANH = 256
 MER_LN_OUT_F16 = 8
@@ -119,10 +121,11 @@ def gemm(A, W, out, *, bias=None, res=None, gelu=False, round_out=False, split_o
          a_phase_stride=0, a_row_stride=None, a_batch_stride=0,
          out_bstride=0, out_row0=0, res_bstride=0, res_row0=0,
          ld_out=None, ld_res=None, force_block_n=0, cluster=0, vt=None, vt_col0=0, gelu_libm=False,
-         f16_out=False, a_row0=0, a_cols=0, a_col_group=0, relu=False, gelu_tanh=False):
+         f16_out=False, a_row0=0, a_cols=0, a_col_group=0, relu=False, gelu_tanh=False, quick_gelu=False):
     """out = epilogue(A @ W.T).  A, W: fp32 CUDA tensors of LOGICAL shape [rows, K] / [N, K] (holding
     tf32-rounded fp32, or split bf16 hi|lo bytes when mode is BF16X3; fp16 tensors when mode is F16);
-    see MerGemmDesc in mer_b200.h."""
+    see MerGemmDesc in mer_b200.h.  a_phase_stride defaults to K_inner when P == 1; a nonzero value is passed through
+    (the tensor map's phase dimension then has the stride a caller's own descriptor would give it)."""
     N, K = W.shape
     d = MerGemmDesc()
     d.A, d.W = A.data_ptr(), W.data_ptr()
@@ -133,7 +136,7 @@ def gemm(A, W, out, *, bias=None, res=None, gelu=False, round_out=False, split_o
     d.a_rows_dim = a_rows_dim if a_rows_dim is not None else d.rows_per_batch
     d.batches = batches
     d.N = N
-    d.a_phase_stride = a_phase_stride if P > 1 else d.K_inner
+    d.a_phase_stride = a_phase_stride if (P > 1 or a_phase_stride) else d.K_inner
     d.a_row_stride = a_row_stride if a_row_stride is not None else K
     d.a_batch_stride = a_batch_stride if batches > 1 else d.a_row_stride * d.a_rows_dim
     d.force_block_n = force_block_n
@@ -148,9 +151,9 @@ def gemm(A, W, out, *, bias=None, res=None, gelu=False, round_out=False, split_o
     d.ep.ld_out = ld_out if ld_out is not None else N
     d.ep.ld_res = ld_res if ld_res is not None else N
     d.ep.flags = ((MER_EPI_GELU if gelu else 0) | (MER_EPI_ROUND_TF32 if round_out else 0)
-                  | (MER_EPI_SPLIT_BF16 if split_out else 0) | (8 if gelu_libm else 0)
+                  | (MER_EPI_SPLIT_BF16 if split_out else 0) | (MER_EPI_GELU_LIBM if gelu_libm else 0)
                   | (MER_EPI_OUT_F16 if f16_out else 0) | (MER_EPI_RELU if relu else 0)
-                  | (MER_EPI_GELU_TANH if gelu_tanh else 0))
+                  | (MER_EPI_GELU_TANH if gelu_tanh else 0) | (MER_EPI_QUICK_GELU if quick_gelu else 0))
     d.ep.split_off = N
     if vt is not None:
         d.ep.vt, d.ep.vt_ld, d.ep.vt_col0 = vt.data_ptr(), vt.shape[1], vt_col0

@@ -468,6 +468,20 @@ int mer_gemm_launch(const MerGemmDesc* g, cudaStream_t stream) {
   MER_REQUIRE(g->a_col_group == 0 || g->force_block_n == 128 || g->force_block_n == 256,
               "mer_gemm: a_col_group needs force_block_n (the weights are built for one block width)");
   MER_REQUIRE(!(g->ep.vt && (g->ep.flags & MER_EPI_GELU)), "mer_gemm: GELU + transposed side output is not supported");
+  // the epilogue routes whole column pairs (n, n + 1), n even, to vt or out and writes vt row n - vt_col0
+  MER_REQUIRE(g->ep.vt == nullptr || (g->ep.vt_col0 >= 0 && g->ep.vt_col0 < g->N && g->ep.vt_col0 % 2 == 0),
+              "mer_gemm: vt_col0=%d must be even and in [0, N=%d)", g->ep.vt_col0, g->N);
+  // flags the kernel would otherwise ignore or resolve silently
+  MER_REQUIRE(!((g->ep.flags & MER_EPI_GELU_LIBM) && !(g->ep.flags & MER_EPI_GELU)),
+              "mer_gemm: MER_EPI_GELU_LIBM selects the erf form of MER_EPI_GELU and needs it");
+  MER_REQUIRE(!((g->ep.flags & MER_EPI_ROUND_TF32) && (g->ep.flags & MER_EPI_SPLIT_BF16)),
+              "mer_gemm: a tf32-rounded output excludes the bf16-split output");
+  // the epilogue loads bias / res as float2 and stores out as float2 (fp32) or as an fp16 pair (uint32)
+  const uintptr_t out_align = (g->ep.flags & MER_EPI_OUT_F16) ? 4 : 8;
+  MER_REQUIRE(reinterpret_cast<uintptr_t>(g->ep.out) % out_align == 0 &&
+                  reinterpret_cast<uintptr_t>(g->ep.res) % 8 == 0 && reinterpret_cast<uintptr_t>(g->ep.bias) % 8 == 0,
+              "mer_gemm: out must be %d-byte aligned, res and bias 8-byte aligned (out %p res %p bias %p)",
+              (int)out_align, (const void*)g->ep.out, (const void*)g->ep.res, (const void*)g->ep.bias);
   const int m_tiles = (g->rows_per_batch + BLOCK_M - 1) / BLOCK_M;
   const long long tiles256 = (g->N % 256 == 0) ? (long long)g->batches * m_tiles * (g->N / 256) : 0;
   // 128 x 256 tiles whenever they fill the machine; 128 x 128 for small problems / N % 256 != 0
