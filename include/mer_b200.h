@@ -551,6 +551,26 @@ MER_API int mer_causal_alibi_attention_f16(const void* qkv16, const void* vt16, 
 MER_API int mer_layernorm_f16(const float* x, const float* gamma, const float* beta, void* y16, float* y32, float* acc,
                               long long rows, int dim, float eps, void* stream);
 
+/* ---- DeBERTa / DeBERTa-v2 encoders (extract_text_huggingface.py:164-166 and the AutoModel branch; orchestrated from the
+ * host in mertools_b200/extract/deberta_text.py over this, mer_gemm, mer_layernorm / mer_layernorm_f16 and
+ * mer_segment_reduce). ---- */
+/* Disentangled self-attention (HF DisentangledSelfAttention, pos_att_type c2p | p2c, head_dim 64) per (sequence, head):
+ *   score[i, j] = scale * (q_i . k_j + q_i . pos_k[row] + k_j . pos_q[row]),  row = rel_row[i - j + max_seqlen - 1],
+ *   ctx_i = softmax_j(score[i, :]) . V,
+ * i and j counted from the sequence start.  qkv, vt, cu_seqlens, tokens, max_seqlen, heads and ctx as mer_attention's
+ * V^T form (V columns of qkv not read); pos_k / pos_q: the layer's projections of the relative-position table, [2 span,
+ * heads*64] with row pitch pos_ld (elements, >= heads*64, multiple of 8 for fp16 / 4 for fp32), in the operand format
+ * of qkv; rel_row: device int32 [2 max_seqlen - 1], values in [0, 2 span) (clamped there).  flags: MER_ATT_QKV_F16 (fp16
+ * qkv / vt / tables, m16n8k16) or none (tf32-rounded fp32, m16n8k8), plus at most one of MER_EPI_OUT_F16,
+ * MER_EPI_ROUND_TF32, MER_EPI_SPLIT_BF16 for ctx (fp32 otherwise).  qkv, vt, pos_k and pos_q 16-byte aligned.  No
+ * length cap.  fp32 scores, softmax statistics and O: attention_rel.cu.  Refused with a "mer_disentangled_attention:"
+ * message: heads outside 1 .. 65535, n_seq outside 1 .. 65535, span <= 0, a NULL operand or table, a V^T or table pitch
+ * that is too small or misaligned, max_seqlen outside 1 .. tokens, other flags. */
+MER_API int mer_disentangled_attention(const void* qkv, const void* vt, long long vt_ld, const void* pos_k,
+                                       const void* pos_q, long long pos_ld, int span, const int32_t* rel_row,
+                                       float scale, void* ctx, const int32_t* cu_seqlens, int n_seq, long long tokens,
+                                       int max_seqlen, int heads, int flags, void* stream);
+
 /* ---- Whisper branch of the audio extractor (extract_audio_huggingface.py:83-91): the two kernels the shared GEMM /
  * LayerNorm / attention entry points do not cover; the encoder / decoder are orchestrated from the host over those
  * (mertools_b200/extract/whisper.py). ---- */

@@ -28,6 +28,7 @@ MER_ATT_QKV_F16 = 32
 MER_LN_ROUND_TF32 = 1
 MER_LN_ACC_INIT = 2
 MER_LN_ACC_ADD = 4
+MER_LN_SPLIT_F16 = 32
 
 
 class MerError(RuntimeError):

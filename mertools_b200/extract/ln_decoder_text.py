@@ -102,10 +102,11 @@ def load_ln_decoder_weights(model_dir, device, family):
     return out
 
 
-def deinterleave_qkv(t, heads):
-    """BLOOM query_key_value rows [head][q, k, v][128] (weight [3 D, D] or bias [3 D]) -> q | k | v blocks."""
+def deinterleave_qkv(t, heads, head_dim=HEAD_DIM):
+    """Fused projection rows interleaved per head as [head][q, k, v][head_dim] (BLOOM's query_key_value, head_dim 128;
+    DeBERTa's in_proj, 64), weight [3 D, D] or bias [3 D] -> q | k | v blocks."""
     shape = t.shape
-    return t.reshape(heads, 3, HEAD_DIM, *shape[1:]).transpose(0, 1).reshape(shape).contiguous()
+    return t.reshape(heads, 3, head_dim, *shape[1:]).transpose(0, 1).reshape(shape).contiguous()
 
 
 # ---- layer orchestration --------------------------------------------------------------------------------------------

@@ -1,7 +1,7 @@
 """Lexical feature extraction — H100 mirror of
-MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; LLaMA-family decoders through
-extract/llama_text.py and BLOOM / OPT through extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU
-run).
+MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; DeBERTa / DeBERTa-v2 through
+extract/deberta_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
+extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU run).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
 model_dir)`` (:139), ``find_start_end_pos`` (:90-114) and the save-dir naming (:148-157).  Token ids
@@ -124,6 +124,25 @@ def _ln_decoder_extractor(model_dir, cfg, device):
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
 
 
+def _deberta_extractor(model_name, model_dir, cfg, device):
+    """The reference's DeBERTa models (:164-166 and the AutoModel branch), fp32 features.  Tokenizer by model name as
+    the reference loads it: BertTokenizer for deberta-chinese-large, AutoTokenizer(use_fast=False) otherwise.  Tokens per
+    launch as in _llama_extractor."""
+    import torch
+    from transformers import AutoTokenizer, BertTokenizer
+
+    from .deberta_text import DebertaTextEncoder, check_deberta_config
+    check_deberta_config(cfg)  # before any weight is read
+    if model_name == "deberta-chinese-large":
+        tokenizer = BertTokenizer.from_pretrained(model_dir, use_fast=False)
+    else:
+        tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
+    enc = DebertaTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    tokens = int(min(16384, max(cfg.max_position_embeddings, free // 2 // enc.bytes_per_token)))
+    return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
+
+
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
                       language="chinese", model_dir=None, config=None, sentences_per_launch=256):
     """Same signature, naming and outputs as the reference (:139-252)."""
@@ -149,12 +168,14 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     from .. import shard
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "llama", "bloom", "opt"), \
-        f"only BERT/RoBERTa encoders and LLaMA / BLOOM / OPT decoders are on the H100 path, got {cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "llama", "bloom", "opt"), \
+        f"only BERT/RoBERTa/DeBERTa encoders and LLaMA / BLOOM / OPT decoders are on the H100 path, got {cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("bloom", "opt"):
         ext = _ln_decoder_extractor(model_dir, cfg, f"cuda:{gpu}")
+    elif cfg.model_type in ("deberta", "deberta-v2"):
+        ext = _deberta_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     else:
         tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
         roberta = cfg.model_type != "bert"

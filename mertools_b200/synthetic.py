@@ -567,6 +567,67 @@ def opt_state_dict(seed=25, vocab=4000, hidden=512, ffn=2048, layers=6, max_pos=
     return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
 
 
+# The two DeBERTa checkpoints of tests/golden/deberta_text_golden.npz: v1 as deberta-large (no absolute positions, c2p |
+# p2c over max_relative_positions, raw relative table) at base width; v2 as deberta-v2-xlarge (log buckets, LayerNorm'd
+# table, share_att_key, conv layer, no token types) at width 512.  HF config keywords.
+DEBERTA_GOLDEN_CFGS = {
+    "v1": dict(vocab_size=None, hidden_size=768, num_attention_heads=12, intermediate_size=1536, num_hidden_layers=4,
+               max_position_embeddings=512, max_relative_positions=-1, relative_attention=True,
+               pos_att_type=["c2p", "p2c"], position_biased_input=False, type_vocab_size=0, layer_norm_eps=1e-7),
+    "v2": dict(vocab_size=None, hidden_size=512, num_attention_heads=8, intermediate_size=1024, num_hidden_layers=5,
+               max_position_embeddings=512, max_relative_positions=-1, relative_attention=True, position_buckets=32,
+               norm_rel_ebd="layer_norm", share_att_key=True, pos_att_type=["p2c", "c2p"], conv_kernel_size=3,
+               conv_act="gelu", position_biased_input=False, type_vocab_size=0, layer_norm_eps=1e-7),
+}
+
+
+def deberta_state_dict(cfg, v2, seed=27, scale=1.0):
+    """Keys of ``transformers.DebertaModel`` (v2 False) / ``DebertaV2Model`` (v2 True) for a dict of HF config keywords
+    (as DEBERTA_GOLDEN_CFGS; vocab_size set).  v1: per-head interleaved ``in_proj`` with ``q_bias`` / ``v_bias`` and
+    ``pos_proj`` / ``pos_q_proj``; v2: query / key / value projections (plus ``pos_key_proj`` / ``pos_query_proj``
+    without share_att_key), ``encoder.LayerNorm`` with norm_rel_ebd, ``encoder.conv`` with conv_kernel_size.  ``scale``
+    multiplies every layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    d, ffn, std = cfg["hidden_size"], cfg["intermediate_size"], 0.03 * scale
+    mr = cfg.get("max_relative_positions", -1)
+    mr = mr if mr >= 1 else cfg["max_position_embeddings"]
+    span = cfg["position_buckets"] if v2 and cfg.get("position_buckets", -1) > 0 else mr
+    g.normal("embeddings.word_embeddings.weight", (cfg["vocab_size"], d), 0.5)
+    if cfg.get("position_biased_input", True):
+        g.normal("embeddings.position_embeddings.weight", (cfg["max_position_embeddings"], d), 0.1)
+    if cfg.get("type_vocab_size", 0) > 0:
+        g.normal("embeddings.token_type_embeddings.weight", (cfg["type_vocab_size"], d), 0.1)
+    g.ln("embeddings.LayerNorm", d)
+    for i in range(cfg["num_hidden_layers"]):
+        p = f"encoder.layer.{i}."
+        a = p + "attention.self."
+        if v2:
+            for n in ("query_proj", "key_proj", "value_proj"):
+                g.linear(a + n, d, d, std)
+            if not cfg.get("share_att_key", False):
+                g.linear(a + "pos_key_proj", d, d, std)
+                g.linear(a + "pos_query_proj", d, d, std)
+        else:
+            g.normal(a + "in_proj.weight", (3 * d, d), std)
+            g.normal(a + "q_bias", (d,), 0.02)
+            g.normal(a + "v_bias", (d,), 0.02)
+            g.normal(a + "pos_proj.weight", (d, d), std)
+            g.linear(a + "pos_q_proj", d, d, std)
+        g.linear(p + "attention.output.dense", d, d, std)
+        g.ln(p + "attention.output.LayerNorm", d)
+        g.linear(p + "intermediate.dense", ffn, d, std)
+        g.linear(p + "output.dense", d, ffn, std)
+        g.ln(p + "output.LayerNorm", d)
+    g.normal("encoder.rel_embeddings.weight", (2 * span, d), 0.5)
+    if v2 and "layer_norm" in cfg.get("norm_rel_ebd", "none"):
+        g.ln("encoder.LayerNorm", d)
+    if v2 and cfg.get("conv_kernel_size", 0) > 0:
+        g.normal("encoder.conv.conv.weight", (d, d, cfg["conv_kernel_size"]), std)
+        g.normal("encoder.conv.conv.bias", (d,), 0.02)
+        g.ln("encoder.conv.LayerNorm", d)
+    return g.sd
+
+
 def fusion_state_dict(seed=3, audio_dim=768, text_dim=768, video_dim=768, hidden=128,
                       out1=6, out2=1, feat_type="utt"):
     """Keys of toolkit/models/attention.py:Attention, nn.Linear / nn.LSTM-style
