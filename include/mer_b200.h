@@ -571,6 +571,29 @@ MER_API int mer_disentangled_attention(const void* qkv, const void* vt, long lon
                                        float scale, void* ctx, const int32_t* cu_seqlens, int n_seq, long long tokens,
                                        int max_seqlen, int heads, int flags, void* stream);
 
+/* ---- XLNet encoders (xlnet-base-cased, xlnet-large-cased, chinese-xlnet-base: the AutoModel branch of
+ * extract_text_huggingface.py; orchestrated from the host in mertools_b200/extract/xlnet_text.py over this, mer_gemm,
+ * mer_layernorm and mer_segment_reduce). ---- */
+/* XLNet relative self-attention (HF XLNetRelativeAttention.rel_attn_core, attn_type "bi", content stream, head_dim 64)
+ * per (sequence, head):
+ *   score[i, j] = scale * ((q_i + r_w_bias) . k_j + (q_i + r_r_bias) . r[row] + (q_i + r_s_bias) . seg_embed[s_ij]),
+ *   row = rel_row[i - j + max_seqlen - 1],  s_ij = (token_type[i] != token_type[j]),  ctx_i = softmax_j . V,
+ * i and j counted from the sequence start.  qkv, vt, cu_seqlens, tokens, max_seqlen, heads and ctx as
+ * mer_disentangled_attention (V columns of qkv not read); r: the layer's projection of the relative-position rows,
+ * [rows, heads*64] with row pitch r_ld (elements, >= heads*64, multiple of 8 for fp16 / 4 for fp32), in the operand
+ * format of qkv; rel_row: device int32 [2 max_seqlen - 1], every value a row of r.  r_w_bias, r_r_bias, r_s_bias:
+ * device fp32 [heads, 64]; seg_embed: device fp32 [2, heads, 64]; all four 8-byte aligned.  token_type: device int32
+ * [tokens] (absolute token index), or NULL for no segment term (the model called without token_type_ids).  flags as
+ * mer_disentangled_attention.  The bias products are fp32 dot products over the operands (q + bias is never rounded to
+ * the operand format).  No length cap.  fp32 scores, softmax statistics and O: attention_xl.cu.  Refused with a
+ * "mer_xlnet_attention:" message: heads or n_seq outside 1 .. 65535, a NULL operand, table or bias, a V^T or R pitch
+ * that is too small or misaligned, a misaligned operand or bias, max_seqlen outside 1 .. tokens, other flags. */
+MER_API int mer_xlnet_attention(const void* qkv, const void* vt, long long vt_ld, const void* r, long long r_ld,
+                                const int32_t* rel_row, const float* r_w_bias, const float* r_r_bias,
+                                const float* r_s_bias, const float* seg_embed, const int32_t* token_type, float scale,
+                                void* ctx, const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
+                                int heads, int flags, void* stream);
+
 /* ---- Whisper branch of the audio extractor (extract_audio_huggingface.py:83-91): the two kernels the shared GEMM /
  * LayerNorm / attention entry points do not cover; the encoder / decoder are orchestrated from the host over those
  * (mertools_b200/extract/whisper.py). ---- */

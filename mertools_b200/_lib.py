@@ -84,6 +84,7 @@ def _declare(l):
         "mer_round_tf32": [vp, i64, vp],
         "mer_split_bf16": [vp, vp, i64, i32, vp],
         "mer_attention": [vp, vp, i64, vp, vp, i32, i64, i32, i32, i32, vp],
+        "mer_xlnet_attention": [vp, vp, i64, vp, i64, vp, vp, vp, vp, vp, vp, f32, vp, vp, i32, i64, i32, i32, i32, vp],
     }
     for name, args in sig.items():
         fn = getattr(l, name)

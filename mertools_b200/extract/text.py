@@ -1,6 +1,6 @@
 """Lexical feature extraction — H100 mirror of
 MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; DeBERTa / DeBERTa-v2 through
-extract/deberta_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
+extract/deberta_text.py and XLNet through extract/xlnet_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
 extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU run).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
@@ -143,6 +143,22 @@ def _deberta_extractor(model_name, model_dir, cfg, device):
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
+def _xlnet_extractor(model_dir, cfg, device):
+    """The reference's XLNet models (the AutoModel + AutoTokenizer(use_fast=False) branch), fp32 features.  The
+    extractor forwards the tokenizer's token_type_ids when it returns them, as model(**inputs) does.  Tokens per launch
+    as in _deberta_extractor, with MAX_LEN (512) for the max_position_embeddings XLNet does not have."""
+    import torch
+    from transformers import AutoTokenizer
+
+    from .xlnet_text import MAX_LEN, XlnetTextEncoder, XlnetTextExtractor, check_xlnet_config
+    check_xlnet_config(cfg)  # before any weight is read
+    tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
+    enc = XlnetTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    tokens = int(min(16384, max(MAX_LEN, free // 2 // enc.bytes_per_token)))
+    return XlnetTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
+
+
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
                       language="chinese", model_dir=None, config=None, sentences_per_launch=256):
     """Same signature, naming and outputs as the reference (:139-252)."""
@@ -168,14 +184,18 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     from .. import shard
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "llama", "bloom", "opt"), \
-        f"only BERT/RoBERTa/DeBERTa encoders and LLaMA / BLOOM / OPT decoders are on the H100 path, got {cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "xlnet", "llama", "bloom",
+                              "opt"), \
+        f"only BERT/RoBERTa/DeBERTa/XLNet encoders and LLaMA / BLOOM / OPT decoders are on the H100 path, got " \
+        f"{cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("bloom", "opt"):
         ext = _ln_decoder_extractor(model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("deberta", "deberta-v2"):
         ext = _deberta_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
+    elif cfg.model_type == "xlnet":
+        ext = _xlnet_extractor(model_dir, cfg, f"cuda:{gpu}")
     else:
         tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
         roberta = cfg.model_type != "bert"

@@ -628,6 +628,42 @@ def deberta_state_dict(cfg, v2, seed=27, scale=1.0):
     return g.sd
 
 
+# The two XLNet checkpoints of tests/golden/xlnet_text_golden.npz: "base" as chinese-xlnet-base (768 wide, 12 heads,
+# relu) at 4 layers; "large" as xlnet-large-cased (1024 wide, 16 heads, gelu) at 3 layers, so that hidden state 0 (the
+# raw word embedding) enters the last-four readout.  HF XLNetConfig keywords.
+XLNET_GOLDEN_CFGS = {
+    "base": dict(vocab_size=None, d_model=768, n_head=12, d_inner=1536, n_layer=4, ff_activation="relu",
+                 layer_norm_eps=1e-12, dropout=0.0),
+    "large": dict(vocab_size=None, d_model=1024, n_head=16, d_inner=2048, n_layer=3, ff_activation="gelu",
+                  layer_norm_eps=1e-12, dropout=0.0),
+}
+
+
+def xlnet_state_dict(cfg, seed=33, scale=1.0):
+    """Keys of ``transformers.XLNetModel`` for a dict of HF config keywords (as XLNET_GOLDEN_CFGS; vocab_size set):
+    ``word_embedding``, ``mask_emb`` and per layer ``rel_attn.{q,k,v,o,r}`` [d_model, n_head, 64] (no bias), the
+    r_w / r_r / r_s biases, ``seg_embed`` [2, n_head, 64], and the post-LN feed-forward.  ``scale`` multiplies every
+    layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    d, ffn, h = cfg["d_model"], cfg["d_inner"], cfg["n_head"]
+    std = 0.03 * scale
+    g.normal("mask_emb", (1, 1, d), 0.02)
+    g.normal("word_embedding.weight", (cfg["vocab_size"], d), 0.5)
+    for i in range(cfg["n_layer"]):
+        a = f"layer.{i}.rel_attn."
+        for n in ("q", "k", "v", "o", "r"):
+            g.normal(a + n, (d, h, d // h), std)
+        for n in ("r_r_bias", "r_s_bias", "r_w_bias"):
+            g.normal(a + n, (h, d // h), 0.3)
+        g.normal(a + "seg_embed", (2, h, d // h), 0.3)
+        g.ln(a + "layer_norm", d)
+        f = f"layer.{i}.ff."
+        g.ln(f + "layer_norm", d)
+        g.linear(f + "layer_1", ffn, d, std)
+        g.linear(f + "layer_2", d, ffn, std)
+    return g.sd
+
+
 def fusion_state_dict(seed=3, audio_dim=768, text_dim=768, video_dim=768, hidden=128,
                       out1=6, out2=1, feat_type="utt"):
     """Keys of toolkit/models/attention.py:Attention, nn.Linear / nn.LSTM-style
