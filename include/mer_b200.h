@@ -41,6 +41,12 @@ MER_API long long mer_launch_count(void);
  * (0 | 1) name CTA-pair forms, which this build does not have (0 launches for cluster 2 or twosm 1); -1 for arguments
  * outside those ranges. */
 MER_API long long mer_gemm_variant_launches(int block_n, int mode, int cluster, int twosm);
+/* launches so far of gemm_kernel with the epilogue that stages the output in shared memory and stores it with TMA
+ * (tma = 1: fp32, tf32 or fp16 output without residual or activation, the out base at out_row0 and its pitches
+ * multiples of 16 bytes, V^T if any starting at a multiple of 32 fp32 / 64 fp16 columns) or with the register epilogue
+ * (tma = 0: every other descriptor, and all of them under the environment variable MER_GEMM_EPI_TMA=0, read at every
+ * launch); -1 for other arguments.  Both write the same bits. */
+MER_API long long mer_gemm_epilogue_launches(int tma);
 /* per-launch CUDA-event timing (roofline in bench.py): enable(1) starts a fresh recording, enable(0)
  * stops; collect sums duration / algorithmic work / launches of one kernel class since the last
  * enable(1).  Classes: MER_GEMM_* (work = 2*M*N*K flop; MER_GEMM_F16 launches of fewer than 2^17 rows are

@@ -166,6 +166,13 @@ def gemm(A, W, out, *, bias=None, res=None, gelu=False, round_out=False, split_o
 gemm_tf32 = gemm
 
 
+def gemm_epilogue_launches():
+    """(register, TMA) epilogue launches of mer_gemm so far in this process (MER_GEMM_EPI_TMA=0 forces the first)."""
+    f = lib().mer_gemm_epilogue_launches
+    f.restype, f.argtypes = C.c_longlong, [C.c_int]
+    return int(f(0)), int(f(1))
+
+
 def layernorm(x, gamma, beta, y, *, eps, y_split=None, acc=None, flags=0):
     rows = x.numel() // x.shape[-1]
     check(lib().mer_layernorm(ptr(x), ptr(gamma), ptr(beta), ptr(y), ptr(y_split), ptr(acc), rows,

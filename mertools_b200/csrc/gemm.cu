@@ -16,8 +16,9 @@
 //   warpgroup 0 (warp 0)  TMA producer: A/B tiles -> 128B-swizzled smem ring (mbarrier full/empty)
 //   warpgroups 1, 2       consumers: rows [0, 64) / [64, 128) of the tile; wgmma.mma_async 64 x 128 x (32 bytes
 //                         of K) per instruction (two per K step for BLOCK_N = 256), fp32 accumulators in
-//                         registers; then the epilogue straight from the accumulator fragment (bias / activation /
-//                         residual / output format, 8 rows x 32 contiguous bytes per store instruction)
+//                         registers; then the epilogue (bias / activation / residual / output format): outputs
+//                         without residual or activation go through shared-memory slots and TMA stores (64-row
+//                         sub-tiles); every other form is stored straight from the accumulator fragment
 // The producer runs ahead across tile boundaries, so the next tile's operands stream in during the epilogue.
 //
 // Three arithmetic modes share the pipeline (128 bytes of K per smem row and stage in each):
@@ -55,9 +56,10 @@ struct GemmCfg {
   static constexpr int kBBytes = BLOCK_N * kRowBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = BLOCK_N == 256 ? 4 : 6;  // 192 KB of operands either way (227 KB usable)
+  static constexpr int kSlotsBytes = 2 * 2 * 64 * 128;     // TMA epilogue: 2 slot pairs of 2 x 8 KB
   static constexpr int kBarBytes = 256;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024;
-  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
+  static constexpr int smem_bytes(bool tma) { return kStages * kStageBytes + (tma ? kSlotsBytes : 0) + kBarBytes + 1024; }
+  static_assert(smem_bytes(true) <= 227 * 1024, "shared memory budget");
 };
 
 // internal epilogue flag (set by mer_gemm_launch when MER_GELU_PACKED=1): erf-GELU on value pairs through the
@@ -170,12 +172,126 @@ __device__ __forceinline__ void epi_tile(float (&acc)[NH][64], const MerGemmEpil
   }
 }
 
-template <int BLOCK_N, int MODE>
+// ---- TMA epilogue (outputs without residual or activation: the QKV form) ----
+// Output slots: 64 rows x 128 bytes (32 fp32 / 64 fp16 columns) in the 128B-swizzled layout of one TMA box, so a slot
+// is one cp.async.bulk.tensor store.  Slots come in pairs, one per consumer warpgroup; a warpgroup's u-th sub-tile
+// (u counts on across tiles) uses pair u % kSlotPairs.  The warpgroup waits only until a slot has been read out by its
+// previous store, never for the global write, so a tile's output traffic runs under the next tile's MMAs.
+constexpr int kSlotBytes = 64 * 128;
+constexpr int kSlotPairs = 2;
+
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the bulk stores committed before the last N groups have finished reading shared memory
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// named barrier over the 128 threads of consumer warpgroup wg (1 | 2); id 0 is __syncthreads
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg) : "memory"); }
+
+// epi_tile<NH, 0, OUT, false>'s arithmetic on one pair (bias, then the tf32 rounding of OUT == 1), in its order
+template <int OUT>
+__device__ __forceinline__ void epi_bias_round(float& v0, float& v1, const float* bias, int n) {
+  if (bias) {
+    const float2 q = __ldg(reinterpret_cast<const float2*>(bias + n));
+    v0 += q.x;
+    v1 += q.y;
+  }
+  if (OUT == 1) {
+    v0 = round_tf32(v0);
+    v1 = round_tf32(v1);
+  }
+}
+
+// TMA epilogue of one consumer warpgroup (OUT: 0 fp32, 1 TF32-rounded fp32, 3 fp16; no activation, no residual): the
+// same fragment and values as epi_tile<NH, 0, OUT, false>, but each 64 x (32 fp32 | 64 fp16) sub-tile is written into
+// a slot and stored by one thread with TMA, which clips rows past rows_per_batch.  Sub-tiles at or past vt_col0 (a
+// multiple of the sub-tile width) keep epi_tile's V^T stores and use no slot.  slots: this warpgroup's slot of pair 0;
+// q: slot uses so far.
+template <int NH, int OUT>
+__device__ __forceinline__ void epi_tile_tma(float (&acc)[NH][64], const MerGemmEpilogue& ep, const CUtensorMap* tmap_out,
+                                             uint8_t* slots, uint32_t& q, int n_base, int m_base, int b,
+                                             int rows_per_batch, long long out_row_b, int wg_row0, int wg) {
+  static_assert(OUT == 0 || OUT == 1 || OUT == 3, "fp32, tf32 or fp16 output");
+  constexpr int kEl = OUT == 3 ? 2 : 4;
+  constexpr int kCols = 128 / kEl;  // columns per slot
+  constexpr int kJ = kCols / 8;     // 8-column fragment groups per slot
+  constexpr int kSub = NH * 128 / kCols;
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int g = lane >> 2, t = lane & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+#pragma unroll
+  for (int s = 0; s < kSub; ++s) {
+    const int hh = s * kCols / 128, j0 = (s * kCols % 128) / 8;
+    const int n0 = n_base + s * kCols;
+    if (ep.vt != nullptr && n0 >= ep.vt_col0) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int m = m_base + wg_row0 + 16 * w + g + 8 * i;
+        if (m >= rows_per_batch) continue;
+        const long long orow = out_row_b + m;
+#pragma unroll
+        for (int jj = 0; jj < kJ; ++jj) {
+          const int n = n0 + 8 * jj + 2 * t;
+          float v0 = acc[hh][4 * (j0 + jj) + 2 * i], v1 = acc[hh][4 * (j0 + jj) + 2 * i + 1];
+          epi_bias_round<OUT>(v0, v1, ep.bias, n);
+          const long long vo = (long long)(n - ep.vt_col0) * ep.vt_ld + orow;
+          if (OUT == 3) {
+            uint16_t* vt16 = reinterpret_cast<uint16_t*>(ep.vt) + vo;
+            const uint32_t p = pack_f16x2(v0, v1);
+            vt16[0] = (uint16_t)(p & 0xffffu);
+            vt16[ep.vt_ld] = (uint16_t)(p >> 16);
+          } else {
+            ep.vt[vo] = v0;
+            ep.vt[vo + ep.vt_ld] = v1;
+          }
+        }
+      }
+      continue;
+    }
+    uint8_t* slot = slots + (q % kSlotPairs) * 2 * kSlotBytes;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = 16 * w + g + 8 * i;  // slot row; r % 8 == g
+#pragma unroll
+      for (int jj = 0; jj < kJ; ++jj) {
+        float v0 = acc[hh][4 * (j0 + jj) + 2 * i], v1 = acc[hh][4 * (j0 + jj) + 2 * i + 1];
+        epi_bias_round<OUT>(v0, v1, ep.bias, n0 + 8 * jj + 2 * t);
+        // byte (8 jj + 2 t) * kEl of the row, 16-byte chunks XOR-swizzled by r % 8
+        const int byte = (8 * jj + 2 * t) * kEl;
+        uint8_t* at = slot + r * 128 + ((((byte >> 4) ^ g) << 4) | (byte & 15));
+        if (OUT == 3) *reinterpret_cast<uint32_t*>(at) = pack_f16x2(v0, v1);
+        else *reinterpret_cast<float2*>(at) = make_float2(v0, v1);
+      }
+    }
+    fence_proxy_async();
+    // before the barrier: the slot of the NEXT use has been read out by its previous store
+    if (leader) bulk_wait_read<kSlotPairs - 2>();
+    wg_sync(wg);
+    if (leader) {
+      tma_store_3d(tmap_out, slot, n0, m_base + wg_row0, b);
+      bulk_commit();
+    }
+    ++q;
+  }
+}
+
+// TMA: the TMA epilogue (epi_tile_tma, for a descriptor without residual or activation) instead of epi_tile.  Two
+// kernels rather than a run-time switch, so that the register epilogue keeps its own code and register allocation.
+template <int BLOCK_N, int MODE, bool TMA>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
-            const __grid_constant__ CUtensorMap tmap_b, const MerGemmEpilogue ep,
+            const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_out,
+            const MerGemmEpilogue ep,
             int rows_per_batch, int batches, int N, int K, int K_inner, int P, int a_row0, int a_col_group) {
   using Cfg = GemmCfg<BLOCK_N, MODE>;
+  static_assert(Cfg::kSlotsBytes == 2 * kSlotPairs * kSlotBytes, "epilogue slot budget");
   constexpr int NH = BLOCK_N / 128;  // 64 x 128 accumulator blocks per consumer thread
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by OFFSET (not through an integer round trip) so the compiler keeps the
@@ -183,7 +299,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint8_t* slots = smem + Cfg::kStages * Cfg::kStageBytes;  // TMA: [pair][warpgroup] x kSlotBytes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(slots + (TMA ? Cfg::kSlotsBytes : 0));
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
 
@@ -199,6 +316,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if (TMA) tma_prefetch_desc(&tmap_out);
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full_bar[i], 1);                // the producer's expect-tx arrival
       mbar_init(&empty_bar[i], 4 * CONSUMERS);   // one arrival per consumer warp
@@ -266,6 +384,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const int kind = gelu_kind * 4 + out_kind;
   int stage = 0;
   uint32_t phase = 0;
+  uint32_t slot_uses = 0;  // TMA: this warpgroup's slot uses so far
   float acc[NH][64];
   for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
     const int n_blk = t % n_tiles;
@@ -316,6 +435,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const int m_base = mt * BLOCK_M;
     const long long out_row_b = (long long)b * ep.out_bstride + ep.out_row0;
     const long long res_row_b = (long long)b * ep.res_bstride + ep.res_row0;
+    if constexpr (TMA) {  // the host sends only fp32 / tf32 / fp16 outputs without residual or activation here
+      if (out_kind == 3)
+        epi_tile_tma<NH, 3>(acc, ep, &tmap_out, slots + (wg - 1) * kSlotBytes, slot_uses, n_base, m_base, b,
+                            rows_per_batch, out_row_b, wg_row0, wg);
+      else if (out_kind == 1)
+        epi_tile_tma<NH, 1>(acc, ep, &tmap_out, slots + (wg - 1) * kSlotBytes, slot_uses, n_base, m_base, b,
+                            rows_per_batch, out_row_b, wg_row0, wg);
+      else
+        epi_tile_tma<NH, 0>(acc, ep, &tmap_out, slots + (wg - 1) * kSlotBytes, slot_uses, n_base, m_base, b,
+                            rows_per_batch, out_row_b, wg_row0, wg);
+    } else {
 #define MER_EPI(G, O, R) epi_tile<NH, G, O, R>(acc, ep, n_base, m_base, rows_per_batch, out_row_b, res_row_b, wg_row0)
     if (ep.res != nullptr) {  // uniform across the kernel; each variant is straight-line code
       if (gelu_kind == 4) MER_EPI(4, 0, true);        // relu(acc + bias + res)
@@ -348,18 +478,41 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a,
       }
     }
 #undef MER_EPI
+    }
   }
+  if (TMA && (threadIdx.x & 127) == 0) bulk_wait_all();  // the last stores have landed before the CTA retires
 }
 
 // launches per kernel instantiation (tests assert that the variant a configuration is benchmarked on is the one a
 // parity test exercised): index = mode | (BLOCK_N == 256) << 2
 long long g_variant_launches[8] = {};
+// launches per epilogue: [0] register, [1] TMA
+long long g_epilogue_launches[2] = {};
+
+// Whether a launch takes the TMA epilogue: an fp32, tf32 or fp16 output without residual or activation (the QKV form;
+// measured on an H100, the residual and activation forms ran no faster through the slots, see DESIGN §7), the out base
+// (at out_row0) 16-byte aligned, its row and batch pitches multiples of 16 bytes and no narrower than N, and V^T (if
+// any) starting at a sub-tile boundary (32 fp32 / 64 fp16 columns).  MER_GEMM_EPI_TMA=0, read at every launch so that
+// both epilogues can be compared in one process, forces the register epilogue.
+bool use_tma_epilogue(const MerGemmDesc* g) {
+  const MerGemmEpilogue& ep = g->ep;
+  const char* e = getenv("MER_GEMM_EPI_TMA");
+  if ((e && *e && atoi(e) == 0) || ep.res ||
+      (ep.flags & (MER_EPI_SPLIT_BF16 | MER_EPI_GELU | MER_EPI_QUICK_GELU | MER_EPI_RELU | MER_EPI_GELU_TANH)))
+    return false;
+  const long long el = (ep.flags & MER_EPI_OUT_F16) ? 2 : 4;
+  if ((reinterpret_cast<uintptr_t>(ep.out) + ep.out_row0 * ep.ld_out * el) % 16 || ep.ld_out * el % 16 ||
+      ep.ld_out < g->N || (g->batches > 1 && ep.out_bstride * ep.ld_out * el % 16))
+    return false;
+  return ep.vt == nullptr || ep.vt_col0 % (128 / el) == 0;
+}
 
 template <int BLOCK_N, int MODE>
 int launch_gemm(const MerGemmDesc* g, cudaStream_t stream) {
   using Cfg = GemmCfg<BLOCK_N, MODE>;
   ++g_variant_launches[(MODE & 3) | (BLOCK_N == 256 ? 4 : 0)];
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, tout;
+  memset(&tout, 0, sizeof(tout));
   const CUtensorMapDataType dt = Cfg::kSplit ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                  : Cfg::kF16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                              : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -384,10 +537,26 @@ int launch_gemm(const MerGemmDesc* g, cudaStream_t stream) {
     const uint32_t box[2] = {(uint32_t)(Cfg::kBlockK * mult), BLOCK_N};
     if (int rc = mer_make_tmap(&tb, dt, 2, g->W, dims, strides, box, sw)) return rc;
   }
+  // TMA epilogue map: (columns, rows_per_batch, batches) over the output from out_row0; the row dimension is exactly
+  // rows_per_batch, so TMA clips the last row tile of every batch entry
+  const bool tma = use_tma_epilogue(g);
+  ++g_epilogue_launches[tma ? 1 : 0];
+  if (tma) {
+    const bool f16 = (g->ep.flags & MER_EPI_OUT_F16) != 0;
+    const uint64_t el = f16 ? 2 : 4, ld = (uint64_t)g->ep.ld_out * el;
+    const uint64_t dims[3] = {(uint64_t)g->N, (uint64_t)g->rows_per_batch, (uint64_t)g->batches};
+    const uint64_t strides[2] = {ld, g->batches > 1 ? (uint64_t)g->ep.out_bstride * ld : (uint64_t)g->rows_per_batch * ld};
+    const uint32_t box[3] = {(uint32_t)(128 / el), 64, 1};
+    if (int rc = mer_make_tmap(&tout, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
+                               reinterpret_cast<const char*>(g->ep.out) + g->ep.out_row0 * ld, dims, strides, box, sw))
+      return rc;
+  }
   static MerPerDevice attr_set;
   if (attr_set.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<BLOCK_N, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::kSmemBytes));
+    MER_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<BLOCK_N, MODE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        Cfg::smem_bytes(false)));
+    MER_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<BLOCK_N, MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        Cfg::smem_bytes(true)));
     attr_set.mark();
   }
   const int m_tiles = (g->rows_per_batch + BLOCK_M - 1) / BLOCK_M;
@@ -410,8 +579,9 @@ int launch_gemm(const MerGemmDesc* g, cudaStream_t stream) {
       if (e && atoi(e) == 1) ep.flags |= EPI_GELU_PACKED;
     }
   }
-  gemm_kernel<BLOCK_N, MODE><<<grid, NUM_THREADS, Cfg::kSmemBytes, stream>>>(
-      ta, tb, ep, g->rows_per_batch, g->batches, g->N, g->K_inner * g->taps, g->K_inner, g->P, g->a_row0,
+  (tma ? gemm_kernel<BLOCK_N, MODE, true> : gemm_kernel<BLOCK_N, MODE, false>)<<<grid, NUM_THREADS,
+                                                                                 Cfg::smem_bytes(tma), stream>>>(
+      ta, tb, tout, ep, g->rows_per_batch, g->batches, g->N, g->K_inner * g->taps, g->K_inner, g->P, g->a_row0,
       g->a_col_group);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
@@ -425,6 +595,11 @@ extern "C" long long mer_gemm_variant_launches(int block_n, int mode, int cluste
   if ((block_n != 128 && block_n != 256) || mode < 0 || mode > 2 || cluster < 1 || cluster > 2) return -1;
   if (cluster != 1 || twosm) return 0;  // sm_90 build: single-CTA tiles only
   return g_variant_launches[(mode & 3) | (block_n == 256 ? 4 : 0)];
+}
+
+extern "C" long long mer_gemm_epilogue_launches(int tma) {
+  if (tma != 0 && tma != 1) return -1;
+  return g_epilogue_launches[tma];
 }
 
 int mer_gemm_launch(const MerGemmDesc* g, cudaStream_t stream) {
