@@ -540,6 +540,13 @@ MER_API int mer_rope_f16(void* qkv16, long long ld, long long tokens, int heads,
 MER_API int mer_causal_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                                      const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
                                      void* stream);
+/* mer_causal_attention_f16 at head_dim 64, 96 or 128 (HF GPT2Attention: gpt2-chinese-cluecorpussmall at 64,
+ * Wenzhong2.0-GPT2-3.5B at 96): qkv16 [tokens, 3 * heads * head_dim], vt16 [heads * head_dim, vt_ld], ctx16 [tokens,
+ * heads * head_dim], scores scaled by 1 / sqrt(head_dim).  Any other head_dim returns an error before any launch.  At
+ * 128 it runs the same kernel as mer_causal_attention_f16. */
+MER_API int mer_causal_attention_hd_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
+                                        const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
+                                        int heads, int head_dim, void* stream);
 
 /* ---- pre-LayerNorm decoders with biases (BLOOM / OPT, extract_text_huggingface.py:170-196; orchestrated from the host
  * in mertools_b200/extract/ln_decoder_text.py over these, mer_gemm (MER_EPI_GELU_TANH, MER_EPI_RELU | MER_EPI_OUT_F16)

@@ -1,13 +1,16 @@
-// attention_causal.cu — causal softmax(Q K^T / sqrt(128)) V for packed variable-length sequences with head_dim 128:
-// the self-attention of HF LlamaAttention (eager / sdpa, is_causal) as the LLaMA text extractor runs it
-// (extract_text_huggingface.py:170-196 -> mertools_b200/extract/llama_text.py).
+// attention_causal.cu — causal softmax(Q K^T / sqrt(HD)) V for packed variable-length sequences: the self-attention of
+// HF LlamaAttention (eager / sdpa, is_causal) as the LLaMA text extractor runs it (extract_text_huggingface.py:170-196
+// -> mertools_b200/extract/llama_text.py) and of OPTAttention at head_dim HD = 128, and of GPT2Attention at HD = 64
+// (gpt2-chinese-cluecorpussmall) and 96 (Wenzhong2.0-GPT2-3.5B) (mertools_b200/extract/ln_decoder_text.py).  The
+// kernel is a template on HD; mer_causal_attention_f16 is the HD = 128 instance, mer_causal_attention_hd_f16 picks one
+// of the three at run time.
 //
 // Operands follow the fp16 V^T kernel of attention_f16.cu: q | k as fp16 rows of the QKV GEMM output
-// ([tokens, 3 * heads * 128], rotary embedding already applied by mer_rope_f16, V columns unused), V^T as the GEMM's
-// fp16 transposed side output ([heads * 128, vt_ld], vt[d, token]); ctx is written as fp16 rows for the fp16 o_proj
-// GEMM.  Flash-style: one CTA = (64-query block, head, sequence), 4 warps x 16 query rows, S = Q K^T and O += P V on
-// mma.sync.m16n8k16 (fp16 in, fp32 accumulate), P rounded to fp16, online-softmax statistics in fp32 registers.
-// K [64 keys][128 d] and V^T [128 d][64 keys] tiles are double-buffered in shared memory by cp.async.
+// ([tokens, 3 * heads * HD], rotary embedding already applied by mer_rope_f16 for LLaMA, V columns unused), V^T as the
+// GEMM's fp16 transposed side output ([heads * HD, vt_ld], vt[d, token]); ctx is written as fp16 rows for the fp16
+// o_proj GEMM.  Flash-style: one CTA = (64-query block, head, sequence), 4 warps x 16 query rows, S = Q K^T and
+// O += P V on mma.sync.m16n8k16 (fp16 in, fp32 accumulate), P rounded to fp16, online-softmax statistics in fp32
+// registers.  K [64 keys][HD d] and V^T [HD d][64 keys] tiles are double-buffered in shared memory by cp.async.
 //
 // Causal work: a query block stops at the key tile holding its last row; only tiles that cross the diagonal (or the
 // sequence start) are masked, and a warp whose 16 rows all lie before a tile skips that tile's MMAs.  Query blocks are
@@ -19,7 +22,7 @@
 // i and key j of a sequence is q_i . k_j / sqrt(128) + slope_h * (j - i), formed in fp32 before the row maximum, with i
 // and j counted from the sequence start (not the packed position).  HF adds slope_h * j; the per-row constant
 // slope_h * i cancels in the softmax, and with (j - i) <= 0 the bias stays bounded however long the row is.  Masked and
-// foreign keys stay -inf.  ALIBI = false is the LLaMA kernel, unchanged.
+// foreign keys stay -inf.  ALIBI = false is the LLaMA kernel, unchanged.  ALiBi is instantiated at HD = 128 only.
 #include "mer_common.cuh"
 #include "mer_kernels.h"
 
@@ -27,16 +30,20 @@ namespace {
 
 using namespace mer;
 
-constexpr int HD = 128;
 constexpr int BQ = 64;
 constexpr int BKV = 64;
 constexpr int THREADS = 128;
-// padded row pitches (fp16 elements): K rows 68 words, V^T rows 36 words -> conflict-free fragment loads
-constexpr int LDK = HD + 8;
+// Padded row pitches (fp16 elements).  A fragment load reads word t of row g (g < 8, t < 4): K rows are (HD + 8) / 2
+// words apart, i.e. 36 / 52 / 68 at head_dim 64 / 96 / 128, so the banks are 4g + t, 20g + t and 4g + t (mod 32), 32
+// distinct banks in each case; V^T rows are 36 words apart.
+template <int HD> constexpr int LDK = HD + 8;
 constexpr int LDV = BKV + 8;
-constexpr int K_TILE = BKV * LDK;
-constexpr int V_TILE = HD * LDV;
-constexpr int SMEM = 2 * (K_TILE + V_TILE) * 2;
+template <int HD> constexpr int K_TILE = BKV * LDK<HD>;
+template <int HD> constexpr int V_TILE = HD * LDV;
+template <int HD> constexpr int SMEM = 2 * (K_TILE<HD> + V_TILE<HD>) * 2;
+// log2(e) / sqrt(head_dim): the softmax runs in base 2 with the score scale folded in
+template <int HD> constexpr float SCALE_LOG2E =
+    (HD == 128 ? 0.08838834764831845f : HD == 96 ? 0.10206207261596575f : 0.125f) * 1.4426950408889634f;
 
 __device__ __forceinline__ void mma_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
@@ -54,14 +61,17 @@ __device__ __forceinline__ float fast_ex2(float x) {
   return y;
 }
 
-template <bool ALIBI>
+template <int HD, bool ALIBI>
 __global__ void __launch_bounds__(THREADS, 2)
 causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __restrict__ vt_, long long vt_ld,
                         uint16_t* __restrict__ ctx, const int* __restrict__ cu_seqlens, long long tokens, int heads,
                         const float* __restrict__ slopes) {
+  static_assert(HD == 64 || HD == 96 || HD == 128, "head_dim 64, 96 or 128");
+  static_assert(!ALIBI || HD == 128, "the ALiBi kernel is head_dim 128 only");
+  constexpr int LDK_ = LDK<HD>, K_TILE_ = K_TILE<HD>, V_TILE_ = V_TILE<HD>;
   extern __shared__ __align__(16) uint8_t smem_att[];
-  uint16_t* Ks = reinterpret_cast<uint16_t*>(smem_att);  // [2][BKV][LDK]
-  uint16_t* Vs = Ks + 2 * K_TILE;                         // [2][HD][LDV]: V^T, keys along the row
+  uint16_t* Ks = reinterpret_cast<uint16_t*>(smem_att);  // [2][BKV][LDK_]
+  uint16_t* Vs = Ks + 2 * K_TILE_;                        // [2][HD][LDV]: V^T, keys along the row
 
   const int seq = blockIdx.z, h = blockIdx.y;
   const int start = cu_seqlens[seq];
@@ -101,18 +111,20 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
 
   auto load_tile = [&](int j, int buf) {
     const int p0 = kstart + j * BKV;  // first key position (absolute token index) of the tile
-    uint16_t* kd = Ks + buf * K_TILE;
-    uint16_t* vd = Vs + buf * V_TILE;
+    uint16_t* kd = Ks + buf * K_TILE_;
+    uint16_t* vd = Vs + buf * V_TILE_;
 #pragma unroll
-    for (int i = 0; i < BKV * (HD / 8) / THREADS; ++i) {  // K: 64 rows x 16 chunks
+    for (int i = 0; i < BKV * (HD / 8) / THREADS; ++i) {  // K: 64 rows x HD / 8 chunks (4 / 6 / 8 per thread)
       const int idx = tid + i * THREADS;
-      const int r = idx >> 4, c = (idx & 15) * 8;
+      // chunk -> (row, column); shift and mask where HD / 8 is a power of two
+      const int r = HD == 96 ? idx / 12 : idx >> (HD == 128 ? 4 : 3);
+      const int c = (HD == 96 ? idx % 12 : idx & (HD / 8 - 1)) * 8;
       const int key = p0 + r;
       const bool kin = key >= start && key < start + len;
-      cp_async16(kd + r * LDK + c, kbase + (long long)(kin ? key : start) * ld + c, kin ? 16 : 0);
+      cp_async16(kd + r * LDK_ + c, kbase + (long long)(kin ? key : start) * ld + c, kin ? 16 : 0);
     }
 #pragma unroll
-    for (int i = 0; i < HD * (BKV / 8) / THREADS; ++i) {  // V^T: 128 rows x 8 chunks
+    for (int i = 0; i < HD * (BKV / 8) / THREADS; ++i) {  // V^T: HD rows x 8 chunks (4 / 6 / 8 per thread)
       const int idx = tid + i * THREADS;
       const int r = idx >> 3, c = (idx & 7) * 8;
       const long long vk = p0 + c;
@@ -123,7 +135,7 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
   };
 
   load_tile(0, 0);
-  constexpr float SL2 = 0.08838834764831845f * 1.4426950408889634f;  // 1/sqrt(128) * log2(e)
+  constexpr float SL2 = SCALE_LOG2E<HD>;
   // ALiBi bias in the units of the raw product q.k (the scale is folded into SL2): slope * sqrt(128) per key step, so
   // that zero slopes leave s, and the output, bit-identical to the plain kernel
   const float slope = ALIBI ? __ldg(slopes + h) * 11.313708498984761f : 0.f;
@@ -139,13 +151,13 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
     __syncthreads();
     const int rel0 = j * BKV - shift;  // key index inside the sequence of tile column 0
     if (rel0 <= warp_last) {           // otherwise every key of the tile is in this warp's future
-      const uint16_t* kt = Ks + buf * K_TILE;
-      const uint16_t* vt = Vs + buf * V_TILE;
+      const uint16_t* kt = Ks + buf * K_TILE_;
+      const uint16_t* vt = Vs + buf * V_TILE_;
       float s[BKV / 8][4];
 #pragma unroll
       for (int nt = 0; nt < BKV / 8; ++nt) {
         s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-        const uint32_t* w = reinterpret_cast<const uint32_t*>(kt + (nt * 8 + g) * LDK);
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(kt + (nt * 8 + g) * LDK_);
 #pragma unroll
         for (int ks = 0; ks < HD / 16; ++ks) mma_f16(s[nt], qa[ks], w[ks * 8 + t], w[ks * 8 + t + 4]);
       }
@@ -237,7 +249,7 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
   }
 }
 
-template <bool ALIBI>
+template <int HD, bool ALIBI>
 int launch_causal(const char* name, const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                   const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
                   const float* slopes, cudaStream_t stream) {
@@ -248,15 +260,14 @@ int launch_causal(const char* name, const void* qkv16, const void* vt16, long lo
               heads, n_seq);
   static MerPerDevice attr_set;
   if (attr_set.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(causal_attention_kernel<ALIBI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        SMEM));
+    MER_CUDA_CHECK(cudaFuncSetAttribute(causal_attention_kernel<HD, ALIBI>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM<HD>));
     attr_set.mark();
   }
   dim3 grid((max_seqlen + BQ - 1) / BQ, heads, n_seq);
-  causal_attention_kernel<ALIBI><<<grid, THREADS, SMEM, stream>>>(static_cast<const uint16_t*>(qkv16),
-                                                                  static_cast<const uint16_t*>(vt16), vt_ld,
-                                                                  static_cast<uint16_t*>(ctx16), cu_seqlens, tokens,
-                                                                  heads, slopes);
+  causal_attention_kernel<HD, ALIBI><<<grid, THREADS, SMEM<HD>, stream>>>(
+      static_cast<const uint16_t*>(qkv16), static_cast<const uint16_t*>(vt16), vt_ld, static_cast<uint16_t*>(ctx16),
+      cu_seqlens, tokens, heads, slopes);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
   return 0;
@@ -267,14 +278,33 @@ int launch_causal(const char* name, const void* qkv16, const void* vt16, long lo
 extern "C" int mer_causal_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                                         const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
                                         int heads, void* stream_) {
-  return launch_causal<false>("mer_causal_attention_f16", qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens,
-                              max_seqlen, heads, nullptr, static_cast<cudaStream_t>(stream_));
+  return launch_causal<128, false>("mer_causal_attention_f16", qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens,
+                                   max_seqlen, heads, nullptr, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int mer_causal_alibi_attention_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                                               const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
                                               int heads, const float* slopes, void* stream_) {
   MER_REQUIRE(slopes, "mer_causal_alibi_attention_f16: null slopes");
-  return launch_causal<true>("mer_causal_alibi_attention_f16", qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens,
-                             max_seqlen, heads, slopes, static_cast<cudaStream_t>(stream_));
+  return launch_causal<128, true>("mer_causal_alibi_attention_f16", qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq,
+                                  tokens, max_seqlen, heads, slopes, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int mer_causal_attention_hd_f16(const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
+                                           const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
+                                           int heads, int head_dim, void* stream_) {
+  const char* name = "mer_causal_attention_hd_f16";
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  MER_REQUIRE(head_dim == 64 || head_dim == 96 || head_dim == 128, "%s: head_dim %d (64, 96 or 128)", name, head_dim);
+  switch (head_dim) {
+    case 64:
+      return launch_causal<64, false>(name, qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens, max_seqlen, heads,
+                                      nullptr, stream);
+    case 96:
+      return launch_causal<96, false>(name, qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens, max_seqlen, heads,
+                                      nullptr, stream);
+    default:
+      return launch_causal<128, false>(name, qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens, max_seqlen, heads,
+                                       nullptr, stream);
+  }
 }

@@ -1,6 +1,8 @@
-"""BLOOM / OPT branch of the text extractor: the pre-LayerNorm decoder LLMs with biases among those the reference loads
-through plain ``AutoModel`` (MERBench/feature_extraction/text/extract_text_huggingface.py:170-172, ``bloom-7b1`` and
-``opt-13b``) and runs in fp16, one sentence per forward (:193-231).  Readout as for every text model:
+"""BLOOM / OPT / GPT-2 branch of the text extractor: the pre-LayerNorm decoder LLMs with biases among those the reference
+loads (MERBench/feature_extraction/text/extract_text_huggingface.py): ``bloom-7b1`` and ``opt-13b`` through plain
+``AutoModel`` (:170-172), run in fp16 (:193-196), and ``gpt2-chinese-cluecorpussmall`` (AutoModel, :188-190) and
+``wenzhong2-gpt2-chinese`` (GPT2Model, :167-169), run in fp32; one sentence per forward (:208-231).  Readout as for
+every text model:
 ``torch.stack(hidden_states)[[-4, -3, -2, -1]].sum(0)``, where the last term is the output of the final LayerNorm
 (``ln_f`` / ``final_layer_norm``) and the other three are raw residual states.
 
@@ -8,14 +10,19 @@ Both families are one orchestration (``LnDecoderNet``) over an ``ops`` backend, 
 - BLOOM: h[0] = word_embeddings_layernorm(E[ids]); causal attention with ALiBi (``mer_causal_alibi_attention_f16``),
   slopes from ``alibi_slopes``; tanh-GELU MLP (``MER_EPI_GELU_TANH``).  The fused ``query_key_value`` rows, interleaved
   per head as [head][q, k, v][128], are de-interleaved into q | k | v blocks at load time.
-- OPT: h[0] = E[ids] + P[pos + 2] (learned positions, offset 2); plain causal attention (``mer_causal_attention_f16``);
-  ReLU MLP (``MER_EPI_RELU | MER_EPI_OUT_F16``).
-``CudaOps``: fp16 weights and GEMM operands, fp32 biases, residual stream and readout, ``mer_layernorm_f16``.
+- OPT: h[0] = E[ids] + P[pos + 2] (learned positions, offset 2); plain causal attention (``mer_causal_attention_hd_f16``
+  at head_dim 128, the kernel of ``mer_causal_attention_f16``); ReLU MLP (``MER_EPI_RELU | MER_EPI_OUT_F16``).
+- GPT-2: h[0] = wte[ids] + wpe[pos] (+ wte[token_type_ids] when the tokenizer returns token types, as GPT2Model adds
+  them); plain causal attention at head_dim 64, 96 or 128 (``mer_causal_attention_hd_f16``); tanh-GELU MLP (gelu_new).
+  The Conv1D weights, stored [in, out], are transposed at load time; c_attn's columns are already q | k | v.
+``CudaOps``: fp16 weights and GEMM operands, fp32 biases, residual stream and readout, ``mer_layernorm_f16`` (for GPT-2
+too, whose reference run is fp32: its features are saved as float32).
 ``TorchOps``: plain torch in HF's order of operations (CPU tests, tests/test_ln_decoder_text.py).
 """
 from __future__ import annotations
 
 import math
+import re
 
 import numpy as np
 import torch
@@ -23,6 +30,8 @@ import torch
 from .llama_text import HEAD_DIM, _checkpoint_files, _iter_tensors
 
 OPT_POS_OFFSET = 2  # OPTLearnedPositionalEmbedding: position p reads row p + 2
+GPT2_HEAD_DIMS = (64, 96, 128)  # the instances of mer_causal_attention_hd_f16
+GPT2_CONV1D = ("attn.c_attn.weight", "attn.c_proj.weight", "mlp.c_fc.weight", "mlp.c_proj.weight")  # [in, out]
 
 
 # ---- configs --------------------------------------------------------------------------------------------------------
@@ -55,8 +64,26 @@ def check_ln_decoder_config(cfg):
         if getattr(cfg, "activation_function", "relu") != "relu":
             raise ValueError(f"OPT path: activation_function {cfg.activation_function!r} is not supported (relu only)")
         _head_check("OPT", cfg.num_attention_heads, cfg.hidden_size)
+    elif cfg.model_type == "gpt2":
+        act = getattr(cfg, "activation_function", "gelu_new")
+        if act not in ("gelu_new", "gelu_pytorch_tanh"):
+            raise ValueError(f"GPT-2 path: activation_function {act!r} is not supported (tanh GELU only)")
+        if not getattr(cfg, "scale_attn_weights", True):
+            raise ValueError("GPT-2 path: scale_attn_weights=False is not supported")
+        if getattr(cfg, "scale_attn_by_inverse_layer_idx", False):
+            raise ValueError("GPT-2 path: scale_attn_by_inverse_layer_idx=True is not supported")
+        if getattr(cfg, "add_cross_attention", False):
+            raise ValueError("GPT-2 path: add_cross_attention=True is not supported")
+        hidden, heads = cfg.hidden_size, cfg.num_attention_heads
+        if hidden % heads or hidden // heads not in GPT2_HEAD_DIMS:
+            raise ValueError(f"GPT-2 path: head_dim {hidden / heads:g} with {heads} heads and hidden {hidden} "
+                             f"(head_dim 64, 96 or 128 only)")
+        if hidden % 256:
+            raise ValueError(f"GPT-2 path: hidden size {hidden} is not a multiple of 256 (mer_layernorm_f16)")
+        if (cfg.n_inner or 4 * hidden) % 128:
+            raise ValueError(f"GPT-2 path: n_inner {cfg.n_inner} is not a multiple of 128")
     else:
-        raise ValueError(f"not a BLOOM / OPT config: model_type {cfg.model_type!r}")
+        raise ValueError(f"not a BLOOM / OPT / GPT-2 config: model_type {cfg.model_type!r}")
 
 
 def alibi_slopes(heads):
@@ -75,27 +102,33 @@ def alibi_slopes(heads):
 
 # ---- streaming checkpoint loader ------------------------------------------------------------------------------------
 def _strip(k, family):
-    """Parameter name of BloomModel (``h.0...``) / of OPTModel.decoder (``layers.0...``), or None to drop."""
+    """Parameter name of BloomModel / GPT2Model (``h.0...``) / of OPTModel.decoder (``layers.0...``), or None to drop:
+    lm_head, and the causal-mask buffers ``h.*.attn.bias`` / ``h.*.attn.masked_bias`` of older GPT-2 checkpoints."""
     if k.startswith("lm_head."):
         return None
-    for p in (("transformer.",) if family == "bloom" else ("model.", "decoder.")):
+    for p in (("model.", "decoder.") if family == "opt" else ("transformer.",)):
         if k.startswith(p):
             k = k[len(p):]
+    if family == "gpt2" and re.fullmatch(r"h\.\d+\.attn\.(bias|masked_bias)", k):
+        return None
     return k
 
 
 def load_ln_decoder_weights(model_dir, device, family):
-    """{name: fp16 tensor on ``device``} of a BLOOM (``family="bloom"``) or OPT (``"opt"``) checkpoint, read one
-    tensor at a time from safetensors or ``.bin`` shards (fp32 / fp16 / bf16).  Names lose the ``transformer.``
-    (BloomForCausalLM) or ``model.`` / ``decoder.`` (OPTForCausalLM / OPTModel) prefixes; ``lm_head`` is dropped.
-    A value that is not finite in fp16 is refused."""
+    """{name: fp16 tensor on ``device``} of a BLOOM (``family="bloom"``), OPT (``"opt"``) or GPT-2 (``"gpt2"``)
+    checkpoint, read one tensor at a time from safetensors or ``.bin`` shards (fp32 / fp16 / bf16).  Names lose the
+    ``transformer.`` (BloomForCausalLM, GPT2LMHeadModel) or ``model.`` / ``decoder.`` (OPTForCausalLM / OPTModel)
+    prefixes; ``lm_head`` and GPT-2's mask buffers are dropped.  GPT-2's Conv1D weights (GPT2_CONV1D, stored [in, out])
+    are transposed to the [out, in] of the other families.  A value that is not finite in fp16 is refused."""
     out = {}
     for path in _checkpoint_files(model_dir):
         for k, v in _iter_tensors(path):
             k = _strip(k, family)
             if k is None:
                 continue
-            t = v.to(device).to(torch.float16)
+            if family == "gpt2" and k.endswith(GPT2_CONV1D):
+                v = v.t()
+            t = v.to(device).to(torch.float16).contiguous()
             if not bool(torch.isfinite(t).all()):
                 raise ValueError(f"{path}: {k} is not finite in fp16")
             out[k] = t
@@ -111,12 +144,12 @@ def deinterleave_qkv(t, heads, head_dim=HEAD_DIM):
 
 # ---- layer orchestration --------------------------------------------------------------------------------------------
 class LnDecoderNet:
-    """Backend-agnostic BloomModel / OPTModel.decoder forward over packed sentences.  ``sd``: {name: tensor} as
-    load_ln_decoder_weights names them; entries are popped as the backend takes them over.  ``family``: "bloom" or
-    "opt".  ``ops``: weight, vector, embedding, embed, batch, layernorm, attention, linear_res, mlp, zeros_like, add_."""
+    """Backend-agnostic BloomModel / OPTModel.decoder / GPT2Model forward over packed sentences.  ``sd``: {name: tensor}
+    as load_ln_decoder_weights names and lays them out; entries are popped as the backend takes them over.  ``family``:
+    "bloom", "opt" or "gpt2".  ``ops``: weight, vector, embedding, embed, batch, layernorm, attention, linear_res, mlp, zeros_like, add_."""
 
     def __init__(self, sd, ops, family, n_layers, heads, eps, max_pos=None):
-        assert family in ("bloom", "opt") and n_layers >= 3, (family, n_layers)
+        assert family in ("bloom", "opt", "gpt2") and n_layers >= 3, (family, n_layers)
         self.ops, self.family, self.n_layers, self.heads, self.eps, self.max_pos = ops, family, n_layers, heads, eps, max_pos
         self.layers = []
         if family == "bloom":
@@ -138,6 +171,23 @@ class LnDecoderNet:
                     up=ops.weight(sd.pop(m + "dense_h_to_4h.weight")), b_up=ops.vector(sd.pop(m + "dense_h_to_4h.bias")),
                     down=ops.weight(sd.pop(m + "dense_4h_to_h.weight")),
                     b_down=ops.vector(sd.pop(m + "dense_4h_to_h.bias"))))
+            self.ln_f = (ops.vector(sd.pop("ln_f.weight")), ops.vector(sd.pop("ln_f.bias")))
+            self.act = "gelu_tanh"
+        elif family == "gpt2":
+            self.embed = ops.embedding(sd.pop("wte.weight"))
+            self.emb_ln = None
+            self.pos = ops.embedding(sd.pop("wpe.weight"))
+            self.slopes = None
+            for i in range(n_layers):
+                p = f"h.{i}."
+                a, m = p + "attn.", p + "mlp."
+                self.layers.append(dict(
+                    ln1=(ops.vector(sd.pop(p + "ln_1.weight")), ops.vector(sd.pop(p + "ln_1.bias"))),
+                    qkv=ops.weight(sd.pop(a + "c_attn.weight")), b_qkv=ops.vector(sd.pop(a + "c_attn.bias")),
+                    o=ops.weight(sd.pop(a + "c_proj.weight")), b_o=ops.vector(sd.pop(a + "c_proj.bias")),
+                    ln2=(ops.vector(sd.pop(p + "ln_2.weight")), ops.vector(sd.pop(p + "ln_2.bias"))),
+                    up=ops.weight(sd.pop(m + "c_fc.weight")), b_up=ops.vector(sd.pop(m + "c_fc.bias")),
+                    down=ops.weight(sd.pop(m + "c_proj.weight")), b_down=ops.vector(sd.pop(m + "c_proj.bias"))))
             self.ln_f = (ops.vector(sd.pop("ln_f.weight")), ops.vector(sd.pop("ln_f.bias")))
             self.act = "gelu_tanh"
         else:
@@ -162,19 +212,23 @@ class LnDecoderNet:
         self.hidden = self.embed.shape[1]
         assert not any(k.startswith(("h.", "layers.")) for k in sd), f"unused layer weights: {sorted(sd)[:4]}"
 
-    def forward(self, ids, lens, return_hidden=False):
-        """ids: int64 [tokens] of packed sentences with lengths ``lens``.  Returns the readout
+    def forward(self, ids, lens, return_hidden=False, token_types=None):
+        """ids: int64 [tokens] of packed sentences with lengths ``lens``; token_types: None or int64 [tokens] (GPT-2 adds
+        wte[token_types], as GPT2Model does when it is passed token_type_ids).  Returns the readout
         h[L-3] + h[L-2] + h[L-1] + ln_f(h[L]) [tokens, hidden] (fp32 on the CUDA backend) and, with return_hidden, the HF
         hidden_states tuple as a list."""
         ops, n = self.ops, self.n_layers
         if self.max_pos is not None and max(lens) > self.max_pos:
             raise ValueError(f"a sentence of {max(lens)} tokens exceeds max_position_embeddings {self.max_pos}")
         b = ops.batch(lens)
+        assert token_types is None or self.family == "gpt2", "token types are a GPT-2 input"
         if self.family == "bloom":
             x = ops.layernorm(ops.embed(self.embed, ids), *self.emb_ln, self.eps, out="f32")
         else:
-            pos = np.concatenate([np.arange(m) for m in lens]) + OPT_POS_OFFSET
+            pos = np.concatenate([np.arange(m) for m in lens]) + (OPT_POS_OFFSET if self.family == "opt" else 0)
             x = ops.embed(self.embed, ids) + ops.embed(self.pos, pos)
+            if token_types is not None:
+                x = x + ops.embed(self.embed, token_types)
         hs = [x.clone()] if return_hidden else None
         acc = ops.zeros_like(x)
         for i, L in enumerate(self.layers):
@@ -197,7 +251,8 @@ class LnDecoderNet:
 
 class TorchOps:
     """Plain torch backend (CPU tests, fp32 by default): the same orchestration on torch operators, HF's order of
-    operations (BloomAttention: baddbmm of alibi and q k^T / sqrt(128); OPTAttention: q scaled before the product)."""
+    operations (BloomAttention: baddbmm of alibi and q k^T / sqrt(128); OPTAttention: q scaled before the product;
+    GPT2Attention scales the product instead, a rounding difference only)."""
 
     def __init__(self, device="cpu", dtype=torch.float32):
         self.device, self.dtype = torch.device(device), dtype
@@ -227,17 +282,18 @@ class TorchOps:
         return y
 
     def attention(self, y, w_qkv, b_qkv, lens, heads, slopes):
-        D = heads * HEAD_DIM
+        D = w_qkv.shape[0] // 3
+        hd = D // heads
         qkv = y @ w_qkv.T + b_qkv
         ctx = torch.empty(y.shape[0], D, dtype=y.dtype, device=y.device)
         o = 0
         for n in lens:
-            q, k, v = (qkv[o:o + n, i * D:(i + 1) * D].view(n, heads, HEAD_DIM).transpose(0, 1) for i in range(3))
+            q, k, v = (qkv[o:o + n, i * D:(i + 1) * D].view(n, heads, hd).transpose(0, 1) for i in range(3))
             if slopes is not None:   # BLOOM: alibi.baddbmm(q, k^T, beta=1, alpha=1/sqrt(128)), alibi = slope * j
                 alibi = slopes[:, None, None] * torch.arange(n, device=y.device, dtype=slopes.dtype)[None, None, :]
-                sc = alibi.to(y.dtype) + (q @ k.transpose(1, 2)) * HEAD_DIM ** -0.5
-            else:                    # OPT: (q * 1/sqrt(128)) k^T
-                sc = (q * HEAD_DIM ** -0.5) @ k.transpose(1, 2)
+                sc = alibi.to(y.dtype) + (q @ k.transpose(1, 2)) * hd ** -0.5
+            else:                    # OPT / GPT-2: (q * 1/sqrt(head_dim)) k^T
+                sc = (q * hd ** -0.5) @ k.transpose(1, 2)
             sc = sc.masked_fill(torch.ones(n, n, dtype=torch.bool, device=y.device).triu(1), float("-inf"))
             p = torch.softmax(sc.to(torch.promote_types(sc.dtype, torch.float32)), dim=-1).to(y.dtype)
             ctx[o:o + n] = (p @ v).transpose(0, 1).reshape(n, D)
@@ -266,7 +322,7 @@ class CudaOps:
         self.L, self.device, self.timing = L, torch.device(device), None
         vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_longlong, C.c_float
         self._ln = L.declare("mer_layernorm_f16", [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp])
-        self._att = L.declare("mer_causal_attention_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, vp])
+        self._att = L.declare("mer_causal_attention_hd_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, i32, vp])
         self._att_alibi = L.declare("mer_causal_alibi_attention_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, vp, vp])
 
     def _run(self, klass, fn):
@@ -315,7 +371,7 @@ class CudaOps:
         return acc if acc is not None else (y16 if y16 is not None else y32)
 
     def attention(self, y, w_qkv, b_qkv, b, heads, slopes):
-        L, T, D = self.L, y.shape[0], heads * HEAD_DIM
+        L, T, D = self.L, y.shape[0], w_qkv.shape[0] // 3
         qkv = torch.empty(T, 3 * D, dtype=torch.float16, device=self.device)     # q | k rows (V columns unused)
         vt = torch.empty(D, (T + 7) // 8 * 8, dtype=torch.float16, device=self.device)
         self._run("gemm", lambda: L.gemm(y, w_qkv, qkv, bias=b_qkv, mode=L.MER_GEMM_F16, f16_out=True, vt=vt,
@@ -325,7 +381,7 @@ class CudaOps:
         if slopes is not None:
             self._run("attention", lambda: L.check(self._att_alibi(*args, L.ptr(slopes), L.stream_ptr())))
         else:  # OPT scales q by 1/sqrt(128) before q k^T; the kernel scales the product: a rounding difference only
-            self._run("attention", lambda: L.check(self._att(*args, L.stream_ptr())))
+            self._run("attention", lambda: L.check(self._att(*args, D // heads, L.stream_ptr())))
         return ctx
 
     def linear_res(self, a, w, bias, x):
@@ -347,17 +403,20 @@ def activation_bytes_per_token(hidden, ffn):
 
 
 def net_dims(cfg):
-    """(family, layers, heads, hidden, ffn, eps, max_pos) of a BLOOM / OPT config."""
+    """(family, layers, heads, hidden, ffn, eps, max_pos) of a BLOOM / OPT / GPT-2 config."""
     if cfg.model_type == "bloom":
         return ("bloom", cfg.num_hidden_layers, cfg.num_attention_heads, cfg.hidden_size, 4 * cfg.hidden_size,
                 float(cfg.layer_norm_epsilon), None)
+    if cfg.model_type == "gpt2":
+        return ("gpt2", cfg.n_layer, cfg.n_head, cfg.n_embd, cfg.n_inner or 4 * cfg.n_embd,
+                float(cfg.layer_norm_epsilon), int(cfg.n_positions))
     return ("opt", cfg.num_hidden_layers, cfg.num_attention_heads, cfg.hidden_size, cfg.ffn_dim, 1e-5,
             int(cfg.max_position_embeddings))
 
 
 class LnDecoderTextEncoder:
     """``forward(id_lists, start, end, want_tokens)`` (the contract TextExtractor drives) over ``LnDecoderNet`` with
-    the CUDA backend.  ``cfg``: the checkpoint's BloomConfig / OPTConfig; ``sd``: {name: tensor}
+    the CUDA backend.  ``cfg``: the checkpoint's BloomConfig / OPTConfig / GPT2Config; ``sd``: {name: tensor}
     (load_ln_decoder_weights)."""
 
     def __init__(self, sd, cfg, device="cuda"):
@@ -375,17 +434,22 @@ class LnDecoderTextEncoder:
         self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                                      C.c_void_p, C.c_void_p])
 
-    def forward(self, id_lists, start=0, end=None, want_tokens=False):
-        """id_lists: non-empty token id sequences.  Returns (utt [n, hidden] = mean over each sentence's kept range
-        [start : len + end], tokens [sum len, hidden] | None), fp32."""
+    def forward(self, id_lists, start=0, end=None, want_tokens=False, token_types=None):
+        """id_lists: non-empty token id sequences; token_types: None, or one int sequence per sentence (GPT-2).  When
+        None, the ``token_types`` attribute TokenTypeTextExtractor attaches to each id list is used if present.  Returns
+        (utt [n, hidden] = mean over each sentence's kept range [start : len + end], tokens [sum len, hidden] | None),
+        fp32."""
+        from .text import packed_token_types
         L = self._L
         lens = [len(x) for x in id_lists]
         assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
+        tt = packed_token_types(id_lists, token_types)
         if self.max_pos is not None and max(lens) > self.max_pos:
             raise ValueError(f"a sentence of {max(lens)} tokens exceeds max_position_embeddings {self.max_pos}")
         ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
         assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
-        acc = self.net.forward(ids, lens)
+        assert tt is None or (tt.min() >= 0 and tt.max() < self.vocab_size), "token type outside the vocabulary"
+        acc = self.net.forward(ids, lens, token_types=tt)
         cu = np.zeros(len(lens) + 1, np.int64)
         cu[1:] = np.cumsum(lens)
         seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)

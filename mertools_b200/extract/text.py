@@ -1,7 +1,8 @@
 """Lexical feature extraction — H100 mirror of
 MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; DeBERTa / DeBERTa-v2 through
 extract/deberta_text.py and XLNet through extract/xlnet_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
-extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU run).
+extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU run; GPT-2 through extract/ln_decoder_text.py,
+float32 like the reference's fp32 run of it).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
 model_dir)`` (:139), ``find_start_end_pos`` (:90-114) and the save-dir naming (:148-157).  Token ids
@@ -93,6 +94,39 @@ class TextExtractor:
                                     feature_level, self.enc.hidden) for i, r in enumerate(res)]
 
 
+class TokenIds(list):
+    """A sentence's token ids, with the ``token_type_ids`` the tokenizer returned next to them (None if it returned
+    none)."""
+    token_types = None
+
+
+class TokenTypeTextExtractor(TextExtractor):
+    """TextExtractor whose token id lists also carry the tokenizer's token_type_ids, so that the encoder adds the
+    token-type term exactly when ``model(**tokenizer(sentence))`` would: XLNet's segment term (transformers 4.x's
+    XLNetTokenizer returned them, 5.x only when the tokenizer config lists them in model_input_names) and GPT-2's
+    ``wte[token_type_ids]`` (BertTokenizer returns them, GPT2Tokenizer does not)."""
+
+    def tokenize(self, sentence):
+        out = self.tokenizer(sentence, return_tensors="pt")
+        ids = TokenIds(out["input_ids"][0].tolist())
+        if "token_type_ids" in out:
+            ids.token_types = out["token_type_ids"][0].tolist()
+        return ids
+
+
+def packed_token_types(id_lists, token_types=None):
+    """int64 [sum len] of the token types of packed id lists, or None: ``token_types`` (one sequence per id list) when
+    given, else the ``token_types`` TokenTypeTextExtractor attached to every id list (all or none of them)."""
+    if token_types is None:
+        found = [getattr(x, "token_types", None) for x in id_lists]
+        assert all(t is None for t in found) or all(t is not None for t in found), "token types for some only"
+        token_types = None if found[0] is None else found
+    if token_types is None:
+        return None
+    assert [len(t) for t in token_types] == [len(x) for x in id_lists], "one token type per token"
+    return np.concatenate([np.asarray(t, dtype=np.int64) for t in token_types])
+
+
 def _llama_extractor(model_name, model_dir, cfg, device):
     """The reference's LLM branch (:170-175, 193-196): LlamaModel + AutoTokenizer(use_fast=False), fp16 features.
     Tokens per launch: what half of the device memory left after the weights holds at the model's activation size."""
@@ -124,6 +158,30 @@ def _ln_decoder_extractor(model_dir, cfg, device):
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
 
 
+def _gpt2_extractor(model_name, model_dir, cfg, device):
+    """The reference's GPT-2 models: wenzhong2-gpt2-chinese as GPT2Model + GPT2Tokenizer(use_fast=False) (:167-169),
+    gpt2-chinese-cluecorpussmall through the AutoModel + AutoTokenizer(use_fast=False) branch (:188-190).  Neither is
+    halved there, so the features are fp32.  The extractor forwards the tokenizer's token_type_ids when it returns them
+    (gpt2-chinese's BertTokenizer does), as model(**inputs) does.  Tokens per launch as in _ln_decoder_extractor."""
+    import torch
+
+    from .ln_decoder_text import LnDecoderTextEncoder, check_ln_decoder_config, load_ln_decoder_weights
+    check_ln_decoder_config(cfg)  # before any weight is read
+    tokenizer = _gpt2_tokenizer(model_name, model_dir)
+    enc = LnDecoderTextEncoder(load_ln_decoder_weights(model_dir, device, "gpt2"), cfg, device=device)
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    tokens = int(min(16384, max(enc.max_pos, free // 2 // enc.bytes_per_token)))
+    return TokenTypeTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
+
+
+def _gpt2_tokenizer(model_name, model_dir):
+    """The tokenizer the reference loads for a GPT-2 model: GPT2Tokenizer for wenzhong2-gpt2-chinese, AutoTokenizer for
+    every other name (gpt2-chinese-cluecorpussmall's config names BertTokenizer), both with use_fast=False."""
+    from transformers import AutoTokenizer, GPT2Tokenizer
+    cls = GPT2Tokenizer if model_name == "wenzhong2-gpt2-chinese" else AutoTokenizer
+    return cls.from_pretrained(model_dir, use_fast=False)
+
+
 def _deberta_extractor(model_name, model_dir, cfg, device):
     """The reference's DeBERTa models (:164-166 and the AutoModel branch), fp32 features.  Tokenizer by model name as
     the reference loads it: BertTokenizer for deberta-chinese-large, AutoTokenizer(use_fast=False) otherwise.  Tokens per
@@ -150,13 +208,13 @@ def _xlnet_extractor(model_dir, cfg, device):
     import torch
     from transformers import AutoTokenizer
 
-    from .xlnet_text import MAX_LEN, XlnetTextEncoder, XlnetTextExtractor, check_xlnet_config
+    from .xlnet_text import MAX_LEN, XlnetTextEncoder, check_xlnet_config
     check_xlnet_config(cfg)  # before any weight is read
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = XlnetTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
     free, _ = torch.cuda.mem_get_info(enc.device)
     tokens = int(min(16384, max(MAX_LEN, free // 2 // enc.bytes_per_token)))
-    return XlnetTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
+    return TokenTypeTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
@@ -185,13 +243,15 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
     assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "xlnet", "llama", "bloom",
-                              "opt"), \
-        f"only BERT/RoBERTa/DeBERTa/XLNet encoders and LLaMA / BLOOM / OPT decoders are on the H100 path, got " \
+                              "opt", "gpt2"), \
+        f"only BERT/RoBERTa/DeBERTa/XLNet encoders and LLaMA / BLOOM / OPT / GPT-2 decoders are on the H100 path, got " \
         f"{cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("bloom", "opt"):
         ext = _ln_decoder_extractor(model_dir, cfg, f"cuda:{gpu}")
+    elif cfg.model_type == "gpt2":
+        ext = _gpt2_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("deberta", "deberta-v2"):
         ext = _deberta_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type == "xlnet":

@@ -31,7 +31,7 @@ import numpy as np
 import torch
 
 from .deberta_text import LN_DIMS, activation_bytes_per_token
-from .text import TextExtractor
+from .text import TokenIds, TokenTypeTextExtractor, packed_token_types  # noqa: F401  (TokenIds: re-exported)
 
 HEAD_DIM = 64
 MAX_LEN = 512   # tokens per sentence the launch sizing assumes (XLNet has no max_position_embeddings)
@@ -348,14 +348,7 @@ class XlnetTextEncoder:
         L = self._L
         lens = [len(x) for x in id_lists]
         assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
-        if token_types is None:
-            found = [getattr(x, "token_types", None) for x in id_lists]
-            assert all(t is None for t in found) or all(t is not None for t in found), "token types for some only"
-            token_types = None if found[0] is None else found
-        tt = None
-        if token_types is not None:
-            assert [len(t) for t in token_types] == lens, "one token type per token"
-            tt = np.concatenate([np.asarray(t, dtype=np.int64) for t in token_types])
+        tt = packed_token_types(id_lists, token_types)
         ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
         assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
         acc = self.net.forward(ids, lens, tt)
@@ -369,20 +362,4 @@ class XlnetTextEncoder:
         return utt, (acc if want_tokens else None)
 
 
-class TokenIds(list):
-    """A sentence's token ids, with the ``token_type_ids`` the tokenizer returned next to them (None if it returned
-    none)."""
-    token_types = None
-
-
-class XlnetTextExtractor(TextExtractor):
-    """TextExtractor whose token id lists also carry the tokenizer's token_type_ids, so that the encoder applies the
-    segment term exactly when ``model(**tokenizer(sentence))`` would: transformers 4.x's XLNetTokenizer returned them,
-    5.x returns them only when the tokenizer config lists them in model_input_names."""
-
-    def tokenize(self, sentence):
-        out = self.tokenizer(sentence, return_tensors="pt")
-        ids = TokenIds(out["input_ids"][0].tolist())
-        if "token_type_ids" in out:
-            ids.token_types = out["token_type_ids"][0].tolist()
-        return ids
+XlnetTextExtractor = TokenTypeTextExtractor   # the token-type hook, under its XLNet name

@@ -567,6 +567,39 @@ def opt_state_dict(seed=25, vocab=4000, hidden=512, ffn=2048, layers=6, max_pos=
     return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
 
 
+# The two GPT-2 checkpoints of tests/golden/gpt2_text_golden.npz, by the reference's model name: gpt2-chinese at head_dim
+# 64 over the BERT fixture vocabulary (tests/golden/text_vocab.txt), Wenzhong at head_dim 96 over the byte-level BPE of
+# tests/golden/opt_tokenizer.
+GPT2_GOLDEN_CFGS = {
+    "gpt2-chinese-cluecorpussmall": dict(seed=29, vocab=2629, hidden=256, heads=4, ffn=1024, layers=6, max_pos=1024),
+    "wenzhong2-gpt2-chinese": dict(seed=31, vocab=4000, hidden=768, heads=8, ffn=3072, layers=6, max_pos=1024),
+}
+
+
+def gpt2_state_dict(seed=29, vocab=2629, hidden=256, ffn=1024, layers=6, max_pos=1024, scale=1.0):
+    """Keys of ``transformers.GPT2Model`` with its Conv1D layout (c_attn / c_proj / c_fc weights [in, out]; c_attn's
+    columns q | k | v).  Values rounded to fp16 and stored as fp32 (as llama_state_dict); ``scale`` multiplies every
+    layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    g.normal("wte.weight", (vocab, hidden), 0.5)
+    g.normal("wpe.weight", (max_pos, hidden), 0.1)
+    std = 0.03 * scale
+
+    def conv1d(prefix, in_dim, out_dim):
+        g.normal(prefix + ".weight", (in_dim, out_dim), std)
+        g.normal(prefix + ".bias", (out_dim,), 0.02)
+    for i in range(layers):
+        p = f"h.{i}."
+        g.ln(p + "ln_1", hidden)
+        conv1d(p + "attn.c_attn", hidden, 3 * hidden)
+        conv1d(p + "attn.c_proj", hidden, hidden)
+        g.ln(p + "ln_2", hidden)
+        conv1d(p + "mlp.c_fc", hidden, ffn)
+        conv1d(p + "mlp.c_proj", ffn, hidden)
+    g.ln("ln_f", hidden)
+    return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
+
+
 # The two DeBERTa checkpoints of tests/golden/deberta_text_golden.npz: v1 as deberta-large (no absolute positions, c2p |
 # p2c over max_relative_positions, raw relative table) at base width; v2 as deberta-v2-xlarge (log buckets, LayerNorm'd
 # table, share_att_key, conv layer, no token types) at width 512.  HF config keywords.

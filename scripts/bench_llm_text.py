@@ -1,5 +1,5 @@
-"""Throughput of the decoder-LLM text-feature paths (LLaMA at 7 B and 13 B shapes; BLOOM-7B1 and OPT-13B on request)
-against the reference's loop.
+"""Throughput of the decoder-LLM text-feature paths (LLaMA at 7 B and 13 B shapes; BLOOM-7B1, OPT-13B and the two GPT-2
+models on request) against the reference's loop.
 
 Packed path: LlamaNet on the CUDA backend (fp16 weights and operands, fp32 residual), sentences packed back to back,
 up to --tokens per pass.  Reference loop (extract_text_huggingface.py:193-231): batch 1, one sentence per forward, fp16,
@@ -10,8 +10,12 @@ Chinese sentencepiece tokenizer (mean ~20 tokens, p99 ~53, capped at 128).  The 
 RMSNorm / RoPE / SwiGLU (LayerNorm for BLOOM / OPT) come from CUDA events around every launch, in a separate pass.
 ``bloom-7b1`` / ``opt-13b`` run LnDecoderNet (extract/ln_decoder_text.py) against HF BloomModel / OPTModel in fp16 at
 batch 1 (a 32000-token vocabulary here: the embedding gather is not part of the timed work that matters).
+``gpt2-chinese`` (gpt2-chinese-cluecorpussmall: 12 x 768, 12 heads of 64) and ``wenzhong-3.5b`` (Wenzhong2.0-GPT2-3.5B:
+30 x 3072, 32 heads of 96) run LnDecoderNet against HF GPT2Model at batch 1 in fp32, the precision the reference runs
+these two in: their speed-up includes fp16 against fp32.
 
-    python scripts/bench_llm_text.py [--shapes 7b,13b,bloom-7b1,opt-13b] [--sentences 1024] [--ref-sentences 64]
+    python scripts/bench_llm_text.py [--shapes 7b,13b,bloom-7b1,opt-13b,gpt2-chinese,wenzhong-3.5b] [--sentences 1024]
+        [--ref-sentences 64]
 """
 import argparse
 import json
@@ -30,7 +34,10 @@ from mertools_b200.extract import ln_decoder_text as LD  # noqa: E402
 SHAPES = {"7b": dict(hidden=4096, heads=32, ffn=11008, layers=32, eps=1e-6),
           "13b": dict(hidden=5120, heads=40, ffn=13824, layers=40, eps=1e-5),
           "bloom-7b1": dict(family="bloom", hidden=4096, heads=32, ffn=16384, layers=30, eps=1e-5),
-          "opt-13b": dict(family="opt", hidden=5120, heads=40, ffn=20480, layers=40, eps=1e-5)}
+          "opt-13b": dict(family="opt", hidden=5120, heads=40, ffn=20480, layers=40, eps=1e-5),
+          "gpt2-chinese": dict(family="gpt2", hidden=768, heads=12, ffn=3072, layers=12, eps=1e-5),
+          "wenzhong-3.5b": dict(family="gpt2", hidden=3072, heads=32, ffn=12288, layers=30, eps=1e-5)}
+MAX_POS = {"bloom": None, "opt": 2048, "gpt2": 1024}
 VOCAB = 32000
 
 
@@ -68,14 +75,15 @@ def random_weights(s, seed, dev):
 
 
 def ln_decoder_weights(s, w):
-    """BloomModel / OPTModel (decoder.*) keys, biases on every linear and LayerNorm."""
+    """BloomModel / OPTModel (decoder.*) / GPT2Model (Conv1D weights [in, out]) keys, biases on every linear and
+    LayerNorm."""
     D, F = s["hidden"], s["ffn"]
 
     def ln(p):
         return {p + ".weight": 1 + w(D, std=0.1), p + ".bias": w(D, std=0.1)}
 
-    def lin(p, o, i):
-        return {p + ".weight": w(o, i), p + ".bias": w(o)}
+    def lin(p, o, i):   # GPT-2's Conv1D: (p, in, out) -> weight [in, out]
+        return {p + ".weight": w(o, i), p + ".bias": w(i if s["family"] == "gpt2" else o)}
     sd = {}
     if s["family"] == "bloom":
         sd.update({"word_embeddings.weight": w(VOCAB, D, std=1.0), **ln("word_embeddings_layernorm"), **ln("ln_f")})
@@ -84,6 +92,12 @@ def ln_decoder_weights(s, w):
             sd.update({**ln(p + "input_layernorm"), **ln(p + "post_attention_layernorm"),
                        **lin(p + "self_attention.query_key_value", 3 * D, D), **lin(p + "self_attention.dense", D, D),
                        **lin(p + "mlp.dense_h_to_4h", F, D), **lin(p + "mlp.dense_4h_to_h", D, F)})
+    elif s["family"] == "gpt2":
+        sd.update({"wte.weight": w(VOCAB, D, std=1.0), "wpe.weight": w(MAX_POS["gpt2"], D, std=0.1), **ln("ln_f")})
+        for i in range(s["layers"]):
+            p = f"h.{i}."
+            sd.update({**ln(p + "ln_1"), **ln(p + "ln_2"), **lin(p + "attn.c_attn", D, 3 * D),
+                       **lin(p + "attn.c_proj", D, D), **lin(p + "mlp.c_fc", D, F), **lin(p + "mlp.c_proj", F, D)})
     else:
         sd.update({"decoder.embed_tokens.weight": w(VOCAB, D, std=1.0), "decoder.embed_positions.weight":
                    w(2050, D, std=0.1), **ln("decoder.final_layer_norm")})
@@ -97,7 +111,10 @@ def ln_decoder_weights(s, w):
 
 
 def hf_config(s):
-    from transformers import BloomConfig, LlamaConfig, OPTConfig
+    from transformers import BloomConfig, GPT2Config, LlamaConfig, OPTConfig
+    if s.get("family") == "gpt2":
+        return GPT2Config(vocab_size=VOCAB, n_positions=MAX_POS["gpt2"], n_embd=s["hidden"], n_layer=s["layers"],
+                          n_head=s["heads"], n_inner=s["ffn"], layer_norm_epsilon=s["eps"])
     if s.get("family") == "bloom":
         return BloomConfig(vocab_size=VOCAB, hidden_size=s["hidden"], n_head=s["heads"], n_layer=s["layers"])
     if s.get("family") == "opt":
@@ -125,27 +142,29 @@ def run_packed(net, ids, max_tokens):
 
 
 def reference_loop(s, sd, ids, dev):
-    """Batch-1 fp16 forwards with output_hidden_states and the last-four sum, as the reference script does."""
+    """Batch-1 forwards with output_hidden_states and the last-four sum, as the reference script does: fp16, except
+    GPT-2, which the reference does not halve."""
     try:
-        from transformers import BloomModel, LlamaModel, OPTModel
-        cls = {"bloom": BloomModel, "opt": OPTModel}.get(s.get("family"), LlamaModel)
+        from transformers import BloomModel, GPT2Model, LlamaModel, OPTModel
+        cls = {"bloom": BloomModel, "opt": OPTModel, "gpt2": GPT2Model}.get(s.get("family"), LlamaModel)
         cfg = hf_config(s)
         dt = torch.get_default_dtype()
-        torch.set_default_dtype(torch.float16)
+        ref_dtype = torch.float32 if s.get("family") == "gpt2" else torch.float16
+        torch.set_default_dtype(ref_dtype)
         try:
             with torch.device(dev):
                 m = cls(cfg).eval()
         finally:
             torch.set_default_dtype(dt)
         m.load_state_dict(sd, strict=True)
-        which = f"HF {cls.__name__} fp16"
+        which = f"HF {cls.__name__} {'fp32' if ref_dtype == torch.float32 else 'fp16'}"
         start = 0 if s.get("family") == "bloom" else 1
 
         def fwd(x):
             hs = m(torch.from_numpy(x)[None].to(dev), output_hidden_states=True).hidden_states
             return torch.stack(hs)[[-4, -3, -2, -1]].sum(0)[0, start:].cpu().numpy()
     except ImportError:
-        assert "family" not in s, "the BLOOM / OPT reference loop needs transformers"
+        assert "family" not in s, "the BLOOM / OPT / GPT-2 reference loop needs transformers"
         net = LT.LlamaNet(dict(sd), LT.TorchOps(dev, torch.float16), s["layers"], s["heads"], s["eps"], 10000.0, 4096)
         which = "torch restatement fp16 (transformers not importable)"
 
@@ -214,8 +233,10 @@ def main():
         ref_tok = sum(len(x) for x in ref_ids)
         if "family" in s:
             ops = LD.CudaOps(dev)
-            net = LD.LnDecoderNet({LD._strip(k, s["family"]): v for k, v in sd.items()}, ops, s["family"], s["layers"],
-                                  s["heads"], s["eps"], 2048 if s["family"] == "opt" else None)
+            conv1d = s["family"] == "gpt2"   # as load_ln_decoder_weights lays GPT-2's Conv1D weights out
+            net = LD.LnDecoderNet({LD._strip(k, s["family"]): (v.T if conv1d and k.endswith(LD.GPT2_CONV1D) else v)
+                                   for k, v in sd.items()}, ops, s["family"], s["layers"], s["heads"], s["eps"],
+                                  MAX_POS[s["family"]])
             linear_flops = 4 * s["hidden"] ** 2 + 2 * s["hidden"] * s["ffn"]
         else:
             ops = LT.CudaOps(dev)
@@ -249,7 +270,7 @@ def main():
         print(f"{shape}: packed {r['packed_sentences_per_s']:.1f} sentences/s, {r['packed_tokens_per_s']:.0f} tokens/s "
               f"({r['tflops']:.0f} TFLOP/s in the linears); reference loop ({which}) "
               f"{r['reference_sentences_per_s']:.2f} sentences/s, {r['reference_tokens_per_s']:.0f} tokens/s; "
-              f"x{r['speedup']:.1f}")
+              f"x{r['speedup']:.1f}" + (" (includes fp16 against the reference's fp32)" if "fp32" in which else ""))
         print(f"{shape}: time shares (per-launch events) " + ", ".join(f"{k} {v:.3f}" for k, v in r["shares"].items()))
         del net, ops
         torch.cuda.empty_cache()

@@ -1,7 +1,7 @@
 """Small launches of every hand-synchronised kernel family, for compute-sanitizer (scripts/sanitize.sh):
 the wgmma GEMM in its three operand modes and both tile widths, both V^T attention kernels
-on ragged batches, the LLaMA kernels (causal head-dim-128 attention, RoPE, RMSNorm, SwiGLU), the BLOOM / OPT
-kernels (ALiBi attention, wide LayerNorm, tanh-GELU / fp16 ReLU epilogues), LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
+on ragged batches, the LLaMA kernels (causal head-dim-128 attention, RoPE, RMSNorm, SwiGLU), the BLOOM / OPT / GPT-2
+kernels (ALiBi attention, causal attention at head_dim 64 / 96 / 128, wide LayerNorm, tanh-GELU / fp16 ReLU epilogues), LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
 fused fusion step (cluster kernel with DSMEM exchange + weight-gradient kernel).  Sizes are tiny: racecheck is slow."""
 import os
 import sys
@@ -86,8 +86,9 @@ def llama():
 
 
 def ln_decoders():
-    """The BLOOM / OPT kernels: causal attention with ALiBi on ragged rows with unaligned starts, the wide LayerNorm in
-    its three output modes, the tanh-GELU and fp16 ReLU GEMM epilogues, then a 3-layer LnDecoderNet forward per family."""
+    """The BLOOM / OPT / GPT-2 kernels: causal attention with ALiBi, and without at head_dim 64, 96 and 128, on ragged
+    rows with unaligned starts, the wide LayerNorm in its three output modes, the tanh-GELU and fp16 ReLU GEMM
+    epilogues, then a 3-layer LnDecoderNet forward per family."""
     from mertools_b200.extract import ln_decoder_text as LD
     heads, lens = 3, [5, 70, 1, 129, 17]
     tokens, D = sum(lens), heads * 128
@@ -99,6 +100,14 @@ def ln_decoders():
     ctx = torch.empty(tokens, D, dtype=torch.float16, device=dev)
     L.check(ops._att_alibi(L.ptr(qkv), L.ptr(vt), vt.shape[1], L.ptr(ctx), L.ptr(cu), len(lens), tokens, max(lens),
                            heads, L.ptr(LD.alibi_slopes(heads).to(dev)), L.stream_ptr()))
+    for hd in LD.GPT2_HEAD_DIMS:
+        Dh = heads * hd
+        qkv_h = torch.randn(tokens, 3 * Dh, device=dev).half()
+        vt_h = torch.zeros(Dh, (tokens + 7) // 8 * 8, dtype=torch.float16, device=dev)
+        vt_h[:, :tokens] = qkv_h[:, 2 * Dh:].T
+        L.check(ops._att(L.ptr(qkv_h), L.ptr(vt_h), vt_h.shape[1], L.ptr(torch.empty(tokens, Dh, dtype=torch.float16,
+                                                                                     device=dev)),
+                         L.ptr(cu), len(lens), tokens, max(lens), heads, hd, L.stream_ptr()))
     x = torch.randn(tokens, 512, device=dev)
     g, b = torch.ones(512, device=dev), torch.zeros(512, device=dev)
     ops.layernorm(x, g, b, 1e-5)
@@ -115,6 +124,9 @@ def ln_decoders():
     LD.LnDecoderNet(bsd, ops, "bloom", 3, 4, 1e-5).forward(ids, lens)
     osd = {LD._strip(k, "opt"): torch.from_numpy(v) for k, v in S.opt_state_dict(vocab=300, layers=3, max_pos=256).items()}
     LD.LnDecoderNet(osd, ops, "opt", 3, 4, 1e-5, 256).forward(ids, lens)
+    gsd = {LD._strip(k, "gpt2"): (torch.from_numpy(v).T if k.endswith(LD.GPT2_CONV1D) else torch.from_numpy(v))
+           for k, v in S.gpt2_state_dict(vocab=300, layers=3, max_pos=256).items()}
+    LD.LnDecoderNet(gsd, ops, "gpt2", 3, 4, 1e-5, 256).forward(ids, lens, token_types=np.zeros_like(ids))
     torch.cuda.synchronize()
     print("ln_decoders ok")
 
