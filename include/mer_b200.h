@@ -31,7 +31,8 @@ extern "C" {
 /* ---- library ------------------------------------------------------------------------- */
 MER_API const char* mer_last_error(void);
 MER_API int mer_abi_version(void); /* 4: model structs may only grow at the tail; zero-filled tails = the older behaviour */
-/* 0 when the current device is compute capability 10.x, non-zero (and an error string) otherwise */
+/* 0 when the current device is compute capability 9.0 (H100; the library holds sm_90a code only), non-zero (and an
+ * error string) otherwise */
 MER_API int mer_check_device(void);
 
 /* cumulative number of CUDA kernels this library has launched in this process (bench.py's
@@ -153,7 +154,9 @@ enum { MER_LN_ROUND_TF32 = 1, MER_LN_ACC_INIT = 2, MER_LN_ACC_ADD = 4,
  * MER_LN_ROUND_TF32) and y_split (bf16 hi|lo rows, the BF16X3 GEMM operand) are both optional;
  * at least one must be given.  Optional side buffer acc
  * (same shape): acc = y (ACC_INIT) or acc += y (ACC_ADD) — the "sum of the last four hidden
- * states" readout of extract_audio_huggingface.py:98 / extract_text_huggingface.py:226. */
+ * states" readout of extract_audio_huggingface.py:98 / extract_text_huggingface.py:226.  acc and y_split take the fp32
+ * value before y's tf32 / fp16 rounding; ACC_INIT wins over ACC_ADD; without either flag acc is not touched.  fp16
+ * outputs saturate at +-65504.  y == x and y_split == x are allowed (not an fp16 y); rows <= 0 is a no-op. */
 MER_API int mer_layernorm(const float* x, const float* gamma, const float* beta, float* y,
                           void* y_split, float* acc, long long rows, int dim, float eps, int flags,
                           void* stream);
@@ -166,12 +169,18 @@ MER_API int mer_round_tf32(float* x, long long n, void* stream);
  * Q | K | V column blocks, sequences packed back to back, cu_seqlens[n_seq+1] (device, int32),
  * tokens = cu_seqlens[n_seq] (host copy, sizes the TMA descriptors).  vt (optional): V^T, [heads*64,
  * vt_ld] with vt[d, token] = V[token, d] (vt_ld >= tokens, multiple of 4; of 8 for fp16), as written by mer_gemm's
- * transposed side output.  With vt and max_seqlen <= 253 the V^T kernel runs and the V columns of qkv are not
- * read; otherwise the kernel that reads V from qkv.
- * ctx is [tokens, heads*64].  flags: MER_EPI_ROUND_TF32 rounds ctx for a TF32 out-proj GEMM,
- * MER_EPI_SPLIT_BF16 writes ctx as bf16 hi|lo rows for a BF16X3 out-proj GEMM, MER_EPI_OUT_F16 writes
- * ctx as fp16 for an F16 out-proj GEMM (V^T kernels only); with MER_ATT_QKV_F16 the inputs are
- * fp16 as well (attention_f16.cu: fp16 MMAs, half the traffic; up to 505 tokens).
+ * transposed side output.  Three routes, chosen from flags, vt and max_seqlen (not from the lengths in cu_seqlens):
+ *  1. MER_ATT_QKV_F16: qkv and vt are fp16 (attention_f16.cu: fp16 MMAs, half the traffic); vt is required and
+ *     max_seqlen <= 505, anything else is refused.  ctx in any of the four forms below.
+ *  2. fp32 qkv, vt given and max_seqlen <= 253: the tf32 V^T kernel; the V columns of qkv are not read.  ctx in any of
+ *     the four forms.
+ *  3. fp32 qkv otherwise (no vt, or max_seqlen >= 254; every call when the environment variable MER_ATTENTION_LEGACY
+ *     is set at the first call): the kernel that reads V from qkv (attention.cu), any length; vt is not read.
+ *     ctx fp32, tf32-rounded or split; MER_EPI_OUT_F16 is refused.
+ * ctx is [tokens, heads*64].  flags: none = fp32; MER_EPI_ROUND_TF32 rounds ctx for a TF32 out-proj GEMM;
+ * MER_EPI_SPLIT_BF16 writes ctx as bf16 hi|lo rows for a BF16X3 out-proj GEMM; MER_EPI_OUT_F16 writes ctx as fp16 for
+ * an F16 out-proj GEMM (OUT_F16 wins over SPLIT_BF16, which wins over ROUND_TF32).  n_seq <= 65535, heads <= 65535;
+ * on route 3 n_seq <= 0 or max_seqlen <= 0 is a no-op and the rows of a sequence beyond max_seqlen are not written.
  * Replaces HF eager/sdpa attention (modeling_vit.py:171-196, modeling_hubert.py:262-345). */
 MER_API int mer_attention(const float* qkv, const float* vt, long long vt_ld, float* ctx,
                           const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
@@ -443,7 +452,8 @@ typedef struct MerHubertModel {
 
 /* per-row zero-mean / unit-variance (eps 1e-7) of HF Wav2Vec2FeatureExtractor(do_normalize=True)
  * (feature_extraction_wav2vec2.py:78-97), as called at extract_audio_huggingface.py:94.
- * in/out: fp32 [batch, n_samples] with row pitches ld_in / ld_out (floats). */
+ * in/out: fp32 [batch, n_samples] with row pitches ld_in / ld_out (floats, each >= n_samples; a shorter pitch is
+ * refused).  Mean and variance are taken in double; a row of variance 0 (and any row of one sample) comes out as zeros. */
 MER_API int mer_wave_normalize(const float* in, float* out, int batch, int n_samples, long long ld_in,
                                long long ld_out, void* stream);
 

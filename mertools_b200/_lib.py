@@ -28,6 +28,7 @@ MER_ATT_QKV_F16 = 32
 MER_LN_ROUND_TF32 = 1
 MER_LN_ACC_INIT = 2
 MER_LN_ACC_ADD = 4
+MER_LN_GELU = 16
 MER_LN_SPLIT_F16 = 32
 
 
@@ -221,6 +222,70 @@ def attention(qkv, ctx, cu_seqlens, max_seqlen, heads, round_out=False, vt=None,
         return ctx
     check(lib().mer_attention(ptr(qkv), ptr(vt), vt.shape[1] if vt is not None else 0, ptr(ctx),
                               ptr(cu_seqlens), cu_seqlens.numel() - 1, qkv.shape[0], max_seqlen, heads,
-                              MER_EPI_OUT_F16 if f16_out else (MER_EPI_ROUND_TF32 if round_out else 0),
+                              MER_EPI_OUT_F16 if f16_out else
+                              (MER_EPI_SPLIT_BF16 if split_out else (MER_EPI_ROUND_TF32 if round_out else 0)),
                               stream_ptr()))
     return ctx
+
+
+def last_error() -> str:
+    return lib().mer_last_error().decode(errors="replace")
+
+
+def launch_count() -> int:
+    f = lib().mer_launch_count
+    f.restype, f.argtypes = C.c_longlong, []
+    return int(f())
+
+
+def segment_reduce(x, begins, ends, out, *, dim, mean=False, n_seg=None):
+    """out[s] = sum | mean of the rows x[begins[s] : ends[s]] (begins / ends: int32 CUDA tensors)."""
+    f = declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                       C.c_void_p])
+    check(f(ptr(x), ptr(begins), ptr(ends), begins.numel() if n_seg is None else n_seg, dim, 1 if mean else 0,
+            ptr(out), stream_ptr()))
+    return out
+
+
+def wave_normalize(x, out, *, batch, n_samples, ld_in, ld_out):
+    f = declare("mer_wave_normalize", [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_longlong, C.c_longlong,
+                                       C.c_void_p])
+    check(f(ptr(x), ptr(out), batch, n_samples, ld_in, ld_out, stream_ptr()))
+    return out
+
+
+def wavlm_gate(x, w, b, c, gate, *, tokens, heads):
+    f = declare("mer_wavlm_gate", [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p])
+    check(f(ptr(x), tokens, heads, ptr(w), ptr(b), ptr(c), ptr(gate), stream_ptr()))
+    return gate
+
+
+def biased_attention(qkv, bias, rowscale, ctx, *, batch, T, heads, round_out=False):
+    f = declare("mer_biased_attention", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                         C.c_int, C.c_void_p])
+    check(f(ptr(qkv), ptr(bias), ptr(rowscale), batch, T, heads, ptr(ctx), 1 if round_out else 0, stream_ptr()))
+    return ctx
+
+
+def small_attention(q, k, v, out, *, ld_q, ld_k, ld_v, ld_out, batch, heads, nq, nk, causal=False):
+    """q / k / v / out may be views into wider buffers: their data pointers carry the column offset."""
+    f = declare("mer_small_attention", [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                        C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p])
+    check(f(ptr(q), ld_q, ptr(k), ld_k, ptr(v), ld_v, batch, heads, nq, nk, 1 if causal else 0, ptr(out), ld_out,
+            stream_ptr()))
+    return out
+
+
+def swiglu(x, out, *, rows, hidden, round_out=False):
+    f = declare("mer_swiglu", [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_void_p])
+    check(f(ptr(x), ptr(out), rows, hidden, 1 if round_out else 0, stream_ptr()))
+    return out
+
+
+def videomae_patchify(frames, mean, std, out, *, n_clips):
+    """frames: uint8 CUDA tensor [n_clips * 16, 224, 224, 3] (BGR); mean / std: three host floats each (RGB)."""
+    f = declare("mer_videomae_patchify", [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p,
+                                          C.c_void_p])
+    check(f(ptr(frames), n_clips, (C.c_float * 3)(*mean), (C.c_float * 3)(*std), ptr(out), stream_ptr()))
+    return out

@@ -330,6 +330,9 @@ conv0_ln_kernel(const float* __restrict__ wave, long long ld_wave, const float* 
 int mer_wave_normalize_launch(const float* in, float* out, int B, int L, long long ld_in,
                               long long ld_out, cudaStream_t stream, const int* lengths) {
   MER_REQUIRE(in && out && B > 0 && L > 0, "mer_wave_normalize: bad arguments");
+  // a pitch below the row length would make row b + 1 start inside row b: the rows' outputs would overwrite each other
+  MER_REQUIRE(ld_in >= L && ld_out >= L, "mer_wave_normalize: row pitches %lld / %lld shorter than the %d samples of a row",
+              ld_in, ld_out, L);
   if (lengths)
     wave_normalize_ragged_kernel<<<B, 1024, 0, stream>>>(in, out, lengths, L, ld_in, ld_out);
   else

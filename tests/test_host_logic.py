@@ -768,11 +768,8 @@ class _TorchVideoMaeOps(_TorchWhisperOps):
     (rows = (clip, tubelet, patch row, patch column); K = (channel RGB, frame-in-tubelet, dy, dx))."""
 
     def patchify(self, frames, mean, std):
-        n = frames.shape[0] // 16
-        x = torch.from_numpy(np.ascontiguousarray(np.asarray(frames)[..., ::-1])).float() / 255.0
-        x = (x - torch.tensor(mean)) / torch.tensor(std)                              # [n*16, 224, 224, 3] RGB
-        x = x.reshape(n, 8, 2, 14, 16, 14, 16, 3).permute(0, 1, 3, 5, 7, 2, 4, 6)    # n, tt, py, px, c, dt, dy, dx
-        return x.reshape(n * 1568, 1536)
+        from _kernel_refs import videomae_patches   # the one definition, shared with the kernel's own GPU test
+        return videomae_patches(torch.from_numpy(np.ascontiguousarray(np.asarray(frames))), mean, std).float()
 
     def layernorm(self, x, g, b, operand, eps=1e-5):
         return torch.nn.functional.layer_norm(x, (x.shape[-1],), g, b, eps)
