@@ -148,9 +148,15 @@ MER_API int mer_split_bf16(const float* in, void* out, long long rows, int K, vo
 enum { MER_LN_ROUND_TF32 = 1, MER_LN_ACC_INIT = 2, MER_LN_ACC_ADD = 4,
        MER_LN_OUT_F16 = 8, /* y is an fp16 array (the MER_GEMM_F16 operand) */
        MER_LN_GELU = 16,   /* GELU(erf) after the affine (HubertLayerNormConvLayer) */
-       MER_LN_SPLIT_F16 = 32 /* y_split is an fp16 array (the MER_GEMM_F16 operand) written NEXT TO the fp32 y:
-                                the post-LN stacks keep y as their residual stream */ };
-/* y = LayerNorm(x) * gamma + beta over the last dim (512, 768, 1024, 1280 or 1536).  y (fp32, tf32-rounded when
+       MER_LN_SPLIT_F16 = 32, /* y_split is an fp16 array (the MER_GEMM_F16 operand) written NEXT TO the fp32 y:
+                                the post-LN stacks keep y as their residual stream */
+       MER_LN_PAD = 64 /* dim is the valid width of rows padded to the next multiple of 128 (x, y, y_split, acc, gamma
+                          and beta all have the padded width): mean and variance over the first dim columns only, and
+                          every output (y, y_split, acc) is written as exactly 0 in the pad columns, whatever x, gamma
+                          and beta hold there (albert_chinese_tiny: 312 valid columns in 384).  Always the default
+                          (round-2) kernel form. */ };
+/* y = LayerNorm(x) * gamma + beta over the last dim (128, 384, 512, 768, 1024, 1280 or 1536; with MER_LN_PAD, any dim
+ * whose next multiple of 128 is one of them).  y (fp32, tf32-rounded when
  * MER_LN_ROUND_TF32) and y_split (bf16 hi|lo rows, the BF16X3 GEMM operand) are both optional;
  * at least one must be given.  Optional side buffer acc
  * (same shape): acc = y (ACC_INIT) or acc += y (ACC_ADD) — the "sum of the last four hidden
@@ -185,6 +191,19 @@ MER_API int mer_round_tf32(float* x, long long n, void* stream);
 MER_API int mer_attention(const float* qkv, const float* vt, long long vt_ld, float* ctx,
                           const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen,
                           int heads, int flags, void* stream);
+/* mer_attention's V^T route (routes 1 and 2) at head_dim 32 or 64 with an explicit score scale: softmax(scale Q K^T) V
+ * (HF AlbertSdpaAttention / eager attention: scale 1 / sqrt(hidden / heads)).  qkv [tokens, 3 * heads * head_dim] with
+ * Q | K column blocks (V columns not read), vt [heads * head_dim, vt_ld] (vt_ld >= tokens, multiple of 8 for fp16 / 4
+ * for fp32), ctx [tokens, heads * head_dim].  flags: MER_ATT_QKV_F16 (fp16 qkv / vt) or none (tf32-rounded fp32), plus
+ * MER_EPI_OUT_F16 / MER_EPI_SPLIT_BF16 / MER_EPI_ROUND_TF32 for ctx as in mer_attention.  Rows of up to 512 tokens, on
+ * both operand formats.  A head zero-padded to 32 columns (ALBERT's 26) gives the unpadded result when scale is that of
+ * the unpadded head, and zero ctx in the pad columns.  head_dim 64 at scale 0.125 runs what mer_attention runs for rows
+ * it accepts (bit for bit).  Refused before any launch with a "mer_attention_hd:" message: head_dim other than 32 / 64,
+ * scale outside (0, 1] or NaN, a NULL operand, other flags, a V^T pitch that is too small or misaligned, max_seqlen
+ * outside 1 .. min(512, tokens), heads or n_seq outside 1 .. 65535.  attention_f16.cu. */
+MER_API int mer_attention_hd(const void* qkv, const void* vt, long long vt_ld, void* ctx, const int32_t* cu_seqlens,
+                             int n_seq, long long tokens, int max_seqlen, int heads, int head_dim, float scale,
+                             int flags, void* stream);
 
 /* ---- segment reduce (readouts) ------------------------------------------------------------ */
 enum { MER_SEG_SUM = 0, MER_SEG_MEAN = 1 };

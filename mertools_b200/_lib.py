@@ -30,6 +30,7 @@ MER_LN_ACC_INIT = 2
 MER_LN_ACC_ADD = 4
 MER_LN_GELU = 16
 MER_LN_SPLIT_F16 = 32
+MER_LN_PAD = 64
 
 
 class MerError(RuntimeError):

@@ -1,5 +1,6 @@
 // attention_f16.cu — softmax(Q K^T / 8) V for packed variable-length sequences (head_dim 64) that reads V
 // transposed: the form the QKV GEMM epilogue writes (V^T [heads*64, vt_ld], vt[d, token], keys contiguous).
+// mer_attention_hd runs the same kernel at head_dim 32 and with the score scale as an argument (ALBERT).
 //
 // Two operand formats share one flash-style kernel:
 //   fp16 : q | k fp16 rows of qkv16, fp16 V^T; S = Q K^T and O += P V on mma.sync.m16n8k16 (fp16 in, fp32
@@ -26,20 +27,23 @@ namespace {
 
 using namespace mer;
 
-constexpr int HD = 64;
 constexpr int BQ = 64;
 constexpr int BKV = 64;
 constexpr int THREADS = 128;
 constexpr int MAX_SEQ = 505;  // longest sequence the stacks send here (10 s audio rows, CLIP L/14)
+constexpr int MAX_SEQ_HD = 512;  // mer_attention_hd: ALBERT's position table
 
-template <bool F16>
+template <bool F16, int HD>
 struct AttCfg {
   static constexpr int kElem = F16 ? 2 : 4;
   static constexpr int kPerChunk = 16 / kElem;  // elements per 16-byte copy
-  // padded row pitch in elements: conflict-free fragment loads (fp16: 36 words, tf32: 68 words per row)
-  static constexpr int kLds = F16 ? 72 : 68;
-  static constexpr int kTile = BKV * kLds;  // elements of one K (or V^T) tile
-  static constexpr int kSmem = 2 * 2 * kTile * kElem;
+  // padded row pitches in elements: conflict-free fragment loads.  K rows (HD wide) are 36 (HD 64) / 20 (HD 32) words
+  // apart for fp16 and 68 / 36 for tf32; V^T rows (64 keys wide) are 36 (fp16) / 68 (tf32) words apart at every HD.
+  static constexpr int kLdsV = F16 ? 72 : 68;
+  static constexpr int kLdsK = HD == 64 ? kLdsV : (F16 ? 40 : 36);
+  static constexpr int kTileK = BKV * kLdsK;  // elements of one K tile
+  static constexpr int kTileV = HD * kLdsV;   // elements of one V^T tile
+  static constexpr int kSmem = 2 * (kTileK + kTileV) * kElem;
 };
 
 __device__ __forceinline__ void mma_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -64,17 +68,29 @@ __device__ __forceinline__ float fast_ex2(float x) {
   return y;
 }
 
-// out_mode: 0 fp32, 1 tf32-rounded fp32, 2 bf16 hi | lo split rows, 3 fp16
-template <bool F16>
+// scale * log2(e): 1/8 (head_dim 64) as a compile-time constant when the kernel has no scale argument, else the argument
+template <typename... S>
+__device__ __forceinline__ float score_l2(S... sl2) {
+  if constexpr (sizeof...(S) == 0) return 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+  else return (sl2 + ...);
+}
+
+// out_mode: 0 fp32, 1 tf32-rounded fp32, 2 bf16 hi | lo split rows, 3 fp16.  sl2: empty (scores scaled by 1/8), or one
+// float, scale * log2(e) (mer_attention_hd).  The scale is an empty pack rather than a default argument so that the
+// head_dim-64 instances mer_attention runs keep their parameter list and code.
+template <bool F16, int HD = 64, typename... S>
 __global__ void __launch_bounds__(THREADS, 3)
 attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_, long long vt_ld, void* __restrict__ ctx,
-                    const int* __restrict__ cu_seqlens, long long tokens, int heads, int out_mode) {
-  using Cfg = AttCfg<F16>;
+                    const int* __restrict__ cu_seqlens, long long tokens, int heads, int out_mode, S... sl2) {
+  static_assert(HD == 32 || HD == 64, "head_dim 32 or 64");
+  using Cfg = AttCfg<F16, HD>;
   using T = typename std::conditional<F16, uint16_t, float>::type;
-  constexpr int LDS = Cfg::kLds;
+  // (V^T rows are Cfg::kLdsV apart: a local constexpr for it reorders the front end's output, and the head_dim-64
+  // instances are meant to keep their SASS)
+  constexpr int LDS = Cfg::kLdsK;   // K rows
   extern __shared__ __align__(16) uint8_t smem_att[];
   T* Ks = reinterpret_cast<T*>(smem_att);  // [2][BKV][LDS]
-  T* Vs = Ks + 2 * Cfg::kTile;             // [2][HD][LDS]: V^T, keys along the row
+  T* Vs = Ks + 2 * Cfg::kTileK;            // [2][HD][Cfg::kLdsV]: V^T, keys along the row
 
   const int seq = blockIdx.z, h = blockIdx.y;
   const int start = cu_seqlens[seq];
@@ -92,7 +108,7 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
   const T* vtbase = static_cast<const T*>(vt_) + (long long)h * HD * vt_ld;
 
   // ---- Q fragments ----
-  constexpr int QK_STEPS = F16 ? 4 : 8;  // k-steps over head_dim
+  constexpr int QK_STEPS = F16 ? HD / 16 : HD / 8;  // k-steps over head_dim
   uint32_t qa[QK_STEPS][4];
   {
     const T* q_lo = qbase + (long long)min(q0 + warp * 16 + g, len - 1) * ld;
@@ -112,34 +128,54 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
     }
   }
 
-  float o[8][4];
+  float o[HD / 8][4];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  for (int i = 0; i < HD / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
   const int n_kv = (shift + len + BKV - 1) / BKV;
 
   auto load_tile = [&](int j, int buf) {
     const int p0 = kstart + j * BKV;  // first key position (absolute token index) of the tile
-    T* kd = Ks + buf * Cfg::kTile;
-    T* vd = Vs + buf * Cfg::kTile;
-    constexpr int CPR = HD / Cfg::kPerChunk;  // 16-byte chunks per 64-element row
+    T* kd = Ks + buf * Cfg::kTileK;
+    T* vd = Vs + buf * Cfg::kTileV;
+    if constexpr (HD == BKV) {
+      constexpr int CPR = HD / Cfg::kPerChunk;  // 16-byte chunks per 64-element row
 #pragma unroll
-    for (int i = 0; i < BKV * CPR / THREADS; ++i) {
-      const int idx = tid + i * THREADS;
-      const int r = idx / CPR, c = (idx % CPR) * Cfg::kPerChunk;
-      // K row r = key p0 + r (zero outside the sequence); V^T row r = head dim r, keys p0 + c ..
-      const int key = p0 + r;
-      const bool kin = key >= start && key < start + len;
-      cp_async16(kd + r * LDS + c, kbase + (long long)(kin ? key : start) * ld + c, kin ? 16 : 0);
-      const long long vk = p0 + c;
-      const int vbytes = vk >= tokens ? 0 : (int)min(16ll, (tokens - vk) * Cfg::kElem);
-      cp_async16(vd + r * LDS + c, vtbase + (long long)r * vt_ld + (vbytes ? vk : 0), vbytes);
+      for (int i = 0; i < BKV * CPR / THREADS; ++i) {
+        const int idx = tid + i * THREADS;
+        const int r = idx / CPR, c = (idx % CPR) * Cfg::kPerChunk;
+        // K row r = key p0 + r (zero outside the sequence); V^T row r = head dim r, keys p0 + c ..
+        const int key = p0 + r;
+        const bool kin = key >= start && key < start + len;
+        cp_async16(kd + r * LDS + c, kbase + (long long)(kin ? key : start) * ld + c, kin ? 16 : 0);
+        const long long vk = p0 + c;
+        const int vbytes = vk >= tokens ? 0 : (int)min(16ll, (tokens - vk) * Cfg::kElem);
+        cp_async16(vd + r * Cfg::kLdsV + c, vtbase + (long long)r * vt_ld + (vbytes ? vk : 0), vbytes);
+      }
+    } else {  // K: BKV rows of HD; V^T: HD rows of BKV keys
+      constexpr int CPK = HD / Cfg::kPerChunk, CPV = BKV / Cfg::kPerChunk;
+#pragma unroll
+      for (int i = 0; i < BKV * CPK / THREADS; ++i) {
+        const int idx = tid + i * THREADS;
+        const int r = idx / CPK, c = (idx % CPK) * Cfg::kPerChunk;
+        const int key = p0 + r;
+        const bool kin = key >= start && key < start + len;
+        cp_async16(kd + r * LDS + c, kbase + (long long)(kin ? key : start) * ld + c, kin ? 16 : 0);
+      }
+#pragma unroll
+      for (int i = 0; i < HD * CPV / THREADS; ++i) {
+        const int idx = tid + i * THREADS;
+        const int r = idx / CPV, c = (idx % CPV) * Cfg::kPerChunk;
+        const long long vk = p0 + c;
+        const int vbytes = vk >= tokens ? 0 : (int)min(16ll, (tokens - vk) * Cfg::kElem);
+        cp_async16(vd + r * Cfg::kLdsV + c, vtbase + (long long)r * vt_ld + (vbytes ? vk : 0), vbytes);
+      }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
 
   load_tile(0, 0);
-  constexpr float SL2 = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+  const float SL2 = score_l2(sl2...);  // scale * log2(e)
 
   for (int j = 0; j < n_kv; ++j) {
     const int buf = j & 1;
@@ -150,8 +186,8 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
       asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
     __syncthreads();
-    const T* kt = Ks + buf * Cfg::kTile;
-    const T* vt = Vs + buf * Cfg::kTile;
+    const T* kt = Ks + buf * Cfg::kTileK;
+    const T* vt = Vs + buf * Cfg::kTileV;
 
     // ---- S = Q K^T: 16 x 64 per warp ----
     float s[8][4];
@@ -210,7 +246,7 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
     l_lo = l_lo * sc_lo + ps_lo;
     l_hi = l_hi * sc_hi + ps_hi;
 #pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
+    for (int dt = 0; dt < HD / 8; ++dt) {
       o[dt][0] *= sc_lo; o[dt][1] *= sc_lo; o[dt][2] *= sc_hi; o[dt][3] *= sc_hi;
     }
     // ---- O += P V ----
@@ -223,8 +259,8 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
         pa[2] = pack_f16x2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
         pa[3] = pack_f16x2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
 #pragma unroll
-        for (int dt = 0; dt < 8; ++dt) {
-          const uint32_t* w = reinterpret_cast<const uint32_t*>(vt + (dt * 8 + g) * LDS + ks * 16);
+        for (int dt = 0; dt < HD / 8; ++dt) {
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(vt + (dt * 8 + g) * Cfg::kLdsV + ks * 16);
           mma_f16(o[dt], pa, w[t], w[t + 4]);
         }
       }
@@ -237,9 +273,9 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
         pa[2] = __float_as_uint(round_tf32(s[ks][1]));
         pa[3] = __float_as_uint(round_tf32(s[ks][3]));
 #pragma unroll
-        for (int dt = 0; dt < 8; ++dt) {
+        for (int dt = 0; dt < HD / 8; ++dt) {
           const float2 w = *reinterpret_cast<const float2*>(
-              reinterpret_cast<const float*>(vt) + (dt * 8 + g) * LDS + ks * 8 + 2 * t);
+              reinterpret_cast<const float*>(vt) + (dt * 8 + g) * Cfg::kLdsV + ks * 8 + 2 * t);
           mma_tf32(o[dt], pa, __float_as_uint(w.x), __float_as_uint(w.y));
         }
       }
@@ -256,7 +292,7 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
   const int row_lo = q0 + warp * 16 + g, row_hi = row_lo + 8;
   const long long ldc = (long long)heads * HD;
 #pragma unroll
-  for (int dt = 0; dt < 8; ++dt) {
+  for (int dt = 0; dt < HD / 8; ++dt) {
     const int col = h * HD + dt * 8 + 2 * t;
     float2 a = make_float2(o[dt][0] * inv_lo, o[dt][1] * inv_lo);
     float2 b = make_float2(o[dt][2] * inv_hi, o[dt][3] * inv_hi);
@@ -281,31 +317,42 @@ attention_vt_kernel(const void* __restrict__ qkv_, const void* __restrict__ vt_,
   }
 }
 
-template <bool F16>
+// max_cap: the longest row the caller routes here (MAX_SEQ for mer_attention, MAX_SEQ_HD for mer_attention_hd; the
+// kernel itself loops over any number of 64-key tiles).  scale is read by the RT_SCALE instances only.
+template <bool F16, int HD = 64, bool RT_SCALE = false>
 int launch_vt(const void* qkv, const void* vt, long long vt_ld, void* ctx, const int* cu_seqlens, int n_seq,
-              long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream) {
+              long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream, int max_cap = MAX_SEQ,
+              float scale = 0.125f) {
   MER_REQUIRE(qkv && vt && ctx && cu_seqlens, "mer_attention (V^T): null operand");
   MER_REQUIRE(out_mode >= 0 && out_mode <= 3, "mer_attention (V^T): out_mode %d", out_mode);
-  using Cfg = AttCfg<F16>;
+  using Cfg = AttCfg<F16, HD>;
   MER_REQUIRE(vt_ld >= tokens && vt_ld % Cfg::kPerChunk == 0,
               "mer_attention (V^T): V^T pitch %lld must be a multiple of %d >= tokens", vt_ld, Cfg::kPerChunk);
-  MER_REQUIRE(max_seqlen > 0 && max_seqlen <= MAX_SEQ, "mer_attention (V^T): max_seqlen %d (1 .. %d)", max_seqlen,
-              MAX_SEQ);
+  MER_REQUIRE(max_seqlen > 0 && max_seqlen <= max_cap, "mer_attention (V^T): max_seqlen %d (1 .. %d)", max_seqlen,
+              max_cap);
   MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535, "mer_attention (V^T): bad grid (%d heads, %d seqs)",
               heads, n_seq);
   if (n_seq <= 0 || tokens <= 0) return 0;
   static MerPerDevice attr_set;
   if (attr_set.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(attention_vt_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::kSmem));
+    if constexpr (RT_SCALE)
+      MER_CUDA_CHECK(cudaFuncSetAttribute(attention_vt_kernel<F16, HD, float>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+    else
+      MER_CUDA_CHECK(cudaFuncSetAttribute(attention_vt_kernel<F16, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          Cfg::kSmem));
     attr_set.mark();
   }
   const double s_avg = (double)tokens / n_seq;  // exact for equal-length batches (ViT frames)
   const int prof = mer_prof_begin(F16 ? MER_PROF_ATT_F16 : MER_PROF_ATT_TC,
                                   4.0 * s_avg * s_avg * HD * (double)n_seq * heads, stream);
   dim3 grid((max_seqlen + BQ - 1) / BQ, heads, n_seq);
-  attention_vt_kernel<F16><<<grid, THREADS, Cfg::kSmem, stream>>>(qkv, vt, vt_ld, ctx, cu_seqlens, tokens, heads,
-                                                                   out_mode);
+  if constexpr (RT_SCALE)
+    attention_vt_kernel<F16, HD, float><<<grid, THREADS, Cfg::kSmem, stream>>>(
+        qkv, vt, vt_ld, ctx, cu_seqlens, tokens, heads, out_mode, scale * 1.4426950408889634f);
+  else
+    attention_vt_kernel<F16, HD><<<grid, THREADS, Cfg::kSmem, stream>>>(qkv, vt, vt_ld, ctx, cu_seqlens, tokens, heads,
+                                                                        out_mode);
   mer_prof_end(prof, stream);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
@@ -338,4 +385,48 @@ int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_l
 int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
                             int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream) {
   return launch_vt<false>(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream);
+}
+
+// mer_attention's V^T route at head_dim 32 or 64 with an explicit score scale (ALBERT: 1 / sqrt(hidden / heads), also
+// for heads zero-padded from 26 to 32 columns).  head_dim 64 at scale 1/8 runs exactly what mer_attention runs (the
+// kernel of attention_short.cu for fp16 rows of up to 249 tokens, then the compile-time-scale instances); every other
+// case runs the tiled kernel with the scale as an argument.  Rows up to MAX_SEQ_HD tokens.
+extern "C" int mer_attention_hd(const void* qkv, const void* vt, long long vt_ld, void* ctx, const int32_t* cu_seqlens,
+                                int n_seq, long long tokens, int max_seqlen, int heads, int head_dim, float scale,
+                                int flags, void* stream_) {
+  const char* name = "mer_attention_hd";
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  MER_REQUIRE(head_dim == 32 || head_dim == 64, "%s: head_dim %d (32 or 64)", name, head_dim);
+  MER_REQUIRE(scale > 0.f && scale <= 1.f, "%s: scale %g (0 < scale <= 1)", name, (double)scale);
+  MER_REQUIRE(qkv && vt && ctx && cu_seqlens, "%s: null operand", name);
+  MER_REQUIRE((flags & ~(MER_ATT_QKV_F16 | MER_EPI_OUT_F16 | MER_EPI_SPLIT_BF16 | MER_EPI_ROUND_TF32)) == 0,
+              "%s: flags 0x%x", name, flags);
+  const bool f16 = (flags & MER_ATT_QKV_F16) != 0;
+  const int chunk = f16 ? 8 : 4;
+  MER_REQUIRE(vt_ld >= tokens && vt_ld % chunk == 0, "%s: V^T pitch %lld must be a multiple of %d >= tokens", name,
+              vt_ld, chunk);
+  MER_REQUIRE(tokens > 0 && max_seqlen > 0 && max_seqlen <= MAX_SEQ_HD && max_seqlen <= tokens,
+              "%s: max_seqlen %d (1 .. min(%d, tokens %lld))", name, max_seqlen, MAX_SEQ_HD, tokens);
+  MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq > 0 && n_seq <= 65535, "%s: bad grid (%d heads, %d seqs)", name,
+              heads, n_seq);
+  const int out_mode = (flags & MER_EPI_OUT_F16) ? 3 : (flags & MER_EPI_SPLIT_BF16) ? 2 : ((flags & MER_EPI_ROUND_TF32) ? 1 : 0);
+  if (head_dim == 64 && scale == 0.125f) {
+    if (f16 && max_seqlen <= MAX_SEQ)
+      return mer_attention_f16_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode,
+                                      stream);
+    return f16 ? launch_vt<true>(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream,
+                                 MAX_SEQ_HD)
+               : launch_vt<false>(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream,
+                                  MAX_SEQ_HD);
+  }
+#define MER_ATT_HD(F, H)                                                                                           \
+  return launch_vt<F, H, true>(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream, \
+                               MAX_SEQ_HD, scale)
+  if (head_dim == 32) {
+    if (f16) MER_ATT_HD(true, 32);
+    MER_ATT_HD(false, 32);
+  }
+  if (f16) MER_ATT_HD(true, 64);
+  MER_ATT_HD(false, 64);
+#undef MER_ATT_HD
 }

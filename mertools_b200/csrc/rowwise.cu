@@ -92,12 +92,31 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
 // per SM, each alternating between a load phase (3 KB in flight) and a reduce / store phase with nothing in flight.  Here a warp
 // fits 64 registers at 768 columns (four blocks = 32 warps per SM) and requests its NEXT row before it reduces and stores the
 // current one, so loads stay in flight through the whole loop.
-template <int VEC>
+// 1 / (the width the statistics run over): DIM, or the valid width of a padded row (MER_LN_PAD)
+template <int DIM, typename... P>
+__device__ __forceinline__ float ln_inv_width(P... valid) {
+  if constexpr (sizeof...(P) == 0) return 1.0f / DIM;
+  else return 1.0f / (float)(valid + ...);
+}
+// zero the elements of float4 slot `slot` (columns 4 slot .. 4 slot + 3) at or beyond column `valid`
+__device__ __forceinline__ void zero_pad4(float4& v, int slot, int valid) {
+  const int c = 4 * slot;
+  if (c >= valid) v.x = 0.f;
+  if (c + 1 >= valid) v.y = 0.f;
+  if (c + 2 >= valid) v.z = 0.f;
+  if (c + 3 >= valid) v.w = 0.f;
+}
+
+// valid: empty, or (MER_LN_PAD) one int, the valid width of rows padded to DIM: the statistics run over the first
+// `valid` columns and every output is zero beyond them.  An empty pack keeps the unpadded instances' parameter list and
+// code.
+template <int VEC, typename... P>
 __global__ void __launch_bounds__(256, VEC <= 6 ? 4 : VEC <= 8 ? 3 : 2)
 layernorm2_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                   const float* __restrict__ beta, float* __restrict__ y, void* __restrict__ ys,
-                  float* __restrict__ acc, long long rows, float eps, int flags) {
+                  float* __restrict__ acc, long long rows, float eps, int flags, P... valid) {
   constexpr int DIM = 128 * VEC;
+  constexpr bool PAD = sizeof...(P) > 0;
   __shared__ float4 gs[32 * VEC], bs[32 * VEC];
   for (int i = threadIdx.x; i < 32 * VEC; i += blockDim.x) {
     gs[i] = __ldg(reinterpret_cast<const float4*>(gamma) + i);
@@ -117,17 +136,22 @@ layernorm2_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
     for (int i = 0; i < VEC; ++i) v[i] = xr[lane + 32 * i];
   }
   for (; row < rows; row += warps_total) {
+    if constexpr (PAD) {
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) zero_pad4(v[i], lane + 32 * i, (valid + ...));
+    }
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-    const float mean = warp_sum(s) * (1.0f / DIM);
+    const float mean = warp_sum(s) * ln_inv_width<DIM>(valid...);
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       v[i].x -= mean; v[i].y -= mean; v[i].z -= mean; v[i].w -= mean;
+      if constexpr (PAD) zero_pad4(v[i], lane + 32 * i, (valid + ...));
       q += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
     }
-    const float rstd = 1.0f / sqrtf(warp_sum(q) * (1.0f / DIM) + eps);
+    const float rstd = 1.0f / sqrtf(warp_sum(q) * ln_inv_width<DIM>(valid...) + eps);
     float4* yr = (y && !y16) ? reinterpret_cast<float4*>(y + row * DIM) : nullptr;
     uint2* yh = (y && y16) ? reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(y) + row * DIM) : nullptr;
     float* ysr = (ys && !ys16) ? reinterpret_cast<float*>(ys) + row * DIM : nullptr;  // split row: DIM 4-byte slots
@@ -148,12 +172,14 @@ layernorm2_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
       if (flags & MER_LN_GELU) {
         o.x = gelu_erf_fast(o.x); o.y = gelu_erf_fast(o.y); o.z = gelu_erf_fast(o.z); o.w = gelu_erf_fast(o.w);
       }
+      if constexpr (PAD) zero_pad4(o, lane + 32 * i, (valid + ...));
       if (ar) {
         if (flags & MER_LN_ACC_INIT) {
           ar[lane + 32 * i] = o;
         } else if (flags & MER_LN_ACC_ADD) {
           float4 a = ar[lane + 32 * i];
           a.x += o.x; a.y += o.y; a.z += o.z; a.w += o.w;
+          if constexpr (PAD) zero_pad4(a, lane + 32 * i, (valid + ...));
           ar[lane + 32 * i] = a;
         }
       }
@@ -225,8 +251,13 @@ int mer_layernorm_launch(const float* x, const float* gamma, const float* beta, 
   // not alias x: its rows are half as long.)
   MER_REQUIRE(!((flags & MER_LN_OUT_F16) && (const void*)y == (const void*)x),
               "mer_layernorm: an fp16 output cannot alias the input");
-  MER_REQUIRE(dim == 768 || dim == 512 || dim == 1024 || dim == 1280 || dim == 1536,
-              "mer_layernorm: dim %d not supported (512, 768, 1024, 1280, 1536)", dim);
+  // MER_LN_PAD: dim is the valid width of rows padded to the next multiple of 128
+  const bool pad = (flags & MER_LN_PAD) != 0;
+  const int width = pad ? (dim + 127) / 128 * 128 : dim;
+  MER_REQUIRE(dim > 0 && (width == 768 || width == 512 || width == 1024 || width == 1280 || width == 1536 ||
+                          width == 128 || width == 384),
+              "mer_layernorm: dim %d not supported (512, 768, 1024, 1280, 1536) (also 128 and 384; with MER_LN_PAD, "
+              "a valid width whose next multiple of 128 is one of these)", dim);
   if (rows <= 0) return 0;
   const int warps_per_block = 8;
   long long blocks = (rows + warps_per_block - 1) / warps_per_block;
@@ -235,18 +266,23 @@ int mer_layernorm_launch(const float* x, const float* gamma, const float* beta, 
   // algorithmic bytes: the fp32 row in, each output row (fp16: 2 B/elem), the accumulator (write, or read+write)
   const double out_b = (y ? ((flags & MER_LN_OUT_F16) ? 2.0 : 4.0) : 0.0) + (y_split ? 4.0 : 0.0) +
                        (acc ? ((flags & MER_LN_ACC_ADD) ? 8.0 : 4.0) : 0.0);
-  const int prof = mer_prof_begin(MER_PROF_LAYERNORM, (double)rows * dim * (4.0 + out_b), stream);
+  const int prof = mer_prof_begin(MER_PROF_LAYERNORM, (double)rows * width * (4.0 + out_b), stream);
   const char* ver = getenv("MER_LN_VER");  // read at every launch: tests run both forms in one process
   const bool v1 = ver && atoi(ver) == 1;
 #define MER_LN_LAUNCH(VEC)                                                                                          \
   do {                                                                                                              \
-    if (v1) layernorm_kernel<VEC><<<(int)blocks, 256, 0, stream>>>(x, gamma, beta, y, y_split, acc, rows, eps, flags);  \
+    if (pad) layernorm2_kernel<VEC, int><<<(int)blocks, 256, 0, stream>>>(x, gamma, beta, y, y_split, acc, rows, eps,  \
+                                                                         flags, dim);                                 \
+    else if (v1) layernorm_kernel<VEC><<<(int)blocks, 256, 0, stream>>>(x, gamma, beta, y, y_split, acc, rows, eps,   \
+                                                                        flags);                                       \
     else layernorm2_kernel<VEC><<<(int)blocks, 256, 0, stream>>>(x, gamma, beta, y, y_split, acc, rows, eps, flags);    \
   } while (0)
-  if (dim == 768) MER_LN_LAUNCH(6);
-  else if (dim == 1024) MER_LN_LAUNCH(8);
-  else if (dim == 1280) MER_LN_LAUNCH(10);  // whisper-large-v2
-  else if (dim == 1536) MER_LN_LAUNCH(12);  // dinov2-giant
+  if (width == 768) MER_LN_LAUNCH(6);
+  else if (width == 1024) MER_LN_LAUNCH(8);
+  else if (width == 1280) MER_LN_LAUNCH(10);  // whisper-large-v2
+  else if (width == 1536) MER_LN_LAUNCH(12);  // dinov2-giant
+  else if (width == 128) MER_LN_LAUNCH(1);    // ALBERT's embedding LayerNorm
+  else if (width == 384) MER_LN_LAUNCH(3);    // albert_chinese_small; albert_chinese_tiny's 312 padded to 384
   else MER_LN_LAUNCH(4);
 #undef MER_LN_LAUNCH
   mer_prof_end(prof, stream);

@@ -1,6 +1,6 @@
 """Lexical feature extraction — H100 mirror of
 MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; DeBERTa / DeBERTa-v2 through
-extract/deberta_text.py and XLNet through extract/xlnet_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
+extract/deberta_text.py, XLNet through extract/xlnet_text.py and ALBERT through extract/albert_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
 extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU run; GPT-2 through extract/ln_decoder_text.py,
 float32 like the reference's fp32 run of it).
 
@@ -217,6 +217,21 @@ def _xlnet_extractor(model_dir, cfg, device):
     return TokenTypeTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
+def _albert_extractor(model_name, model_dir, cfg, device):
+    """The reference's ALBERT models, fp32 features: albert_chinese_tiny / _small with BertTokenizer (:164-166), the
+    English v2 models through the AutoModel + AutoTokenizer(use_fast=False) branch.  Tokens per launch as in
+    _xlnet_extractor, with max_position_embeddings for the row length."""
+    import torch
+
+    from .albert_text import AlbertTextEncoder, albert_tokenizer, check_albert_config
+    check_albert_config(cfg)  # before any weight is read
+    tokenizer = albert_tokenizer(model_name, model_dir)
+    enc = AlbertTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    tokens = int(min(16384, max(cfg.max_position_embeddings, free // 2 // enc.bytes_per_token)))
+    return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
+
+
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
                       language="chinese", model_dir=None, config=None, sentences_per_launch=256):
     """Same signature, naming and outputs as the reference (:139-252)."""
@@ -242,10 +257,10 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     from .. import shard
     gpu = shard.device_index(gpu)
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "xlnet", "llama", "bloom",
-                              "opt", "gpt2"), \
-        f"only BERT/RoBERTa/DeBERTa/XLNet encoders and LLaMA / BLOOM / OPT / GPT-2 decoders are on the H100 path, got " \
-        f"{cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "xlnet", "albert", "llama",
+                              "bloom", "opt", "gpt2"), \
+        f"only BERT/RoBERTa/DeBERTa/XLNet/ALBERT encoders and LLaMA / BLOOM / OPT / GPT-2 decoders are on the H100 " \
+        f"path, got {cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("bloom", "opt"):
@@ -256,6 +271,8 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
         ext = _deberta_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type == "xlnet":
         ext = _xlnet_extractor(model_dir, cfg, f"cuda:{gpu}")
+    elif cfg.model_type == "albert":
+        ext = _albert_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     else:
         tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
         roberta = cfg.model_type != "bert"

@@ -697,6 +697,55 @@ def xlnet_state_dict(cfg, seed=33, scale=1.0):
     return g.sd
 
 
+# ALBERT (AlbertConfig keywords).  Goldens: albert_chinese_tiny (312 = 12 heads of 26, padded to 32 on the device),
+# albert_chinese_small (384 = 12 x 32) and albert-base-v2 at 3 layers (hidden state 0 enters the readout).  PUBLISHED:
+# the five checkpoints' shapes, for the bench and the full-width tests (seeded weights; vocab and depth as given).
+ALBERT_GOLDEN_CFGS = {
+    "tiny": dict(vocab_size=None, embedding_size=128, hidden_size=312, num_attention_heads=12, intermediate_size=1248,
+                 num_hidden_layers=4, hidden_act="gelu", layer_norm_eps=1e-12, hidden_dropout_prob=0.0,
+                 attention_probs_dropout_prob=0.0, classifier_dropout_prob=0.0),
+    "small": dict(vocab_size=None, embedding_size=128, hidden_size=384, num_attention_heads=12, intermediate_size=1536,
+                  num_hidden_layers=4, hidden_act="gelu", layer_norm_eps=1e-12, hidden_dropout_prob=0.0,
+                  attention_probs_dropout_prob=0.0, classifier_dropout_prob=0.0),
+    "base": dict(vocab_size=None, embedding_size=128, hidden_size=768, num_attention_heads=12, intermediate_size=3072,
+                 num_hidden_layers=3, hidden_act="gelu_new", layer_norm_eps=1e-12, hidden_dropout_prob=0.0,
+                 attention_probs_dropout_prob=0.0, classifier_dropout_prob=0.0),
+}
+ALBERT_PUBLISHED_CFGS = {
+    "albert_chinese_tiny": dict(ALBERT_GOLDEN_CFGS["tiny"], vocab_size=21128),
+    "albert_chinese_small": dict(ALBERT_GOLDEN_CFGS["small"], vocab_size=21128, num_hidden_layers=6),
+    "albert-base-v2": dict(ALBERT_GOLDEN_CFGS["base"], vocab_size=30000, num_hidden_layers=12),
+    "albert-large-v2": dict(ALBERT_GOLDEN_CFGS["base"], vocab_size=30000, hidden_size=1024, num_attention_heads=16,
+                            intermediate_size=4096, num_hidden_layers=24),
+    "albert-xxlarge-v2": dict(ALBERT_GOLDEN_CFGS["base"], vocab_size=30000, hidden_size=4096, num_attention_heads=64,
+                              intermediate_size=16384, num_hidden_layers=12),
+}
+
+
+def albert_state_dict(cfg, seed=41, scale=1.0):
+    """Keys of ``transformers.AlbertModel`` (with pooler) for a dict of AlbertConfig keywords (as ALBERT_GOLDEN_CFGS;
+    vocab_size set): the 128-wide embeddings and their LayerNorm, ``encoder.embedding_hidden_mapping_in`` and the ONE
+    shared layer ``encoder.albert_layer_groups.0.albert_layers.0``.  ``scale`` multiplies every layer matrix (stress
+    checkpoints)."""
+    g = _Gen(seed)
+    e, d, ffn = cfg["embedding_size"], cfg["hidden_size"], cfg["intermediate_size"]
+    std = 0.03 * scale
+    g.normal("embeddings.word_embeddings.weight", (cfg["vocab_size"], e), 0.5)
+    g.normal("embeddings.position_embeddings.weight", (cfg.get("max_position_embeddings", 512), e), 0.1)
+    g.normal("embeddings.token_type_embeddings.weight", (cfg.get("type_vocab_size", 2), e), 0.1)
+    g.ln("embeddings.LayerNorm", e)
+    g.linear("encoder.embedding_hidden_mapping_in", d, e, 0.08)
+    p = "encoder.albert_layer_groups.0.albert_layers.0."
+    g.ln(p + "full_layer_layer_norm", d)
+    for n in ("query", "key", "value", "dense"):
+        g.linear(p + "attention." + n, d, d, std)
+    g.ln(p + "attention.LayerNorm", d)
+    g.linear(p + "ffn", ffn, d, std)
+    g.linear(p + "ffn_output", d, ffn, std)
+    g.linear("pooler", d, d, 0.02)
+    return g.sd
+
+
 def fusion_state_dict(seed=3, audio_dim=768, text_dim=768, video_dim=768, hidden=128,
                       out1=6, out2=1, feat_type="utt"):
     """Keys of toolkit/models/attention.py:Attention, nn.Linear / nn.LSTM-style
