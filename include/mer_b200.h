@@ -712,7 +712,10 @@ MER_API int mer_fusion_forward(const MerFusionDims* dims, const float* params, c
  * parallelism so that an all-reduce SUM of grads gives the reference's batch-mean gradient).
  * dropout_p > 0: keep-masks come from a counter hash of (seed, *step_counter, index) unless
  * ext_masks (HOST array of 4 device pointers: audio [B,Da], text, video, concat [B,3H]; entries may
- * be NULL) supplies them (parity tests inject the reference's masks).
+ * be NULL) supplies them (parity tests inject the reference's masks).  The hash index is the element's LOCAL
+ * index (row * dim + col of this call's batch), so data-parallel callers must give every rank its own seed:
+ * ranks that share one drop the same elements of their local rows, and the all-reduced gradient carries
+ * world-size-fold correlated dropout noise (the Python wrappers derive one per rank, fusion.rank_dropout_seed).
  * loss_out: device float[3] = {CE mean, MSE mean, total}. */
 MER_API int mer_fusion_fwd_bwd(const MerFusionDims* dims, const float* params, float* grads,
                                const float* audios, const float* texts, const float* videos,

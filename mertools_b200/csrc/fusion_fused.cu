@@ -1237,8 +1237,12 @@ int launch_rows_fast(const RowArgs& a, const FastPlan& pl, cudaStream_t st) {
 
 int launch_rows(const RowArgs& a, cudaStream_t st) {
   static const bool no_fast = getenv("MER_FUSION_GENERIC") != nullptr;  // A/B and fallback testing
+  // the fast kernel stages the input rows with 16-byte loads (its widths are multiples of 4, so every row is aligned
+  // when the base pointer is); a caller's view that starts off a 16-byte boundary takes the general kernel
+  bool aligned = true;
+  for (int m = 0; m < 3; ++m) aligned = aligned && (reinterpret_cast<uintptr_t>(a.x[m]) & 15) == 0;
   FastPlan pl;
-  if (!no_fast && fast_plan_for(a.d, &pl)) return launch_rows_fast(a, pl, st);
+  if (!no_fast && aligned && fast_plan_for(a.d, &pl)) return launch_rows_fast(a, pl, st);
   // 8 rows per cluster once there are enough rows to fill the GPU with clusters and the plan fits shared memory
   if (a.B >= 128 && a.d.hidden <= 128) return launch_rows_t<8>(a, st);
   return launch_rows_t<4>(a, st);

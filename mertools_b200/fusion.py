@@ -39,6 +39,30 @@ LSTM_PARAMS = ("rnn.weight_ih_l0", "rnn.weight_hh_l0", "rnn.bias_ih_l0", "rnn.bi
                "linear_1.weight", "linear_1.bias")
 
 
+_M64 = (1 << 64) - 1
+
+
+def rank_dropout_seed(seed, rank, world_size):
+    """The dropout seed one data-parallel rank hands the kernels.  The keep-masks hash (seed, mask tensor, step, LOCAL
+    element index), so ranks that share a seed would drop the same elements of their local rows, and the all-reduced
+    gradient would carry W-fold correlated dropout noise.  At world_size 1 the seed is returned unchanged; otherwise it
+    is a splitmix64 output for (seed, rank): a bijection of the seed for each rank, different for every rank."""
+    seed = int(seed) & _M64
+    if world_size == 1:
+        return seed
+    z = (seed + 0x9E3779B97F4A7C15 * (int(rank) + 1)) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def _dist_seed(seed, world):
+    if world == 1:
+        return seed
+    import torch.distributed as dist
+    return rank_dropout_seed(seed, dist.get_rank(), world)
+
+
 def param_names(feat_type="utt"):
     names = []
     for e in ENC:
@@ -231,11 +255,12 @@ class FusionNet:
         inv = 1.0 / (global_batch if global_batch is not None else B * world)
         masks = self._masks(ext_masks)
         clip = self.grad_clip if self.grad_clip != -1 else 0.0
+        seed = _dist_seed(self.seed, world)
         if not self.frm and world == 1 and fused_adam:  # the whole step in two kernels, Adam fused into the weight gradients
             hyper = MerAdamHyper(lr, betas[0], betas[1], eps, wd, clip)
             L.check(self._step(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg),
                                L.ptr(self.exp_avg_sq), L.ptr(a), L.ptr(t), L.ptr(v), L.ptr(emo), L.ptr(val), B,
-                               inv, self.dropout, self.seed, L.ptr(self.step_counter), masks, C.byref(hyper),
+                               inv, self.dropout, seed, L.ptr(self.step_counter), masks, C.byref(hyper),
                                L.ptr(self.ws), self.ws.numel(), L.ptr(self.loss), L.ptr(feats), L.ptr(emos_out),
                                L.ptr(vals_out), L.stream_ptr()))
             return
@@ -243,13 +268,13 @@ class FusionNet:
             ws = self._frm_ws(B, a, t, v)
             L.check(self._fb_frm(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(a), L.ptr(t),
                                  L.ptr(v), a.shape[1], t.shape[1], v.shape[1], L.ptr(emo), L.ptr(val), B,
-                                 inv, self.dropout, self.seed, L.ptr(self.step_counter), masks,
+                                 inv, self.dropout, seed, L.ptr(self.step_counter), masks,
                                  L.ptr(ws), ws.numel(), L.ptr(self.loss), L.ptr(feats), L.ptr(emos_out),
                                  L.ptr(vals_out), L.stream_ptr()))
         else:
             L.check(self._fb(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(a), L.ptr(t),
                              L.ptr(v), L.ptr(emo), L.ptr(val), B, inv, self.dropout,
-                             self.seed, L.ptr(self.step_counter), masks, L.ptr(self.ws), self.ws.numel(),
+                             seed, L.ptr(self.step_counter), masks, L.ptr(self.ws), self.ws.numel(),
                              L.ptr(self.loss), L.ptr(feats), L.ptr(emos_out), L.ptr(vals_out), L.stream_ptr()))
         if world > 1:
             import torch.distributed as dist
@@ -446,7 +471,8 @@ class TopnFusionNet:
         d = self.dims
         out = [torch.empty(B, n, dtype=torch.float32, device=self.device) for n in (d.hidden, d.out1, d.out2)]
         L.check(self._step(C.byref(d), L.ptr(self.params), L.ptr(self.grads), C.cast(fp, C.c_void_p), L.ptr(emo),
-                           L.ptr(val), B, 1.0 / (B * world), self.dropout if emo is not None else 0.0, self.seed,
+                           L.ptr(val), B, 1.0 / (B * world), self.dropout if emo is not None else 0.0,
+                           _dist_seed(self.seed, world),
                            L.ptr(self.step_counter), C.cast(mp, C.c_void_p) if mp is not None else None,
                            L.ptr(self.ws), self.ws.numel(), L.ptr(self.loss), L.ptr(out[0]), L.ptr(out[1]),
                            L.ptr(out[2]), L.stream_ptr()))

@@ -34,8 +34,8 @@ def _lstm_encoder(sd, prefix, x, mask, p):
     b_ih, b_hh = sd[f"{prefix}.rnn.bias_ih_l0"], sd[f"{prefix}.rnn.bias_hh_l0"]
     B, T, _ = x.shape
     H = w_hh.shape[1]
-    h = torch.zeros(B, H, dtype=x.dtype)
-    c = torch.zeros(B, H, dtype=x.dtype)
+    h = torch.zeros(B, H, dtype=x.dtype, device=x.device)
+    c = torch.zeros(B, H, dtype=x.dtype, device=x.device)
     for t in range(T):
         g = F.linear(x[:, t], w_ih, b_ih) + F.linear(h, w_hh, b_hh)
         i, f, gg, o = g.chunk(4, dim=1)

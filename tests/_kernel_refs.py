@@ -1,11 +1,12 @@
-"""float64 restatements of the row-wise and fp32 attention entry points of include/mer_b200.h, and the small helpers the
-kernel-level GPU tests share (environment switches, guarded output buffers).  Every function takes torch tensors on any
-device and computes in float64 on that device; tests/test_kernel_refs.py checks them on the CPU against torch's own
-operators."""
+"""float64 restatements of the row-wise and fp32 attention entry points of include/mer_b200.h, of the fusion nets'
+dropout hash, loss, gradients and Adam, and the small helpers the kernel-level GPU tests share (environment switches,
+guarded output buffers).  Every function takes torch tensors on any device and computes in float64 on that device;
+tests/test_kernel_refs.py checks them on the CPU against torch's own operators."""
 import contextlib
 import math
 import os
 
+import numpy as np
 import torch
 
 U32 = 2.0 ** -24  # unit roundoff of fp32 (round to nearest)
@@ -181,3 +182,73 @@ def videomae_patches(frames_bgr, mean, std):
                                                                                       device=x.device)
     x = x.reshape(n, 8, 2, 14, 16, 14, 16, 3).permute(0, 1, 3, 5, 7, 2, 4, 6)    # n, tt, py, px, c, dt, dy, dx
     return x.reshape(n * 1568, 1536)
+
+
+# ---- fusion nets: dropout hash, float64 loss / gradients, Adam -------------------------------------------------------
+_M64 = (1 << 64) - 1
+
+
+def keep_mask(seed, m, step, n, p):
+    """Elements 0 .. n-1 of keep-mask tensor m at step counter `step` as the fusion kernels draw them, as a bool numpy
+    array: keep_hash of fusion_fused.cu (seed + 0x1000 (m + 1) + 0x9E37.. (step + 1) + 0xD1B5.. (i + 1), the splitmix64
+    finaliser, u = top 24 bits / 2^24, keep when u >= p in fp32).  m = None is fus_dropout_mask_kernel's form of fusion.cu,
+    whose seed already carries the tensor's 0x1000 (m + 1)."""
+    base = (int(seed) + (0 if m is None else 0x1000 * (m + 1)) + 0x9E3779B97F4A7C15 * (int(step) + 1)) & _M64
+    z = np.arange(1, n + 1, dtype=np.uint64) * np.uint64(0xD1B54A32D192ED03) + np.uint64(base)  # wraps mod 2^64
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    z ^= z >> np.uint64(31)
+    u = (z >> np.uint64(40)).astype(np.float32) * np.float32(2.0 ** -24)
+    return u >= np.float32(p)
+
+
+def keep_probability(p):
+    """Exact keep probability of keep_mask: u takes the 2^24 values k / 2^24, and u >= p for all but ceil(p 2^24)."""
+    return 1.0 - math.ceil(float(np.float32(p)) * 2 ** 24) / 2 ** 24
+
+
+def fusion_f64(sd, inputs, p=0.0, masks=None, emo=None, val=None, upstream=None):
+    """The fusion net in float64 through the oracle's own dtype-generic forward (oracle/fusion.py): Attention when `inputs`
+    is (audios, texts, videos) with a state dict of audio_encoder.* keys (utterance or frame level), Attention_TOPN when
+    the state dict has encoder0.* keys and `inputs` is the list of features.  Parameters, inputs and keep-masks are double
+    copies of what the kernels read.  Returns dict(out=(features, emos, vals), and with emo / val: loss=(ce, mse, total)
+    and grads={name: d total / d param}; with upstream=(w_features, w_emos, w_vals): up={name: d sum(out * w) / d param})."""
+    from oracle import fusion as OF
+    dev = inputs[0].device
+    sd64 = {k: torch.as_tensor(v).to(dev, torch.float64).requires_grad_(True) for k, v in sd.items()}
+    xs = [x.to(torch.float64) for x in inputs]
+    mk = None if masks is None else [None if mm is None else torch.as_tensor(mm).to(dev, torch.float64) for mm in masks]
+    if "encoder0.linear_1.weight" in sd64:
+        out = OF.attention_topn_forward(sd64, xs, mk, p)
+    else:
+        out = OF.attention_forward(sd64, *xs, masks=mk, p=p)
+    res = dict(out=tuple(o.detach() for o in out))
+    names, leaves = list(sd64), list(sd64.values())
+    if emo is not None:
+        ce, mse = OF.losses(out[1], out[2], emo.to(dev), val.to(dev, torch.float64))
+        total = ce + mse
+        g = torch.autograd.grad(total, leaves, retain_graph=upstream is not None, allow_unused=True)
+        res["loss"] = tuple(float(x.detach()) for x in (ce, mse, total))
+        res["grads"] = {n: torch.zeros_like(x) if gi is None else gi for n, x, gi in zip(names, leaves, g)}
+    if upstream is not None:
+        s = sum((o * w.to(torch.float64)).sum() for o, w in zip(out, upstream))
+        g = torch.autograd.grad(s, leaves, allow_unused=True)
+        res["up"] = {n: torch.zeros_like(x) if gi is None else gi for n, x, gi in zip(names, leaves, g)}
+    return res
+
+
+def adam_f64(param, grad, exp_avg, exp_avg_sq, t, lr, beta1, beta2, eps, weight_decay, grad_scale=1.0, clip=0.0):
+    """torch.optim.Adam(lr, (beta1, beta2), eps, weight_decay) step t (1-based) in float64, after clip_grad_value_(clip)
+    (clip > 0) of grad * grad_scale; coupled L2 (weight_decay * param added to the clipped gradient).  The hyper-
+    parameters are taken at their fp32 values, as the kernels receive them.  Returns (param, exp_avg, exp_avg_sq)."""
+    h = [float(np.float32(x)) for x in (lr, beta1, beta2, eps, weight_decay, grad_scale, clip)]
+    lr, beta1, beta2, eps, weight_decay, grad_scale, clip = h
+    p, g, m, v = (x.to(torch.float64) for x in (param, grad, exp_avg, exp_avg_sq))
+    g = g * grad_scale
+    if clip > 0:
+        g = g.clamp(-clip, clip)
+    g = g + weight_decay * p
+    m = beta1 * m + (1.0 - beta1) * g
+    v = beta2 * v + (1.0 - beta2) * g * g
+    denom = v.sqrt() / math.sqrt(1.0 - beta2 ** t) + eps
+    return p - lr / (1.0 - beta1 ** t) * m / denom, m, v

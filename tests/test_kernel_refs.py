@@ -1,6 +1,9 @@
 """CPU checks of tests/_kernel_refs.py: the float64 references the kernel-level GPU tests compare with are themselves
 compared with torch's operators (or a second, independent formula) at small shapes."""
+import math
+
 import numpy as np
+import pytest
 import torch
 import torch.nn.functional as F
 
@@ -116,3 +119,125 @@ def test_videomae_patch_layout_is_the_conv3d_unfold():
     w = torch.randn(2, 3, 2, 16, 16, generator=_g(30)).double()
     want = F.conv3d(vid, w, stride=(2, 16, 16)).flatten(2).transpose(1, 2)[0]     # [1568, 2]
     assert float((rows @ w.reshape(2, -1).T - want).abs().max()) < 1e-9
+
+
+# ---- the fusion nets' dropout hash, float64 network and Adam ------------------------------------------------------------
+HASH_PS = (0.2, 0.3, 0.5, 0.9)
+HASH_N = 1 << 22          # 4M draws per statistic
+HASH_SEED, HASH_W = 7, 768
+
+
+def _within_5_sigma(hits, n, prob):
+    sigma = math.sqrt(prob * (1.0 - prob) / n)
+    return abs(hits / n - prob) <= 5 * sigma, f"{hits / n:.6f} vs {prob:.6f} (5 sigma = {5 * sigma:.1e})"
+
+
+def test_keep_mask_both_seeding_forms_agree():
+    """keep_hash (seed and tensor index passed apart) and fus_dropout_mask_kernel (seed + 0x1000 (m + 1) passed in) are
+    the same draw; seeds past 2^63 wrap as the kernels' unsigned 64-bit arithmetic does."""
+    for seed, m, step in ((7, 0, 0), (7, 3, 41), ((1 << 64) - 5, 18, 123456)):
+        a = R.keep_mask(seed, m, step, 4096, 0.5)
+        b = R.keep_mask((seed + 0x1000 * (m + 1)) & ((1 << 64) - 1), None, step, 4096, 0.5)
+        assert a.dtype == np.bool_ and np.array_equal(a, b)
+    # a hand-evaluated element: seed 0, tensor 0, step 0, i = 0 (z = 0x1000 + 0x9E37.. + 0xD1B5.. mod 2^64)
+    z = (0x1000 + 0x9E3779B97F4A7C15 + 0xD1B54A32D192ED03) & ((1 << 64) - 1)
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & ((1 << 64) - 1)
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & ((1 << 64) - 1)
+    z ^= z >> 31
+    for p in (0.1, 0.5, 0.9):
+        assert bool(R.keep_mask(0, 0, 0, 1, p)[0]) == ((z >> 40) / 2 ** 24 >= np.float32(p))
+
+
+@pytest.mark.parametrize("p", HASH_PS)
+def test_keep_mask_keep_rate_is_one_minus_p(p):
+    q = R.keep_probability(p)
+    assert q == 1.0 - math.ceil(float(np.float32(p)) * 2 ** 24) / 2 ** 24
+    for seed, m, step in ((HASH_SEED, 0, 0), (HASH_SEED, 3, 41)):
+        ok, msg = _within_5_sigma(int(R.keep_mask(seed, m, step, HASH_N, p).sum()), HASH_N, q)
+        assert ok, f"p={p} m={m} step={step}: keep fraction {msg}"
+
+
+@pytest.mark.parametrize("p", HASH_PS)
+def test_keep_mask_pairs_are_uncorrelated(p):
+    """Two independent keep draws agree with probability q^2 + (1 - q)^2.  A hash whose neighbouring indices, rows,
+    tensors or steps were correlated (or identical) would move the fraction of equal pairs far past 5 sigma."""
+    q = R.keep_probability(p)
+    e = q * q + (1 - q) * (1 - q)
+    base = R.keep_mask(HASH_SEED, 1, 5, HASH_N + HASH_W, p)
+    pairs = {
+        "neighbouring elements": (base[:HASH_N], base[1:HASH_N + 1]),
+        "same column, neighbouring rows": (base[:HASH_N], base[HASH_W:HASH_N + HASH_W]),
+        "tensors m, m + 1": (base[:HASH_N], R.keep_mask(HASH_SEED, 2, 5, HASH_N, p)),
+        "steps s, s + 1": (base[:HASH_N], R.keep_mask(HASH_SEED, 1, 6, HASH_N, p)),
+    }
+    for what, (x, y) in pairs.items():
+        ok, msg = _within_5_sigma(int((x == y).sum()), HASH_N, e)
+        assert ok, f"p={p} {what}: equal-pair fraction {msg}"
+
+
+def test_fusion_f64_matches_the_fp32_oracle_trainer():
+    """fusion_f64 runs the oracle's network in float64: its losses and gradients agree with the fp32 oracle Trainer
+    (same masks) to fp32 accuracy, for the utterance-level, frame-level and top-N nets."""
+    from mertools_b200 import synthetic as S
+    from oracle import fusion as OF
+    g = _g(40)
+    B, p = 5, 0.3
+    cases = []
+    sd = S.fusion_state_dict(seed=3, audio_dim=12, text_dim=8, video_dim=4, hidden=8, out1=3, out2=2)
+    xs = [torch.randn(B, d, generator=g) for d in (12, 8, 4)]
+    cases.append((sd, xs, [(torch.rand(B, d, generator=g) >= p).float() for d in (12, 8, 4, 24)]))
+    sd = S.fusion_state_dict(seed=4, audio_dim=6, text_dim=5, video_dim=3, hidden=8, out1=3, out2=1,
+                             feat_type="frm_align")
+    xs = [torch.randn(B, T, d, generator=g) for T, d in ((3, 6), (1, 5), (4, 3))]
+    cases.append((sd, xs, [(torch.rand(B, d, generator=g) >= p).float() for d in (8, 8, 8, 24)]))
+    sd = S.fusion_topn_state_dict([7, 3], seed=5, hidden=8, out1=4, out2=1)
+    xs = [torch.randn(B, d, generator=g) for d in (7, 3)]
+    cases.append((sd, xs, [(torch.rand(B, d, generator=g) >= p).float() for d in (7, 3, 16)]))
+    for sd, xs, masks in cases:
+        out1 = sd["fc_out_1.weight"].shape[0]
+        emo = torch.randint(0, out1, (B,), generator=g)
+        val = torch.randn(B, sd["fc_out_2.weight"].shape[0], generator=g)   # [B, out2]: MSE over every element / B
+        ref = R.fusion_f64(sd, xs, p, masks, emo, val)
+        tr = OF.Trainer(sd, dropout=p)
+        args = (xs, None, None) if "encoder0.linear_1.weight" in sd else tuple(xs)  # Attention_TOPN takes the list
+        ce, mse, tot, eo, vo, grads = tr.step(*args, emo, val, masks)
+        assert abs(ref["loss"][2] - tot) <= 1e-5 * max(1.0, tot) and abs(ref["loss"][0] - ce) <= 1e-5 * max(1.0, ce)
+        assert float((ref["out"][1] - eo.double()).abs().max()) <= 1e-5
+        for n, r in ref["grads"].items():
+            assert r.dtype == torch.float64
+            assert float((r - grads[n].double()).abs().max()) <= 1e-5 * max(1.0, float(r.abs().max())), n
+    # the upstream form is the gradient of sum(out * w)
+    sd = S.fusion_state_dict(seed=3, audio_dim=12, text_dim=8, video_dim=4, hidden=8, out1=3, out2=2)
+    xs = [torch.randn(B, d, generator=g) for d in (12, 8, 4)]
+    ws = [torch.randn(B, n, generator=g) for n in (8, 3, 2)]
+    up = R.fusion_f64(sd, xs, upstream=ws)["up"]
+    sdd = {k: torch.tensor(v, dtype=torch.float64, requires_grad=True) for k, v in sd.items()}
+    out = OF.attention_forward(sdd, *(x.double() for x in xs))
+    sum((o * w.double()).sum() for o, w in zip(out, ws)).backward()
+    for n, x in sdd.items():
+        assert torch.allclose(up[n], x.grad, rtol=0, atol=1e-13), n
+
+
+def test_adam_f64_is_torch_adam_after_clip_grad_value():
+    g = _g(41)
+    p0 = torch.randn(257, generator=g, dtype=torch.float64)
+    hp = dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5)
+    for clip, scale in ((0.0, 1.0), (0.01, 1.0), (0.0, 0.5)):
+        w = p0.clone().requires_grad_(True)
+        # hyper-parameters already at fp32 values, so that adam_f64's rounding of them to fp32 changes nothing
+        hp32 = dict(lr=float(np.float32(1e-3)), betas=(float(np.float32(0.9)), float(np.float32(0.999))),
+                    eps=float(np.float32(1e-8)), weight_decay=float(np.float32(1e-5)))
+        opt = torch.optim.Adam([w], **hp32)
+        p, m, v = p0.clone(), torch.zeros(257, dtype=torch.float64), torch.zeros(257, dtype=torch.float64)
+        for t in range(1, 6):
+            grad = torch.randn(257, generator=g, dtype=torch.float64) * 0.05
+            w.grad = grad * scale
+            if clip > 0:
+                torch.nn.utils.clip_grad_value_([w], float(np.float32(clip)))  # the kernels take the fp32 value
+            opt.step()
+            p, m, v = R.adam_f64(p, grad, m, v, t, hp["lr"], *hp["betas"], hp["eps"], hp["weight_decay"],
+                                 grad_scale=scale, clip=clip)
+            st = opt.state[w]
+            # torch moves exp_avg by lerp (m + (1 - beta1) (g - m)): the two forms differ by float64 roundings only
+            for mine, theirs in ((p, w.detach()), (m, st["exp_avg"]), (v, st["exp_avg_sq"])):
+                assert float((mine - theirs).abs().max()) <= 1e-14 * float(theirs.abs().max())
