@@ -476,6 +476,25 @@ typedef struct MerHubertModel {
 MER_API int mer_wave_normalize(const float* in, float* out, int batch, int n_samples, long long ld_in,
                                long long ld_out, void* stream);
 
+/* The first layer of the feature encoder on its own: conv0 (Conv1d 1 -> 512, kernel 10, stride 5) of every row of
+ * wave (fp32 [batch, n_samples], row pitch ld_wave >= n_samples floats), then
+ *   model->feat_norm_layer == 0: GroupNorm(512 groups, eps 1e-5, biased variance over the clip's frames; conv0_w,
+ *     gn_g, gn_b) and exact GELU (HF HubertGroupNormConvLayer).  The statistics come from the waveform's tap moments,
+ *     summed in double; `frames`: NULL (every clip has T0 = (n_samples - 10) / 5 + 1 frames) or a DEVICE int32 [batch]
+ *     of per-clip frame counts in 1 .. T0, over which clip b's statistics are taken (mer_hubert_forward_ragged).
+ *   model->feat_norm_layer == 1: + conv_b[0] (NULL: no bias), LayerNorm over the 512 channels (eps 1e-5; conv_ln_g[0],
+ *     conv_ln_b[0]) and exact GELU per frame (HF HubertLayerNormConvLayer); `frames` is ignored.
+ * out: rows [clip][frame][512] at clip stride out_bstride (elements, >= T0 * 512); out_format MER_EPI_SPLIT_BF16:
+ * split-bf16 rows (the BF16X3 operand of conv1), or -- GroupNorm family only, even out_bstride -- MER_EPI_OUT_F16:
+ * fp16 rows (the MER_GEMM_F16 operand).  Rows T0 .. of a clip's stride are not written; rows at or past a clip's own
+ * frame count are finite and unspecified.  workspace: >= mer_hubert_conv0_workspace_bytes(batch) bytes, 16-byte
+ * aligned (GroupNorm statistics; unused by the LayerNorm family).  Refused before any launch: a workspace that is
+ * too small or misaligned, a pitch or stride shorter than a row, an output format the family does not write. */
+MER_API int mer_hubert_conv0(const MerHubertModel* model, const float* wave, int batch, int n_samples,
+                             long long ld_wave, const int* frames, int out_format, void* out, long long out_bstride,
+                             void* workspace, long long workspace_bytes, void* stream);
+MER_API long long mer_hubert_conv0_workspace_bytes(int batch); /* 5120 * batch */
+
 /* frames produced for n_samples input samples (conv kernels 10,3,3,3,3,2,2 / strides 5,2,2,2,2,2,2) */
 MER_API int mer_hubert_num_frames(int n_samples);
 MER_API long long mer_hubert_workspace_bytes(int batch, int n_samples);               /* base dims */

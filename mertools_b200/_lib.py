@@ -255,6 +255,29 @@ def wave_normalize(x, out, *, batch, n_samples, ld_in, ld_out):
     return out
 
 
+def hubert_conv0_workspace_bytes(batch):
+    f = lib().mer_hubert_conv0_workspace_bytes
+    f.restype, f.argtypes = C.c_longlong, [C.c_int]
+    return int(f(batch))
+
+
+def hubert_conv0(model, wave, out, *, batch, n_samples, ld_wave, out_bstride, frames=None, f16_out=False,
+                 workspace=None, workspace_bytes=None):
+    """mer_hubert_conv0 on a MerHubertModel (ctypes struct, encoders.py).  out: split-bf16 rows in an fp32-typed tensor,
+    or fp16 rows (f16_out); frames: optional int32 CUDA tensor of per-clip frame counts; workspace: a CUDA tensor
+    (default: a fresh one of mer_hubert_conv0_workspace_bytes(batch))."""
+    import torch
+    if workspace is None:
+        workspace = torch.empty(max(hubert_conv0_workspace_bytes(batch), 16), dtype=torch.uint8, device=wave.device)
+    f = declare("mer_hubert_conv0", [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_int,
+                                     C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p])
+    check(f(C.byref(model), ptr(wave), batch, n_samples, ld_wave, ptr(frames),
+            MER_EPI_OUT_F16 if f16_out else MER_EPI_SPLIT_BF16, ptr(out), out_bstride, ptr(workspace),
+            workspace.numel() * workspace.element_size() if workspace_bytes is None else workspace_bytes,
+            stream_ptr()))
+    return out
+
+
 def wavlm_gate(x, w, b, c, gate, *, tokens, heads):
     f = declare("mer_wavlm_gate", [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p])

@@ -432,3 +432,37 @@ extern "C" int mer_wave_normalize(const float* in, float* out, int batch, int n_
   return mer_wave_normalize_launch(in, out, batch, n_samples, ld_in, ld_out,
                                    static_cast<cudaStream_t>(stream));
 }
+
+extern "C" int mer_hubert_conv0(const MerHubertModel* model, const float* wave, int batch, int n_samples,
+                                long long ld_wave, const int* frames, int out_format, void* out, long long out_bstride,
+                                void* workspace, long long workspace_bytes, void* stream) {
+  MER_REQUIRE(model && wave && out && batch > 0 && model->conv0_w, "mer_hubert_conv0: bad arguments");
+  const int T0 = n_samples >= K0 ? (n_samples - K0) / S0 + 1 : 0;
+  MER_REQUIRE(T0 > 0, "mer_hubert_conv0: waveform too short (%d samples)", n_samples);
+  MER_REQUIRE(ld_wave >= n_samples, "mer_hubert_conv0: row pitch %lld shorter than the %d samples of a row", ld_wave,
+              n_samples);
+  MER_REQUIRE(out_bstride >= (long long)T0 * C0, "mer_hubert_conv0: output batch stride %lld shorter than %d rows of %d",
+              out_bstride, T0, C0);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (model->feat_norm_layer) {
+    MER_REQUIRE(out_format == MER_EPI_SPLIT_BF16, "mer_hubert_conv0: the LayerNorm family writes split-bf16 rows only");
+    MER_REQUIRE(model->conv_ln_g[0] && model->conv_ln_b[0], "mer_hubert_conv0: LayerNorm affine missing");
+    return mer_hubert_conv0_ln_launch(wave, ld_wave, batch, n_samples, model->conv0_w, model->conv_b[0],
+                                      model->conv_ln_g[0], model->conv_ln_b[0], static_cast<float*>(out), out_bstride, s);
+  }
+  MER_REQUIRE(out_format == MER_EPI_SPLIT_BF16 || (out_format == MER_EPI_OUT_F16 && out_bstride % 2 == 0),
+              "mer_hubert_conv0: output format %d (split-bf16 = %d, or fp16 = %d with an even batch stride)", out_format,
+              (int)MER_EPI_SPLIT_BF16, (int)MER_EPI_OUT_F16);
+  MER_REQUIRE(model->gn_g && model->gn_b, "mer_hubert_conv0: GroupNorm affine missing");
+  const long long need = mer_hubert_conv0_workspace_bytes(batch);
+  MER_REQUIRE(workspace && workspace_bytes >= need && reinterpret_cast<uintptr_t>(workspace) % 16 == 0,
+              "mer_hubert_conv0: workspace %lld B < required %lld B, or not 16-byte aligned", workspace_bytes, need);
+  return mer_hubert_conv0_launch(wave, ld_wave, batch, n_samples, model->conv0_w, model->gn_g, model->gn_b,
+                                 static_cast<double*>(workspace), static_cast<float*>(out), out_bstride,
+                                 out_format == MER_EPI_OUT_F16 ? 2 : 1, s, frames);
+}
+
+// the moments ([batch, 128] doubles, MOM_LD used) and then the coefficients ([batch, 512] float2)
+extern "C" long long mer_hubert_conv0_workspace_bytes(int batch) {
+  return batch > 0 ? (long long)batch * (128 * sizeof(double) + C0 * sizeof(float2)) : 0;
+}

@@ -8,6 +8,7 @@ import os
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 U32 = 2.0 ** -24  # unit roundoff of fp32 (round to nearest)
 
@@ -103,6 +104,253 @@ def wave_normalize(x):
     mu = x.mean(-1, keepdim=True)
     var = ((x - mu) ** 2).mean(-1, keepdim=True)
     return (x - mu) / torch.sqrt(var + 1e-7)
+
+
+# ---- HuBERT front end: conv0 (mer_hubert_conv0) ------------------------------------------------------------------------
+# Elementwise bounds of the kernels against the float64 reference on the same fp32 samples, u = 2^-24, A = |w| * |x|
+# (the conv of the absolute values; + |bias| for the LayerNorm form), n = the clip's frame count.
+#
+# GroupNorm form (conv0_moments / conv0_coef / conv0_apply(2)):
+#   conv     the fp32 chain of 10 fma: <= 10 u A (every rounding is <= u times a partial sum, and |partial| <= A).
+#   mean     rounded to float: u |mean|; its double sums add <= (n + 11) 2^-53 mean_t(A).
+#   variance q / n - mean^2 from double moments: each moment is a sum of n exact products (in chunks, in any order),
+#            and q combines the 55 products with 55 more fma, so |dvar| <= (3 n + 100) 2^-53 mean_t(A^2).  Relative to
+#            var + eps this is the conditioning kappa = mean_t(A^2) / (var + eps) times (3 n + 100) 2^-53: a clip with a
+#            DC offset has a large kappa (the cancellation the double moments exist to absorb).
+#   scale    g = gamma * float(1 / sqrt(var + eps)): relative 0.5 |dvar| / (var + eps) + 2 u (the float conversion and
+#            the fp32 product with gamma).
+#   affine   d = y - mean rounds (u |d|), z = d g + beta rounds once or twice (u (|z| + |d g|)); d carries the conv and
+#            mean errors, g its relative error: |dz| <= |g| (10 u A + u |mean| + u |d|) + |d g| rg + u (|z| + |d g|).
+#   GELU     slope <= 1.13; gelu_erf_fast's own error <= min(4.7e-7, 2.9e-7 |z|) (mer_common.cuh), + u |GELU|.
+#   output   split bf16 hi + lo: 2^-17 relative; fp16: half an ulp, max(2^-11 |v|, 2^-25).
+# Second-order terms (a u-sized error of a u-sized error) are covered by the +1 in 11 u for the conv chain.
+#
+# LayerNorm form (conv0_ln_kernel): the conv + bias chain (11 fma, <= 11 u A) carried through the LayerNorm's
+# derivative, |gamma| / sigma (|e| + mean_c |e| + |zhat| mean_c(|zhat| |e|)), plus the two-pass fp32 LayerNorm's own
+# error (layernorm_bound), then GELU and the output rounding as above.
+#
+# What the bounds tell apart (tests/test_kernel_refs.py): a variance divided by n - 1 instead of n (relative 1 / n:
+# 6e-5 on a 5 s clip) and an eps of 1e-7 instead of 1e-5 on channels whose variance is not far above eps.
+CONV0_EPS = 1e-5
+GELU_SLOPE = 1.13
+U53 = 2.0 ** -53
+
+
+def gelu_fast_error(z):
+    return torch.minimum(torch.full_like(z, 4.7e-7), 2.9e-7 * z.abs())
+
+
+def out_rounding(v, f16):
+    return torch.clamp(2.0 ** -11 * v.abs(), min=2.0 ** -25) if f16 else 2.0 ** -17 * v.abs()
+
+
+def speech_like(n, seed, dc=0.0, noise=1.0):
+    """A seeded fp32 [n] waveform: a few amplitude-modulated harmonics plus white noise, then `dc` added."""
+    g = torch.Generator().manual_seed(seed)
+    t = torch.arange(n, dtype=torch.float64) / 16000.0
+    f0 = 110.0 + 60.0 * float(torch.rand(1, generator=g))
+    x = sum(torch.sin(2 * math.pi * f0 * h * t + float(torch.rand(1, generator=g)) * 6.0) / h for h in (1, 2, 3, 5))
+    x = x * (0.6 + 0.4 * torch.sin(2 * math.pi * 3.0 * t))
+    return (x + noise * 0.3 * torch.randn(n, generator=g, dtype=torch.float64) + dc).float()
+
+
+def conv0_weights(seed):
+    """(w0 [512, 10], gamma, beta, bias) for conv0 tests: He-scaled taps, with every third channel scaled by 1e-3 and
+    every third by 3e-3, so that a normalised clip gives channel variances around eps (1e-5) as well as around 2."""
+    g = torch.Generator().manual_seed(seed)
+    w = torch.randn(512, 10, generator=g) * math.sqrt(2.0 / 10)
+    w[1::3] *= 1e-3
+    w[2::3] *= 3e-3
+    gamma = 1.0 + 0.1 * torch.randn(512, generator=g)
+    beta = 0.1 * torch.randn(512, generator=g)
+    bias = 0.05 * torch.randn(512, generator=g)
+    return w, gamma, beta, bias
+
+
+def conv0(wave, w0, bias=None):
+    """Conv1d(1 -> 512, k 10, s 5) in float64: (y, A) as [B, T0, 512], A = |w| * |x| (+ |bias|)."""
+    x = wave.double()[:, None]
+    w = w0.double().reshape(512, 1, 10)
+    y = F.conv1d(x, w, None if bias is None else bias.double(), stride=5).transpose(1, 2)
+    a = F.conv1d(x.abs(), w.abs(), None if bias is None else bias.double().abs(), stride=5).transpose(1, 2)
+    return y, a
+
+
+def conv0_moments(wave, n):
+    """The 10 tap sums X_k = sum_t x[5 t + k] and the 10 x 10 tap products R_kk' of the first n frames of each row."""
+    x = wave.double()
+    taps = torch.stack([x[:, k:k + 5 * (n - 1) + 1:5] for k in range(10)], -1)   # [B, n, 10]
+    return taps.sum(1), taps.transpose(1, 2) @ taps
+
+
+def conv0_stats_from_moments(X, R, w0, n):
+    """Per-channel (mean, biased variance) of conv0 from the moments: sum_k w_k X_k / n and w R w^T / n - mean^2."""
+    w = w0.double().reshape(512, 10)
+    mean = X @ w.T / n
+    q = torch.einsum("ck,bkl,cl->bc", w, R, w)
+    return mean, q / n - mean * mean
+
+
+def hubert_conv0(wave, w0, gamma, beta, family="group", bias=None, frames=None, f16=False, eps=CONV0_EPS,
+                 var_div=None):
+    """First layer of the feature encoder in float64: conv0, then GroupNorm(512 groups, biased variance over the clip's
+    first frames[b] frames, or all) -- family "group" -- or conv bias + LayerNorm(512) -- family "layer" -- then exact
+    GELU.  Returns (out [B, T0, 512], elementwise bound of the kernel's error, see above; f16: fp16 output rows).
+    var_div (tests of the bound only): divide the sum of squares by frames + var_div instead of frames."""
+    y, A = conv0(wave, w0, bias if family == "layer" else None)
+    B, T0, _ = y.shape
+    g = gamma.double()
+    if family == "layer":
+        mu = y.mean(-1, keepdim=True)
+        sig = torch.sqrt(((y - mu) ** 2).mean(-1, keepdim=True) + eps)
+        zh = (y - mu) / sig
+        z = zh * g + beta.double()
+        e = 11 * U32 * A
+        dz = g.abs() / sig * (e + e.mean(-1, keepdim=True) + zh.abs() * (zh.abs() * e).mean(-1, keepdim=True))
+        dz = dz + layernorm_bound(y, gamma, z, eps)
+    else:
+        ns = [T0] * B if frames is None else [int(f) for f in frames]
+        mean = torch.stack([y[b, :ns[b]].mean(0) for b in range(B)])[:, None]            # [B, 1, 512]
+        ss = torch.stack([((y[b, :ns[b]] - mean[b]) ** 2).sum(0) for b in range(B)])[:, None]
+        n = torch.tensor(ns, dtype=torch.float64, device=y.device)[:, None, None]
+        var = ss / (n + (var_div or 0))
+        A2 = torch.stack([(A[b, :ns[b]] ** 2).mean(0) for b in range(B)])[:, None]
+        A1 = torch.stack([A[b, :ns[b]].mean(0) for b in range(B)])[:, None]
+        rg = 0.5 * (3 * n + 100) * U53 * A2 / (var + eps) + 2 * U32
+        gs = g / torch.sqrt(var + eps)
+        d = y - mean
+        z = d * gs + beta.double()
+        dg = (d * gs).abs()
+        dz = gs.abs() * (11 * U32 * A + U32 * mean.abs() + (n + 11) * U53 * A1 + U32 * d.abs()) + dg * rg + \
+            U32 * (z.abs() + dg)
+    out = gelu_erf(z)
+    bound = GELU_SLOPE * dz + gelu_fast_error(z) + U32 * out.abs()
+    return out, bound + out_rounding(out, f16 and family != "layer")
+
+
+# ---- HuBERT front end: hidden_states[0] (mer_hubert_frontend) ----------------------------------------------------------
+# The reference is oracle.encoders.hubert_hidden_states(layers=0) in float64, restated stage by stage so that each stage
+# can carry an elementwise error bound e next to its value v:
+#   linear / conv  v = W a (+ b).  Every error here is treated as the sum of independent, mean-zero roundings (the
+#                  probabilistic analysis of Higham and Mary, with lambda = 4 standard deviations): the error carried in,
+#                  sqrt(W^2 e^2), plus the stage's own, 4 sqrt(u_op^2 + K u^2) sqrt(W^2 a^2): u_op = the operands'
+#                  unit (split bf16 hi + lo for activations and weights, the dropped lo * lo: 2^-15; fp16 or tf32
+#                  activations of fp16-exact weights: 2^-11; fp16 rows already rounded: 0), K u the fp32 accumulation
+#                  of K products.  The worst case, |W| e and (u_op + K u) |W| |a|, grows by ~sqrt(K) per stage (~40 for
+#                  K = 1536, 40^6 over the conv stack) and would bound nothing.
+#   GELU           |GELU'(z)| e + 0.4 e^2 (|GELU''| <= 0.8), + gelu_erf_fast's own error and u |v|.
+#   LayerNorm      the derivative's gain |gamma| / sigma times e (the rest of the derivative is an orthogonal projection,
+#                  which does not enlarge independent errors), + layernorm_bound.
+#   rows           + 2^-17 |v| for split-bf16 rows, max(2^-11 |v|, 2^-25) for fp16 rows, u |v| for an fp32 add.
+# Unlike the conv0 bound this one is not a worst case; it is far above the errors the front end makes and far below
+# the error of a misplaced frame or channel.
+LAMBDA = 4.0
+
+
+def _lin_err(conv, v, e, w, u_op, K):
+    return torch.sqrt(conv(e * e, w * w).clamp(min=0.0)) + \
+        LAMBDA * math.sqrt(u_op ** 2 + K * U32 ** 2) * torch.sqrt(conv(v * v, w * w).clamp(min=0.0))
+
+
+def _ln_err(x, e, gamma, beta, eps):
+    mu = x.mean(-1, keepdim=True)
+    sig = torch.sqrt(((x - mu) ** 2).mean(-1, keepdim=True) + eps)
+    zh = (x - mu) / sig
+    y = zh * gamma + beta
+    return y, gamma.abs() / sig * e + layernorm_bound(x, gamma, y, eps)
+
+
+def _gelu_err(z, e):
+    g = gelu_erf(z)
+    slope = (0.5 * (1.0 + torch.erf(z / math.sqrt(2.0))) + z * torch.exp(-0.5 * z * z) / math.sqrt(2 * math.pi)).abs()
+    return g, slope * e + 0.4 * e * e + gelu_fast_error(z) + U32 * g.abs()
+
+
+def fp16_exact_front_end(sd):
+    """A copy of a HuBERT-family state dict whose fp16-operand weights are fp16-exact: the positional conv stored as its
+    folded `weight` (no weight norm) rounded to fp16, conv1 and conv2, and the data2vec chain's convs."""
+    from mertools_b200.encoders import fold_pos_conv_weight
+    r16 = lambda v: np.asarray(v, np.float32).astype(np.float16).astype(np.float32)  # noqa: E731
+    out = dict(sd)
+    pre = "encoder.pos_conv_embed.conv."
+    if pre + "parametrizations.weight.original0" in sd:
+        out[pre + "weight"] = r16(fold_pos_conv_weight(sd))
+        del out[pre + "parametrizations.weight.original0"], out[pre + "parametrizations.weight.original1"]
+    for k in list(out):
+        if k.startswith(("feature_extractor.conv_layers.1.conv.weight", "feature_extractor.conv_layers.2.conv.weight",
+                         "encoder.pos_conv_embed.layers.")) and k.endswith("conv.weight"):
+            out[k] = r16(out[k])
+    return out
+
+
+def hubert_hidden0(sd, wave, conv_f16=False, ln_eps=1e-5):
+    """(hidden_states[0] [B, T, D], bound) of the HuBERT-family front end on fp32 input values `wave` [B, n] (already
+    normalised when the model normalises).  conv_f16: conv1 and conv2 on fp16 operands (group-norm feature encoder).
+    The positional conv's unit is 2^-11 in both of its forms (fp16 activations in the windowed GEMM, tf32 in the
+    mma.sync kernel).  The fp16-operand weights must be fp16-exact (fp16_exact_front_end): the bound has no term for
+    their rounding."""
+    dev = wave.device
+    t = lambda k: torch.as_tensor(np.asarray(sd[k])).to(dev, torch.float64)  # noqa: E731
+    cl = "feature_extractor.conv_layers."
+    ln_convs = cl + "1.layer_norm.weight" in sd
+    data2vec = "encoder.pos_conv_embed.layers.0.conv.weight" in sd
+    stable = ln_convs and not data2vec
+    w0 = t(cl + "0.conv.weight").reshape(512, 10)
+    b0 = t(cl + "0.conv.bias") if cl + "0.conv.bias" in sd else None
+    a, e = hubert_conv0(wave, w0, t(cl + "0.layer_norm.weight"), t(cl + "0.layer_norm.bias"),
+                        family="layer" if ln_convs else "group", bias=b0, f16=conv_f16)
+    a, e = a.transpose(1, 2), e.transpose(1, 2)                                  # [B, 512, T]
+    for i in range(1, 7):
+        w = t(cl + f"{i}.conv.weight")
+        bias = t(cl + f"{i}.conv.bias") if cl + f"{i}.conv.bias" in sd else None
+        conv = lambda x, ww: F.conv1d(x, ww, stride=2)  # noqa: E731
+        f16_in = conv_f16 and i <= 2
+        z = F.conv1d(a, w, bias, stride=2)
+        ez = _lin_err(conv, a, e, w, 0.0 if f16_in else 2.0 ** -15, w.shape[1] * w.shape[2])
+        if bias is not None:
+            ez = ez + U32 * bias.abs()[:, None]
+        if ln_convs:
+            z, ez = (v.transpose(1, 2) for v in _ln_err(z.transpose(1, 2), ez.transpose(1, 2),
+                                                        t(cl + f"{i}.layer_norm.weight"),
+                                                        t(cl + f"{i}.layer_norm.bias"), 1e-5))
+        a, e = _gelu_err(z, ez)
+        if i < 6:
+            e = e + out_rounding(a, conv_f16 and i == 1)
+    a, e = _ln_err(a.transpose(1, 2), e.transpose(1, 2), t("feature_projection.layer_norm.weight"),
+                   t("feature_projection.layer_norm.bias"), ln_eps)
+    e = e + out_rounding(a, False)
+    w = t("feature_projection.projection.weight")
+    x0 = a @ w.T + t("feature_projection.projection.bias")
+    e0 = _lin_err(lambda x, ww: x @ ww.T, a, e, w, 2.0 ** -15, w.shape[1]) + U32 * x0.abs()
+    D = x0.shape[-1]
+    g = 16
+    if data2vec:
+        p, ep, l = x0.transpose(1, 2), e0.transpose(1, 2), 0
+        while f"encoder.pos_conv_embed.layers.{l}.conv.weight" in sd:
+            w = t(f"encoder.pos_conv_embed.layers.{l}.conv.weight")
+            k = w.shape[-1]
+            conv = lambda x, ww: F.conv1d(x, ww, padding=k // 2, groups=g)  # noqa: E731
+            z = F.conv1d(p, w, t(f"encoder.pos_conv_embed.layers.{l}.conv.bias"), padding=k // 2, groups=g)
+            ez = _lin_err(conv, p, ep, w, 2.0 ** -11, w.shape[1] * k) + U32 * z.abs()
+            ones = torch.ones(D, dtype=torch.float64, device=dev)
+            z, ez = _ln_err(z.transpose(1, 2), ez.transpose(1, 2), ones, ones * 0, 1e-5)
+            p, ep = (v.transpose(1, 2) for v in _gelu_err(z, ez))
+            l += 1
+        x = x0 + p.transpose(1, 2)
+        ex = e0 + ep.transpose(1, 2) + U32 * x.abs()
+    else:
+        from oracle.encoders import hubert_pos_conv_weight
+        w = hubert_pos_conv_weight(sd, torch.float64).to(dev)
+        conv = lambda x, ww: F.conv1d(x, ww, padding=64, groups=g)[:, :, :-1]  # noqa: E731
+        xt, et = x0.transpose(1, 2), e0.transpose(1, 2)
+        z = conv(xt, w) + t("encoder.pos_conv_embed.conv.bias")[:, None]
+        ez = _lin_err(conv, xt, et, w, 2.0 ** -11, w.shape[1] * 128) + U32 * z.abs()
+        p, ep = _gelu_err(z, ez)
+        x = x0 + p.transpose(1, 2)
+        ex = e0 + ep.transpose(1, 2) + U32 * x.abs()
+    if not stable:
+        x, ex = _ln_err(x, ex, t("encoder.layer_norm.weight"), t("encoder.layer_norm.bias"), ln_eps)
+    return x, ex
 
 
 def attention_packed(qkv, cu, heads):

@@ -241,3 +241,93 @@ def test_adam_f64_is_torch_adam_after_clip_grad_value():
             # torch moves exp_avg by lerp (m + (1 - beta1) (g - m)): the two forms differ by float64 roundings only
             for mine, theirs in ((p, w.detach()), (m, st["exp_avg"]), (v, st["exp_avg_sq"])):
                 assert float((mine - theirs).abs().max()) <= 1e-14 * float(theirs.abs().max())
+
+
+# ---- HuBERT conv0 ------------------------------------------------------------------------------------------------------
+def _normalised(x):
+    return R.wave_normalize(x[None]).float()
+
+
+@pytest.mark.parametrize("frames", [1, 2, 1024, 1025, 15999])
+def test_conv0_statistics_from_tap_moments_are_group_norms(frames):
+    """The identity the GroupNorm statistics kernels rest on: per channel, the mean and biased variance of conv0 over a
+    clip follow from the 10 tap sums and the 55 tap products of the waveform, so the normalised output equals
+    F.group_norm's (num_groups = channels) in float64 -- on a normalised clip and on one with a DC offset 100x its
+    noise.  Three samples past the last window make no frame and must not count."""
+    w0, _, _, _ = R.conv0_weights(0)
+    n = 5 * (frames - 1) + 10 + 3
+    for x in (_normalised(R.speech_like(n, 1)), R.speech_like(n, 2, dc=30.0)[None]):
+        y, _ = R.conv0(x, w0)
+        assert y.shape[1] == frames
+        X, Rm = R.conv0_moments(x, frames)
+        mean, var = R.conv0_stats_from_moments(X, Rm, w0, frames)
+        var = var.clamp(min=0.0)
+        yt = y.transpose(1, 2)
+        # (F.group_norm refuses one value per group; over a single frame it is F.layer_norm over time)
+        want = (F.group_norm(yt, 512, None, None, R.CONV0_EPS) if frames > 1 else
+                F.layer_norm(yt, (1,), None, None, R.CONV0_EPS)).transpose(1, 2)
+        got = (y - mean[:, None]) / torch.sqrt(var[:, None] + R.CONV0_EPS)
+        assert float((got - want).abs().max()) < 1e-7, frames
+
+
+def test_conv0_reference_is_the_oracles_first_layer():
+    """hubert_conv0 = conv0 -> GroupNorm -> GELU (HubertGroupNormConvLayer) and conv0 + bias -> LayerNorm -> GELU
+    (HubertLayerNormConvLayer) in float64; with `frames`, GroupNorm over each clip's own first frames."""
+    w0, gamma, beta, bias = R.conv0_weights(3)
+    x = torch.stack([_normalised(R.speech_like(4005, s))[0] for s in (4, 5)])
+    w = w0.double().view(512, 1, 10)
+    y = F.conv1d(x.double()[:, None], w, stride=5)
+    want = F.gelu(F.group_norm(y, 512, gamma.double(), beta.double(), 1e-5)).transpose(1, 2)
+    got, _ = R.hubert_conv0(x, w0, gamma, beta)
+    assert float((got - want).abs().max()) < 1e-12
+    yb = F.conv1d(x.double()[:, None], w, bias.double(), stride=5).transpose(1, 2)
+    want = F.gelu(F.layer_norm(yb, (512,), gamma.double(), beta.double(), 1e-5))
+    got, _ = R.hubert_conv0(x, w0, gamma, beta, family="layer", bias=bias)
+    assert float((got - want).abs().max()) < 1e-12
+    got, _ = R.hubert_conv0(x, w0, gamma, beta, frames=[799, 300])
+    for b, n in ((0, 799), (1, 300)):
+        one = F.gelu(F.group_norm(y[b:b + 1, :, :n], 512, gamma.double(), beta.double(), 1e-5)).transpose(1, 2)[0]
+        assert float((got[b, :n] - one).abs().max()) < 1e-12
+
+
+def test_conv0_bound_rejects_the_statistics_mutations():
+    """The GroupNorm-form bound is tight enough to tell apart, on a 5 s clip (15,999 frames): a variance divided by
+    n - 1 (a relative change of 6e-5), and an eps of 1e-7 instead of 1e-5 (on the channels whose variance is near
+    eps).  It holds the float64 reference itself and, for a DC offset 100x the noise (normalize off), the
+    conditioning kappa = mean(A^2) / (var + eps) that the double moments must absorb stays within the bound's reach."""
+    w0, gamma, beta, _ = R.conv0_weights(6)
+    x = _normalised(R.speech_like(80000, 7))
+    ref, bound = R.hubert_conv0(x, w0, gamma, beta)
+    for kw in (dict(var_div=-1), dict(eps=1e-7)):
+        mut, _ = R.hubert_conv0(x, w0, gamma, beta, **kw)
+        assert float(((mut - ref).abs() / bound).max()) > 4, kw
+    # the LayerNorm form's eps on quiet frames (amplitude 1e-3, no bias: the channel variance is ~1e-6 there)
+    q = x * 1e-3
+    ref, bound = R.hubert_conv0(q, w0, gamma, beta, family="layer")
+    mut, _ = R.hubert_conv0(q, w0, gamma, beta, family="layer", eps=1e-6)
+    assert float(((mut - ref).abs() / bound).max()) > 4
+    # a DC offset 100x the noise: kappa is pinned, and the cancellation term it costs stays below 1e-5 of var + eps
+    xd = R.speech_like(80000, 8, dc=100.0, noise=1.0)[None]
+    y, A = R.conv0(xd, w0)
+    kappa = float(((A ** 2).mean(1) / (y.var(1, unbiased=False) + R.CONV0_EPS)).max())
+    assert 1e3 < kappa < 1e6, kappa
+    assert (3 * 16000 + 100) * R.U53 * kappa < 1e-5
+
+
+@pytest.mark.parametrize("family", ["base", "large", "large_gn", "data2vec"])
+def test_hidden0_reference_is_the_oracle_at_layer_0(family):
+    """hubert_hidden0 (the stage-by-stage restatement that carries the error bound) equals the oracle's hidden_states[0]
+    in float64: hubert_hidden_states(layers=0) for the post-LN families, the input of layer 0 for the stable one."""
+    from mertools_b200.synthetic import hubert_state_dict
+    from oracle.encoders import hubert_hidden_states
+    kw = dict(base={}, large=dict(large=True), large_gn=dict(large=True, group_norm=True),
+              data2vec=dict(data2vec=True))[family]
+    sd = R.fp16_exact_front_end(hubert_state_dict(seed=5, layers=1, **kw))
+    sdt = {k: torch.as_tensor(np.asarray(v)) for k, v in sd.items()}
+    x = torch.stack([_normalised(R.speech_like(6407, s))[0] for s in (8, 9)])
+    got, bound = R.hubert_hidden0(sd, x)
+    heads = 16 if family.startswith("large") else 12
+    want = hubert_hidden_states(sdt, x, layers=1 if family == "large" else 0, heads=heads, dtype=torch.float64)[0]
+    assert got.shape == want.shape == (2, 19, 1024 if family.startswith("large") else 768)
+    assert float((got - want).abs().max()) < 1e-10
+    assert bool((bound > 0).all()) and float((bound / want.abs().clamp(min=1e-3)).median()) < 5e-2
