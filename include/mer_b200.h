@@ -580,6 +580,12 @@ MER_API int mer_rmsnorm(const float* x, const float* w, void* y16, float* acc, l
  * A position outside [0, max_pos) turns the token's q | k into NaN. */
 MER_API int mer_rope_f16(void* qkv16, long long ld, long long tokens, int heads, const int32_t* cu_seqlens, int n_seq,
                          const int32_t* positions, const float* cos_t, const float* sin_t, int max_pos, void* stream);
+/* mer_rope_f16 over the first rot_heads heads of head_dim 64 or 128 of each row (Falcon: 71 q heads + its one k head),
+ * cos_t / sin_t [max_pos, head_dim / 2].  At head_dim 128 with rot_heads = 2 * heads it computes what mer_rope_f16
+ * does.  Any other head_dim returns an error before any launch. */
+MER_API int mer_rope_hd_f16(void* qkv16, long long ld, long long tokens, int rot_heads, int head_dim,
+                            const int32_t* cu_seqlens, int n_seq, const int32_t* positions, const float* cos_t,
+                            const float* sin_t, int max_pos, void* stream);
 /* Causal softmax(Q K^T / sqrt(128)) V per (sequence, head), head_dim 128 (HF LlamaAttention).  qkv16: fp16 [tokens,
  * 3 * heads * 128] with Q | K column blocks (V columns not read), sequences packed back to back, cu_seqlens [n_seq + 1]
  * (device int32); vt16: fp16 V^T [heads * 128, vt_ld] (vt_ld >= tokens, multiple of 8) as written by mer_gemm's
@@ -611,6 +617,24 @@ MER_API int mer_causal_alibi_attention_f16(const void* qkv16, const void* vt16, 
  * last-four readout). */
 MER_API int mer_layernorm_f16(const float* x, const float* gamma, const float* beta, void* y16, float* y32, float* acc,
                               long long rows, int dim, float eps, void* stream);
+
+/* ---- Falcon-7B (HF FalconModel, parallel attention, multi-query; extract_text_huggingface.py:188-196; orchestrated from
+ * the host in mertools_b200/extract/ln_decoder_text.py over these, mer_gemm (MER_EPI_GELU | MER_EPI_OUT_F16) and
+ * mer_layernorm_ld_f16, with hidden-wide rows padded to a multiple of 128 columns). ---- */
+/* mer_causal_attention_hd_f16 at head_dim 64 with one K / V head shared by every query head (HF FalconAttention,
+ * multi_query): qkv16 fp16 [tokens, qkv_ld] with Q in columns [0, heads * 64) and K in [heads * 64, heads * 64 + 64)
+ * (other columns not read); vt16 fp16 V^T [64, vt_ld] (vt_ld >= tokens, multiple of 8); ctx16 fp16 [tokens, heads * 64].
+ * Scores scaled by 1 / 8; same masking and limits as mer_causal_attention_f16.  Refused with a
+ * "mer_causal_mqa_attention_f16:" message before any launch: heads outside 1 .. 65535, qkv_ld below (heads + 1) * 64 or
+ * not a multiple of 8, a bad V^T pitch, n_seq outside 1 .. 65535, max_seqlen outside 1 .. tokens, a NULL operand. */
+MER_API int mer_causal_mqa_attention_f16(const void* qkv16, long long qkv_ld, const void* vt16, long long vt_ld,
+                                         void* ctx16, const int32_t* cu_seqlens, int n_seq, long long tokens,
+                                         int max_seqlen, int heads, void* stream);
+/* mer_layernorm_f16 over the first dim columns (dim % 64 == 0, <= 8192) of fp32 rows of pitch ld (ld >= dim, multiple
+ * of 4); y16 / y32 / acc have the same pitch and only their first dim columns are written.  With ld == dim it computes
+ * what mer_layernorm_f16 does. */
+MER_API int mer_layernorm_ld_f16(const float* x, long long ld, const float* gamma, const float* beta, void* y16,
+                                 float* y32, float* acc, long long rows, int dim, float eps, void* stream);
 
 /* ---- DeBERTa / DeBERTa-v2 encoders (extract_text_huggingface.py:164-166 and the AutoModel branch; orchestrated from the
  * host in mertools_b200/extract/deberta_text.py over this, mer_gemm, mer_layernorm / mer_layernorm_f16 and

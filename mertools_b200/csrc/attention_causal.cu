@@ -23,6 +23,11 @@
 // and j counted from the sequence start (not the packed position).  HF adds slope_h * j; the per-row constant
 // slope_h * i cancels in the softmax, and with (j - i) <= 0 the bias stays bounded however long the row is.  Masked and
 // foreign keys stay -inf.  ALIBI = false is the LLaMA kernel, unchanged.  ALiBi is instantiated at HD = 128 only.
+//
+// Multi-query variant (template MQA = true; HF FalconAttention with multi_query, mertools_b200/extract/ln_decoder_text.py):
+// every query head reads the one K head and the one V^T head.  Q is columns [0, heads * HD) of qkv rows of pitch qkv_ld,
+// K the next HD columns, V^T is [HD, vt_ld].  Only the row pitch, the K column base and the V^T row base differ from the
+// plain kernel; nothing is expanded to `heads` copies.  Instantiated at HD = 64 only.
 #include "mer_common.cuh"
 #include "mer_kernels.h"
 
@@ -61,13 +66,14 @@ __device__ __forceinline__ float fast_ex2(float x) {
   return y;
 }
 
-template <int HD, bool ALIBI>
+template <int HD, bool ALIBI, bool MQA>
 __global__ void __launch_bounds__(THREADS, 2)
 causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __restrict__ vt_, long long vt_ld,
                         uint16_t* __restrict__ ctx, const int* __restrict__ cu_seqlens, long long tokens, int heads,
-                        const float* __restrict__ slopes) {
+                        const float* __restrict__ slopes, long long qkv_ld) {
   static_assert(HD == 64 || HD == 96 || HD == 128, "head_dim 64, 96 or 128");
   static_assert(!ALIBI || HD == 128, "the ALiBi kernel is head_dim 128 only");
+  static_assert(!MQA || (HD == 64 && !ALIBI), "the multi-query kernel is head_dim 64 only, without ALiBi");
   constexpr int LDK_ = LDK<HD>, K_TILE_ = K_TILE<HD>, V_TILE_ = V_TILE<HD>;
   extern __shared__ __align__(16) uint8_t smem_att[];
   uint16_t* Ks = reinterpret_cast<uint16_t*>(smem_att);  // [2][BKV][LDK_]
@@ -82,10 +88,10 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
-  const long long ld = 3ll * heads * HD;
+  const long long ld = MQA ? qkv_ld : 3ll * heads * HD;
   const uint16_t* qbase = qkv + (long long)start * ld + h * HD;
-  const uint16_t* kbase = qkv + heads * HD + h * HD;  // row = absolute token index
-  const uint16_t* vtbase = vt_ + (long long)h * HD * vt_ld;
+  const uint16_t* kbase = qkv + heads * HD + (MQA ? 0 : h * HD);  // row = absolute token index
+  const uint16_t* vtbase = vt_ + (MQA ? 0ll : (long long)h * HD * vt_ld);
 
   const int row_lo = q0 + warp * 16 + g, row_hi = row_lo + 8;
   // last key each row may see (rows past the sequence end are computed on clamped data and never stored)
@@ -249,10 +255,10 @@ causal_attention_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __rest
   }
 }
 
-template <int HD, bool ALIBI>
+template <int HD, bool ALIBI, bool MQA = false>
 int launch_causal(const char* name, const void* qkv16, const void* vt16, long long vt_ld, void* ctx16,
                   const int32_t* cu_seqlens, int n_seq, long long tokens, int max_seqlen, int heads,
-                  const float* slopes, cudaStream_t stream) {
+                  const float* slopes, cudaStream_t stream, long long qkv_ld = 0) {
   MER_REQUIRE(qkv16 && vt16 && ctx16 && cu_seqlens, "%s: null operand", name);
   MER_REQUIRE(vt_ld >= tokens && vt_ld % 8 == 0, "%s: V^T pitch %lld must be a multiple of 8 >= tokens", name, vt_ld);
   MER_REQUIRE(max_seqlen > 0 && max_seqlen <= tokens, "%s: max_seqlen %d (1 .. tokens %lld)", name, max_seqlen, tokens);
@@ -260,14 +266,14 @@ int launch_causal(const char* name, const void* qkv16, const void* vt16, long lo
               heads, n_seq);
   static MerPerDevice attr_set;
   if (attr_set.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(causal_attention_kernel<HD, ALIBI>,
+    MER_CUDA_CHECK(cudaFuncSetAttribute(causal_attention_kernel<HD, ALIBI, MQA>,
                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM<HD>));
     attr_set.mark();
   }
   dim3 grid((max_seqlen + BQ - 1) / BQ, heads, n_seq);
-  causal_attention_kernel<HD, ALIBI><<<grid, THREADS, SMEM<HD>, stream>>>(
+  causal_attention_kernel<HD, ALIBI, MQA><<<grid, THREADS, SMEM<HD>, stream>>>(
       static_cast<const uint16_t*>(qkv16), static_cast<const uint16_t*>(vt16), vt_ld, static_cast<uint16_t*>(ctx16),
-      cu_seqlens, tokens, heads, slopes);
+      cu_seqlens, tokens, heads, slopes, qkv_ld);
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
   return 0;
@@ -307,4 +313,15 @@ extern "C" int mer_causal_attention_hd_f16(const void* qkv16, const void* vt16, 
       return launch_causal<128, false>(name, qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens, max_seqlen, heads,
                                        nullptr, stream);
   }
+}
+
+extern "C" int mer_causal_mqa_attention_f16(const void* qkv16, long long qkv_ld, const void* vt16, long long vt_ld,
+                                            void* ctx16, const int32_t* cu_seqlens, int n_seq, long long tokens,
+                                            int max_seqlen, int heads, void* stream_) {
+  const char* name = "mer_causal_mqa_attention_f16";
+  MER_REQUIRE(heads > 0 && heads <= 65535, "%s: %d heads (1 .. 65535)", name, heads);
+  MER_REQUIRE(qkv_ld >= (heads + 1ll) * 64 && qkv_ld % 8 == 0,
+              "%s: qkv pitch %lld must be a multiple of 8 >= (heads + 1) * 64 = %lld", name, qkv_ld, (heads + 1ll) * 64);
+  return launch_causal<64, false, true>(name, qkv16, vt16, vt_ld, ctx16, cu_seqlens, n_seq, tokens, max_seqlen, heads,
+                                        nullptr, static_cast<cudaStream_t>(stream_), qkv_ld);
 }

@@ -47,10 +47,11 @@ def rope_theta(cfg):
     return float(rope.get("rope_theta", getattr(cfg, "rope_theta", 10000.0)))
 
 
-def rope_tables(max_pos, theta):
-    """cos / sin [max_pos, 64] fp32 built as HF LlamaRotaryEmbedding builds them: fp32 inv_freq, fp32 angle
-    pos * inv_freq, torch.cos / torch.sin (the table's columns j and j + 64 of HF's cat(freqs, freqs) are equal)."""
-    inv_freq = 1.0 / (theta ** (torch.arange(0, HEAD_DIM, 2, dtype=torch.int64).to(torch.float32) / HEAD_DIM))
+def rope_tables(max_pos, theta, head_dim=HEAD_DIM):
+    """cos / sin [max_pos, head_dim / 2] fp32 built as HF LlamaRotaryEmbedding (and FalconRotaryEmbedding) builds them:
+    fp32 inv_freq, fp32 angle pos * inv_freq, torch.cos / torch.sin (the table's columns j and j + head_dim / 2 of HF's
+    cat(freqs, freqs) are equal)."""
+    inv_freq = 1.0 / (theta ** (torch.arange(0, head_dim, 2, dtype=torch.int64).to(torch.float32) / head_dim))
     freqs = torch.arange(max_pos, dtype=torch.int64).to(torch.float32)[:, None] * inv_freq[None, :]
     return freqs.cos().contiguous(), freqs.sin().contiguous()
 

@@ -1,7 +1,8 @@
 """Lexical feature extraction — H100 mirror of
 MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; DeBERTa / DeBERTa-v2 through
 extract/deberta_text.py, XLNet through extract/xlnet_text.py and ALBERT through extract/albert_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
-extract/ln_decoder_text.py, saved as float16 like the reference's fp16 GPU run; GPT-2 through extract/ln_decoder_text.py,
+extract/ln_decoder_text.py (BLOOM / OPT / Falcon), saved as float16 like the reference's fp16 GPU run; GPT-2 through
+extract/ln_decoder_text.py,
 float32 like the reference's fp32 run of it).
 
 Keeps ``extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu, punc_case, language,
@@ -144,8 +145,8 @@ def _llama_extractor(model_name, model_dir, cfg, device):
 
 
 def _ln_decoder_extractor(model_dir, cfg, device):
-    """The same LLM branch for BLOOM / OPT (:170-172, 193-196): BloomModel / OPTModel + AutoTokenizer(use_fast=False),
-    fp16 features; tokens per launch as in _llama_extractor."""
+    """The same LLM branch for BLOOM / OPT (:170-172, 193-196) and Falcon (:188-190, 193-196): BloomModel / OPTModel /
+    FalconModel + AutoTokenizer(use_fast=False), fp16 features; tokens per launch as in _llama_extractor."""
     import torch
     from transformers import AutoTokenizer
 
@@ -232,6 +233,17 @@ def _albert_extractor(model_name, model_dir, cfg, device):
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
+def _refuse_remote_code_falcon(model_dir):
+    """AutoConfig does not know the legacy RefinedWebModel / RefinedWeb model types at all; refuse them with a message
+    that says what they are, before any weight is read."""
+    import json
+    path = os.path.join(model_dir, "config.json")
+    if os.path.exists(path):
+        from .ln_decoder_text import refuse_refinedweb
+        with open(path) as f:
+            refuse_refinedweb(json.load(f).get("model_type"))
+
+
 def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, punc_case=None,
                       language="chinese", model_dir=None, config=None, sentences_per_launch=256):
     """Same signature, naming and outputs as the reference (:139-252)."""
@@ -256,14 +268,15 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     assert gpu != -1, "mertools_b200 has no CPU path (reference: gpu=-1 means CPU)"
     from .. import shard
     gpu = shard.device_index(gpu)
+    _refuse_remote_code_falcon(model_dir)
     cfg = AutoConfig.from_pretrained(model_dir)
     assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "xlnet", "albert", "llama",
-                              "bloom", "opt", "gpt2"), \
-        f"only BERT/RoBERTa/DeBERTa/XLNet/ALBERT encoders and LLaMA / BLOOM / OPT / GPT-2 decoders are on the H100 " \
-        f"path, got {cfg.model_type}"
+                              "bloom", "opt", "gpt2", "falcon"), \
+        f"only BERT/RoBERTa/DeBERTa/XLNet/ALBERT encoders and LLaMA / BLOOM / OPT / GPT-2 / Falcon decoders are on the " \
+        f"H100 path, got {cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
-    elif cfg.model_type in ("bloom", "opt"):
+    elif cfg.model_type in ("bloom", "opt", "falcon"):
         ext = _ln_decoder_extractor(model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type == "gpt2":
         ext = _gpt2_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")

@@ -567,6 +567,30 @@ def opt_state_dict(seed=25, vocab=4000, hidden=512, ffn=2048, layers=6, max_pos=
     return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
 
 
+# The Falcon checkpoint of tests/golden/falcon_text_golden.npz: head_dim 64 like falcon-7b, with a hidden size (7 x 64 = 448)
+# and a QKV width (9 x 64 = 576) that, like falcon-7b's 4544 and 4672, are not multiples of 128.
+FALCON_SMALL_CFG = dict(vocab=4000, hidden=448, heads=7, ffn=1792, layers=6, max_pos=2048)
+
+
+def falcon_state_dict(seed=43, vocab=4000, hidden=448, heads=7, ffn=1792, layers=6, scale=1.0):
+    """Keys of ``transformers.FalconModel`` with parallel attention, multi-query and no biases: query_key_value rows
+    heads x 64 q | 64 k | 64 v.  Values rounded to fp16 and stored as fp32 (as llama_state_dict); ``scale`` multiplies
+    every layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    hd = hidden // heads
+    g.normal("word_embeddings.weight", (vocab, hidden), 0.5)
+    std = 0.03 * scale
+    for i in range(layers):
+        p = f"h.{i}."
+        g.ln(p + "input_layernorm", hidden)
+        g.normal(p + "self_attention.query_key_value.weight", (hidden + 2 * hd, hidden), std)
+        g.normal(p + "self_attention.dense.weight", (hidden, hidden), std)
+        g.normal(p + "mlp.dense_h_to_4h.weight", (ffn, hidden), std)
+        g.normal(p + "mlp.dense_4h_to_h.weight", (hidden, ffn), std)
+    g.ln("ln_f", hidden)
+    return {k: v.astype(np.float16).astype(np.float32) for k, v in g.sd.items()}
+
+
 # The two GPT-2 checkpoints of tests/golden/gpt2_text_golden.npz, by the reference's model name: gpt2-chinese at head_dim
 # 64 over the BERT fixture vocabulary (tests/golden/text_vocab.txt), Wenzhong at head_dim 96 over the byte-level BPE of
 # tests/golden/opt_tokenizer.

@@ -1,5 +1,5 @@
-"""Throughput of the decoder-LLM text-feature paths (LLaMA at 7 B and 13 B shapes; BLOOM-7B1, OPT-13B and the two GPT-2
-models on request) against the reference's loop.
+"""Throughput of the decoder-LLM text-feature paths (LLaMA at 7 B and 13 B shapes; BLOOM-7B1, OPT-13B, Falcon-7B and the
+two GPT-2 models on request) against the reference's loop.
 
 Packed path: LlamaNet on the CUDA backend (fp16 weights and operands, fp32 residual), sentences packed back to back,
 up to --tokens per pass.  Reference loop (extract_text_huggingface.py:193-231): batch 1, one sentence per forward, fp16,
@@ -10,11 +10,14 @@ Chinese sentencepiece tokenizer (mean ~20 tokens, p99 ~53, capped at 128).  The 
 RMSNorm / RoPE / SwiGLU (LayerNorm for BLOOM / OPT) come from CUDA events around every launch, in a separate pass.
 ``bloom-7b1`` / ``opt-13b`` run LnDecoderNet (extract/ln_decoder_text.py) against HF BloomModel / OPTModel in fp16 at
 batch 1 (a 32000-token vocabulary here: the embedding gather is not part of the timed work that matters).
+``falcon-7b`` (32 x 4544, 71 query heads of 64 sharing one K / V head, FFN 18176, no biases) runs LnDecoderNet against
+HF FalconModel in fp16 at batch 1, as the reference halves it.
 ``gpt2-chinese`` (gpt2-chinese-cluecorpussmall: 12 x 768, 12 heads of 64) and ``wenzhong-3.5b`` (Wenzhong2.0-GPT2-3.5B:
 30 x 3072, 32 heads of 96) run LnDecoderNet against HF GPT2Model at batch 1 in fp32, the precision the reference runs
 these two in: their speed-up includes fp16 against fp32.
 
-    python scripts/bench_llm_text.py [--shapes 7b,13b,bloom-7b1,opt-13b,gpt2-chinese,wenzhong-3.5b] [--sentences 1024]
+    python scripts/bench_llm_text.py [--shapes 7b,13b,bloom-7b1,opt-13b,falcon-7b,gpt2-chinese,wenzhong-3.5b]
+        [--sentences 1024]
         [--ref-sentences 64]
 """
 import argparse
@@ -35,9 +38,10 @@ SHAPES = {"7b": dict(hidden=4096, heads=32, ffn=11008, layers=32, eps=1e-6),
           "13b": dict(hidden=5120, heads=40, ffn=13824, layers=40, eps=1e-5),
           "bloom-7b1": dict(family="bloom", hidden=4096, heads=32, ffn=16384, layers=30, eps=1e-5),
           "opt-13b": dict(family="opt", hidden=5120, heads=40, ffn=20480, layers=40, eps=1e-5),
+          "falcon-7b": dict(family="falcon", hidden=4544, heads=71, ffn=18176, layers=32, eps=1e-5),
           "gpt2-chinese": dict(family="gpt2", hidden=768, heads=12, ffn=3072, layers=12, eps=1e-5),
           "wenzhong-3.5b": dict(family="gpt2", hidden=3072, heads=32, ffn=12288, layers=30, eps=1e-5)}
-MAX_POS = {"bloom": None, "opt": 2048, "gpt2": 1024}
+MAX_POS = {"bloom": None, "opt": 2048, "gpt2": 1024, "falcon": 2048}
 VOCAB = 32000
 
 
@@ -76,7 +80,7 @@ def random_weights(s, seed, dev):
 
 def ln_decoder_weights(s, w):
     """BloomModel / OPTModel (decoder.*) / GPT2Model (Conv1D weights [in, out]) keys, biases on every linear and
-    LayerNorm."""
+    LayerNorm; FalconModel keys (multi-query query_key_value, no linear biases)."""
     D, F = s["hidden"], s["ffn"]
 
     def ln(p):
@@ -92,6 +96,13 @@ def ln_decoder_weights(s, w):
             sd.update({**ln(p + "input_layernorm"), **ln(p + "post_attention_layernorm"),
                        **lin(p + "self_attention.query_key_value", 3 * D, D), **lin(p + "self_attention.dense", D, D),
                        **lin(p + "mlp.dense_h_to_4h", F, D), **lin(p + "mlp.dense_4h_to_h", D, F)})
+    elif s["family"] == "falcon":
+        sd.update({"word_embeddings.weight": w(VOCAB, D, std=1.0), **ln("ln_f")})
+        for i in range(s["layers"]):
+            p = f"h.{i}."
+            sd.update({**ln(p + "input_layernorm"), p + "self_attention.query_key_value.weight": w(D + 128, D),
+                       p + "self_attention.dense.weight": w(D, D), p + "mlp.dense_h_to_4h.weight": w(F, D),
+                       p + "mlp.dense_4h_to_h.weight": w(D, F)})
     elif s["family"] == "gpt2":
         sd.update({"wte.weight": w(VOCAB, D, std=1.0), "wpe.weight": w(MAX_POS["gpt2"], D, std=0.1), **ln("ln_f")})
         for i in range(s["layers"]):
@@ -111,7 +122,11 @@ def ln_decoder_weights(s, w):
 
 
 def hf_config(s):
-    from transformers import BloomConfig, GPT2Config, LlamaConfig, OPTConfig
+    from transformers import BloomConfig, FalconConfig, GPT2Config, LlamaConfig, OPTConfig
+    if s.get("family") == "falcon":
+        return FalconConfig(vocab_size=VOCAB, hidden_size=s["hidden"], num_attention_heads=s["heads"],
+                            ffn_hidden_size=s["ffn"], num_hidden_layers=s["layers"], layer_norm_epsilon=s["eps"],
+                            max_position_embeddings=MAX_POS["falcon"])
     if s.get("family") == "gpt2":
         return GPT2Config(vocab_size=VOCAB, n_positions=MAX_POS["gpt2"], n_embd=s["hidden"], n_layer=s["layers"],
                           n_head=s["heads"], n_inner=s["ffn"], layer_norm_epsilon=s["eps"])
@@ -145,8 +160,9 @@ def reference_loop(s, sd, ids, dev):
     """Batch-1 forwards with output_hidden_states and the last-four sum, as the reference script does: fp16, except
     GPT-2, which the reference does not halve."""
     try:
-        from transformers import BloomModel, GPT2Model, LlamaModel, OPTModel
-        cls = {"bloom": BloomModel, "opt": OPTModel, "gpt2": GPT2Model}.get(s.get("family"), LlamaModel)
+        from transformers import BloomModel, FalconModel, GPT2Model, LlamaModel, OPTModel
+        cls = {"bloom": BloomModel, "opt": OPTModel, "gpt2": GPT2Model, "falcon": FalconModel}.get(s.get("family"),
+                                                                                                  LlamaModel)
         cfg = hf_config(s)
         dt = torch.get_default_dtype()
         ref_dtype = torch.float32 if s.get("family") == "gpt2" else torch.float16
@@ -158,13 +174,13 @@ def reference_loop(s, sd, ids, dev):
             torch.set_default_dtype(dt)
         m.load_state_dict(sd, strict=True)
         which = f"HF {cls.__name__} {'fp32' if ref_dtype == torch.float32 else 'fp16'}"
-        start = 0 if s.get("family") == "bloom" else 1
+        start = 0 if s.get("family") in ("bloom", "falcon") else 1
 
         def fwd(x):
             hs = m(torch.from_numpy(x)[None].to(dev), output_hidden_states=True).hidden_states
             return torch.stack(hs)[[-4, -3, -2, -1]].sum(0)[0, start:].cpu().numpy()
     except ImportError:
-        assert "family" not in s, "the BLOOM / OPT / GPT-2 reference loop needs transformers"
+        assert "family" not in s, "the BLOOM / OPT / GPT-2 / Falcon reference loop needs transformers"
         net = LT.LlamaNet(dict(sd), LT.TorchOps(dev, torch.float16), s["layers"], s["heads"], s["eps"], 10000.0, 4096)
         which = "torch restatement fp16 (transformers not importable)"
 
@@ -237,7 +253,10 @@ def main():
             net = LD.LnDecoderNet({LD._strip(k, s["family"]): (v.T if conv1d and k.endswith(LD.GPT2_CONV1D) else v)
                                    for k, v in sd.items()}, ops, s["family"], s["layers"], s["heads"], s["eps"],
                                   MAX_POS[s["family"]])
-            linear_flops = 4 * s["hidden"] ** 2 + 2 * s["hidden"] * s["ffn"]
+            if s["family"] == "falcon":   # q | one k | one v, dense, the two FFN matrices
+                linear_flops = s["hidden"] * (s["hidden"] + 128) + s["hidden"] ** 2 + 2 * s["hidden"] * s["ffn"]
+            else:
+                linear_flops = 4 * s["hidden"] ** 2 + 2 * s["hidden"] * s["ffn"]
         else:
             ops = LT.CudaOps(dev)
             net = LT.LlamaNet(sd, ops, s["layers"], s["heads"], s["eps"], 10000.0, 4096)
