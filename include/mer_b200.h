@@ -706,7 +706,7 @@ typedef struct MerBertModel {
   const MerLayerWeights* layers;
   /* zero-initialised = the base models; bert-large-uncased / roberta-large / chinese-roberta-wwm-ext-large /
    * chinese-macbert-large ... (extract_text_huggingface.py:21,26,41,49): 1024 / 4096 / 16 */
-  int hidden;               /* 0 = 768; 768 or 1024 (embedding tables are then [*, hidden]) */
+  int hidden;               /* 0 = 768; 768, 1024 or 256 (embedding tables are then [*, hidden]) */
   int ffn;                  /* 0 = 3072 */
   int heads;                /* 0 = 12; hidden / 64 */
   /* optional: the same layers with fp16 GEMM weights -> the 12 layers run on fp16 operands (one MMA per product
@@ -727,6 +727,32 @@ MER_API int mer_bert_forward(const MerBertModel* model, const int32_t* ids, cons
                              const int32_t* seg_begins, const int32_t* seg_ends, void* workspace,
                              long long workspace_bytes, float* out_tokens, float* out_utt,
                              float* opt_hidden, void* stream);
+
+/* ELECTRA's factorised embedding (HF ElectraEmbeddings + embeddings_project, modeling_electra.py), for checkpoints whose
+ * embedding_size E differs from hidden_size H (ELECTRA-small: E 128, H 256):
+ *     e  = LayerNorm_E(word[ids] + pos[pos_ids] + type[0])      (eps: the model's ln_eps)
+ *     h0 = e proj_w^T + proj_b                                  (hidden state 0)
+ * followed by the model's post-LN layers.  The tables below replace the model's word_emb / pos_emb / type_emb0 /
+ * emb_ln_g / emb_ln_b, which are not read.  May only grow at the tail; zero-filled tails = the older behaviour. */
+typedef struct MerBertEmbedProjection {
+  int emb_dim;              /* E: 128 or 256; 2 E <= the model's ffn (the E-wide rows live in the idle FFN buffer) */
+  const float* word_emb;    /* [V, E] */
+  const float* pos_emb;     /* [P, E] */
+  const float* type_emb0;   /* token_type_embeddings[0], [E] */
+  const float* emb_ln_g;    /* [E] */
+  const float* emb_ln_b;    /* [E] */
+  const float* proj_w;      /* [H, E] as split bf16 rows (read when the model's layers_f16 is NULL: the BF16X3 stack) */
+  const void* proj_w_f16;   /* [H, E] fp16 (read when layers_f16 is set: the F16 stack) */
+  const float* proj_b;      /* [H] */
+} MerBertEmbedProjection;
+
+/* mer_bert_forward with the factorised embedding above (proj != NULL; NULL is exactly mer_bert_forward).  Same
+ * arguments, workspace (mer_bert_model_workspace_bytes) and outputs; opt_hidden[0] is the projected h0. */
+MER_API int mer_bert_forward_projected(const MerBertModel* model, const MerBertEmbedProjection* proj,
+                                       const int32_t* ids, const int32_t* pos_ids, const int32_t* cu_seqlens, int n_seq,
+                                       int tokens, int max_seqlen, const int32_t* seg_begins, const int32_t* seg_ends,
+                                       void* workspace, long long workspace_bytes, float* out_tokens, float* out_utt,
+                                       float* opt_hidden, void* stream);
 
 /* ---- Attention fusion network: forward, loss, backward, Adam ------------------------------------ */
 /* toolkit/models/attention.py:8-57 (feat_type 'utt': three MLPEncoders 768->H->H->H, attention MLP

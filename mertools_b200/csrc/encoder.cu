@@ -843,21 +843,24 @@ long long mer_bert_model_workspace_bytes(const MerBertModel* m, int tokens, int 
   return bert_ws(tokens, bert_dim(m), bert_ffn(m));
 }
 
-int mer_bert_forward(const MerBertModel* m, const int32_t* ids, const int32_t* pos_ids,
-                     const int32_t* cu_seqlens, int n_seq, int tokens, int max_seqlen,
-                     const int32_t* seg_begins, const int32_t* seg_ends, void* workspace,
-                     long long workspace_bytes, float* out_tokens, float* out_utt, float* opt_hidden,
-                     void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// proj == NULL: BERT / RoBERTa / ELECTRA with embedding_size == hidden_size; otherwise ELECTRA's factorised embedding
+// (LayerNorm at width E, then the E -> H projection writes hidden state 0)
+static int bert_forward_impl(const MerBertModel* m, const MerBertEmbedProjection* proj, const int32_t* ids,
+                             const int32_t* pos_ids, const int32_t* cu_seqlens, int n_seq, int tokens, int max_seqlen,
+                             const int32_t* seg_begins, const int32_t* seg_ends, void* workspace,
+                             long long workspace_bytes, float* out_tokens, float* out_utt, float* opt_hidden,
+                             cudaStream_t stream) {
   MER_REQUIRE(m && ids && pos_ids && cu_seqlens && workspace, "mer_bert_forward: null operand");
   MER_REQUIRE(n_seq > 0 && tokens > 0 && max_seqlen > 0, "mer_bert_forward: empty batch");
   MER_REQUIRE(m->n_layers >= 4, "mer_bert_forward: the last-four readout needs >= 4 layers");
-  // model dims: zero-initialised fields = the base models (768 / 12 heads / 3072); -large: 1024 / 16 / 4096
+  // model dims: zero-initialised fields = the base models (768 / 12 heads / 3072); -large: 1024 / 16 / 4096;
+  // ELECTRA-small / LERT-small: 256 / 4 / 1024
   const int D = bert_dim(m), DFF = bert_ffn(m), HEADS = m->heads > 0 ? m->heads : ::HEADS, DQKV = 3 * D;
-  MER_REQUIRE((D == 768 || D == 1024) && HEADS * 64 == D && DFF % 128 == 0,
+  MER_REQUIRE((D == 768 || D == 1024 || D == 256) && HEADS * 64 == D && DFF % 128 == 0,
               "mer_bert_forward: hidden %d / heads %d / ffn %d not supported", D, HEADS, DFF);
   MER_REQUIRE(workspace_bytes >= bert_ws(tokens, D, DFF), "mer_bert_forward: workspace %lld B < required %lld B",
               workspace_bytes, bert_ws(tokens, D, DFF));
+  const bool f16 = m->layers_f16 != nullptr;
   const long long M = tokens;
   float* x = static_cast<float*>(workspace);
   float* xs = x + M * D;
@@ -866,14 +869,36 @@ int mer_bert_forward(const MerBertModel* m, const int32_t* ids, const int32_t* p
   float* h = qkv + M * DQKV;
   float* acc = h + M * DFF;
   float* vt = acc + M * D;
-  MER_TRY(mer_bert_embed_launch(ids, pos_ids, m->word_emb, m->pos_emb, m->type_emb0, m->emb_ln_g,
-                                m->emb_ln_b, m->ln_eps, tokens, x, xs, stream, D));
+  if (proj) {
+    const int E = proj->emb_dim;
+    MER_REQUIRE((E == 128 || E == 256) && E != D, "mer_bert_forward_projected: embedding size %d (128 or 256, != hidden %d)",
+                E, D);
+    // the E-wide LayerNorm output and its GEMM operand live in the FFN buffer, idle before layer 1
+    MER_REQUIRE(2 * E <= DFF, "mer_bert_forward_projected: embedding size %d needs 2 x %d <= ffn %d", E, E, DFF);
+    MER_REQUIRE(proj->word_emb && proj->pos_emb && proj->type_emb0 && proj->emb_ln_g && proj->emb_ln_b && proj->proj_b &&
+                    (f16 ? proj->proj_w_f16 != nullptr : proj->proj_w != nullptr),
+                "mer_bert_forward_projected: null table or weight (the %s projection)", f16 ? "fp16" : "split bf16");
+    float* e32 = h;           // [M, E] fp32 LayerNorm_E output
+    float* eop = h + M * E;   // [M, E] its GEMM operand: split bf16 rows (E 4-byte slots) or fp16 rows
+    MER_TRY(mer_bert_embed_launch(ids, pos_ids, proj->word_emb, proj->pos_emb, proj->type_emb0, proj->emb_ln_g,
+                                  proj->emb_ln_b, m->ln_eps, tokens, e32, f16 ? nullptr : eop, stream, E));
+    if (f16) MER_TRY(mer_cast_f16_launch(e32, eop, M * E, stream));
+    const float* pw = f16 ? static_cast<const float*>(proj->proj_w_f16) : proj->proj_w;
+    MER_TRY(linear(f16 ? MER_GEMM_F16 : MER_GEMM_BF16X3, eop, pw, proj->proj_b, nullptr, x, M, D, E, 0, stream));
+    // the stack's operand copy of hidden state 0
+    if (f16) MER_TRY(mer_cast_f16_launch(x, xs, M * D, stream));
+    else MER_TRY(mer_split_bf16(x, xs, M, D, stream));
+  } else {
+    MER_REQUIRE(m->word_emb && m->pos_emb && m->type_emb0 && m->emb_ln_g && m->emb_ln_b,
+                "mer_bert_forward: null embedding table");
+    MER_TRY(mer_bert_embed_launch(ids, pos_ids, m->word_emb, m->pos_emb, m->type_emb0, m->emb_ln_g,
+                                  m->emb_ln_b, m->ln_eps, tokens, x, xs, stream, D));
+    if (f16) MER_TRY(mer_cast_f16_launch(x, xs, M * D, stream));  // the embedding LayerNorm's fp16 copy (operand)
+  }
   if (opt_hidden)
     MER_CUDA_CHECK(cudaMemcpyAsync(opt_hidden, x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, stream));
   MerStackArgs a;
   memset(&a, 0, sizeof(a));
-  const bool f16 = m->layers_f16 != nullptr;
-  if (f16) MER_TRY(mer_cast_f16_launch(x, xs, M * D, stream));  // the embedding LayerNorm's fp16 copy (operand)
   a.layers = f16 ? m->layers_f16 : m->layers;
   a.n_layers = m->n_layers;
   a.pre_ln = 0;
@@ -903,6 +928,24 @@ int mer_bert_forward(const MerBertModel* m, const int32_t* ids, const int32_t* p
   if (out_utt && seg_begins && seg_ends)
     MER_TRY(mer_segment_reduce_launch(acc, seg_begins, seg_ends, n_seq, D, MER_SEG_MEAN, out_utt, stream));
   return 0;
+}
+
+int mer_bert_forward(const MerBertModel* m, const int32_t* ids, const int32_t* pos_ids,
+                     const int32_t* cu_seqlens, int n_seq, int tokens, int max_seqlen,
+                     const int32_t* seg_begins, const int32_t* seg_ends, void* workspace,
+                     long long workspace_bytes, float* out_tokens, float* out_utt, float* opt_hidden,
+                     void* stream) {
+  return bert_forward_impl(m, nullptr, ids, pos_ids, cu_seqlens, n_seq, tokens, max_seqlen, seg_begins, seg_ends,
+                           workspace, workspace_bytes, out_tokens, out_utt, opt_hidden, static_cast<cudaStream_t>(stream));
+}
+
+int mer_bert_forward_projected(const MerBertModel* m, const MerBertEmbedProjection* proj, const int32_t* ids,
+                               const int32_t* pos_ids, const int32_t* cu_seqlens, int n_seq, int tokens, int max_seqlen,
+                               const int32_t* seg_begins, const int32_t* seg_ends, void* workspace,
+                               long long workspace_bytes, float* out_tokens, float* out_utt, float* opt_hidden,
+                               void* stream) {
+  return bert_forward_impl(m, proj, ids, pos_ids, cu_seqlens, n_seq, tokens, max_seqlen, seg_begins, seg_ends,
+                           workspace, workspace_bytes, out_tokens, out_utt, opt_hidden, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -167,7 +167,8 @@ segment_reduce_kernel(const float* __restrict__ in, const int* __restrict__ begi
 
 // BERT/RoBERTa embeddings (HF modeling_bert.py BertEmbeddings / modeling_roberta.py:56-122):
 // (word[id] + token_type[0]) + position[pos] -> LayerNorm -> x (fp32) and its split-bf16 copy.
-// One warp per token; hidden size 128 * VEC (VEC 6: the base models, VEC 8: the -large ones).
+// One warp per token; width 128 * VEC (VEC 6: the base models, VEC 8: the -large ones, VEC 2: LERT-small's hidden 256,
+// VEC 1: ELECTRA-small's factorised 128-wide embedding).
 template <int VEC>
 __global__ void __launch_bounds__(256)
 bert_embed_ln_kernel(const int* __restrict__ ids, const int* __restrict__ pos_ids,
@@ -285,13 +286,16 @@ int mer_bert_embed_launch(const int* ids, const int* pos_ids, const float* word,
                           const float* type0, const float* gamma, const float* beta, float eps,
                           int tokens, float* out, void* out_split, cudaStream_t stream, int dim) {
   if (tokens <= 0) return 0;
-  MER_REQUIRE(dim == 768 || dim == 1024, "mer_bert_embed: hidden size %d (768 or 1024)", dim);
-  if (dim == 1024)
-    bert_embed_ln_kernel<8><<<(tokens + 7) / 8, 256, 0, stream>>>(ids, pos_ids, word, pos, type0, gamma, beta, eps,
-                                                                  tokens, out, out_split);
-  else
-    bert_embed_ln_kernel<6><<<(tokens + 7) / 8, 256, 0, stream>>>(ids, pos_ids, word, pos, type0, gamma, beta, eps,
-                                                                  tokens, out, out_split);
+  MER_REQUIRE(dim == 768 || dim == 1024 || dim == 128 || dim == 256,
+              "mer_bert_embed: hidden size %d (768 or 1024; also 128 and 256)", dim);
+#define MER_EMBED_LAUNCH(VEC)                                                                                       \
+  bert_embed_ln_kernel<VEC><<<(tokens + 7) / 8, 256, 0, stream>>>(ids, pos_ids, word, pos, type0, gamma, beta, eps, \
+                                                                  tokens, out, out_split)
+  if (dim == 1024) MER_EMBED_LAUNCH(8);
+  else if (dim == 768) MER_EMBED_LAUNCH(6);
+  else if (dim == 256) MER_EMBED_LAUNCH(2);
+  else MER_EMBED_LAUNCH(1);
+#undef MER_EMBED_LAUNCH
   MER_CUDA_CHECK(cudaGetLastError());
   mer_count_launches(1);
   return 0;

@@ -255,8 +255,8 @@ int mer_layernorm_launch(const float* x, const float* gamma, const float* beta, 
   const bool pad = (flags & MER_LN_PAD) != 0;
   const int width = pad ? (dim + 127) / 128 * 128 : dim;
   MER_REQUIRE(dim > 0 && (width == 768 || width == 512 || width == 1024 || width == 1280 || width == 1536 ||
-                          width == 128 || width == 384),
-              "mer_layernorm: dim %d not supported (512, 768, 1024, 1280, 1536) (also 128 and 384; with MER_LN_PAD, "
+                          width == 128 || width == 384 || width == 256),
+              "mer_layernorm: dim %d not supported (512, 768, 1024, 1280, 1536) (also 128, 384 and 256; with MER_LN_PAD, "
               "a valid width whose next multiple of 128 is one of these)", dim);
   if (rows <= 0) return 0;
   const int warps_per_block = 8;
@@ -283,6 +283,7 @@ int mer_layernorm_launch(const float* x, const float* gamma, const float* beta, 
   else if (width == 1536) MER_LN_LAUNCH(12);  // dinov2-giant
   else if (width == 128) MER_LN_LAUNCH(1);    // ALBERT's embedding LayerNorm
   else if (width == 384) MER_LN_LAUNCH(3);    // albert_chinese_small; albert_chinese_tiny's 312 padded to 384
+  else if (width == 256) MER_LN_LAUNCH(2);    // ELECTRA-small / LERT-small (hidden 256)
   else MER_LN_LAUNCH(4);
 #undef MER_LN_LAUNCH
   mer_prof_end(prof, stream);

@@ -1193,56 +1193,102 @@ class MerBertModel(C.Structure):
                 ("layers_f16", C.POINTER(W.MerLayerWeights))]
 
 
+class MerBertEmbedProjection(C.Structure):
+    _fields_ = [("emb_dim", C.c_int), ("word_emb", C.c_void_p), ("pos_emb", C.c_void_p), ("type_emb0", C.c_void_p),
+                ("emb_ln_g", C.c_void_p), ("emb_ln_b", C.c_void_p), ("proj_w", C.c_void_p), ("proj_w_f16", C.c_void_p),
+                ("proj_b", C.c_void_p)]
+
+
+# keys of an ElectraForPreTraining / ElectraForMaskedLM checkpoint that ElectraModel does not have (the prefix
+# ``electra.`` is already gone, common.normalise_hf_keys), and the registered buffers some checkpoints carry
+_BERT_IGNORED_PREFIXES = ("discriminator_predictions.", "generator_predictions.", "generator_lm_head.")
+_BERT_IGNORED_KEYS = ("embeddings.position_ids", "embeddings.token_type_ids")
+
+
+def bert_model_state(state_dict):
+    """The tensors of the base model (BertModel / RobertaModel / ElectraModel) in a prefix-free checkpoint, as numpy:
+    ELECTRA's discriminator / generator heads and the position / token-type id buffers are dropped."""
+    return {k: v for k, v in W._np(state_dict).items()
+            if k not in _BERT_IGNORED_KEYS and not k.startswith(_BERT_IGNORED_PREFIXES)}
+
+
 class BertEncoder:
-    """BERT-architecture encoders (HF ``BertModel`` / ``RobertaModel`` / ``ElectraModel`` with embedding_size ==
-    hidden_size; hidden 768 or 1024: BERT, RoBERTa, MacBERT, PERT, LERT, ELECTRA base and large) over a packed
-    variable-length batch + the reference readout (sum of the last four hidden states, strip specials, mean).
+    """BERT-architecture encoders (HF ``BertModel`` / ``RobertaModel`` / ``ElectraModel``; hidden 768 or 1024: BERT,
+    RoBERTa, MacBERT, PERT, LERT, ELECTRA base and large; hidden 256: LERT-small, and ELECTRA-small with its factorised
+    128-wide embedding + ``embeddings_project``) over a packed variable-length batch + the reference readout (sum of
+    the last four hidden states, strip specials, mean).
 
     Reference: MERBench/feature_extraction/text/extract_text_huggingface.py:222-249."""
 
     def __init__(self, state_dict, device="cuda", ln_eps=1e-12, position_offset=0, precision=None):
         """precision: operand format of the layers' linear products.  "f16" (default for the 12-layer base models since
-        round 2; env MER_TEXT_PRECISION): one fp16 MMA per product, readout error 2.9e-4 at 12 layers; "bf16x3"
-        (default for the 24-layer -large models): three bf16 MMAs on (hi, lo) pairs, 3.5e-5
-        (scripts/precision_table.py)."""
+        round 2; env MER_TEXT_PRECISION): one fp16 MMA per product, readout error 2.9e-4 at 12 layers; "bf16x3" (default
+        for the 24-layer -large models and the hidden-256 small ones): three bf16 MMAs on (hi, lo) pairs, 3.5e-5
+        (scripts/precision_table.py; hidden 256: scripts/precision_table_electra.py)."""
         L.check(L.lib().mer_check_device())
-        sd = W._np(state_dict)
+        sd = bert_model_state(state_dict)
         self.device = torch.device(device)
         pk = self.pk = W.Packed(self.device)
         self.position_offset = position_offset  # 0 = BERT, 2 = RoBERTa (pad_token_id + 1)
         self.n_layers = W.count_layers(sd, "encoder.layer.{i}.output.LayerNorm.weight")
-        assert "embeddings_project.weight" not in sd, \
-            "ELECTRA-small style checkpoints (embedding_size != hidden_size) are not on the H100 path"
         m = MerBertModel()
         m.n_layers, m.ln_eps = self.n_layers, ln_eps
         self.word = pk.keep(sd["embeddings.word_embeddings.weight"])
         self.pos = pk.keep(sd["embeddings.position_embeddings.weight"])
         self.vocab_size, self.max_pos = self.word.shape[0], self.pos.shape[0]
-        # base (768 / 12 heads / 3072) or -large (1024 / 16 / 4096) BERT-architecture checkpoints
-        self.hidden = int(self.word.shape[1])
+        # ELECTRA with embedding_size != hidden_size: the E-wide embedding is projected to the hidden size
+        projected = "embeddings_project.weight" in sd
+        self.emb_dim = int(self.word.shape[1])
+        # base (768 / 12 heads / 3072), -large (1024 / 16 / 4096) or small (256 / 4 / 1024) checkpoints
+        self.hidden = int(sd["embeddings_project.weight"].shape[0]) if projected else self.emb_dim
         ffn = int(sd["encoder.layer.0.intermediate.dense.weight"].shape[0])
-        assert self.hidden in (768, 1024) and ffn % 128 == 0, (self.hidden, ffn)
+        assert self.hidden in (256, 768, 1024) and ffn % 128 == 0, \
+            f"hidden {self.hidden} / ffn {ffn}: hidden 256, 768 or 1024 and ffn % 128 == 0 are on the H100 path"
+        assert not projected or (self.emb_dim in (128, 256) and self.emb_dim != self.hidden and 2 * self.emb_dim <= ffn), \
+            f"embedding size {self.emb_dim} -> hidden {self.hidden}: a projected embedding of 128 or 256 is on the H100 path"
         m.hidden, m.ffn, m.heads = self.hidden, ffn, self.hidden // 64
-        m.word_emb, m.pos_emb = self.word.data_ptr(), self.pos.data_ptr()
-        m.type_emb0 = pk.keep(sd["embeddings.token_type_embeddings.weight"][0]).data_ptr()
-        m.emb_ln_g = pk.keep(sd["embeddings.LayerNorm.weight"]).data_ptr()
-        m.emb_ln_b = pk.keep(sd["embeddings.LayerNorm.bias"]).data_ptr()
+        emb = dict(word_emb=self.word.data_ptr(), pos_emb=self.pos.data_ptr(),
+                   type_emb0=pk.keep(sd["embeddings.token_type_embeddings.weight"][0]).data_ptr(),
+                   emb_ln_g=pk.keep(sd["embeddings.LayerNorm.weight"]).data_ptr(),
+                   emb_ln_b=pk.keep(sd["embeddings.LayerNorm.bias"]).data_ptr())
         self.layers = W.pack_layers(sd, W.BERT_NAMES, self.n_layers, pk, split=True)
         m.layers = self.layers
         import os as _os
+        # hidden 256: bf16x3, the emulated f16 readout error of the x5 stress checkpoint is 1.1e-2 at 12 layers
         self.precision = precision or _os.environ.get("MER_TEXT_PRECISION", "f16" if self.hidden == 768 else "bf16x3")
         assert self.precision in ("bf16x3", "f16"), self.precision
         if self.precision == "f16":
             self.layers_f16 = W.pack_layers(sd, W.BERT_NAMES, self.n_layers, pk, f16=True)
             m.layers_f16 = self.layers_f16
+        self.proj = None
+        if projected:  # the tables go to the projection struct; the model's stay NULL (not read)
+            pr = self.proj = MerBertEmbedProjection()
+            pr.emb_dim = self.emb_dim
+            for k, v in emb.items():
+                setattr(pr, k, v)
+            w = sd["embeddings_project.weight"]
+            if self.precision == "f16":
+                pr.proj_w_f16 = pk.keep(w, f16=True).data_ptr()
+            else:
+                pr.proj_w = pk.keep(w, split=True).data_ptr()
+            pr.proj_b = pk.keep(sd["embeddings_project.bias"]).data_ptr()
+        else:
+            for k, v in emb.items():
+                setattr(m, k, v)
         self.model = m
         self.ws = _Workspace(self.device)
         lib = L.lib()
         lib.mer_bert_model_workspace_bytes.restype = C.c_longlong
         lib.mer_bert_model_workspace_bytes.argtypes = [C.POINTER(MerBertModel), C.c_int, C.c_int]
         vp, i32 = C.c_void_p, C.c_int
-        self._fwd = L.declare("mer_bert_forward", [C.POINTER(MerBertModel), vp, vp, vp, i32, i32, i32,
-                                                   vp, vp, vp, C.c_longlong, vp, vp, vp, vp])
+        if projected:
+            fwd = L.declare("mer_bert_forward_projected", [C.POINTER(MerBertModel), C.POINTER(MerBertEmbedProjection),
+                                                           vp, vp, vp, i32, i32, i32, vp, vp, vp, C.c_longlong, vp, vp,
+                                                           vp, vp])
+            self._fwd = lambda model, *args: fwd(model, C.byref(self.proj), *args)
+        else:
+            self._fwd = L.declare("mer_bert_forward", [C.POINTER(MerBertModel), vp, vp, vp, i32, i32, i32,
+                                                       vp, vp, vp, C.c_longlong, vp, vp, vp, vp])
 
     def forward_packed(self, ids, seqlen, start=1, end=-1):
         """Device fast path for n sentences of identical length: ids int32 CUDA [n, seqlen].  Position

@@ -1,5 +1,5 @@
 """Lexical feature extraction — H100 mirror of
-MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa branch; DeBERTa / DeBERTa-v2 through
+MERBench/feature_extraction/text/extract_text_huggingface.py (BERT / RoBERTa / ELECTRA branch; DeBERTa / DeBERTa-v2 through
 extract/deberta_text.py, XLNet through extract/xlnet_text.py and ALBERT through extract/albert_text.py, float32 like BERT; LLaMA-family decoders through extract/llama_text.py and BLOOM / OPT through
 extract/ln_decoder_text.py (BLOOM / OPT / Falcon), saved as float16 like the reference's fp16 GPU run; GPT-2 through
 extract/ln_decoder_text.py,
@@ -233,6 +233,37 @@ def _albert_extractor(model_name, model_dir, cfg, device):
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
+def check_electra_config(cfg):
+    """Refuse, before any weight is read, the ELECTRA configs mer_bert_forward does not compute exactly: BERT's post-LN
+    layers with erf GELU and absolute positions, heads of 64, hidden 256 / 768 / 1024, and an embedding of 128 or 256
+    projected to the hidden size (or as wide as it), at least 4 layers for the last-four readout."""
+    act = getattr(cfg, "hidden_act", "gelu")
+    assert act == "gelu", f"ELECTRA hidden_act {act!r}: only 'gelu' (erf) is on the H100 path"
+    pet = getattr(cfg, "position_embedding_type", "absolute")
+    assert pet == "absolute", f"ELECTRA position_embedding_type {pet!r}: only 'absolute' is on the H100 path"
+    H, heads = cfg.hidden_size, cfg.num_attention_heads
+    assert H % heads == 0 and H // heads == 64, \
+        f"ELECTRA num_attention_heads {heads} (hidden_size {H}): only head_dim 64 is on the H100 path"
+    assert H in (256, 768, 1024), f"ELECTRA hidden_size {H}: only 256, 768 or 1024 is on the H100 path"
+    E = getattr(cfg, "embedding_size", H)
+    assert E in (128, 256, H), f"ELECTRA embedding_size {E}: only 128, 256 or hidden_size ({H}) is on the H100 path"
+    assert cfg.intermediate_size % 128 == 0 and (E == H or 2 * E <= cfg.intermediate_size), \
+        f"ELECTRA intermediate_size {cfg.intermediate_size}: a multiple of 128 (and >= 2 x embedding_size) is needed"
+    assert cfg.num_hidden_layers >= 4, \
+        f"ELECTRA num_hidden_layers {cfg.num_hidden_layers}: the last-four readout needs at least 4 layers"
+
+
+def _electra_extractor(model_dir, cfg, device):
+    """The reference's ELECTRA models (the AutoModel + AutoTokenizer(use_fast=False) branch, :188-190): ElectraModel is
+    BERT's post-LN stack, behind the factorised 128-wide embedding and its projection for the small models; fp32
+    features, position ids from 0, the checkpoint's LayerNorm eps."""
+    from transformers import AutoTokenizer
+    check_electra_config(cfg)  # before any weight is read
+    tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
+    return TextExtractor(common.load_hf_state_dict(model_dir), tokenizer, device=device, ln_eps=cfg.layer_norm_eps,
+                         position_offset=0)
+
+
 def _refuse_remote_code_falcon(model_dir):
     """AutoConfig does not know the legacy RefinedWebModel / RefinedWeb model types at all; refuse them with a message
     that says what they are, before any weight is read."""
@@ -270,10 +301,10 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
     gpu = shard.device_index(gpu)
     _refuse_remote_code_falcon(model_dir)
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "deberta", "deberta-v2", "xlnet", "albert", "llama",
-                              "bloom", "opt", "gpt2", "falcon"), \
-        f"only BERT/RoBERTa/DeBERTa/XLNet/ALBERT encoders and LLaMA / BLOOM / OPT / GPT-2 / Falcon decoders are on the " \
-        f"H100 path, got {cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta", "xlm-roberta", "electra", "deberta", "deberta-v2", "xlnet", "albert",
+                              "llama", "bloom", "opt", "gpt2", "falcon"), \
+        f"only BERT/RoBERTa/ELECTRA/DeBERTa/XLNet/ALBERT encoders and LLaMA / BLOOM / OPT / GPT-2 / Falcon decoders are " \
+        f"on the H100 path, got {cfg.model_type}"
     if cfg.model_type == "llama":
         ext = _llama_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type in ("bloom", "opt", "falcon"):
@@ -286,6 +317,8 @@ def extract_embedding(model_name, trans_dir, save_dir, feature_level, gpu=-1, pu
         ext = _xlnet_extractor(model_dir, cfg, f"cuda:{gpu}")
     elif cfg.model_type == "albert":
         ext = _albert_extractor(model_name, model_dir, cfg, f"cuda:{gpu}")
+    elif cfg.model_type == "electra":
+        ext = _electra_extractor(model_dir, cfg, f"cuda:{gpu}")
     else:
         tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
         roberta = cfg.model_type != "bert"

@@ -5,8 +5,8 @@ The host side is the reference's: split the transcript into words and sentences 
 sentence as pre-split words (:232), and, after the encoder, merge sub-word embeddings back into one vector per
 word (:254-291, ``combine_type`` mean | sum | last), then the FRAME / UTTERANCE save rules (:296-309).  The
 encoder pass (sum of the last four hidden states of every real token, :236-238) runs in libmer_b200.so over
-all sentences of a transcript as one packed batch.  BERT / RoBERTa-base style checkpoints only (the
-reference's list also names ALBERT, XLNet, GPT, T5, DeBERTa, which are outside the H100 path).
+all sentences of a transcript as one packed batch.  BERT / RoBERTa / ELECTRA checkpoints only (the reference's list
+also names ALBERT, XLNet, GPT, T5, DeBERTa, which this path does not run).
 """
 from __future__ import annotations
 
@@ -135,10 +135,14 @@ def extract_bert_embedding_english(model_name, trans_dir, save_dir, feature_leve
         raise Exception(f'==> Error: csv out dir "{dir_name}" already exists, set overwrite=TRUE if needed!')
     model_dir = os.path.join(config.PATH_TO_PRETRAINED_MODELS, f"transformers/{model_name}")
     cfg = AutoConfig.from_pretrained(model_dir)
-    assert cfg.model_type in ("bert", "roberta"), f"only BERT/RoBERTa-base encoders are on the H100 path, got {cfg.model_type}"
+    assert cfg.model_type in ("bert", "roberta", "electra"), \
+        f"only BERT/RoBERTa/ELECTRA encoders are on the H100 path, got {cfg.model_type}"
+    if cfg.model_type == "electra":
+        from .text import check_electra_config
+        check_electra_config(cfg)  # before any weight is read
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = BertEncoder(common.load_hf_state_dict(model_dir), device=f"cuda:{gpu}", ln_eps=cfg.layer_norm_eps,
-                      position_offset=(cfg.pad_token_id + 1) if cfg.model_type != "bert" else 0)
+                      position_offset=(cfg.pad_token_id + 1) if cfg.model_type == "roberta" else 0)
     lower = "uncased" in model_name or "albert" in model_name or "electra" in model_name
     df = pd.read_csv(trans_dir)
     for idx, row in df.iterrows():

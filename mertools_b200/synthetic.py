@@ -897,3 +897,59 @@ def write_mer2023_corpus(root, n_train=32, n_test=8, dim=768, seed=0, frame_leve
                 shape = (int(rng.integers(2, hi)), dim) if hi else (dim,)
                 np.save(os.path.join(feats, fname, name + ".npy"), rng.standard_normal(shape).astype(np.float32))
     return label_path, feats
+
+
+# ELECTRA (ElectraConfig keywords).  Goldens: ``small`` (the factorised 128-wide embedding + embeddings_project into
+# hidden 256, 4 heads of 64, FFN 1024), ``base`` (embedding_size == hidden_size: BERT's graph) and ``lert_small`` (a
+# hidden-256 BertModel, as chinese-lert-small).  PUBLISHED: the checkpoints' shapes (seeded weights; vocab as given).
+ELECTRA_GOLDEN_CFGS = {
+    "small": dict(vocab_size=None, embedding_size=128, hidden_size=256, num_attention_heads=4, intermediate_size=1024,
+                  num_hidden_layers=5, hidden_act="gelu", layer_norm_eps=1e-12, hidden_dropout_prob=0.0,
+                  attention_probs_dropout_prob=0.0),
+    "base": dict(vocab_size=None, embedding_size=768, hidden_size=768, num_attention_heads=12, intermediate_size=3072,
+                 num_hidden_layers=4, hidden_act="gelu", layer_norm_eps=1e-12, hidden_dropout_prob=0.0,
+                 attention_probs_dropout_prob=0.0),
+    "lert_small": dict(vocab_size=None, embedding_size=256, hidden_size=256, num_attention_heads=4,
+                       intermediate_size=1024, num_hidden_layers=4, hidden_act="gelu", layer_norm_eps=1e-12,
+                       hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0),
+}
+ELECTRA_PUBLISHED_CFGS = {
+    "chinese-electra-180g-small": dict(ELECTRA_GOLDEN_CFGS["small"], vocab_size=21128, num_hidden_layers=12),
+    "chinese-lert-small": dict(ELECTRA_GOLDEN_CFGS["lert_small"], vocab_size=21128, num_hidden_layers=12),
+    "chinese-electra-180g-base": dict(ELECTRA_GOLDEN_CFGS["base"], vocab_size=21128, num_hidden_layers=12),
+    "chinese-electra-180g-large": dict(ELECTRA_GOLDEN_CFGS["base"], vocab_size=21128, embedding_size=1024,
+                                       hidden_size=1024, num_attention_heads=16, intermediate_size=4096,
+                                       num_hidden_layers=24),
+}
+
+
+def electra_state_dict(cfg, seed=51, scale=1.0, pretraining=False):
+    """Keys of ``transformers.ElectraModel`` for a dict of ElectraConfig keywords (as ELECTRA_GOLDEN_CFGS; vocab_size
+    set): the E-wide embeddings and their LayerNorm, ``embeddings_project`` when embedding_size != hidden_size, and
+    BERT's post-LN layers.  ``pretraining``: the keys of ``ElectraForPreTraining`` instead (``electra.`` prefix and the
+    discriminator head).  ``scale`` multiplies every layer matrix (stress checkpoints)."""
+    g = _Gen(seed)
+    e, d, ffn = cfg["embedding_size"], cfg["hidden_size"], cfg["intermediate_size"]
+    std = 0.03 * scale
+    g.normal("embeddings.word_embeddings.weight", (cfg["vocab_size"], e), 0.5)
+    g.normal("embeddings.position_embeddings.weight", (cfg.get("max_position_embeddings", 512), e), 0.1)
+    g.normal("embeddings.token_type_embeddings.weight", (cfg.get("type_vocab_size", 2), e), 0.1)
+    g.ln("embeddings.LayerNorm", e)
+    if e != d:
+        g.linear("embeddings_project", d, e, 0.08)
+    for i in range(cfg["num_hidden_layers"]):
+        p = f"encoder.layer.{i}."
+        for n in ("query", "key", "value"):
+            g.linear(p + f"attention.self.{n}", d, d, std)
+        g.linear(p + "attention.output.dense", d, d, std)
+        g.ln(p + "attention.output.LayerNorm", d)
+        g.linear(p + "intermediate.dense", ffn, d, std)
+        g.linear(p + "output.dense", d, ffn, std)
+        g.ln(p + "output.LayerNorm", d)
+    if not pretraining:
+        return g.sd
+    sd = {"electra." + k: v for k, v in g.sd.items()}
+    g.sd = sd
+    g.linear("discriminator_predictions.dense", d, d, 0.02)
+    g.linear("discriminator_predictions.dense_prediction", 1, d, 0.02)
+    return g.sd
