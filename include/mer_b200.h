@@ -205,6 +205,20 @@ MER_API int mer_attention_hd(const void* qkv, const void* vt, long long vt_ld, v
                              int n_seq, long long tokens, int max_seqlen, int heads, int head_dim, float scale,
                              int flags, void* stream);
 
+/* Longest row of mer_attention_long, and of the HuBERT / wav2vec2 stacks' fp16 V^T attention (82 s of audio; a 60 s
+ * clip is 2,999 frames).  Longer rows of those stacks take the kernel of attention.cu (route 3 above). */
+#define MER_ATT_LONG_MAX 4096
+/* mer_attention's fp16 route (route 1) for rows of up to MER_ATT_LONG_MAX tokens: qkv fp16 [tokens, 3 * heads * 64]
+ * (V columns not read), vt fp16 [heads * 64, vt_ld], ctx [tokens, heads * 64] in the format the flags name
+ * (MER_EPI_OUT_F16, MER_EPI_SPLIT_BF16, MER_EPI_ROUND_TF32 or none = fp32).  Rows of up to 505 tokens run exactly what
+ * mer_attention runs; longer ones the same tiled kernel over more 64-key tiles (fp16 P, fp32 softmax statistics).  The
+ * HuBERT / wav2vec2 stacks route their rows of 506 .. MER_ATT_LONG_MAX tokens here (not under MER_ATTENTION_LEGACY).
+ * Refused before any launch with a "mer_attention_long:" message: a NULL operand, other flags, tokens outside
+ * 1 .. 2^31 - 1, a V^T pitch below tokens or not a multiple of 8, max_seqlen outside 1 .. min(MER_ATT_LONG_MAX,
+ * tokens), heads or n_seq outside 1 .. 65535.  attention_f16.cu. */
+MER_API int mer_attention_long(const void* qkv, const void* vt, long long vt_ld, void* ctx, const int32_t* cu_seqlens,
+                               int n_seq, long long tokens, int max_seqlen, int heads, int flags, void* stream);
+
 /* ---- segment reduce (readouts) ------------------------------------------------------------ */
 enum { MER_SEG_SUM = 0, MER_SEG_MEAN = 1 };
 /* out[s, :] = sum or mean of in[begins[s] : ends[s], :] (dim % 4 == 0; begins/ends device int32,
@@ -416,7 +430,7 @@ MER_API int mer_vggish_forward(const MerVggishModel* model, const float* example
 
 /* ---- HuBERT-base audio encoder ------------------------------------------------------------------ */
 typedef struct MerHubertModel {
-  int n_layers;  /* 12 (>= 4: the readout sums the last four hidden states) */
+  int n_layers;  /* 12 (>= 4 for the readout that sums the last four hidden states; see `readout`) */
   float ln_eps;  /* 1e-5 */
   const float* conv0_w;    /* [512, 10] */
   const float* gn_g;       /* GroupNorm(512 groups) affine, [512] */
@@ -467,7 +481,15 @@ typedef struct MerHubertModel {
    * writes fp16 rows, conv2 split-bf16 rows for conv3).  conv1 + conv2 are 77 % of the conv stack's flops; emulated
    * readout error with fp16 layers: 3.5e-4 against 3.2e-4 (profiles/r2_precision_conv_layers.json). */
   const void* conv_w_f16[2];
+  /* ---- readout (0 = MER_HUBERT_READOUT_LAST4: the sum of the last four hidden states, as described at
+   * mer_hubert_forward) ----
+   * MER_HUBERT_READOUT_LAST: hidden_states[-1] alone (MER2023/feature_extraction/audio/extract_transformers_embedding.py,
+   * layer_ids = [-1]) into the same out_frames / out_utt: the last layer's output for the post-LN family, the output of
+   * encoder.layer_norm after the last layer for the stable-layer-norm family.  Needs n_layers >= 1 (LAST4: >= 4). */
+  int readout;
 } MerHubertModel;
+#define MER_HUBERT_READOUT_LAST4 0
+#define MER_HUBERT_READOUT_LAST 1
 
 /* per-row zero-mean / unit-variance (eps 1e-7) of HF Wav2Vec2FeatureExtractor(do_normalize=True)
  * (feature_extraction_wav2vec2.py:78-97), as called at extract_audio_huggingface.py:94.
@@ -504,7 +526,8 @@ MER_API long long mer_hubert_model_workspace_bytes(const MerHubertModel* model, 
  * clip at a time, or 10 s rows from split_into_batch, extract_audio_huggingface.py:40-50,95).
  * normalize != 0 applies the Wav2Vec2FeatureExtractor zero-mean/unit-variance step per row (:94).
  * Then HubertModel forward (HF modeling_hubert.py) and the readout
- * torch.stack(hidden_states)[[-4,-3,-2,-1]].sum(0) (:98).
+ * torch.stack(hidden_states)[[-4,-3,-2,-1]].sum(0) (:98), or hidden_states[-1] (model->readout).
+ * Rows of more than 505 frames (clips over 10.1 s) run attention on the fp16 V^T kernel up to MER_ATT_LONG_MAX frames.
  * out_frames: NULL or [batch*T, 768] (FRAME level, :100); out_utt: NULL or [batch, 768] = mean over
  * each row's T frames (UTTERANCE level for clips <= 10 s, :105-108). */
 MER_API int mer_hubert_forward(const MerHubertModel* model, const float* wave, int batch, int n_samples,

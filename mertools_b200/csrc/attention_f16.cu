@@ -32,6 +32,9 @@ constexpr int BKV = 64;
 constexpr int THREADS = 128;
 constexpr int MAX_SEQ = 505;  // longest sequence the stacks send here (10 s audio rows, CLIP L/14)
 constexpr int MAX_SEQ_HD = 512;  // mer_attention_hd: ALBERT's position table
+// whole-clip audio rows (MER2023's extractor: a 60 s clip is 2,999 HuBERT frames); the emulated fp16-P readout error is
+// measured up to this length (scripts/precision_table_long_audio.py)
+constexpr int MAX_SEQ_LONG = MER_ATT_LONG_MAX;
 
 template <bool F16, int HD>
 struct AttCfg {
@@ -370,6 +373,21 @@ bool mer_attention_f16_supported(int max_seqlen) {
   return (e == nullptr || atoi(e) != 0) && max_seqlen <= MAX_SEQ;
 }
 
+// rows of 506 .. MAX_SEQ_LONG tokens: the HuBERT / wav2vec2 stacks (MerStackArgs::long_rows), not mer_attention
+bool mer_attention_f16_long_supported(int max_seqlen) {
+  return max_seqlen > MAX_SEQ && max_seqlen <= MAX_SEQ_LONG && !mer_attention_legacy();
+}
+
+int mer_attention_f16_long_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
+                                  int n_seq, long long tokens, int heads, int max_seqlen, int out_mode,
+                                  cudaStream_t stream) {
+  if (max_seqlen <= MAX_SEQ)
+    return mer_attention_f16_launch(qkv16, vt16, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode,
+                                    stream);
+  return launch_vt<true>(qkv16, vt16, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode, stream,
+                         MAX_SEQ_LONG);
+}
+
 // qkv16: fp16 [tokens, 3*heads*64] (V columns unused), vt16: fp16 [heads*64, vt_ld] with vt[d, token];
 // ctx [tokens, heads*64] in the format `out_mode` names (3 fp16, 2 bf16 hi | lo split rows, 1 tf32-rounded fp32, 0 fp32).
 // Rows of up to 249 tokens take the one-CTA-per-(sequence, head) kernel of attention_short.cu.
@@ -429,4 +447,22 @@ extern "C" int mer_attention_hd(const void* qkv, const void* vt, long long vt_ld
   if (f16) MER_ATT_HD(true, 64);
   MER_ATT_HD(false, 64);
 #undef MER_ATT_HD
+}
+
+// the fp16 route of mer_attention for rows of up to MAX_SEQ_LONG tokens (mer_b200.h)
+extern "C" int mer_attention_long(const void* qkv, const void* vt, long long vt_ld, void* ctx, const int32_t* cu_seqlens,
+                                  int n_seq, long long tokens, int max_seqlen, int heads, int flags, void* stream) {
+  const char* name = "mer_attention_long";
+  MER_REQUIRE(qkv && vt && ctx && cu_seqlens, "%s: null operand", name);
+  MER_REQUIRE((flags & ~(MER_EPI_OUT_F16 | MER_EPI_SPLIT_BF16 | MER_EPI_ROUND_TF32)) == 0, "%s: flags 0x%x", name, flags);
+  MER_REQUIRE(tokens > 0 && tokens < (1ll << 31), "%s: tokens %lld (1 .. 2^31 - 1: int32 cu_seqlens)", name, tokens);
+  MER_REQUIRE(vt_ld >= tokens && vt_ld % 8 == 0, "%s: V^T pitch %lld must be a multiple of 8 >= tokens %lld", name, vt_ld,
+              tokens);
+  MER_REQUIRE(max_seqlen > 0 && max_seqlen <= MAX_SEQ_LONG && max_seqlen <= tokens,
+              "%s: max_seqlen %d (1 .. min(MER_ATT_LONG_MAX = %d, tokens %lld))", name, max_seqlen, MAX_SEQ_LONG, tokens);
+  MER_REQUIRE(heads > 0 && heads <= 65535 && n_seq > 0 && n_seq <= 65535, "%s: bad grid (%d heads, %d seqs)", name,
+              heads, n_seq);
+  const int out_mode = (flags & MER_EPI_OUT_F16) ? 3 : (flags & MER_EPI_SPLIT_BF16) ? 2 : ((flags & MER_EPI_ROUND_TF32) ? 1 : 0);
+  return mer_attention_f16_long_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode,
+                                       static_cast<cudaStream_t>(stream));
 }

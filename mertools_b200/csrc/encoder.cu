@@ -58,6 +58,17 @@ int linear(int mode, const float* A, const float* W, const float* bias, const fl
     if (int _rc = (expr)) return _rc; \
   } while (0)
 
+// mer_attention_launch, except that with `long_rows` (fp16 q | k | V^T rows of 506 .. MER_ATT_LONG_MAX tokens, which
+// mer_attention refuses) the call goes to the long-row launch of the same fp16 V^T kernel
+int attend(bool long_rows, const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
+           int n_seq, long long tokens, int max_seqlen, int heads, int flags, cudaStream_t stream) {
+  if (!long_rows)
+    return mer_attention_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, max_seqlen, heads, flags, stream);
+  const int out_mode = (flags & MER_EPI_OUT_F16) ? 3 : (flags & MER_EPI_SPLIT_BF16) ? 2 : ((flags & MER_EPI_ROUND_TF32) ? 1 : 0);
+  return mer_attention_f16_long_launch(qkv, vt, vt_ld, ctx, cu_seqlens, n_seq, tokens, heads, max_seqlen, out_mode,
+                                       stream);
+}
+
 }  // namespace
 
 int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
@@ -79,8 +90,11 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
     const bool split = a.mode == MER_GEMM_BF16X3;
     // V^T attention (sequences <= 253): the QKV GEMM writes V transposed into a.vt instead of
     // the V columns of qkv
-    // (254 .. 505 tokens: the fp16 V^T kernel, which takes fp16 q | k | V^T whatever the stack's operand format)
-    const bool long_att = a.vt && !mer_attention_uses_tc(a.max_seqlen) && mer_attention_f16_supported(a.max_seqlen);
+    // (254 .. 505 tokens, and up to MER_ATT_LONG_MAX with a.long_rows: the fp16 V^T kernel, which takes fp16
+    // q | k | V^T whatever the stack's operand format)
+    const bool f16_long = a.long_rows && a.vt && mer_attention_f16_long_supported(a.max_seqlen);
+    const bool f16_rows = f16_long || mer_attention_f16_supported(a.max_seqlen);
+    const bool long_att = a.vt && !mer_attention_uses_tc(a.max_seqlen) && f16_rows;
     float* vt = (a.vt && (long_att || mer_attention_uses_tc(a.max_seqlen))) ? a.vt : nullptr;
     // the TF32 / BF16X3 stacks: QKV epilogue and attention flags (q | k | v tf32-rounded fp32, or fp16 = the same 10-bit
     // mantissa, for the long-key kernel)
@@ -92,14 +106,14 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
       // into the (fp32-sized) scratch buffers; only the residual stream x stays fp32
       float* xn16 = a.xn;  // fp16 [M, 768]
       float* h16 = a.h;    // fp16 [M, 3072]
-      const bool f16_att = vt != nullptr && mer_attention_f16_supported(a.max_seqlen);
+      const bool f16_att = vt != nullptr && f16_rows;
       MER_TRY(mer_layernorm_launch(a.x, w.ln1_g, w.ln1_b, xn16, nullptr, nullptr, M, D, a.eps, MER_LN_OUT_F16,
                                    stream));
       if (f16_att) {
         MER_TRY(linear(a.mode, xn16, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, MER_EPI_OUT_F16, stream,
                        vt, a.vt_ld, 2 * D));
-        MER_TRY(mer_attention_launch(a.qkv, vt, a.vt_ld, xn16, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
-                                     MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
+        MER_TRY(attend(f16_long, a.qkv, vt, a.vt_ld, xn16, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
+                       MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
         MER_TRY(linear(a.mode, xn16, w.w_o, w.b_o, a.x, a.x, M, D, D, 0, stream));
       } else {
         // sequences beyond the fp16 attention kernel (CLIP L/14: 257 tokens): the linear layers stay on fp16
@@ -121,8 +135,8 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
                                    nullptr, M, D, a.eps, MER_LN_ROUND_TF32, stream));
       MER_TRY(linear(a.mode, a.xn, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, qkv_fl, stream,
                      vt, a.vt_ld, 2 * D));
-      MER_TRY(mer_attention_launch(a.qkv, vt, a.vt_ld, a.xn, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
-                                   opnd | att_in, stream));
+      MER_TRY(attend(f16_long, a.qkv, vt, a.vt_ld, a.xn, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
+                     opnd | att_in, stream));
       MER_TRY(linear(a.mode, a.xn, w.w_o, w.b_o, a.x, a.x, M, D, D, 0, stream));
       MER_TRY(mer_layernorm_launch(a.x, w.ln2_g, w.ln2_b, split ? nullptr : a.xn, split ? a.xn : nullptr,
                                    nullptr, M, D, a.eps, MER_LN_ROUND_TF32, stream));
@@ -135,12 +149,12 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
       float* x16 = a.xs;
       float* c16 = a.xn;   // fp16 ctx; later the fp32 pre-LN sum of the FFN half
       float* h16 = a.h;
-      const bool f16_att = vt != nullptr && mer_attention_f16_supported(a.max_seqlen);
+      const bool f16_att = vt != nullptr && f16_rows;
       if (f16_att) {
         MER_TRY(linear(a.mode, x16, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, MER_EPI_OUT_F16, stream, vt,
                        a.vt_ld, 2 * D));
-        MER_TRY(mer_attention_launch(a.qkv, vt, a.vt_ld, c16, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
-                                     MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
+        MER_TRY(attend(f16_long, a.qkv, vt, a.vt_ld, c16, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
+                       MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
         MER_TRY(linear(a.mode, c16, w.w_o, w.b_o, a.x, a.qkv, M, D, D, 0, stream));  // qkv is dead: holds the sum
       } else {
         // rows beyond the fp16 attention kernel (> 249 frames): TF32-rounded fp32 q | k | v (same 10-bit mantissa)
@@ -169,8 +183,8 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
       const float* xop = split ? a.xs : a.x;
       MER_TRY(linear(a.mode, xop, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, qkv_fl, stream,
                      vt, a.vt_ld, 2 * D));
-      MER_TRY(mer_attention_launch(a.qkv, vt, a.vt_ld, a.xn, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
-                                   opnd | att_in, stream));
+      MER_TRY(attend(f16_long, a.qkv, vt, a.vt_ld, a.xn, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
+                     opnd | att_in, stream));
       // the pre-LN sum goes to the (now dead) qkv buffer: ctx in xn is still being read
       MER_TRY(linear(a.mode, a.xn, w.w_o, w.b_o, a.x, a.qkv, M, D, D, 0, stream));
       MER_TRY(mer_layernorm_launch(a.qkv, w.ln1_g, w.ln1_b, a.x, split ? a.xs : nullptr, nullptr, M, D,
@@ -487,7 +501,11 @@ static int hubert_forward_impl(const MerHubertModel* m, const float* wave, int B
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   MER_REQUIRE(m && wave && workspace, "mer_hubert_forward: null operand");
   MER_REQUIRE(B > 0 && L > 0, "mer_hubert_forward: batch=%d n_samples=%d", B, L);
-  MER_REQUIRE(m->n_layers >= 4, "mer_hubert_forward: the last-four readout needs >= 4 layers");
+  MER_REQUIRE(m->readout == MER_HUBERT_READOUT_LAST4 || m->readout == MER_HUBERT_READOUT_LAST,
+              "mer_hubert_forward: readout %d (MER_HUBERT_READOUT_LAST4 = 0 or MER_HUBERT_READOUT_LAST = 1)", m->readout);
+  const bool last_only = m->readout == MER_HUBERT_READOUT_LAST;
+  MER_REQUIRE(m->n_layers >= (last_only ? 1 : 4), "mer_hubert_forward: the %s readout needs >= %d layers (n_layers %d)",
+              last_only ? "last-layer" : "last-four", last_only ? 1 : 4, m->n_layers);
   const int D = hub_dim(m), DFF = hub_ffn(m), HEADS = hub_heads(m);
   MER_REQUIRE((D == 768 || D == 1024) && HEADS * 64 == D && DFF % 128 == 0,
               "mer_hubert_forward: hidden %d / heads %d / ffn %d not supported", D, HEADS, DFF);
@@ -744,6 +762,7 @@ static int hubert_forward_impl(const MerHubertModel* m, const float* wave, int B
   a.vt = reinterpret_cast<float*>(ws + p.off_vt);
   a.vt_ld = (M + 7) & ~7ll;
   a.hidden0_done = 1;
+  a.long_rows = 1;
   const size_t hs_bytes = (size_t)M * D * 4;
   if (!m->stable_layer_norm) {
     // encoder.layer_norm -> x ; post-LN layers; readout = sum of the last four LayerNorm outputs
@@ -758,7 +777,7 @@ static int hubert_forward_impl(const MerHubertModel* m, const float* wave, int B
     a.pre_ln = 0;
     a.mode = f16 ? MER_GEMM_F16 : MER_GEMM_BF16X3;
     a.acc = acc;
-    a.acc_last = 4;
+    a.acc_last = last_only ? 1 : 4;  // hidden_states[-1] alone: the last layer's LayerNorm initialises acc
     a.opt_hidden = opt_hidden;
     MER_TRY(mer_run_stack(a, stream));
   } else {
@@ -783,16 +802,24 @@ static int hubert_forward_impl(const MerHubertModel* m, const float* wave, int B
       done += n;
       return rc;
     };
-    MER_TRY(run(L0 + 1));                                        // x = x_{L-4}
-    MER_TRY(mer_accumulate_launch(x, acc, M * D, 1, stream));
-    for (int k = 0; k < 2; ++k) {
-      MER_TRY(run(1));                                           // x_{L-3}, x_{L-2}
-      MER_TRY(mer_accumulate_launch(x, acc, M * D, 0, stream));
+    if (last_only) {
+      // hidden_states[-1] alone = encoder.layer_norm of the last layer's output
+      MER_TRY(run(m->n_layers));
+      float* last = opt_hidden ? opt_hidden + (size_t)m->n_layers * M * D : xn;
+      MER_TRY(mer_layernorm_launch(x, m->enc_ln_g, m->enc_ln_b, last, nullptr, acc, M, D, m->ln_eps, MER_LN_ACC_INIT,
+                                   stream));
+    } else {
+      MER_TRY(run(L0 + 1));                                      // x = x_{L-4}
+      MER_TRY(mer_accumulate_launch(x, acc, M * D, 1, stream));
+      for (int k = 0; k < 2; ++k) {
+        MER_TRY(run(1));                                         // x_{L-3}, x_{L-2}
+        MER_TRY(mer_accumulate_launch(x, acc, M * D, 0, stream));
+      }
+      MER_TRY(run(1));                                           // x_{L-1}
+      float* last = opt_hidden ? opt_hidden + (size_t)m->n_layers * M * D : xn;
+      MER_TRY(mer_layernorm_launch(x, m->enc_ln_g, m->enc_ln_b, last, nullptr, acc, M, D, m->ln_eps,
+                                   MER_LN_ACC_ADD, stream));
     }
-    MER_TRY(run(1));                                             // x_{L-1}
-    float* last = opt_hidden ? opt_hidden + (size_t)m->n_layers * M * D : xn;
-    MER_TRY(mer_layernorm_launch(x, m->enc_ln_g, m->enc_ln_b, last, nullptr, acc, M, D, m->ln_eps,
-                                 MER_LN_ACC_ADD, stream));
   }
   if (out_frames)
     MER_CUDA_CHECK(cudaMemcpyAsync(out_frames, acc, hs_bytes, cudaMemcpyDeviceToDevice, stream));

@@ -44,6 +44,9 @@ bool mer_attention_uses_tc(int max_seqlen);  // the tf32 V^T kernel takes this l
 bool mer_attention_legacy();  // MER_ATTENTION_LEGACY set: only the kernel of attention.cu (debug)
 // attention_f16.cu: V^T kernels.  out_mode: 0 fp32, 1 tf32-rounded fp32, 2 bf16 hi | lo split rows, 3 fp16
 bool mer_attention_f16_supported(int max_seqlen);  // fp16 q | k | V^T, up to 505 tokens
+bool mer_attention_f16_long_supported(int max_seqlen);  // 506 .. MER_ATT_LONG_MAX tokens, not under MER_ATTENTION_LEGACY
+int mer_attention_f16_long_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
+                                  int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
                              int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
@@ -113,5 +116,7 @@ struct MerStackArgs {
   int acc_last;
   float* opt_hidden;         // optional [(n_layers+1), tokens, 768]
   int hidden0_done;          // caller already wrote opt_hidden[0] (post-LN: the un-rounded LN)
+  int long_rows;             // 1 (HuBERT / wav2vec2): rows of 506 .. MER_ATT_LONG_MAX tokens take the fp16 V^T kernel
+                             // like the 254 .. 505-token rows; 0: they take the kernel of attention.cu
 };
 int mer_run_stack(const MerStackArgs& a, cudaStream_t stream);

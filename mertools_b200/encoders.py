@@ -972,7 +972,10 @@ class MerHubertModel(C.Structure):
                 ("conv_ln_b", C.c_void_p * 7), ("pos_window", C.c_int), ("layers_f16", C.POINTER(W.MerLayerWeights)),
                 ("n_pos_layers", C.c_int), ("pos_taps", C.c_int), ("pos_layers_w", C.c_void_p * 8),
                 ("pos_layers_b", C.c_void_p * 8), ("ln_ones", C.c_void_p), ("ln_zeros", C.c_void_p),
-                ("conv_w_f16", C.c_void_p * 2)]
+                ("conv_w_f16", C.c_void_p * 2), ("readout", C.c_int)]
+
+
+MER_HUBERT_READOUT_LAST4, MER_HUBERT_READOUT_LAST = 0, 1   # MerHubertModel.readout (mer_b200.h)
 
 
 def block_diagonal_pos_conv_weight(wpos, block_n=256, window=320, group=48):
@@ -1021,7 +1024,9 @@ class HubertEncoder:
     Reference: MERBench/feature_extraction/audio/extract_audio_huggingface.py:18-36,93-110."""
 
     def __init__(self, state_dict, device="cuda", ln_eps=1e-5, stable_layer_norm=None, stack_precision=None,
-                 conv_precision=None):
+                 conv_precision=None, last_layer_only=False):
+        """last_layer_only: the readout is ``hidden_states[-1]`` alone (MER2023's extract_transformers_embedding.py,
+        ``layer_ids = [-1]``) instead of the sum of the last four."""
         L.check(L.lib().mer_check_device())
         sd = W._np(state_dict)
         self.device = torch.device(device)
@@ -1029,6 +1034,7 @@ class HubertEncoder:
         self.n_layers = W.count_layers(sd, "encoder.layers.{i}.layer_norm.weight")
         m = MerHubertModel()
         m.n_layers, m.ln_eps = self.n_layers, ln_eps
+        m.readout = MER_HUBERT_READOUT_LAST if last_layer_only else MER_HUBERT_READOUT_LAST4
         w0 = sd["feature_extractor.conv_layers.0.conv.weight"]
         assert w0.shape == (512, 1, 10), f"wav2vec2-style feature extractor (512 x 10 conv0) only, got {w0.shape}"
         assert "feature_extractor.conv_layers.0.layer_norm.weight" in sd

@@ -47,17 +47,19 @@ def split_into_batch(input_values, maxlen=MAXLEN):
 
 class AudioExtractor:
     def __init__(self, state_dict, device="cuda", max_rows_per_launch=128, ragged=None, max_samples_per_launch=128 * MAXLEN // 2,
-                 do_normalize=True):
+                 do_normalize=True, last_layer_only=False):
         """ragged (default on; env MER_AUDIO_RAGGED=0 switches it off): clips of different lengths share one device pass
         (``HubertEncoder.forward_ragged``: every clip computed as if alone) instead of one pass per distinct
-        length; sorted by length and cut into launches of at most ``max_samples_per_launch`` padded samples."""
+        length; sorted by length and cut into launches of at most ``max_samples_per_launch`` padded samples.
+        last_layer_only: read out ``hidden_states[-1]`` instead of the sum of the last four (HuBERT / wav2vec2 only)."""
         if "encoder.layers.0.attention.gru_rel_pos_linear.weight" in state_dict:   # WavLMModel (wavlm-base / -large)
             from .wavlm import WavLmEncoder
             self.enc = WavLmEncoder(state_dict, device=device)
             assert not ragged, "ragged batches are implemented for the HuBERT / wav2vec2 families only"  # None: default
+            assert not last_layer_only, "the last-layer readout is implemented for the HuBERT / wav2vec2 families only"
             ragged = False
         else:
-            self.enc = HubertEncoder(state_dict, device=device)
+            self.enc = HubertEncoder(state_dict, device=device, last_layer_only=last_layer_only)
         self.device = self.enc.device
         self.max_rows = max_rows_per_launch
         # ragged batches: one launch chain for clips of any length instead of one pass per distinct length; results
@@ -88,6 +90,50 @@ class AudioExtractor:
             outs.append(fr.clone())
         return torch.cat(outs)
 
+    def _extract_ragged(self, waves, clips, feature_level, res):
+        """Clips ``clips`` (indices into waves) through ``forward_ragged``: sorted by length, cut into launches of at most
+        ``max_rows`` clips and ``max_samples`` padded samples; res[i] receives clip i's frames [T, D] or mean [D]."""
+        order = sorted(clips, key=lambda i: len(waves[i]))
+        launches, s0 = [], 0
+        while s0 < len(order):   # launches of consecutive (sorted) clips: rows * longest <= max_samples
+            e = s0 + 1
+            while (e < len(order) and e - s0 < self.max_rows
+                   and (e - s0 + 1) * len(waves[order[e]]) <= self.max_samples):
+                e += 1
+            launches.append(order[s0:e])
+            s0 = e
+        # Two persistent pinned staging buffers (a fresh pinned allocation per launch cost as much as the launch's
+        # device time) and a one-launch-deep pipeline: launch k is enqueued, the host fills the buffer of launch
+        # k + 1 while the GPU works, and only then are the results of launch k read back -- in ONE device-to-host
+        # copy per launch (round 2's first build synchronised once per clip).
+        want_frames = feature_level != "UTTERANCE"
+
+        def finish(p):
+            idxs, utt, frames = p
+            if want_frames:
+                for r, i in enumerate(idxs):
+                    res[i] = frames[r].cpu().numpy()
+            else:
+                u = utt.cpu().numpy()
+                for r, i in enumerate(idxs):
+                    res[i] = u[r].copy()
+
+        pending = None
+        for k, idxs in enumerate(launches):
+            lens = [len(waves[i]) for i in idxs]
+            host = self._staging(k & 1, len(idxs), max(lens))
+            hn = host.numpy()            # shares the pinned memory; the assignment converts float64 -> float32 in place
+            for r, i in enumerate(idxs):
+                hn[r, :lens[r]] = waves[i]
+                hn[r, lens[r]:] = 0.0
+            utt, frames = self.enc.forward_ragged(host.to(self.device, non_blocking=True), lens,
+                                                  normalize=self.do_normalize, want_frames=want_frames)
+            if pending is not None:
+                finish(pending)          # (synchronises: buffer k & 1 is free again two launches later)
+            pending = (idxs, utt, frames)
+        if pending is not None:
+            finish(pending)
+
     def extract_waves(self, waves, feature_level="UTTERANCE", save_files=None):
         """waves: list of 1-D float arrays (what ``sf.read`` returns, 16 kHz mono).  Returns the
         arrays the reference would ``np.save`` (:103-110)."""
@@ -99,46 +145,7 @@ class AudioExtractor:
             if len(w) <= MAXLEN:
                 short.setdefault(len(w), []).append(i)
         if self.ragged and len(short) > 1:
-            order = sorted((i for idxs in short.values() for i in idxs), key=lambda i: len(waves[i]))
-            launches, s0 = [], 0
-            while s0 < len(order):   # launches of consecutive (sorted) clips: rows * longest <= max_samples
-                e = s0 + 1
-                while (e < len(order) and e - s0 < self.max_rows
-                       and (e - s0 + 1) * len(waves[order[e]]) <= self.max_samples):
-                    e += 1
-                launches.append(order[s0:e])
-                s0 = e
-            # Two persistent pinned staging buffers (a fresh pinned allocation per launch cost as much as the launch's
-            # device time) and a one-launch-deep pipeline: launch k is enqueued, the host fills the buffer of launch
-            # k + 1 while the GPU works, and only then are the results of launch k read back -- in ONE device-to-host
-            # copy per launch (round 2's first build synchronised once per clip).
-            want_frames = feature_level != "UTTERANCE"
-
-            def finish(p):
-                idxs, utt, frames = p
-                if want_frames:
-                    for r, i in enumerate(idxs):
-                        res[i] = frames[r].cpu().numpy()
-                else:
-                    u = utt.cpu().numpy()
-                    for r, i in enumerate(idxs):
-                        res[i] = u[r].copy()
-
-            pending = None
-            for k, idxs in enumerate(launches):
-                lens = [len(waves[i]) for i in idxs]
-                host = self._staging(k & 1, len(idxs), max(lens))
-                hn = host.numpy()            # shares the pinned memory; the assignment converts float64 -> float32 in place
-                for r, i in enumerate(idxs):
-                    hn[r, :lens[r]] = waves[i]
-                    hn[r, lens[r]:] = 0.0
-                utt, frames = self.enc.forward_ragged(host.to(self.device, non_blocking=True), lens,
-                                                      normalize=self.do_normalize, want_frames=want_frames)
-                if pending is not None:
-                    finish(pending)          # (synchronises: buffer k & 1 is free again two launches later)
-                pending = (idxs, utt, frames)
-            if pending is not None:
-                finish(pending)
+            self._extract_ragged(waves, [i for idxs in short.values() for i in idxs], feature_level, res)
             short = {}
         # clips <= 10 s: batch by identical length; normalisation fused on the device
         for n, idxs in short.items():
