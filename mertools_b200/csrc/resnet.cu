@@ -659,9 +659,11 @@ maskmul_kernel(const float* __restrict__ src, int s_ld, int s0, const float* __r
 
 struct CnnPlan { long long off_buf[CNN_BUFS], off_col, off_cu, off_z, off_scale, total; };
 
-int pool_out(int in, int pad, int ceil_mode) {  // torch MaxPool2d(3, 2, pad, ceil_mode) output size
-  const int num = in + 2 * pad - 3;
-  int o = (ceil_mode ? (num + 1) / 2 : num / 2) + 1;
+// torch MaxPool2d(3, 2, pad, ceil_mode) output size (pooling_output_shape: floor division); < 1 where torch raises
+// (pad 0 with in = 1, or in = 2 in floor mode: the window does not fit)
+int pool_out(int in, int pad, int ceil_mode) {
+  const int num = in + 2 * pad - 3 + (ceil_mode ? 1 : 0);
+  int o = (num >= 0 ? num / 2 : -((1 - num) / 2)) + 1;
   if (ceil_mode && (o - 1) * 2 >= in + pad) --o;  // the last window must start inside the (left-padded) input
   return o;
 }
@@ -700,6 +702,9 @@ int cnn_walk(const MerCnnModel* m, int n_frames, bool exec, CnnPlan* plan, char*
         const MerResnetConv& cv = m->convs[op.conv];
         MER_REQUIRE(cv.k == 7 && cv.stride == 2 && cv.pad == 3 && cv.cin == 3 && cv.kpad == (split ? 160 : 192),
                     "mer_cnn: the stem is a 7x7 / 2 convolution packed to %d columns", split ? 160 : 192);
+        MER_REQUIRE(cv.cout > 0 && cv.cout <= cv.cout_pad && cv.cout_pad % 128 == 0 && m->in_h > 0 && m->in_w > 0,
+                    "mer_cnn: op %d stem geometry (cout %d stored as %d, frames %d x %d)", i, cv.cout, cv.cout_pad,
+                    m->in_h, m->in_w);
         const int OH = (m->in_h + 6 - 7) / 2 + 1, OW = (m->in_w + 6 - 7) / 2 + 1;
         const long long rows = n * OH * OW, total = rows * cv.kpad;
         MER_REQUIRE(rows < (1ll << 31), "mer_cnn: too many frames per call");
@@ -746,6 +751,15 @@ int cnn_walk(const MerCnnModel* m, int n_frames, bool exec, CnnPlan* plan, char*
         const int c0 = op.p[0];  // the conv reads channels [c0, c0 + cin) of src
         MER_REQUIRE(full.H > 0 && c0 >= 0 && c0 % 4 == 0 && c0 + cv.cin <= full.C && op.src != op.dst,
                     "mer_cnn: op %d reads channels [%d, %d) of a %d-channel buffer", i, c0, c0 + cv.cin, full.C);
+        // what conv() and mer_gemm_launch require, checked here so that a table they would refuse is refused by
+        // mer_cnn_workspace_bytes and by mer_cnn_forward before its first launch
+        const int K = cv.k * cv.k * cv.cin;
+        MER_REQUIRE(cv.k > 0 && cv.stride > 0 && cv.pad >= 0 && cv.cin > 0 && cv.cin % 8 == 0 && cv.kpad == K &&
+                        K % (split ? 32 : 64) == 0 && cv.cout > 0 && cv.cout <= cv.cout_pad && cv.cout_pad % 128 == 0,
+                    "mer_cnn: op %d conv geometry (k %d stride %d pad %d, cin %d, kpad %d for K %d, cout %d stored as "
+                    "%d)", i, cv.k, cv.stride, cv.pad, cv.cin, cv.kpad, K, cv.cout, cv.cout_pad);
+        MER_REQUIRE(full.H + 2 * cv.pad >= cv.k && full.W + 2 * cv.pad >= cv.k,
+                    "mer_cnn: op %d %dx%d conv (pad %d) of a %d x %d map", i, cv.k, cv.k, cv.pad, full.H, full.W);
         const Shape in{full.H, full.W, cv.cin, full.Cs};
         const int OH = (in.H + 2 * cv.pad - cv.k) / cv.stride + 1, OW = (in.W + 2 * cv.pad - cv.k) / cv.stride + 1;
         const long long rows = n * OH * OW;
@@ -781,6 +795,8 @@ int cnn_walk(const MerCnnModel* m, int n_frames, bool exec, CnnPlan* plan, char*
           break;
         }
         const int OH = pool_out(in.H, op.pad, op.ceil_mode), OW = pool_out(in.W, op.pad, op.ceil_mode);
+        MER_REQUIRE((op.pad == 0 || op.pad == 1) && OH > 0 && OW > 0,
+                    "mer_cnn: op %d 3x3 max-pool (pad %d) of a %d x %d map", i, op.pad, in.H, in.W);
         define(op.dst, Shape{OH, OW, in.C, in.Cs});
         if (!exec) break;
         const long long total = n * OH * OW * (in.Cs / 4);

@@ -500,3 +500,293 @@ def adam_f64(param, grad, exp_avg, exp_avg_sq, t, lr, beta1, beta2, eps, weight_
     v = beta2 * v + (1.0 - beta2) * g * g
     denom = v.sqrt() / math.sqrt(1.0 - beta2 ** t) + eps
     return p - lr / (1.0 - beta1 ** t) * m / denom, m, v
+
+
+# ---- table-driven CNN executor (mer_cnn_forward, resnet.cu) -----------------------------------------------------------
+# GEMM operand formats.  MER_GEMM_F16 converts each fp32 activation with cvt.rn.satfinite (round to nearest even, clamp
+# to +-65504, NaN stays NaN); MER_GEMM_BF16X3 stores hi = bf16(x) and lo = bf16(x - hi) (both round to nearest even)
+# and its MMAs add hi hi + hi lo + lo hi: the lo lo product is left out (tests/test_gemm_gpu.py).
+GEMM_F16, GEMM_BF16X3 = 2, 1
+
+
+def f16_satfinite(x):
+    """cvt.rn.satfinite.f16.f32 on fp32 values, returned as fp32."""
+    return x.float().clamp(-65504.0, 65504.0).half().float()
+
+
+def split_bf16(x):
+    """(hi, lo) of the split-bf16 operand of fp32 values: hi = RNE bf16 of x, lo = RNE bf16 of x - hi (exact in fp32)."""
+    x = x.float()
+    hi = round_bf16_nearest_even(x)
+    return hi, round_bf16_nearest_even(x - hi)
+
+
+def stem_operand(frames_bgr, scale, mean, std):
+    """The value im2col_stem_kernel computes for each pixel, bit for bit: fma(pix, scale, -mean[c]) rounded once to fp32
+    (pix * scale is exact in float64 for 8-bit pixels and an fp32 scale, and so is its difference with an fp32 mean),
+    then an IEEE fp32 division by std[c]; channels in RGB order (BGR input).  frames: uint8 [n, H, W, 3] -> fp32."""
+    f32 = lambda v: torch.tensor([float(np.float32(t)) for t in v], dtype=torch.float64)  # noqa: E731
+    pix = torch.as_tensor(np.ascontiguousarray(np.asarray(frames_bgr)[..., ::-1])).double()
+    num = (pix * float(np.float32(scale)) - f32(mean)).float()
+    return num / f32(std).float()
+
+
+def cnn_conv(x, w, b, k, stride, pad, mode=None, res=None):
+    """NHWC convolution of the operand values of x [n, H, W, cin] with w [cout_pad, >= k k cin] in (ky, kx, c) order
+    and bias b, in float64: mode None computes on x and w as given, GEMM_F16 on their satfinite fp16 values,
+    GEMM_BF16X3 on split operands without the lo lo product.  Returns (y, a): a = |x| |w| + |b| (+ |res|) on the same
+    operands, the scale the GEMM's accumulation error is measured against."""
+    x, w = x.float(), torch.as_tensor(w).float()
+    cin, co = x.shape[-1], w.shape[0]
+    kk = k * k * cin
+    wt = lambda v: v[:, :kk].reshape(co, k, k, cin).permute(0, 3, 1, 2).double()  # noqa: E731
+    cv = lambda v, ww: F.conv2d(v.permute(0, 3, 1, 2).double(), ww, stride=stride, padding=pad)  # noqa: E731
+    if mode == GEMM_BF16X3:
+        (xh, xl), (wh, wl) = split_bf16(x), split_bf16(w)
+        y = cv(xh, wt(wh) + wt(wl)) + cv(xl, wt(wh))
+        a = cv(xh.abs(), wt(wh).abs() + wt(wl).abs()) + cv(xl.abs(), wt(wh).abs())
+    else:
+        if mode == GEMM_F16:
+            x, w = f16_satfinite(x), f16_satfinite(w)
+        y, a = cv(x, wt(w)), cv(x.abs(), wt(w).abs())
+    b = torch.as_tensor(b).double()
+    y, a = (y + b[:, None, None]).permute(0, 2, 3, 1), (a + b.abs()[:, None, None]).permute(0, 2, 3, 1)
+    if res is not None:
+        assert tuple(res.shape) == tuple(y.shape), f"residual {tuple(res.shape)} for an output {tuple(y.shape)}"
+        y, a = y + res.double(), a + res.double().abs()
+    return y, a
+
+
+def cnn_plan(m, n):
+    """Workspace layout of mer_cnn_forward for an op table (cnn_walk's planning pass): per buffer the largest
+    n H W Cs fp32 map any op defines there, each 256-byte aligned in index order, then the im2col operand, the
+    average pool's offsets and the SE means and gates.  Returns (dict of byte offsets and total, {buffer: (H, W, C,
+    Cs)} as the last op left them)."""
+    al = lambda v: (v + 255) & ~255  # noqa: E731
+    vb = 4 if m.gemm_mode == GEMM_BF16X3 else 2
+    sh, need, col, se_c = {}, [0] * 24, 0, 0
+
+    def define(bi, s):
+        sh[bi] = s
+        need[bi] = max(need[bi], n * s[0] * s[1] * s[3])
+    for i in range(m.n_ops):
+        op = m.ops[i]
+        p = [op.p[j] for j in range(4)]
+        if op.kind == 0:                                                             # STEM
+            c = m.convs[op.conv]
+            oh, ow = (m.in_h - 1) // 2 + 1, (m.in_w - 1) // 2 + 1
+            col = max(col, n * oh * ow * c.kpad * vb)
+            define(op.dst, (oh, ow, c.cout, c.cout_pad))
+        elif op.kind == 1:                                                           # CONV
+            c, s = m.convs[op.conv], sh[op.src]
+            oh, ow = (s[0] + 2 * c.pad - c.k) // c.stride + 1, (s[1] + 2 * c.pad - c.k) // c.stride + 1
+            col = max(col, n * oh * ow * c.kpad * vb)
+            define(op.dst, (oh, ow, c.cout, c.cout_pad))
+        elif op.kind == 2:                                                           # MAXPOOL
+            s = sh[op.src]
+            if op.k == 2:
+                define(op.dst, (s[0] // 2, s[1] // 2, s[2], s[3]))
+            else:
+                po = [pool_out_size(v, op.pad, op.ceil_mode) for v in s[:2]]
+                define(op.dst, (po[0], po[1], s[2], s[3]))
+        elif op.kind in (4, 8):                                                      # SE, CBAM
+            if op.kind == 4:
+                se_c = max(se_c, sh[op.src][2])
+            define(op.dst, sh[op.src])
+        elif op.kind == 5:                                                           # CROP
+            s = sh[op.src]
+            define(op.dst, (p[2], p[3], s[2], s[3]))
+        elif op.kind == 6:                                                           # SHAPE
+            s = sh[op.src]
+            define(op.dst, (s[0], s[1], p[0], p[0]))
+        elif op.kind == 9:                                                           # AFFINE
+            s, c = sh[op.src], m.convs[op.conv].cout
+            define(op.dst, (s[0], s[1], c, c))
+        elif op.kind == 10:                                                          # UPADD
+            define(op.dst, sh[op.res])
+    off, o = {}, 0
+    for bi in range(24):
+        off[bi] = o
+        o += al(need[bi] * 4)
+    for name, size in (("col", col), ("cu", (n + 1) * 4), ("z", n * se_c * 4), ("scale", n * se_c * 4)):
+        off[name] = o
+        o += al(size)
+    off["total"] = o
+    return off, sh
+
+
+def pool_out_size(v, pad, ceil_mode):
+    """torch MaxPool2d(3, 2, pad, ceil_mode) output length (aten pooling_output_shape); < 1 where torch raises."""
+    o = (v + 2 * pad - 3 + (1 if ceil_mode else 0)) // 2 + 1
+    if ceil_mode and (o - 1) * 2 >= v + pad:
+        o -= 1
+    return o
+
+
+def interpret_cnn_tables(m, store, frames_bgr=None, dtype=torch.float32, bufs=None, operands=False):
+    """Interpreter of a mer_cnn_forward op table (include/mer_b200.h: MerCnnOp) with the buffer / shape semantics of
+    resnet.cu's executor, on NHWC maps with padded channel counts, in `dtype`.  store maps the w / b addresses of the
+    table's MerResnetConv entries to their fp32 values (numpy or torch).  bufs: {index: [n, H, W, Cs] tensor} of
+    buffer contents to start from (what a test wrote into the workspace; a SHAPE op keeps a buffer given here).
+    operands: convolutions compute on the GEMM operands of m.gemm_mode (cnn_conv) and the stem on stem_operand, as
+    the kernels do; otherwise on the exact values (the network's own semantics).
+    Returns (out_feats [n, feat_dim], {index: tensor} of every buffer as the last op left it)."""
+    n = len(frames_bgr) if frames_bgr is not None else next(iter(bufs.values())).shape[0]
+    T = lambda v: torch.as_tensor(np.asarray(v, np.float32)).to(dtype)  # noqa: E731
+    mode = m.gemm_mode if operands else None
+    buf = {i: v.to(dtype).clone() for i, v in (bufs or {}).items()}
+    real = {i: v.shape[-1] for i, v in buf.items()}
+    given = set(buf)
+    out = torch.full((n, m.feat_dim), float("nan"), dtype=dtype)
+    mean, std = [m.mean[i] for i in range(3)], [m.std[i] for i in range(3)]
+
+    def conv(x, c, res=None):
+        kk = c.k * c.k * c.cin
+        assert c.kpad == kk or (c.cin == 3 and c.kpad in (160, 192))
+        return cnn_conv(x, T(store[c.w]), T(store[c.b]), c.k, c.stride, c.pad, mode, res)[0].to(dtype)
+    for i in range(m.n_ops):
+        op = m.ops[i]
+        p = [op.p[j] for j in range(4)]
+        res = buf[op.res] if op.res >= 0 and op.kind in (0, 1) else None
+        if op.kind == 0:                                                             # STEM
+            c = m.convs[op.conv]
+            if operands:
+                x0 = stem_operand(frames_bgr, m.scale, mean, std)
+            else:
+                pix = torch.as_tensor(np.ascontiguousarray(np.asarray(frames_bgr)[..., ::-1])).to(dtype)
+                x0 = (pix * m.scale - torch.tensor(mean, dtype=dtype)) / torch.tensor(std, dtype=dtype)
+            y = conv(x0, c, res)
+            buf[op.dst], real[op.dst] = (torch.relu(y) if op.relu else y), c.cout
+        elif op.kind == 1:                                                           # CONV
+            c = m.convs[op.conv]
+            assert op.src != op.dst and p[0] + c.cin <= real[op.src]
+            y = conv(buf[op.src][..., p[0]:p[0] + c.cin], c, res)
+            buf[op.dst], real[op.dst] = (torch.relu(y) if op.relu else y), c.cout
+        elif op.kind == 2:                                                           # MAXPOOL
+            assert op.k in (2, 3) and op.stride == 2 and op.src != op.dst
+            xin = buf[op.src].permute(0, 3, 1, 2)
+            y = F.max_pool2d(xin, 2, 2) if op.k == 2 else F.max_pool2d(xin, 3, 2, op.pad, ceil_mode=bool(op.ceil_mode))
+            buf[op.dst], real[op.dst] = y.permute(0, 2, 3, 1), real[op.src]
+        elif op.kind == 9:                                                           # AFFINE
+            af = m.convs[op.conv]
+            v = buf[op.src][..., p[0]:p[0] + af.cout] * T(store[af.w]) + T(store[af.b])
+            assert op.src != op.dst
+            buf[op.dst], real[op.dst] = (torch.relu(v) if op.relu else v), af.cout
+        elif op.kind == 10:                                                          # UPADD
+            up = buf[op.src].repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
+            buf[op.dst], real[op.dst] = buf[op.res] + up, real[op.res]
+        elif op.kind == 11:                                                          # MASKMUL
+            mask = buf[op.res][..., :p[3]].sum(dim=3, keepdim=True)
+            buf[op.dst][..., p[1]:p[1] + p[2]] = buf[op.src][..., p[0]:p[0] + p[2]] * mask
+        elif op.kind == 4:                                                           # SE
+            dn, up = m.convs[op.conv], m.convs[op.k]
+            y = buf[op.src]
+            d = torch.relu(y.mean(dim=(1, 2)) @ T(store[dn.w]).T + T(store[dn.b]))
+            g = torch.sigmoid(d @ T(store[up.w]).T + T(store[up.b]))
+            buf[op.dst], real[op.dst] = torch.relu(g[:, None, None, :] * y + buf[op.res]), real[op.src]
+        elif op.kind == 5:                                                           # CROP
+            buf[op.dst], real[op.dst] = buf[op.src][:, p[0]:p[0] + p[2], p[1]:p[1] + p[3]].clone(), real[op.src]
+        elif op.kind == 6:                                                           # SHAPE
+            if op.dst not in given:
+                hh, ww = buf[op.src].shape[1:3]
+                buf[op.dst] = torch.full((n, hh, ww, p[0]), float("nan"), dtype=dtype)
+            real[op.dst] = p[0]
+        elif op.kind == 7:                                                           # SLICE
+            v = buf[op.src][..., p[0]:p[0] + p[2]]
+            v = torch.relu(v) if op.relu == 1 else v
+            if op.res >= 0:
+                v = v + buf[op.res][..., p[3]:p[3] + p[2]]
+            buf[op.dst][..., p[1]:p[1] + p[2]] = torch.relu(v) if op.relu == 2 else v
+        elif op.kind == 8:                                                           # CBAM
+            l1, l2, sp = m.convs[op.conv], m.convs[p[0]], m.convs[p[1]]
+            y = buf[op.src]
+            assert y.shape[-1] == real[op.src] == l1.cin
+
+            def mlp(v):
+                return torch.relu(v @ T(store[l1.w]).T + T(store[l1.b])) @ T(store[l2.w]).T + T(store[l2.b])
+            y1 = y * torch.sigmoid(mlp(y.mean(dim=(1, 2))) + mlp(y.amax(dim=(1, 2))))[:, None, None, :]
+            comp = torch.stack((y1.amax(dim=3), y1.mean(dim=3)), dim=1)              # [n, 2, H, W]: max, mean
+            sg = torch.sigmoid(F.conv2d(comp, T(store[sp.w]).reshape(1, 2, 7, 7), T(store[sp.b]), padding=3))
+            buf[op.dst], real[op.dst] = torch.relu(y1 * sg[:, 0, :, :, None] + buf[op.res]), real[op.src]
+        else:
+            assert op.kind == 3                                                      # GAP
+            v = buf[op.src][..., :real[op.src]].mean(dim=(1, 2)) / max(p[2], 1)
+            cols = slice(p[0], p[0] + real[op.src])
+            out[:, cols] = out[:, cols] + v if p[1] else v
+    return out, buf
+
+
+def cnn_model(convs, ops, gemm_mode, in_hw, feat_dim, scale=1.0, mean=(0.0, 0.0, 0.0), std=(1.0, 1.0, 1.0)):
+    """A MerCnnModel from plain lists: convs of dicts of MerResnetConv fields, ops of dicts of MerCnnOp fields (missing
+    ones: conv / res -1, src / dst 0, the rest 0).  Returns (model, keep-alive list)."""
+    import ctypes as C
+
+    from mertools_b200 import encoders as En
+    ca = (En.MerResnetConv * len(convs))()
+    for c, d in zip(ca, convs):
+        for k, v in d.items():
+            setattr(c, k, v)
+    oa = (En.MerCnnOp * len(ops))()
+    for o, d in zip(oa, ops):
+        o.conv, o.res = -1, -1
+        for k, v in d.items():
+            if k == "p":
+                o.p = (C.c_int * 4)(*(list(v) + [0] * (4 - len(v))))
+            else:
+                setattr(o, k, v)
+    m = En.MerCnnModel()
+    m.convs, m.n_convs, m.ops, m.n_ops = ca, len(convs), oa, len(ops)
+    m.gemm_mode, (m.in_h, m.in_w), m.scale, m.feat_dim = gemm_mode, in_hw, scale, feat_dim
+    m.mean, m.std = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
+    return m, [ca, oa]
+
+
+def cnn_refused_tables(w=0x7F0000000000, b=0x7F0000001000):
+    """(name, model, keep-alive, expected mer_last_error fragment) of op tables the executor cannot run: each would
+    launch the stem's gather (and GEMM) before conv() or mer_gemm_launch refused it, so the planning pass refuses them.
+    Every convolution entry points at w and b: the default addresses are never dereferenced while the planner refuses
+    these tables on a machine without a GPU; a GPU test passes real zeroed buffers (>= 192 * 192 * 4 bytes for w,
+    >= 192 * 4 for b) so that a table wrongly accepted runs on readable memory and fails on its launch count."""
+    from mertools_b200 import _lib as L
+
+    def conv(cin, cout, cout_pad, k, stride, pad, kpad=None):
+        return dict(w=w, b=b, cin=cin, cout=cout, cout_pad=cout_pad, k=k, stride=stride, pad=pad,
+                    kpad=k * k * cin if kpad is None else kpad)
+    stem = conv(3, 64, 128, 7, 2, 3, 192)
+    stem_s = conv(3, 64, 128, 7, 2, 3, 160)
+    shape = lambda c: [dict(kind=6, src=0, dst=1, p=(c,))]  # noqa: E731
+    F16, BF = L.MER_GEMM_F16, L.MER_GEMM_BF16X3
+    # (name, gemm mode, frame h x w, convs, ops between the stem and the GAP, expected message); a frame of 3 x 3
+    # gives a 2 x 2 stem output, 1 x 1 a 1 x 1 one.  With a second conv entry the table ends in CONV 1 -> 2 + GAP 2,
+    # otherwise in a GAP of the last op's dst.
+    cases = [
+        # f16 3x3 over 32 channels: K = 288 is no multiple of the f16 GEMM's 64-wide K step
+        ("f16 K 288", F16, (3, 3), [stem, conv(32, 128, 128, 3, 1, 1)], shape(32), "conv geometry"),
+        ("split K 72", BF, (3, 3), [stem_s, conv(8, 128, 128, 3, 1, 1)], shape(8), "conv geometry"),
+        ("kpad != k k cin", F16, (3, 3), [stem, conv(64, 128, 128, 1, 1, 0, kpad=128)], shape(64), "conv geometry"),
+        ("cin % 8", BF, (3, 3), [stem_s, conv(4, 128, 128, 4, 1, 0)], shape(4), "conv geometry"),
+        ("cout_pad % 128", F16, (3, 3), [stem, conv(64, 64, 64, 1, 1, 0)], shape(64), "conv geometry"),
+        ("cout > cout_pad", F16, (3, 3), [stem, conv(64, 256, 128, 1, 1, 0)], shape(64), "conv geometry"),
+        ("stride 0", F16, (3, 3), [stem, conv(64, 128, 128, 1, 0, 0)], shape(64), "conv geometry"),
+        ("k 0", F16, (3, 3), [stem, conv(64, 128, 128, 0, 1, 0, kpad=0)], shape(64), "conv geometry"),
+        ("7x7 of a 2 x 2 map", F16, (3, 3), [stem, conv(64, 128, 128, 7, 1, 0)], shape(64),
+         "conv (pad 0) of a 2 x 2 map"),
+        ("stem cout_pad 192", F16, (3, 3), [conv(3, 64, 192, 7, 2, 3, 192)], [], "stem geometry"),
+        ("stem cout > cout_pad", F16, (3, 3), [conv(3, 256, 128, 7, 2, 3, 192)], [], "stem geometry"),
+        ("3x3/2 pool pad 0 of 1 x 1", F16, (1, 1), [stem], [dict(kind=2, src=0, dst=1, k=3, stride=2, pad=0)],
+         "max-pool (pad 0) of a 1 x 1 map"),
+        ("3x3/2 floor pool pad 0 of 2 x 2", F16, (3, 3), [stem],
+         [dict(kind=5, src=0, dst=2, p=(0, 0, 2, 2)), dict(kind=2, src=2, dst=1, k=3, stride=2, pad=0)],
+         "max-pool (pad 0) of a 2 x 2 map"),
+        ("3x3/2 pool pad 2", F16, (3, 3), [stem], [dict(kind=2, src=0, dst=1, k=3, stride=2, pad=2)], "max-pool (pad 2)"),
+    ]
+    out = []
+    for name, mode, hw, convs, mid, msg in cases:
+        ops = [dict(kind=0, conv=0, dst=0, relu=1)] + mid
+        if len(convs) > 1:
+            ops += [dict(kind=1, conv=1, src=1, dst=2), dict(kind=3, src=2)]
+        else:
+            ops.append(dict(kind=3, src=ops[-1]["dst"]))
+        m, keep = cnn_model(convs, ops, mode, hw, 256)
+        out.append((name, m, keep, msg))
+    return out

@@ -311,90 +311,58 @@ def test_cnn_executor_plans_the_ferplus_tables_without_a_gpu():
     assert dll.mer_cnn_workspace_bytes(C.byref(m), 1) == -1 and b"SE shortcut shape" in dll.mer_last_error()
 
 
-def _interpret_cnn_tables(m, store, frames_bgr):
-    """Test-side interpreter of a mer_cnn_forward op table (include/mer_b200.h: MerCnnOp): the same buffer / shape
-    semantics as resnet.cu's executor, in torch fp32 on NHWC maps with padded channel counts, so that the tables a
-    Python builder emits can be checked against a golden without a GPU."""
-    import torch.nn.functional as F
+def test_cnn_planner_refuses_tables_the_executor_cannot_run():
+    """mer_cnn_workspace_bytes (the planning pass mer_cnn_forward also runs before its first launch) returns -1 with a
+    message for convolution geometry the im2col gather or the GEMM cannot run, a stem whose output width is no GEMM
+    column block, and a 3x3 / 2 max-pool whose window does not fit the map (torch raises for those sizes).  The same
+    tables with the defect removed plan normally."""
+    import ctypes as C
+
+    from mertools_b200 import _lib
     from mertools_b200 import encoders as En
-    n = len(frames_bgr)
-    mean = torch.tensor([m.mean[i] for i in range(3)])
-    std = torch.tensor([m.std[i] for i in range(3)])
-    x0 = (torch.from_numpy(np.ascontiguousarray(frames_bgr[..., ::-1])).float() * m.scale - mean) / std  # NHWC, RGB
-    buf, real = [None] * 24, [0] * 24
-    out = torch.full((n, m.feat_dim), float("nan"))
-    T = torch.from_numpy
+    dll = _lib.lib()
+    dll.mer_cnn_workspace_bytes.restype = C.c_longlong
+    dll.mer_cnn_workspace_bytes.argtypes = [C.POINTER(En.MerCnnModel), C.c_int]
+    import _kernel_refs as R
+    for name, m, _keep, msg in R.cnn_refused_tables():
+        assert dll.mer_cnn_workspace_bytes(C.byref(m), 2) == -1, name
+        err = dll.mer_last_error().decode()
+        assert msg in err, (name, err)
+    # controls: the f16 conv at 64 channels (K 576), split at 8 channels 2x2 (K 32), pad 0 ceil-mode pool of 2 x 2
+    fake = 0x7F0000000000
+    conv = lambda cin, k, kpad: dict(w=fake, b=fake, cin=cin, cout=128, cout_pad=128, k=k, stride=1, pad=1,  # noqa
+                                     kpad=kpad)
+    for mode, c, ch in ((_lib.MER_GEMM_F16, conv(64, 3, 576), 64), (_lib.MER_GEMM_BF16X3, conv(8, 2, 32), 8)):
+        stem = dict(conv(3, 7, 192 if mode == _lib.MER_GEMM_F16 else 160), stride=2, pad=3)
+        m, _k = R.cnn_model([stem, c], [dict(kind=0, conv=0, dst=0), dict(kind=6, src=0, dst=1, p=(ch,)),
+                                        dict(kind=1, conv=1, src=1, dst=2), dict(kind=3, src=2)], mode, (3, 3), 128)
+        assert dll.mer_cnn_workspace_bytes(C.byref(m), 2) == R.cnn_plan(m, 2)[0]["total"]
+    m, _k = R.cnn_model([dict(conv(3, 7, 192), stride=2, pad=3)],
+                        [dict(kind=0, conv=0, dst=0), dict(kind=2, src=0, dst=1, k=3, stride=2, pad=0, ceil_mode=1),
+                         dict(kind=3, src=1)], _lib.MER_GEMM_F16, (3, 3), 128)
+    assert dll.mer_cnn_workspace_bytes(C.byref(m), 1) == R.cnn_plan(m, 1)[0]["total"]
+    assert R.cnn_plan(m, 1)[1][1][:2] == (1, 1)
 
-    def conv(x, c):
-        w, b = store[c.w], store[c.b]                       # [cout_pad, kpad], [cout_pad]
-        kk = c.k * c.k * c.cin
-        assert c.kpad == kk or (c.cin == 3 and c.kpad in (160, 192))
-        wt = T(w[:, :kk]).reshape(c.cout_pad, c.k, c.k, c.cin).permute(0, 3, 1, 2)
-        y = F.conv2d(x.permute(0, 3, 1, 2), wt, T(b), stride=c.stride, padding=c.pad)
-        return y.permute(0, 2, 3, 1)
-    for i in range(m.n_ops):
-        op = m.ops[i]
-        p = [op.p[j] for j in range(4)]
-        if op.kind in (En.CNN_STEM, En.CNN_CONV):
-            c = m.convs[op.conv]
-            if op.kind == En.CNN_STEM:
-                y = conv(x0, c)
-            else:
-                assert op.src != op.dst and p[0] + c.cin <= real[op.src]
-                y = conv(buf[op.src][..., p[0]:p[0] + c.cin], c)
-            if op.res >= 0:
-                assert buf[op.res].shape == y.shape
-                y = y + buf[op.res]
-            buf[op.dst], real[op.dst] = (torch.relu(y) if op.relu else y), c.cout
-        elif op.kind == En.CNN_MAXPOOL:
-            assert op.k in (2, 3) and op.stride == 2 and op.src != op.dst
-            xin = buf[op.src].permute(0, 3, 1, 2)
-            y = F.max_pool2d(xin, 2, 2) if op.k == 2 else F.max_pool2d(xin, 3, 2, op.pad, ceil_mode=bool(op.ceil_mode))
-            buf[op.dst], real[op.dst] = y.permute(0, 2, 3, 1), real[op.src]
-        elif op.kind == En.CNN_AFFINE:
-            af = m.convs[op.conv]
-            v = buf[op.src][..., p[0]:p[0] + af.cout] * T(store[af.w]) + T(store[af.b])
-            assert op.src != op.dst
-            buf[op.dst], real[op.dst] = (torch.relu(v) if op.relu else v), af.cout
-        elif op.kind == En.CNN_UPADD:
-            up = buf[op.src].repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-            buf[op.dst], real[op.dst] = buf[op.res] + up, real[op.res]
-        elif op.kind == En.CNN_MASKMUL:
-            mask = buf[op.res][..., :p[3]].sum(dim=3, keepdim=True)
-            buf[op.dst][..., p[1]:p[1] + p[2]] = buf[op.src][..., p[0]:p[0] + p[2]] * mask
-        elif op.kind == En.CNN_SE:
-            dn, up = m.convs[op.conv], m.convs[op.k]
-            y = buf[op.src]
-            d = torch.relu(y.mean(dim=(1, 2)) @ T(store[dn.w]).T + T(store[dn.b]))
-            g = torch.sigmoid(d @ T(store[up.w]).T + T(store[up.b]))
-            buf[op.dst], real[op.dst] = torch.relu(g[:, None, None, :] * y + buf[op.res]), real[op.src]
-        elif op.kind == En.CNN_CROP:
-            buf[op.dst], real[op.dst] = buf[op.src][:, p[0]:p[0] + p[2], p[1]:p[1] + p[3]].clone(), real[op.src]
-        elif op.kind == En.CNN_SHAPE:
-            hh, ww = buf[op.src].shape[1:3]
-            buf[op.dst], real[op.dst] = torch.full((n, hh, ww, p[0]), float("nan")), p[0]
-        elif op.kind == En.CNN_SLICE:
-            v = buf[op.src][..., p[0]:p[0] + p[2]]
-            v = torch.relu(v) if op.relu == 1 else v
-            if op.res >= 0:
-                v = v + buf[op.res][..., p[3]:p[3] + p[2]]
-            buf[op.dst][..., p[1]:p[1] + p[2]] = torch.relu(v) if op.relu == 2 else v
-        elif op.kind == En.CNN_CBAM:
-            l1, l2, sp = m.convs[op.conv], m.convs[p[0]], m.convs[p[1]]
-            y = buf[op.src]
-            assert y.shape[-1] == real[op.src] == l1.cin
 
-            def mlp(v):
-                return torch.relu(v @ T(store[l1.w]).T + T(store[l1.b])) @ T(store[l2.w]).T + T(store[l2.b])
-            y1 = y * torch.sigmoid(mlp(y.mean(dim=(1, 2))) + mlp(y.amax(dim=(1, 2))))[:, None, None, :]
-            comp = torch.stack((y1.amax(dim=3), y1.mean(dim=3)), dim=1)              # [n, 2, H, W]: max, mean
-            sg = torch.sigmoid(F.conv2d(comp, T(store[sp.w]).reshape(1, 2, 7, 7), T(store[sp.b]), padding=3))
-            buf[op.dst], real[op.dst] = torch.relu(y1 * sg[:, 0, :, :, None] + buf[op.res]), real[op.src]
-        else:
-            assert op.kind == En.CNN_GAP
-            v = buf[op.src][..., :real[op.src]].mean(dim=(1, 2)) / max(p[2], 1)
-            cols = slice(p[0], p[0] + real[op.src])
-            out[:, cols] = out[:, cols] + v if p[1] else v
+def test_pool_output_size_matches_torch():
+    """The planner's MaxPool2d(3, 2) output size (mirrored by _kernel_refs.pool_out_size) against torch's own, including
+    the sizes torch refuses."""
+    import _kernel_refs as R
+    import torch.nn.functional as F
+    for pad in (0, 1):
+        for ceil in (0, 1):
+            for h in range(1, 120):
+                try:
+                    want = F.max_pool2d(torch.zeros(1, 1, h, 1 + 2 * pad + 2), 3, 2, pad, ceil_mode=bool(ceil)).shape[2]
+                except RuntimeError:
+                    want = 0
+                assert max(R.pool_out_size(h, pad, ceil), 0) == want, (h, pad, ceil)
+
+
+def _interpret(m, store, frames_bgr):
+    """out_feats of the float64 interpreter of the op semantics (tests/_kernel_refs.py), every column written."""
+    import _kernel_refs as R
+    out, _ = R.interpret_cnn_tables(m, store, frames_bgr, dtype=torch.float64)
     assert not torch.isnan(out).any(), "some output columns were never written"
     return out.numpy()
 
@@ -404,7 +372,7 @@ def test_ferplus_op_tables_reproduce_the_reference_golden_on_a_cpu_interpreter(s
     """The conv / op tables FerplusResnet50Encoder hands to mer_cnn_forward (BN folding, (ky, kx, c) weight layout,
     channel padding, caffe-style strides, shortcut wiring, SE layer indices), run by a torch interpreter of the op
     semantics, against outputs of the unmodified reference extractor.  Checks the host side of the CUDA path; the
-    kernels themselves are covered by the GPU tests."""
+    kernels themselves are compared with the same interpreter op by op in tests/test_cnn_kernels_gpu.py."""
     import importlib.util
     from mertools_b200 import encoders as En
     from oracle import pipeline as P
@@ -422,7 +390,7 @@ def test_ferplus_op_tables_reproduce_the_reference_golden_on_a_cpu_interpreter(s
     m, _keep = En.ferplus_resnet50_tables(S.ferplus_resnet50_state_dict(int(g["seed"]), se=se), pack)
     frames = mod.golden_clips()["vidA"][:2]                       # 256 x 256: Resize(256) is the identity
     crop = frames[:, 16:240, 16:240]                              # CenterCrop(224), as frame_features slices it
-    got = _interpret_cnn_tables(m, store, crop)
+    got = _interpret(m, store, crop)
     ref = g[f"{prefix}fra_vidA"][:2]
     assert got.shape == ref.shape and np.abs(got - ref).max() / np.abs(ref).max() < 1e-4
     enc_geom = En.FerplusResnet50Encoder.preprocess_geometry(None, 200, 300)
@@ -485,7 +453,7 @@ def test_manet_op_tables_reproduce_the_reference_golden_on_a_cpu_interpreter():
         store[len(store) + 1] = np.asarray(b, np.float32)
         return len(store) - 1, len(store)
     m, _keep = En.manet_tables(S.manet_state_dict(int(g["seed"])), pack)
-    got = _interpret_cnn_tables(m, store, mod.golden_clips()["vidA"][:2])
+    got = _interpret(m, store, mod.golden_clips()["vidA"][:2])
     ref = g["fra_vidA"][:2]
     assert got.shape == ref.shape and np.abs(got - ref).max() / np.abs(ref).max() < 1e-4
     dll = _lib.lib()
@@ -515,7 +483,7 @@ def test_emonet_op_tables_reproduce_the_reference_golden_on_a_cpu_interpreter():
         store[len(store) + 1] = np.asarray(b, np.float32)
         return len(store) - 1, len(store)
     m, _keep = En.emonet_tables(S.emonet_state_dict(int(g["seed"])), pack)
-    got = _interpret_cnn_tables(m, store, mod.golden_clips()["vidA"][:1])           # 256 x 256: no resize needed
+    got = _interpret(m, store, mod.golden_clips()["vidA"][:1])                      # 256 x 256: no resize needed
     ref = g["fra_vidA"][:1]
     assert got.shape == ref.shape and np.abs(got - ref).max() / np.abs(ref).max() < 1e-4
     dll = _lib.lib()

@@ -331,3 +331,75 @@ def test_hidden0_reference_is_the_oracle_at_layer_0(family):
     assert got.shape == want.shape == (2, 19, 1024 if family.startswith("large") else 768)
     assert float((got - want).abs().max()) < 1e-10
     assert bool((bound > 0).all()) and float((bound / want.abs().clamp(min=1e-3)).median()) < 5e-2
+
+
+# ---- table-driven CNN executor ----------------------------------------------------------------------------------------
+def test_cnn_operand_formats():
+    x = torch.tensor([1.0, 1.0 + 2.0 ** -11, 1.0 + 3 * 2.0 ** -11, 65504.0, 65520.0, -1e30, 2.0 ** -25, float("nan")])
+    got = R.f16_satfinite(x)
+    assert got.tolist()[:7] == [1.0, 1.0, 1.0 + 2.0 ** -9, 65504.0, 65504.0, -65504.0, 0.0]      # ties to even, clamped
+    assert math.isnan(got[7]) and got.dtype == torch.float32
+    y = torch.randn(4096, generator=_g(20)) * 50
+    hi, lo = R.split_bf16(y)
+    assert torch.equal(hi, y.bfloat16().float()) and torch.equal(lo, (y - hi).bfloat16().float())
+    assert bool(((y.double() - hi.double() - lo.double()).abs() <= 2.0 ** -16 * y.double().abs()).all())
+
+
+def test_stem_operand_is_the_fused_multiply_add_then_the_division():
+    """pix * scale - mean is exact in float64 for every 8-bit pixel (checked with fractions), so rounding it once to fp32
+    is the fma; the plain fp32 product-then-subtract rounds twice and differs in some operands by an ulp."""
+    from fractions import Fraction
+    mean, std = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+    scale = float(np.float32(1 / 255))
+    for mv in mean:
+        m32 = float(np.float32(mv))
+        for pix in range(256):
+            assert Fraction(pix * scale - m32) == Fraction(pix) * Fraction(scale) - Fraction(m32)
+    frames = np.arange(256, dtype=np.uint8).repeat(3).reshape(1, 16, 16, 3)
+    frames[..., 0] = frames[..., 0][:, ::-1]                    # different pixels in the three channels
+    got = R.stem_operand(frames, 1 / 255, mean, std)
+    rgb = torch.from_numpy(np.ascontiguousarray(frames[..., ::-1])).float()
+    plain = (rgb * np.float32(1 / 255) - torch.tensor(mean)) / torch.tensor(std)
+    # both round the difference once and the quotient once: they differ by at most an ulp of the operands' scale
+    scale_ = (rgb.double() / 255 + torch.tensor(mean).double()) / torch.tensor(std).double()
+    assert bool(((got - plain).double().abs() <= 2.0 ** -22 * scale_).all()) and int((got != plain).sum()) > 0
+    exact = (rgb.double() / 255 - torch.tensor(mean).double()) / torch.tensor(std).double()
+    assert float((got.double() - exact).abs().max()) < 1e-6
+
+
+def test_cnn_conv_reference():
+    x = torch.randn(2, 5, 4, 16, generator=_g(21)) * 3
+    w = torch.randn(128, 3 * 3 * 16 + 8, generator=_g(22))      # padded columns past k k cin are ignored
+    b = torch.randn(128, generator=_g(23))
+    r = torch.randn(2, 3, 2, 128, generator=_g(24))
+    y, a = R.cnn_conv(x, w, b, 3, 2, 1, res=r)
+    wt = w[:, :144].reshape(128, 3, 3, 16).permute(0, 3, 1, 2).double()
+    want = F.conv2d(x.permute(0, 3, 1, 2).double(), wt, b.double(), stride=2, padding=1).permute(0, 2, 3, 1) + r
+    assert float((y - want).abs().max()) < 1e-12 and bool((a >= y.abs() - 1e-12).all())
+    y16, _ = R.cnn_conv(x, w, b, 3, 2, 1, mode=R.GEMM_F16)
+    want16, _ = R.cnn_conv(R.f16_satfinite(x), R.f16_satfinite(w), b, 3, 2, 1)
+    assert torch.equal(y16, want16)
+    ys, _ = R.cnn_conv(x, w, b, 3, 2, 1, mode=R.GEMM_BF16X3)
+    (xh, xl), (wh, wl) = R.split_bf16(x), R.split_bf16(w)
+    full, _ = R.cnn_conv(xh.double() + xl.double(), wh.double() + wl.double(), b, 3, 2, 1)
+    lolo, _ = R.cnn_conv(xl, wl, torch.zeros(128), 3, 2, 1)
+    assert float((ys - (full - lolo)).abs().max()) < 1e-9 and float((full - lolo - full).abs().max()) > 0
+
+
+def test_cnn_plan_mirrors_the_executor_on_the_extractor_tables():
+    """The workspace layout the GPU tests read buffers from equals mer_cnn_workspace_bytes on the FER+ / SENet, MA-Net and
+    EmoNet tables at 1 and 3 frames."""
+    import ctypes as C
+
+    from mertools_b200 import _lib
+    from mertools_b200 import encoders as En
+    from mertools_b200 import synthetic as S
+    dll = _lib.lib()
+    dll.mer_cnn_workspace_bytes.restype = C.c_longlong
+    dll.mer_cnn_workspace_bytes.argtypes = [C.POINTER(En.MerCnnModel), C.c_int]
+    pack = lambda w, b: (1, 1)  # noqa: E731
+    for m, _keep in (En.ferplus_resnet50_tables(S.ferplus_resnet50_state_dict(9), pack),
+                     En.ferplus_resnet50_tables(S.ferplus_resnet50_state_dict(9, se=True), pack),
+                     En.manet_tables(S.manet_state_dict(3), pack), En.emonet_tables(S.emonet_state_dict(3), pack)):
+        for n in (1, 3):
+            assert R.cnn_plan(m, n)[0]["total"] == dll.mer_cnn_workspace_bytes(C.byref(m), n)
