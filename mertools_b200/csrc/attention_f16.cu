@@ -390,7 +390,8 @@ int mer_attention_f16_long_launch(const void* qkv16, const void* vt16, long long
 
 // qkv16: fp16 [tokens, 3*heads*64] (V columns unused), vt16: fp16 [heads*64, vt_ld] with vt[d, token];
 // ctx [tokens, heads*64] in the format `out_mode` names (3 fp16, 2 bf16 hi | lo split rows, 1 tf32-rounded fp32, 0 fp32).
-// Rows of up to 249 tokens take the one-CTA-per-(sequence, head) kernel of attention_short.cu.
+// Rows of 129 .. 208 tokens take the one-CTA-per-(sequence, head) kernel of attention_short.cu
+// (mer_attention_short_enabled; MER_ATT_SHORT=1: every row of up to 249 tokens).
 int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
                              int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream) {
   if (mer_attention_short_enabled(max_seqlen))

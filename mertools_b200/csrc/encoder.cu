@@ -3,7 +3,7 @@
 // mer_run_stack   : the transformer stack shared by the modalities (dims at run time)
 //                   pre-LN  (HF ViTLayer, modeling_vit.py:328-346; CLIPEncoderLayer; the stable-layer-norm
 //                            HuBERT encoder) in fp16 / TF32 / BF16X3 operand formats
-//                   post-LN (HF HubertEncoderLayer, modeling_hubert.py:372-405; BertLayer) in BF16X3
+//                   post-LN (HF HubertEncoderLayer, modeling_hubert.py:372-405; BertLayer) in fp16 / BF16X3
 // mer_vit_forward : frames (uint8 BGR) -> patchify -> patch-embed GEMM (+bias +pos) -> stack ->
 //                   token-sum readout  (reference: extract_vision_huggingface.py:137-144)
 // mer_clip_vision_forward, mer_hubert_forward (base and large families), mer_bert_forward: see each.
@@ -116,7 +116,8 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
                        MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
         MER_TRY(linear(a.mode, xn16, w.w_o, w.b_o, a.x, a.x, M, D, D, 0, stream));
       } else {
-        // sequences beyond the fp16 attention kernel (CLIP L/14: 257 tokens): the linear layers stay on fp16
+        // sequences beyond the fp16 attention kernels (> 505 tokens: a CLIP tower forced to fp16 at a larger image;
+        // no caller at image 224 reaches this): the linear layers stay on fp16
         // operands, attention runs the fp32-operand flash kernel on a TF32-rounded fp32 q | k | v (same 10-bit
         // mantissa) and its fp32 context is cast to the fp16 out-proj operand through the idle FFN buffer
         MER_TRY(linear(a.mode, xn16, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, MER_EPI_ROUND_TF32, stream));
@@ -157,7 +158,8 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
                        MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
         MER_TRY(linear(a.mode, c16, w.w_o, w.b_o, a.x, a.qkv, M, D, D, 0, stream));  // qkv is dead: holds the sum
       } else {
-        // rows beyond the fp16 attention kernel (> 249 frames): TF32-rounded fp32 q | k | v (same 10-bit mantissa)
+        // rows beyond the fp16 attention kernels (> MER_ATT_LONG_MAX frames with long_rows, > 505 tokens without):
+        // TF32-rounded fp32 q | k | v (same 10-bit mantissa)
         // through the fp32-operand attention kernels, fp32 context cast to the fp16 out-proj operand
         MER_TRY(linear(a.mode, x16, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, MER_EPI_ROUND_TF32, stream, vt,
                        a.vt_ld, 2 * D));

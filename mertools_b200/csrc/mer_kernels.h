@@ -52,7 +52,7 @@ int mer_attention_f16_launch(const void* qkv16, const void* vt16, long long vt_l
 int mer_attention_tc_launch(const float* qkv, const float* vt, long long vt_ld, float* ctx, const int* cu_seqlens,
                             int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 // attention_short.cu: the fp16 V^T operands of rows of <= 249 tokens, one CTA per (sequence, head)
-bool mer_attention_short_enabled(int max_seqlen);  // max_seqlen <= 249 and MER_ATT_SHORT is not 0
+bool mer_attention_short_enabled(int max_seqlen);  // 129 .. 208 tokens; MER_ATT_SHORT=1: any <= 249, =0: none
 int mer_attention_short_launch(const void* qkv16, const void* vt16, long long vt_ld, void* ctx, const int* cu_seqlens,
                                int n_seq, long long tokens, int heads, int max_seqlen, int out_mode, cudaStream_t stream);
 
@@ -97,7 +97,7 @@ struct MerStackArgs {
   const MerLayerWeights* layers;
   int n_layers;
   int pre_ln;
-  int mode;                  // MER_GEMM_TF32 | MER_GEMM_BF16X3 | MER_GEMM_F16 (pre-LN only)
+  int mode;                  // MER_GEMM_TF32 | MER_GEMM_BF16X3 | MER_GEMM_F16, either order (no caller runs post-LN TF32)
   int dim, ffn, heads;       // 0 = 768 / 3072 / 12
   int quick_gelu;            // FC1 activation: x * sigmoid(1.702 x) (CLIP) instead of erf-GELU
   float eps;

@@ -178,9 +178,10 @@ class ClipVisionEncoder:
     def __init__(self, state_dict, device="cuda", ln_eps=1e-5, image=224, precision=None, variant=0, mean=CLIP_MEAN,
                  std=CLIP_STD, resize=None):
         """variant / mean / std / resize: set by Dinov2Encoder (same tower, MER_VISION_DINOV2 readout).
-        precision: None = "f16" when the fp16 attention kernel covers the token count (B/32), else "tf32";
-        "f16" forces fp16 linear layers for longer sequences too (L/14: attention then runs the fp32-operand flash
-        kernel between them; env MER_CLIP_PRECISION=f16; not yet measured)."""
+        precision: None = "f16" up to 249 tokens per frame (B/32), else "tf32" (L/14: attention on fp16 q | k | V^T
+        between tf32 linear layers); "f16" forces fp16 linear layers for longer sequences too (L/14: attention then
+        runs the fp16 V^T kernel, past 505 tokens the fp32-operand kernel of attention.cu; env MER_CLIP_PRECISION=f16;
+        not yet measured)."""
         L.check(L.lib().mer_check_device())
         sd = W._np(state_dict)
         self.device = torch.device(device)
@@ -199,7 +200,7 @@ class ClipVisionEncoder:
         kpad = (3 * p * p + 31) // 32 * 32
         wflat = np.zeros((D, kpad), np.float32)
         wflat[:, :3 * p * p] = pw.reshape(D, 3 * p * p)
-        # fp16 operands need the fp16 attention kernel (<= 249 tokens per frame): B/32 yes, L/14 (257) runs TF32
+        # fp16 linear layers by default up to 249 tokens per frame: B/32 yes, L/14 (257) runs TF32
         import os
         precision = precision or os.environ.get("MER_CLIP_PRECISION")
         assert precision in (None, "f16", "tf32"), precision

@@ -376,6 +376,242 @@ def attention_packed(qkv, cu, heads):
     return out, mag, amp
 
 
+# ---- transformer stack: one layer of mer_run_stack (encoder.cu) ---------------------------------------------------------
+# stack_layer restates one layer in float64 from the GPU's own input hidden state, with an elementwise bound built from
+# the pieces above (the lambda = 4 model of the front end).  The stack stores its operands (LN outputs, q | k | v, ctx, the
+# FC1 output) as fp16, tf32 or split bf16; each such store rounds by at most out_rounding(v), and that rounding enters
+# the bound as LAMBDA * out_rounding(v): its standard deviation is at most out_rounding(v), and it is the dominant error
+# of every layer, carried through the next linear stage in quadrature (_lin_err).  Stage by stage (encoder.cu):
+#   LN          _ln_err (mer_layernorm_launch; pre-LN: LN1 / LN2 then the operand store; post-LN: fp32 x, then its copy)
+#   linear      _lin_err with u_op = 0 for fp16 or tf32 operands (fp16- / tf32-exact weights and activations: exact
+#               products), 2^-16 for split bf16 (hi hi + hi lo + lo hi; the dropped lo lo is <= 2^-16 |a| |w|); + u |z|
+#               for the fp32 bias / residual add of the epilogue (linear() of encoder.cu, gemm.cu epilogue)
+#   attention   _attention_err: the kernel's own (2^-11 + 16 u A + 8 u) P |V| (P rounded to fp16 or tf32 for P V in every
+#               route), plus the q | k | v errors carried through softmax; a one-token row is exactly its v
+#   activation  _gelu_err (gelu_erf_fast) or _quick_gelu_err (quick_gelu_fast), gemm.cu epi_act
+# The input operand is applied exactly: post-LN layers read fp16(x) (MER_LN_SPLIT_F16) or split_bf16(x) of the previous
+# LayerNorm's fp32 output, which is the hidden state itself.
+STACK_UNIT = {None: 0.0, "f16": 0.0, "tf32": 0.0, "bf16x3": 2.0 ** -16}
+STACK_OPERAND = {None: None, "f16": "f16", "tf32": "tf32", "bf16x3": "split"}
+ATT_KERNEL = {"short": "attention_short_kernel", "f16": "attention_vt_kernel<true", "long": "attention_vt_kernel<true",
+              "tc": "attention_vt_kernel<false", "fallback": "attention_kernel"}
+
+
+def stack_route(mode, max_seqlen, long_rows=False):
+    """Attention route of mer_run_stack for a stack in `mode` ("f16", "tf32", "bf16x3") whose batch has `max_seqlen`
+    (encoder.cu: f16_long / f16_rows / long_att; attention.cu mer_attention_uses_tc; attention_f16.cu
+    mer_attention_f16_supported; attention_short.cu mer_attention_short_enabled without MER_ATT_SHORT): "short" (fp16
+    q | k | V^T, attention_short.cu, 129 .. 208 tokens), "f16" (fp16 q | k | V^T, tiled),
+    "long" (the same kernel past 505 tokens, long_rows only), "tc" (tf32 q | k | V^T) or "fallback" (tf32 q | k | v read
+    by attention.cu; an fp16 stack casts its fp32 context to fp16)."""
+    tc = max_seqlen <= 253
+    f16_long = long_rows and 505 < max_seqlen <= 4096
+    f16_rows = f16_long or max_seqlen <= 505
+    if mode == "f16":
+        if f16_rows:
+            return "short" if 128 < max_seqlen <= 208 else ("long" if f16_long else "f16")
+        return "fallback"
+    if not tc and f16_rows:
+        return "long" if f16_long else "f16"
+    return "tc" if tc else "fallback"
+
+
+def stack_form(mode, pre_ln, max_seqlen, long_rows=False, quick=False, eps=1e-12, heads=12):
+    return dict(mode=mode, pre_ln=pre_ln, route=None if mode is None else stack_route(mode, max_seqlen, long_rows),
+                act="quick" if quick else "erf", eps=eps, heads=heads)
+
+
+def packed_layer(pk, layers, l, mode):
+    """Layer l's weights exactly as the encoder packed them on the device (MerLayerWeights pointers resolved through the
+    Packed store): fp16 weights as stored (F16), the tf32-rounded copies (TF32), hi + lo of the split rows (BF16X3);
+    LayerNorm parameters and biases fp32.  float64 tensors on the device."""
+    by_ptr = {t.data_ptr(): t for t in pk.tensors}
+    out = {}
+    for name, _ in type(layers[l])._fields_:
+        t = by_ptr[getattr(layers[l], name)]
+        if name.startswith("w_") and mode == "bf16x3":
+            hi, lo = split_halves(t)
+            t = hi.double() + lo.double()
+        out[name] = t.double()
+    return out
+
+
+def layer_from_state_dict(sd, names, l, device="cpu"):
+    """The same dict from an HF state dict (float64, no operand rounding): q | k | v concatenated as pack_layers does."""
+    g = lambda role: torch.as_tensor(np.asarray(sd[names[role].format(i=l)])).to(device, torch.float64)  # noqa: E731
+    return dict(ln1_g=g("ln1_g"), ln1_b=g("ln1_b"), w_qkv=torch.cat([g("q_w"), g("k_w"), g("v_w")]),
+                b_qkv=torch.cat([g("q_b"), g("k_b"), g("v_b")]), w_o=g("o_w"), b_o=g("o_b"), ln2_g=g("ln2_g"),
+                ln2_b=g("ln2_b"), w_fc1=g("fc1_w"), b_fc1=g("fc1_b"), w_fc2=g("fc2_w"), b_fc2=g("fc2_b"))
+
+
+def quick_gelu(x):
+    return x * torch.sigmoid(1.702 * x)
+
+
+def _quick_gelu_err(z, e):
+    """quick_gelu_fast (mer_common.cuh): x * rcp.approx(1 + ex2.approx(-1.702 log2(e) x)).  |q''| <= 0.9, so the carried
+    error is |q'| e + 0.45 e^2.  Own error, relative to |q|: the product and the reciprocal (2 u), the exponent's
+    argument rounded (u |t|, t = 2.46 x, moving 2^t by ln 2 u |t| = 1.70 u |x|) and ex2.approx (2 u), both scaled by
+    1 - sigmoid (the share of 2^t in 1 + 2^t), and the sum 1 + 2^t (u)."""
+    s = torch.sigmoid(1.702 * z)
+    q = z * s
+    slope = (s + 1.702 * z * s * (1 - s)).abs()
+    own = U32 * q.abs() * (3 + (1 - s) * (2 + 1.702 * z.abs()))
+    return q, slope * e + 0.45 * e * e + own + 1e-30
+
+
+def _store(v, e, fmt, emulate):
+    """The stack stores v as fmt (None: fp32): returns (value, bound)."""
+    if fmt is None:
+        return v, e
+    if emulate:
+        return operand(v, fmt).to(v.dtype), e
+    return v, e + LAMBDA * out_rounding(v, fmt != "split")
+
+
+def operand(v, fmt):
+    """Value of fp32 v stored as fmt: "f16" (cvt.rn.satfinite), "tf32" (cvt.rna), "split" (hi + lo)."""
+    if fmt is None:
+        return v
+    if fmt == "f16":
+        return f16_satfinite(v).to(v.dtype)
+    if fmt == "tf32":
+        return round_tf32_ties_away(v.float()).to(v.dtype)
+    hi, lo = split_bf16(v)
+    return (hi.double() + lo.double()).to(v.dtype)
+
+
+def _attention_err(qkv, e, cu, heads, scale=0.125, fault=None):
+    """(ctx, bound) of the stack's attention on packed q | k | v with elementwise bounds e.  The kernel's own error is
+    that of tests/test_attention_fp32_gpu.py (attention_packed's P |V| and A).  Carried errors: a v error reaches ctx
+    through P (in quadrature); a score error ds_ij (q and k errors, in quadrature over the head's 64 columns, / 8) moves
+    ctx by sum_j P_ij (ds_ij - sum_l P_il ds_il) v_j, at most 2 max_j ds_ij P |V|.  A one-token row is v itself."""
+    D = heads * 64
+    ctx, mag, amp = attention_packed(qkv, cu, heads)
+    bound = (2.0 ** -11 + 16 * U32 * amp + 8 * U32) * mag
+    x, e = qkv.double(), e.double()
+    for s in range(len(cu) - 1):
+        a, b = cu[s], cu[s + 1]
+        if b - a == 1:
+            bound[a:b] = e[a:b, 2 * D:]
+            continue
+        hv = lambda t, c: t[a:b, c * D:(c + 1) * D].reshape(b - a, heads, 64).transpose(0, 1)  # noqa: E731
+        q, k, v = hv(x, 0), hv(x, 1), hv(x, 2)
+        eq, ek, ev = hv(e, 0), hv(e, 1), hv(e, 2)
+        p = torch.softmax(q @ k.transpose(1, 2) * 0.125, dim=-1)
+        ds = torch.sqrt((eq * eq) @ (k * k).transpose(1, 2) + (q * q) @ (ek * ek).transpose(1, 2)) * 0.125
+        carried = torch.sqrt((p * p) @ (ev * ev)) + 2 * ds.amax(-1, keepdim=True) * (p @ v.abs())
+        bound[a:b] += carried.transpose(0, 1).reshape(b - a, D)
+    if fault is not None:                   # tests of the bound only: a restatement of a wrong attention
+        ctx = _faulty_attention(x, cu, heads, scale, fault)
+    return ctx, bound
+
+
+def _faulty_attention(x, cu, heads, scale, fault):
+    D = heads * 64
+    q, k, v = x[:, :D], x[:, D:2 * D], x[:, 2 * D:]
+    if fault == "head_k":                   # head h reads head h + 1's keys
+        k = torch.roll(k.view(-1, heads, 64), -1, dims=1).reshape(-1, D)
+    if fault == "key_shift":                # a V^T column offset: token j reads token j + 1's value
+        v = torch.roll(v, -1, dims=0)
+    return attention_packed(torch.cat([q * (scale / 0.125), k, v], 1), cu, heads)[0]
+
+
+def stack_layer(w, x_in, cu, form, fault=None, emulate=False, op_in=None, trace=None):
+    """One layer of mer_run_stack on x_in [tokens, D] (the GPU's hidden state l) with packed cu_seqlens `cu` (a list),
+    weights w (packed_layer / layer_from_state_dict) and `form` (stack_form).  Returns (x_out, bound): float64, or with
+    `emulate` an fp32 evaluation that rounds every stored operand (bound None).  form["mode"] None: no operand rounding
+    anywhere (the network itself, for the comparison with the oracle).
+    For the tests of the bound only: `fault` restates a wrong layer (see STACK_FAULTS); op_in replaces the input operand
+    copy of a post-LN layer; trace (a dict) receives the post-LN layer's fp32 x after LN1 as trace["x1"]."""
+    dt = torch.float32 if emulate else torch.float64
+    x = x_in.to(dt)
+    fmt = STACK_OPERAND[form["mode"]]
+    u_op = STACK_UNIT[form["mode"]]
+    route = form["route"]
+    qkv_fmt = None if fmt is None else ("f16" if route in ("short", "f16", "long") else "tf32")
+    D, eps, heads = x.shape[-1], form["eps"], form["heads"]
+    pre_ln = form["pre_ln"] != (fault == "ln_order")
+    W = {k: v.to(dt) for k, v in w.items()}
+    if fault == "ln_swap":
+        for a, b in (("ln1_g", "ln2_g"), ("ln1_b", "ln2_b")):
+            W[a], W[b] = W[b], W[a]
+    for name in ("b_qkv", "b_o", "b_fc1", "b_fc2", "ln1_b", "ln2_b"):
+        if fault == "drop_" + name:
+            W[name] = torch.zeros_like(W[name])
+    zero = torch.zeros_like(x)
+
+    def ln(v, ev, g, b):
+        if emulate:
+            return F.layer_norm(v, (D,), g, b, eps), None
+        return _ln_err(v, ev, g, b, eps)
+
+    def lin(a, ea, wname, bname, res=None, eres=None):
+        z = a @ W[wname].T + W[bname]
+        if res is not None:
+            z = z + res
+        if emulate:
+            return z, None
+        e = _lin_err(lambda t, ww: t @ ww.T, a, ea, W[wname], u_op, a.shape[-1]) + U32 * z.abs()
+        return z, e if eres is None else e + eres
+
+    if pre_ln:
+        a, ea = _store(*ln(x, zero, W["ln1_g"], W["ln1_b"]), fmt, emulate)
+    else:
+        a = operand(x if op_in is None else op_in.to(dt), fmt)
+        ea = None if emulate else zero
+    qkv, eqkv = _store(*lin(a, ea, "w_qkv", "b_qkv"), qkv_fmt, emulate)
+    scale = 1.0 / math.sqrt(D) if fault == "scale" else 0.125
+    att_fault = fault if fault in ("scale", "head_k", "key_shift") else None
+    if emulate:
+        ctx = _emulated_attention(qkv, cu, heads, "f16" if route in ("short", "f16", "long") else "tf32")
+        ectx = None
+    else:
+        ctx, ectx = _attention_err(qkv, eqkv, cu, heads, scale, att_fault)
+    ctx, ectx = _store(ctx, ectx, fmt, emulate)     # the fp16 fallback's mer_cast_f16 is the same rounding
+    res = None if fault == "no_residual" else x
+    s, es = lin(ctx, ectx, "w_o", "b_o", res, None if emulate else zero)
+    if pre_ln:
+        x1, ex1 = s, es
+        a2, ea2 = _store(*ln(x1, ex1, W["ln2_g"], W["ln2_b"]), fmt, emulate)
+    else:
+        x1, ex1 = ln(s, es, W["ln1_g"], W["ln1_b"])
+        a2, ea2 = _store(x1, ex1, fmt, emulate)
+    if trace is not None:
+        trace["x1"] = x1
+    z, ez = lin(a2, ea2, "w_fc1", "b_fc1")
+    quick = (form["act"] == "quick") != (fault == "act")
+    if emulate:
+        h, eh = (quick_gelu(z) if quick else 0.5 * z * (1 + torch.erf(z / math.sqrt(2.0)))), None
+    else:
+        h, eh = (_quick_gelu_err if quick else _gelu_err)(z, ez)
+    h, eh = _store(h, eh, fmt, emulate)
+    s2, es2 = lin(h, eh, "w_fc2", "b_fc2", x1, ex1)
+    if pre_ln:
+        return s2, es2
+    return ln(s2, es2, W["ln2_g"], W["ln2_b"])
+
+
+STACK_FAULTS = ("act", "drop_b_qkv", "drop_b_o", "drop_b_fc1", "drop_b_fc2", "drop_ln1_b", "drop_ln2_b", "ln_swap",
+                "ln_order", "scale", "head_k", "key_shift", "no_residual", "stale_operand")
+
+
+def _emulated_attention(qkv, cu, heads, p_fmt):
+    """fp32 attention with P rounded to p_fmt for the P V product (fp16 in the fp16 V^T kernels, tf32 ties-away in the
+    tf32 V^T kernel and attention.cu), normalised by the fp32 sum of the unrounded P."""
+    D = heads * 64
+    x = qkv.float()
+    out = torch.zeros(x.shape[0], D, dtype=torch.float32, device=x.device)
+    for s in range(len(cu) - 1):
+        a, b = cu[s], cu[s + 1]
+        q, k, v = (x[a:b, c * D:(c + 1) * D].reshape(b - a, heads, 64).transpose(0, 1) for c in range(3))
+        sc = q @ k.transpose(1, 2) * 0.125
+        p = torch.exp(sc - sc.amax(-1, keepdim=True))
+        pr = p.half().float() if p_fmt == "f16" else round_tf32_ties_away(p.contiguous())
+        out[a:b] = ((pr @ v) / p.sum(-1, keepdim=True)).transpose(0, 1).reshape(b - a, D)
+    return out
+
+
 def biased_attention(qkv, bias, rowscale, batch, T, heads):
     """softmax_j((q_i / 8) . k_j + rowscale[b, i, h] * bias[h, i, j]) v_j.  Returns (ctx, P |V|, S): S is the row's score
     error in units of u for 64 chained fp32 FMAs and one more for the bias: 65 max_j sum_d |q_d k_jd| / 8 + max_j

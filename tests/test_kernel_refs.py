@@ -333,6 +333,125 @@ def test_hidden0_reference_is_the_oracle_at_layer_0(family):
     assert bool((bound > 0).all()) and float((bound / want.abs().clamp(min=1e-3)).median()) < 5e-2
 
 
+# ---- transformer stack: one layer of mer_run_stack ----------------------------------------------------------------------
+def _stack_case(family, tokens=None, scale=1.0):
+    """(state dict, names, oracle hidden states in float64, cu, form kwargs) of a one- or two-layer synthetic model."""
+    from mertools_b200 import synthetic as S
+    from mertools_b200 import weights as W
+    from oracle import encoders as E
+    g = _g(40)
+    if family == "vit":
+        sd = S.vit_state_dict(seed=0, layers=1, scale=scale)
+        n = tokens or 1
+        hs = E.vit_hidden_states(sd, torch.rand(n, 3, 224, 224, generator=g) * 2 - 1, layers=1, dtype=torch.float64)
+        return sd, W.VIT_NAMES, [h.reshape(-1, 768) for h in hs], [197 * i for i in range(n + 1)], dict(pre_ln=True)
+    if family == "clip":
+        sd = S.clip_vision_state_dict(seed=4, variant="b32", layers=1, scale=scale)
+        n = tokens or 2
+        sdt = {k: torch.as_tensor(v) for k, v in sd.items()}
+        _, hs = E.clip_image_features(sdt, torch.rand(n, 3, 224, 224, generator=g) * 2 - 1, layers=1,
+                                      dtype=torch.float64)
+        return sd, W.CLIP_NAMES, [h.reshape(-1, 768) for h in hs], [50 * i for i in range(n + 1)], \
+            dict(pre_ln=True, quick=True, eps=1e-5)
+    if family in ("hubert", "hubert_stable"):
+        stable = family == "hubert_stable"
+        sd = S.hubert_state_dict(seed=1, layers=2, large=stable, scale=scale)
+        sdt = {k: torch.as_tensor(v) for k, v in sd.items()}
+        x = torch.stack([_normalised(R.speech_like(16000, s))[0] for s in (1, 2)])
+        hs = E.hubert_hidden_states(sdt, x, layers=2, heads=16 if stable else 12, dtype=torch.float64)
+        D = 1024 if stable else 768
+        return sd, W.HUBERT_NAMES, [h.reshape(-1, D) for h in hs], [0, 49, 98], \
+            dict(pre_ln=stable, eps=1e-5, heads=D // 64)
+    lens = tokens or [1, 2, 64, 65]
+    large = family == "roberta_large"
+    sd = S.bert_state_dict(300, seed=2, layers=1, large=large, scale=scale, max_pos=514)
+    sdt = {k: torch.as_tensor(v) for k, v in sd.items()}
+    gen = np.random.default_rng(3)
+    seqs = [np.concatenate([[0], gen.integers(1, 299, n - 2), [299]])[:n] if n > 1 else np.array([299]) for n in lens]
+    eps, off = (1e-5, 2) if large else (1e-12, 0)
+    hs = [torch.cat([h[0] for h in t]) for t in zip(*(E.bert_hidden_states(sdt, s, layers=1, heads=16 if large else 12, eps=eps,
+                                                            position_offset=off, dtype=torch.float64) for s in seqs))]
+    hs = [h.reshape(-1, 1024 if large else 768) for h in hs]
+    return sd, W.BERT_NAMES, hs, [int(c) for c in np.cumsum([0] + list(lens))], \
+        dict(pre_ln=False, eps=eps, heads=16 if large else 12)
+
+
+@pytest.mark.parametrize("family", ["vit", "clip", "hubert", "hubert_stable", "bert", "roberta_large"])
+def test_stack_layer_is_the_oracles_layer(family):
+    """stack_layer without operand rounding is one layer of the oracle (vit_hidden_states, clip_image_features,
+    hubert_hidden_states in both layer orders, bert_hidden_states) in float64, on the oracle's own input."""
+    sd, names, hs, cu, kw = _stack_case(family)
+    w = R.layer_from_state_dict(sd, names, 0)
+    form = R.stack_form(None, max_seqlen=max(b - a for a, b in zip(cu, cu[1:])), **kw)
+    got, bound = R.stack_layer(w, hs[0], cu, form)
+    assert float((got - hs[1]).abs().max()) < 1e-12
+    assert bool((bound > 0).all())
+
+
+EMULATED = [("vit", "f16"), ("vit", "tf32"), ("clip", "f16"), ("hubert", "f16"), ("hubert", "bf16x3"),
+            ("hubert_stable", "bf16x3"), ("bert", "f16"), ("bert", "bf16x3")]
+
+
+@pytest.mark.parametrize("family,mode", EMULATED)
+def test_stack_bound_covers_an_fp32_emulation(family, mode):
+    """An fp32 evaluation of the layer that rounds every operand the stack stores (LN output, q | k | v, P, ctx, FC1
+    output) to the form's format lands inside the bound of the float64 restatement."""
+    sd, names, hs, cu, kw = _stack_case(family)
+    w = {k: (R.operand(v.float(), R.STACK_OPERAND[mode]).double() if k.startswith("w_") else v)
+         for k, v in R.layer_from_state_dict(sd, names, 0).items()}
+    form = R.stack_form(mode, max_seqlen=max(b - a for a, b in zip(cu, cu[1:])), **kw)
+    x = hs[0].float()
+    ref, bound = R.stack_layer(w, x, cu, form)
+    emu, _ = R.stack_layer(w, x, cu, form, emulate=True)
+    ratio = float(((emu.double() - ref).abs() / bound).max())
+    print(f"stack layer {family} {mode}: fp32 emulation at {ratio:.3f} of the bound")
+    assert 1e-3 < ratio <= 1.0
+
+
+def test_stack_bound_rejects_the_faults():
+    """Each wiring fault of STACK_FAULTS, restated, leaves the bound by 4x or more on some element in a form the GPU test
+    runs (two ViT frames in fp16; a BERT batch of 1, 2, 64 and 65 tokens in fp16 and split bf16; CLIP B/32 for the
+    activation).  Not listed: erf <-> tanh GELU (<= 3e-4 apart, below fp16's own noise after FC2) and BERT <-> RoBERTa
+    eps (1e-12 vs 1e-5 against unit variances): the GEMM epilogue and LayerNorm tests cover those."""
+    cases = []
+    for family, mode in (("vit", "f16"), ("bert", "f16"), ("bert", "bf16x3"), ("clip", "f16")):
+        sd, names, hs, cu, kw = _stack_case(family, tokens=2 if family == "vit" else None)
+        w = {k: (R.operand(v.float(), R.STACK_OPERAND[mode]).double() if k.startswith("w_") else v)
+             for k, v in R.layer_from_state_dict(sd, names, 0).items()}
+        form = R.stack_form(mode, max_seqlen=max(b - a for a, b in zip(cu, cu[1:])), **kw)
+        x = hs[0].float()
+        cases.append((f"{family} {mode}", w, x, cu, form) + R.stack_layer(w, x, cu, form))
+    worst = {}
+    for fault in R.STACK_FAULTS:
+        for name, w, x, cu, form, ref, bound in cases:
+            if fault == "stale_operand":
+                if form["pre_ln"]:
+                    continue
+                tr = {}                       # LN1's copy of the layer before: its x after the attention half
+                R.stack_layer(w, x, cu, form, trace=tr)
+                got, _ = R.stack_layer(w, x, cu, form, op_in=tr["x1"])
+            else:
+                got, _ = R.stack_layer(w, x, cu, form, fault=fault)
+            r = float(((got - ref).abs() / bound).max())
+            if r > worst.get(fault, ("", 0.0))[1]:
+                worst[fault] = (name, r)
+    print("fault / bound: " + ", ".join(f"{k} {v[1]:.1f} ({v[0]})" for k, v in worst.items()))
+    assert all(worst[f][1] >= 4 for f in R.STACK_FAULTS), worst
+
+
+def test_stack_routes_follow_the_encoder_predicates():
+    """stack_route at each boundary of encoder.cu / attention.cu / attention_f16.cu."""
+    f16 = {1: "f16", 128: "f16", 129: "short", 208: "short", 209: "f16", 249: "f16", 250: "f16", 253: "f16", 254: "f16", 505: "f16", 506: "long", 4096: "long",
+           4097: "fallback"}
+    split = {1: "tc", 253: "tc", 254: "f16", 505: "f16", 506: "long", 4096: "long", 4097: "fallback"}
+    for n, r in f16.items():
+        assert R.stack_route("f16", n, long_rows=True) == r, n
+    for n, r in split.items():
+        assert R.stack_route("bf16x3", n, long_rows=True) == r, n
+    assert R.stack_route("f16", 512) == "fallback" and R.stack_route("bf16x3", 512) == "fallback"   # BERT at 512
+    assert R.stack_route("tf32", 197) == "tc" and R.stack_route("tf32", 257) == "f16"             # ViT / CLIP L/14
+
+
 # ---- table-driven CNN executor ----------------------------------------------------------------------------------------
 def test_cnn_operand_formats():
     x = torch.tensor([1.0, 1.0 + 2.0 ** -11, 1.0 + 3 * 2.0 ** -11, 65504.0, 65520.0, -1e30, 2.0 ** -25, float("nan")])
