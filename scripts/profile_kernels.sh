@@ -6,7 +6,7 @@
 #   gpurun_out/<tag>_fusion.{ncu-rep,json}  the two kernels of one fusion training step (graph replay)
 # Three profiled processes instead of one per kernel: the capture windows are set with MER_CUPROF (runtime.cu).  The
 # GEMM report (source pages of 6 large kernels, ~40 MB) is summarised on the box and dropped: gpurun_out/ comes back only
-# below 64 MiB.  Environment switches (MER_ATT_F16_VER=...) are inherited.
+# below 64 MiB.  Environment switches (MER_ATT_SHORT=...) are inherited.
 set -u
 tag=${1:-r2}
 out=gpurun_out

@@ -1,5 +1,5 @@
 """Small launches of every hand-synchronised kernel family, for compute-sanitizer (scripts/sanitize.sh):
-the wgmma GEMM in its three operand modes and both tile widths, both V^T attention kernels
+the wgmma GEMM in its three operand modes and both tile widths, every tensor-core attention route
 on ragged batches, the LLaMA kernels (causal head-dim-128 attention, RoPE, RMSNorm, SwiGLU), the BLOOM / OPT / GPT-2
 kernels (ALiBi attention, causal attention at head_dim 64 / 96 / 128, wide LayerNorm, tanh-GELU / fp16 ReLU epilogues), LayerNorm, the HuBERT front-end (conv0 + GroupNorm, positional conv) through a 2-layer forward, the
 fused fusion step (cluster kernel with DSMEM exchange + weight-gradient kernel).  Sizes are tiny: racecheck is slow."""
@@ -10,6 +10,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 from mertools_b200 import _lib as L  # noqa: E402
 from mertools_b200 import synthetic as S  # noqa: E402
 
@@ -32,23 +33,20 @@ def gemms():
 
 
 def attention():
-    heads = 2
-    for dtype, env, vers, lens in ((torch.float16, "MER_ATT_F16_VER", (1, 3, 4, 6, 7), [197, 5, 64, 129, 249, 17]),
-                                   (torch.float32, "MER_ATT_TC_VER", (1, 2), [197, 5, 64, 129, 253, 17])):
-        tokens = sum(lens)
-        qkv = (torch.randn(tokens, 3 * heads * 64, device=dev)).to(dtype)
-        if dtype == torch.float32:
-            L.round_tf32_(qkv)
-        al = 8 if dtype == torch.float16 else 4
-        vt = torch.zeros(heads * 64, (tokens + al - 1) // al * al, dtype=dtype, device=dev)
-        vt[:, :tokens] = qkv[:, 2 * heads * 64:].T
-        cu = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int32, device=dev)
-        ctx = torch.empty(tokens, heads * 64, dtype=dtype, device=dev)
-        for v in vers:
-            os.environ[env] = str(v)
-            L.attention(qkv, ctx, cu, max(lens), heads, vt=vt)
-            torch.cuda.synchronize()
-        os.environ.pop(env)
+    """One small launch per route of tests/test_attention_tc_gpu.py (the short kernel, the fp16 / tf32 tiled kernel,
+    mer_attention_hd, mer_attention_long, the causal, ALiBi and multi-query kernels), on ragged rows with an empty
+    sequence and unaligned starts, in the fp32 and fp16 ctx formats."""
+    import _kernel_refs as R
+    from test_attention_tc_gpu import _device_operands, _run
+    for name in R.ATT_TC_CASES:
+        c = R.att_tc_case(name)
+        c["lens"] = [5, 0, 17, 600 if c["entry"] == "long" else min(max(c["lens"]), 300)]
+        ops = R.att_tc_operands(c, 1.5)
+        qkv, vt, cu = _device_operands(c, ops, dev)
+        slopes = None if ops["slopes"] is None else ops["slopes"].to(dev)
+        for fmt in ("f16",) if c["causal"] else ("fp32", "f16"):
+            _run(c, qkv, vt, cu, fmt, slopes)
+    torch.cuda.synchronize()
     print("attention ok")
 
 

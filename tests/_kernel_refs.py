@@ -353,27 +353,353 @@ def hubert_hidden0(sd, wave, conv_f16=False, ln_eps=1e-5):
     return x, ex
 
 
-def attention_packed(qkv, cu, heads):
-    """softmax(Q K^T / 8) V per (sequence, head) of packed [tokens, 3 * heads * 64] rows.  Returns (ctx, P |V|, A): P |V|
-    is the scale of the error a perturbed probability leaves, A [tokens, heads * 64] the row's max_j sum_d |q_d k_jd| / 8,
-    the scale of the error of a score summed in fp32."""
-    D = heads * 64
+def attention_packed(qkv, cu, heads, hd=64, scale=0.125, causal=False, slopes=None, v=None, mqa=False, stats=False):
+    """softmax(scale Q K^T (+ ALiBi)) V per (sequence, head) of packed rows.  qkv [tokens, >= 3 * heads * hd]: Q | K | V
+    column blocks; with `mqa` Q is columns [0, heads * hd) and the one K head the next hd columns (the rest of the row is
+    not read).  v (optional): V as its own [tokens, heads * hd] ([tokens, hd] with mqa) tensor instead of qkv's V block.
+    causal: query i sees keys 0 .. i of its sequence.  slopes [heads]: HF's ALiBi, + slope_h * j with j counted from the
+    sequence start.  Empty sequences in cu are skipped.
+    Returns (ctx, P |V|, A) [tokens, heads * hd]: P |V| is the scale of the error a perturbed probability leaves, A the
+    row's score amplitude max_j scale sum_d |q_d k_jd| (+ max |slope_h (j - i)| over the keys whose probability is not
+    negligible, the bias the kernel adds in fp32), the scale of the error of a score summed in fp32.  stats: a fourth
+    item, dict(tiny = sum_{j: p~_j < 2^-13} |v_j| / sum_j p~_j with p~ = exp(s - max s) (the keys whose probability is an
+    fp16 subnormal or in the lowest normal binade), keys = the number of keys each row sees)."""
+    D = heads * hd
+    kh = 1 if mqa else heads
     x = qkv.double()
+    vv = x[:, 2 * D:3 * D] if v is None else v.double()
     out = torch.zeros(x.shape[0], D, dtype=torch.float64, device=x.device)
     mag, amp = torch.zeros_like(out), torch.zeros_like(out)
+    tiny, keys = torch.zeros_like(out), torch.zeros_like(out)
     for s in range(len(cu) - 1):
         a, b = cu[s], cu[s + 1]
         if b <= a:
             continue
-        q = x[a:b, :D].view(b - a, heads, 64).transpose(0, 1)
-        k = x[a:b, D:2 * D].view(b - a, heads, 64).transpose(0, 1)
-        v = x[a:b, 2 * D:].view(b - a, heads, 64).transpose(0, 1)
-        p = torch.softmax(q @ k.transpose(1, 2) / 8.0, dim=-1)
-        out[a:b] = (p @ v).transpose(0, 1).reshape(b - a, D)
-        mag[a:b] = (p @ v.abs()).transpose(0, 1).reshape(b - a, D)
-        top = (q.abs() @ k.abs().transpose(1, 2) / 8.0).amax(-1)                 # [heads, len]
-        amp[a:b] = top.T[:, :, None].expand(-1, -1, 64).reshape(b - a, D)
+        n = b - a
+        q = x[a:b, :D].reshape(n, heads, hd).transpose(0, 1)
+        k = x[a:b, D:D + kh * hd].reshape(n, kh, hd).transpose(0, 1)
+        vs = vv[a:b, :kh * hd].reshape(n, kh, hd).transpose(0, 1)
+        sc = q @ k.transpose(1, 2) * scale
+        top = q.abs() @ k.abs().transpose(1, 2) * scale                            # [heads, n, n]
+        ii = torch.arange(n, device=x.device)
+        if slopes is not None:
+            sl = slopes.double().to(x.device)[:, None, None]
+            sc = sc + sl * ii[None, None, :]
+        if causal:
+            future = ii[None, :] > ii[:, None]
+            sc = sc.masked_fill(future, float("-inf"))
+            top = top.masked_fill(future, 0.0)
+        p = torch.softmax(sc, dim=-1)
+        top = top.amax(-1)
+        if slopes is not None:
+            top = top + (sl * (ii[None, :] - ii[:, None]) * (p > 1e-30)).abs().amax(-1)
+        flat = lambda t: t.transpose(0, 1).reshape(n, D)  # noqa: E731
+        out[a:b] = flat(p @ vs)
+        mag[a:b] = flat(p @ vs.abs())
+        amp[a:b] = flat(top[..., None].expand(-1, -1, hd))
+        if stats:
+            pt = torch.exp(sc - sc.amax(-1, keepdim=True))
+            tiny[a:b] = flat(((pt < 2.0 ** -13) * (pt > 0)).double() @ vs.abs() / pt.sum(-1, keepdim=True))
+            seen = (ii + 1 if causal else torch.full_like(ii, n)).double()
+            keys[a:b] = seen[:, None].expand(-1, D)
+    if stats:
+        return out, mag, amp, dict(tiny=tiny, keys=keys)
     return out, mag, amp
+
+
+# ---- tensor-core attention: attention_short.cu, attention_f16.cu, attention_causal.cu ----------------------------------
+def ctx_rounding(v, fmt):
+    """Largest error of storing a value of magnitude v in the ctx format: fp16 (cvt.rn.satfinite; subnormal spacing
+    2^-24), tf32 (cvt.rna: half of 10 mantissa bits), split bf16 hi + lo, fp32 (nothing: the kernel's last product)."""
+    if fmt == "f16":
+        return torch.clamp(2.0 ** -11 * v, min=2.0 ** -25)
+    if fmt == "tf32":
+        return 2.0 ** -11 * v
+    if fmt == "split":
+        return 2.0 ** -17 * v
+    return torch.zeros_like(v)
+
+
+def attention_tc_bound(mag, amp, st, ref, fmt):
+    """Elementwise bound of the fp16 / tf32 tensor-core attention kernels against attention_packed(stats=True)'s
+    (ref, mag = P |V|, amp = A, st), u = 2^-24, n = st["keys"].  A = max_j scale sum_d |q_d k_jd| (+ the largest
+    ALiBi bias |slope (j - i)| over the keys that keep a probability), so every scaled score s_j and the row maximum m
+    lie in [-A, A] and |s_j - m| <= 2 A.  The kernels compute, per row (natural-log units for exponents):
+      score      q . k_j on mma.sync, fp32 accumulate: fp16 x fp16 and tf32 x tf32 products are exact, one rounding
+                 (truncation at worst: 2 u) of a partial sum <= sum_d |q_d k_jd| per 16-wide (8-wide tf32) k-step,
+                 <= 8 steps at head_dim <= 128: 16 u A.  ALiBi adds slope * sqrt(128) (rounded: u |bias|) with one
+                 fmaf (u |s_j|): 2 u A.  Together <= 18 u A.
+      exponent   fmaf(s, SL2, -b), b = fl(m SL2), SL2 = fl(scale log2(e)), then ex2.approx.ftz (relative 2^-22 = 4 u).
+                 SL2's rounding scales s - m by (1 + u): u |s - m| <= 2 u A; b's rounding: u |m| <= u A; the fma's
+                 rounding: u |s - m| <= 2 u A; ex2: 4 u.  Together 5 u A + 4 u.
+      rescales   each online rescale multiplies the earlier keys by ex2((m_old - m_new) SL2): the difference, the
+                 product and SL2 each round by u |m_old - m_new|, and the maxima only grow, so their sum over a row's
+                 rescales is <= 2 A: 6 u A; ex2 adds 4 u per rescale, <= n / 64 + 2 of them: (n / 16 + 8) u.
+    So each unnormalised probability is p~_j e^{d_j} with |d_j| <= D = 29 u A + (n / 16 + 12) u (keys whose probability
+    is below 1e-30 may have a larger d_j; they move ctx by nothing an fp32 result can show).  The normaliser is summed
+    from the same perturbed values, so P_j becomes P_j r_j with e^{-2D} <= r_j <= e^{2D}, and ctx moves by at most
+    (e^{2D} - 1) P |V|.
+      P          rounded once for P V, numerator only: fp16 (cvt.rn.satfinite) or tf32 (cvt.rna), 2^-11 relative.  p~ is
+                 formed against the running maximum, which only makes it larger; where it is below 2^-13 (fp16
+                 subnormals and the lowest binade, with room for the factor e^D) the rounding is <= 2^-25 absolute and
+                 later rescales only shrink it: 2^-25 tiny, tiny = sum_{p~_j < 2^-13} |v_j| / sum_j p~_j.
+      O          fp32 accumulation, 2 u per MMA step of 16 keys, <= n / 16 + 5 steps (the up to 7 leading foreign keys,
+                 whole 64-key tiles): (n / 8 + 10) u; one rescale product per tile or chunk: (n / 64 + 2) u.
+      normaliser each thread sums <= 32 values per tile or chunk (31 u), l = l sc + ps rounds twice per tile
+                 ((n / 32 + 4) u), two shuffle adds (2 u): (n / 32 + 37) u relative to l, i.e. to |ctx| <= P |V|.
+      finish     1 / l and the product: 2 u.  O, normaliser and finish: (11 n / 64 + 51) u, + u for the products of
+                 these relative errors.
+    The P, O, normaliser and finish terms act on the perturbed probabilities, whose P |V| is at most e^{2D} P |V|, and
+    the P rounding acts on values already off by those fp32 errors: factor (1 + 2^-10).  Total
+      (e^{2D} - 1) P |V| + e^{2D} ((1 + 2^-10) (2^-11 + (11 n / 64 + 52) u) P |V| + 2^-25 tiny)
+    plus ctx_rounding of |ref| plus that (the ctx store).  A worst case: no constant is fitted to observed errors."""
+    n = st["keys"]
+    d2 = 2 * (29 * U32 * amp + (n / 16 + 12) * U32)
+    grow = torch.exp(d2)
+    own = torch.expm1(d2) * mag + grow * ((1 + 2.0 ** -10) * (2.0 ** -11 + (11 * n / 64 + 52) * U32) * mag +
+                                         2.0 ** -25 * st["tiny"])
+    return own + ctx_rounding(ref.abs() + own, fmt)
+
+
+def bound_ratio(got, ref, bound):
+    """|got - ref| / bound elementwise, 0 where got equals ref (a zero bound on an exact zero, ALBERT's pad columns), inf
+    where got is NaN."""
+    err = (got.double() - ref).abs()
+    return torch.where(err == 0, torch.zeros_like(err), err / bound).nan_to_num(nan=float("inf"))
+
+
+def tc_bound_ratio(got, qkv, cu, heads, fmt, **kw):
+    """Worst |got - attention_packed(qkv, cu, heads, **kw)| / attention_tc_bound over the rows of the sequences in cu
+    (a list): the check of one tensor-core attention launch (ctx `fmt`) against float64.  got: ctx values as fp32 /
+    fp16 (split rows already recombined); computed on qkv's device."""
+    ref, mag, amp, st = attention_packed(qkv, cu, heads, stats=True, **kw)
+    rows = slice(cu[0], cu[-1])
+    r = bound_ratio(got[rows].to(ref.device), ref[rows], attention_tc_bound(mag, amp, st, ref, fmt)[rows])
+    return float(r.max())
+
+
+def ctx_format(x, fmt):
+    """fp32 ctx values as the kernels store them in `fmt` (see ctx_rounding), as fp32."""
+    if fmt == "f16":
+        return f16_satfinite(x)
+    if fmt == "tf32":
+        return round_tf32_ties_away(x.float())
+    if fmt == "split":
+        hi, lo = split_bf16(x)
+        return hi + lo
+    return x.float()
+
+
+# Restated faults of the tensor-core attention kernels (tests/test_kernel_refs.py: each must leave the bound):
+#   bf16_p        P rounded to bf16 for P V (what a wgmma A operand in bf16 would do)
+#   acc16         O accumulated in fp16: rounded to fp16 after every 16-key MMA step
+#   vt_shift      past the first 64-key tile the V^T column is off by one (key j reads token j + 1's value)
+#   causal_diag   the causal mask drops the diagonal key (query i sees keys 0 .. i - 1)
+#   alibi_tile    ALiBi key positions restarting at every 64-key tile (the tile offset rel0 dropped).  An offset common
+#                 to all keys of a row -- ALiBi on packed instead of in-sequence positions -- cancels in the softmax
+#                 and changes nothing: tests/test_kernel_refs.py checks that instead
+#   mqa_head_k    the multi-query kernel reading head h's K columns (heads + h) * hd instead of the one K head
+#   hd96_scale    head_dim 96 scored at 1/8 instead of 1/sqrt(96)
+#   foreign_keys  the up to 7 keys before a sequence start (the 8-token aligned key axis) left unmasked
+ATT_TC_FAULTS = ("bf16_p", "acc16", "vt_shift", "causal_diag", "alibi_tile", "mqa_head_k", "hd96_scale",
+                 "foreign_keys")
+
+
+def attention_tc_emulated(qkv, cu, heads, hd=64, scale=0.125, causal=False, slopes=None, v=None, mqa=False,
+                          p_fmt="f16", fault=None):
+    """An fp32 evaluation with the kernels' arithmetic (fp32 scores, p~ = exp(s - max) in fp32, P rounded to p_fmt
+    ("f16", "tf32") for P V, the normaliser summed from the unrounded p~, fp32 O), before the ctx store (ctx_format).
+    Same arguments as attention_packed; `fault` (ATT_TC_FAULTS) restates a wrong kernel."""
+    D = heads * hd
+    x = qkv.float()
+    T = x.shape[0]
+    vv = x[:, 2 * D:3 * D] if v is None else v.float()
+    kh = 1 if mqa else heads
+    if fault == "hd96_scale" and hd == 96:
+        scale = 0.125
+    out = torch.zeros(T, D, dtype=torch.float32, device=x.device)
+    for s in range(len(cu) - 1):
+        a, b = cu[s], cu[s + 1]
+        if b <= a:
+            continue
+        n = b - a
+        ka = a & ~7 if fault == "foreign_keys" else a                           # first key
+        nk = b - ka
+        q = x[a:b, :D].reshape(n, heads, hd).transpose(0, 1)
+        if fault == "mqa_head_k" and mqa:
+            k = x[ka:b, D:2 * D].reshape(nk, heads, hd).transpose(0, 1)
+        else:
+            k = x[ka:b, D:D + kh * hd].reshape(nk, kh, hd).transpose(0, 1)
+        vs = vv[ka:b, :kh * hd]
+        if fault == "vt_shift":
+            j = torch.arange(n, device=x.device)
+            src = (a + j + 1).clamp(max=T - 1)
+            moved = vv[src, :kh * hd] * (a + j + 1 < T)[:, None]
+            vs = torch.where((j + (a & 7) >= 64)[:, None], moved, vs)
+        vs = vs.reshape(nk, kh, hd).transpose(0, 1)
+        sc = (q @ k.transpose(1, 2)) * scale
+        i = torch.arange(n, device=x.device)[:, None] + (a - ka)                # query index on the key axis
+        jj = torch.arange(nk, device=x.device)[None, :]
+        if slopes is not None:
+            pos = jj % 64 if fault == "alibi_tile" else jj
+            sc = sc + slopes.float().to(x.device)[:, None, None] * (pos - i).float()
+        if causal:
+            sc = sc.masked_fill(jj >= i if fault == "causal_diag" else jj > i, float("-inf"))
+        p = torch.exp(sc - sc.amax(-1, keepdim=True))
+        if p_fmt == "f16" and fault != "bf16_p":
+            pr = p.half().float()
+        elif fault == "bf16_p":
+            pr = p.bfloat16().float()
+        else:
+            pr = round_tf32_ties_away(p.contiguous())
+        if fault == "acc16":
+            o = torch.zeros(heads, n, hd, dtype=torch.float32, device=x.device)
+            for st in range(0, nk, 16):
+                o = (o + pr[..., st:st + 16] @ vs[..., st:st + 16, :]).half().float()
+        else:
+            o = pr @ vs
+        out[a:b] = (o / p.sum(-1, keepdim=True)).transpose(0, 1).reshape(n, D)
+    return out
+
+
+# The operand sets of tests/test_attention_tc_gpu.py, one per (route, shape); tests/test_kernel_refs.py runs the
+# emulation and the faults on the same sets.  Lengths: every kernel boundary +-1 (16-key steps, 64-key tiles, the short
+# kernel's 128-key chunk and its default 129 .. 208 window, 249 / 253 / 505 caps), an odd length first so that most
+# starts are not multiples of 8, and an empty sequence inside cu_seqlens.
+ATT_TC_EDGES = [9, 1, 2, 3, 4, 5, 6, 7, 8, 15, 16, 17, 63, 64, 65, 127, 128, 129, 208, 209, 248, 249]
+
+
+def _lens(*more, top=None):
+    ls = [n for n in ATT_TC_EDGES if top is None or n <= top] + list(more)
+    ls.insert(3, 0)
+    return ls
+
+
+ATT_TC_CASES = {
+    # mer_attention, fp16 q | k | V^T: the short kernel (MER_ATT_SHORT=1: every row <= 249; unset: 129 .. 208)
+    "short": dict(entry="attention", fmt="f16", env="1", kernel="attention_short_kernel", lens=_lens(), heads=3),
+    "short_default": dict(entry="attention", fmt="f16", env=None, kernel="attention_short_kernel",
+                          lens=_lens(top=208), heads=3),
+    # the tiled fp16 kernel (MER_ATT_SHORT=0 at <= 249; 250 .. 505 always)
+    "tile_f16": dict(entry="attention", fmt="f16", env="0", kernel="attention_vt_kernel<true", lens=_lens(), heads=3),
+    "tile_f16_505": dict(entry="attention", fmt="f16", env=None, kernel="attention_vt_kernel<true",
+                         lens=_lens(250, 253, 254, 300, 504, 505), heads=3),
+    # the tf32 kernel, <= 253 tokens
+    "tile_tf32": dict(entry="attention", fmt="tf32", env=None, kernel="attention_vt_kernel<false",
+                      lens=_lens(250, 252, 253), heads=3),
+    # mer_attention_hd: runtime scale, head_dim 32 (26 or 32 valid columns) and 64, rows up to 512
+    "hd32_26_f16": dict(entry="hd", fmt="f16", kernel="attention_vt_kernel<true", lens=_lens(250, 254, 505, 506, 512),
+                        heads=4, hd=32, valid=26),
+    "hd32_32_tf32": dict(entry="hd", fmt="tf32", kernel="attention_vt_kernel<false",
+                         lens=_lens(250, 253, 254, 505, 506, 512), heads=4, hd=32, valid=32),
+    "hd32_26_tf32": dict(entry="hd", fmt="tf32", kernel="attention_vt_kernel<false", lens=_lens(254, 511, 512),
+                         heads=2, hd=32, valid=26),
+    "hd64_f16": dict(entry="hd", fmt="f16", kernel="attention_vt_kernel<true", lens=_lens(250, 505, 506, 511, 512),
+                     heads=3, hd=64, scale=0.1),
+    "hd64_tf32": dict(entry="hd", fmt="tf32", kernel="attention_vt_kernel<false", lens=_lens(253, 254, 300, 512),
+                      heads=3, hd=64, scale=0.1),
+    # mer_attention_long: 506 .. 4096 among short rows
+    "long": dict(entry="long", fmt="f16", kernel="attention_vt_kernel<true",
+                 lens=[4095, 9, 506, 0, 249, 511, 1, 512, 65, 513, 1000, 129, 2999, 17, 4096, 505], heads=2),
+    # causal kernels: mer_causal_attention_hd_f16 at 64 / 96, mer_causal_attention_f16 (128)
+    "causal64": dict(entry="causal", fmt="f16", kernel="causal_attention_kernel<64, false, false>",
+                     lens=_lens(250, 253, 254, 505, 506, 512, 1000, 2048), heads=2, hd=64, causal=True),
+    "causal96": dict(entry="causal", fmt="f16", kernel="causal_attention_kernel<96, false, false>",
+                     lens=_lens(250, 505, 506, 1000, 2048), heads=2, hd=96, causal=True),
+    "causal128": dict(entry="causal128", fmt="f16", kernel="causal_attention_kernel<128, false, false>",
+                      lens=_lens(250, 505, 506, 1000, 2048), heads=2, hd=128, causal=True),
+    # ALiBi (BLOOM), head_dim 128: 4 heads and 40 (not a power of two)
+    "alibi4": dict(entry="alibi", fmt="f16", kernel="causal_attention_kernel<128, true, false>",
+                   lens=_lens(250, 505, 1000, 2048), heads=4, hd=128, causal=True, alibi=True),
+    "alibi40": dict(entry="alibi", fmt="f16", kernel="causal_attention_kernel<128, true, false>", lens=_lens(512),
+                    heads=40, hd=128, causal=True, alibi=True),
+    # multi-query (Falcon), head_dim 64, one K / V head
+    "mqa1": dict(entry="mqa", fmt="f16", kernel="causal_attention_kernel<64, false, true>",
+                 lens=_lens(505, 1000, 2048), heads=1, causal=True, mqa=True),
+    "mqa7": dict(entry="mqa", fmt="f16", kernel="causal_attention_kernel<64, false, true>", lens=_lens(505, 1000),
+                 heads=7, causal=True, mqa=True),
+    "mqa71": dict(entry="mqa", fmt="f16", kernel="causal_attention_kernel<64, false, true>", lens=_lens(),
+                  heads=71, causal=True, mqa=True),
+}
+
+
+def att_tc_case(name):
+    """ATT_TC_CASES[name] with every default filled in: hd, valid columns, score scale (fp32-exact), causal, alibi, mqa."""
+    c = dict(ATT_TC_CASES[name])
+    c.setdefault("hd", 64)
+    c.setdefault("valid", c["hd"])
+    c.setdefault("causal", False)
+    c.setdefault("alibi", False)
+    c.setdefault("mqa", False)
+    c.setdefault("env", None)
+    if "scale" not in c:
+        c["scale"] = 1.0 / math.sqrt(c["valid"])
+    c["scale"] = float(np.float32(c["scale"]))
+    return c
+
+
+def att_tc_operands(case, amp, seed=0):
+    """Host operands of a case at operand scale amp (randn * amp, rounded to fp16 or tf32): dict(qkv, v, cu, slopes,
+    ld).  qkv [tokens, ld]: Q | K | V blocks (mqa: Q, the one K head, then columns no kernel reads, up to (2 heads + 1)
+    * 64 so that a kernel reading head h's K columns reads finite values here); v the values the kernel's V^T holds
+    ([tokens, heads * hd], or [tokens, hd] for mqa).  ALBERT's padded heads: columns valid .. hd of each head are 0."""
+    g = torch.Generator().manual_seed(seed)
+    lens, H, hd = case["lens"], case["heads"], case["hd"]
+    tokens = sum(lens)
+    cu = [0]
+    for n in lens:
+        cu.append(cu[-1] + n)
+    ld = (2 * H + 1) * hd if case["mqa"] else 3 * H * hd
+    x = torch.randn(tokens, ld, generator=g) * amp
+    if case["valid"] < hd:
+        x.view(tokens, ld // hd, hd)[:, :, case["valid"]:] = 0.0
+    x = x.half().float() if case["fmt"] == "f16" else round_tf32_ties_away(x)
+    if case["mqa"]:
+        v = (torch.randn(tokens, hd, generator=g) * amp).half().float()
+    else:
+        v = x[:, 2 * H * hd:3 * H * hd].clone()
+    slopes = None
+    if case["alibi"]:
+        from mertools_b200.extract.ln_decoder_text import alibi_slopes
+        slopes = alibi_slopes(H)
+    return dict(qkv=x, v=v, cu=cu, slopes=slopes, ld=ld)
+
+
+def att_tc_reference(case, ops, device="cpu"):
+    """(ref, mag, amp, st) of attention_packed(stats=True) on a case's operands, in float64 on `device`."""
+    return attention_packed(ops["qkv"].to(device), ops["cu"], case["heads"], case["hd"], case["scale"],
+                            causal=case["causal"], slopes=None if ops["slopes"] is None else ops["slopes"].to(device),
+                            v=ops["v"].to(device), mqa=case["mqa"], stats=True)
+
+
+def attention_kernels(fn):
+    """Run fn under torch.profiler; the names of the attention kernels that ran while fn did.  The profiler's kernel
+    records are not reliably those of its own session: a session can come back without the records of what it ran,
+    and with records of kernels that ran before it started (launched while no session was open).  So each capture is
+    followed by a second, empty session that collects records delivered late, and of both only the kernels whose start
+    lies between fn's start and the synchronize after it (host clock, kineto's time base) count.  The others are
+    reported on stdout with their start relative to fn's.  A capture that found no attention kernel of fn at all is
+    repeated, up to 3 times."""
+    import time
+    from torch.profiler import DeviceType, ProfilerActivity, profile
+    for _ in range(3):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as run:
+            t0 = time.time_ns()
+            out = fn()
+            torch.cuda.synchronize()
+            t1 = time.time_ns()
+        with profile(activities=[ProfilerActivity.CUDA]) as late:
+            torch.cuda.synchronize()
+        kernels = [(e.name(), e.start_ns()) for p in (run, late) for e in p.profiler.kineto_results.events()
+                   if e.device_type() == DeviceType.CUDA and "attention" in e.name()]
+        names = {n for n, t in kernels if t0 <= t <= t1}
+        other = sorted({(n.split("::")[-1].split("(")[0], round((t - t0) / 1e6, 3)) for n, t in kernels if not t0 <= t <= t1})
+        if other:
+            print(f"attention_kernels: record(s) from outside the call (name, start - call start in ms): {other}")
+        if names:
+            break
+    return out, names
 
 
 # ---- transformer stack: one layer of mer_run_stack (encoder.cu) ---------------------------------------------------------

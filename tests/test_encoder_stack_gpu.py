@@ -51,20 +51,6 @@ pytestmark = pytest.mark.gpu
 U = R.U32
 
 
-def _attention_kernels(fn):
-    """Run fn under torch.profiler; the names of the attention kernels it launched.  A capture that recorded no
-    attention kernel at all (the profiler drops a session's kernel records now and then) is repeated, up to 3 times."""
-    from torch.profiler import ProfilerActivity, profile
-    for _ in range(3):
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            out = fn()
-            torch.cuda.synchronize()
-        names = {e.key for e in prof.key_averages() if "attention" in e.key}
-        if names:
-            break
-    return out, names
-
-
 def _assert_route(names, route):
     want = R.ATT_KERNEL[route]
     assert any(want in n for n in names), (route, names)
@@ -144,7 +130,7 @@ def test_vit_stack_layers_and_readout(cuda, precision, route):
     frames = torch.from_numpy(np.random.default_rng(5).integers(0, 256, (2, 224, 224, 3), dtype=np.uint8)).to(cuda)
     enc = VitEncoder(sd, device=cuda, precision=precision)
     feats, hidden = enc.frame_features(frames, return_hidden=True)
-    feats2, names = _attention_kernels(lambda: enc.frame_features(frames).clone())
+    feats2, names = R.attention_kernels(lambda: enc.frame_features(frames).clone())
     assert torch.equal(R.bits(feats), R.bits(feats2))
     form = R.stack_form(precision, True, 197)
     assert form["route"] == route
@@ -179,7 +165,7 @@ def test_clip_dinov2_stack_layers_and_readout(cuda, variant, route):
     for hw, (y0, x0) in (((260, 300), (17, 38)), ((224, 224), (0, 0))):
         frames = torch.from_numpy(rng.integers(0, 256, (2, hw[0], hw[1], 3), dtype=np.uint8)).to(cuda)
         emb, hidden = _clip_forward(enc, frames, y0, x0, True)
-        emb2, names = _attention_kernels(lambda: _clip_forward(enc, frames, y0, x0, False)[0])
+        emb2, names = R.attention_kernels(lambda: _clip_forward(enc, frames, y0, x0, False)[0])
         assert torch.equal(R.bits(emb), R.bits(emb2))
         mode = enc.precision
         T = enc.tokens
@@ -261,7 +247,7 @@ def test_hubert_base_stack_layers_and_readouts(cuda, precision):
         wave = _wave(T, B, cuda, 7 + T)
         assert enc.num_frames(wave.shape[1]) == T
         utt, frames, hidden = enc.forward(wave, want_frames=True, return_hidden=True)
-        (utt2, frames2), names = _attention_kernels(lambda: tuple(t.clone() for t in enc.forward(wave, want_frames=True)))
+        (utt2, frames2), names = R.attention_kernels(lambda: tuple(t.clone() for t in enc.forward(wave, want_frames=True)))
         assert torch.equal(R.bits(frames), R.bits(frames2)) and torch.equal(R.bits(utt), R.bits(utt2))
         form = R.stack_form(precision, False, T, long_rows=True, eps=1e-5)
         assert form["route"] == route
@@ -299,7 +285,7 @@ def test_hubert_large_stable_stack_layers_and_readouts(cuda, precision, lengths)
         B = 2
         wave = _wave(T, B, cuda, 11 + T)
         utt, frames, hidden = enc.forward(wave, want_frames=True, return_hidden=True)
-        (utt2, frames2), names = _attention_kernels(lambda: tuple(t.clone() for t in enc.forward(wave, want_frames=True)))
+        (utt2, frames2), names = R.attention_kernels(lambda: tuple(t.clone() for t in enc.forward(wave, want_frames=True)))
         assert torch.equal(R.bits(frames), R.bits(frames2)) and torch.equal(R.bits(utt), R.bits(utt2))
         form = R.stack_form(mode, True, T, long_rows=True, eps=1e-5, heads=16)
         assert form["route"] == route
@@ -338,7 +324,7 @@ def test_bert_stack_layers_and_readout(cuda, model):
         ids = [np.concatenate([[0], rng.integers(1, vocab - 1, n - 2), [vocab - 1]]) if n > 1 else np.array([vocab - 1])
                for n in lens]
         utt, toks, hidden, cu = enc.forward(ids, want_tokens=True, return_hidden=True)
-        (utt2, toks2), names = _attention_kernels(lambda: tuple(t.clone() for t in enc.forward(ids, want_tokens=True)))
+        (utt2, toks2), names = R.attention_kernels(lambda: tuple(t.clone() for t in enc.forward(ids, want_tokens=True)))
         assert torch.equal(R.bits(toks), R.bits(toks2)) and torch.equal(R.bits(utt), R.bits(utt2))
         form = R.stack_form(mode, False, max(lens), eps=eps, heads=D // 64)
         _assert_route(names, form["route"])

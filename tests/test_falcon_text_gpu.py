@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+import _kernel_refs as R
 from mertools_b200 import _lib as L
 from mertools_b200 import synthetic as S
 from mertools_b200.extract import ln_decoder_text as LD
@@ -63,19 +64,6 @@ def _mqa_operands(lens, heads, cuda, seed=23, extra=40, pad_value=0.0):
     return qkv, ld, v, vt, cu
 
 
-def _mqa_reference(qkv, v, cu, heads):
-    D = heads * HD
-    out = torch.zeros(qkv.shape[0], D, dtype=torch.float64, device=qkv.device)
-    for a, b in zip(cu.tolist()[:-1], cu.tolist()[1:]):
-        n = b - a
-        q = qkv[a:b, :D].double().view(n, heads, HD).transpose(0, 1)
-        k = qkv[a:b, D:D + HD].double()
-        s = (q @ k.T) / HD ** 0.5
-        s = s.masked_fill(torch.ones(n, n, dtype=torch.bool, device=qkv.device).triu(1), float("-inf"))
-        out[a:b] = (torch.softmax(s, -1) @ v[a:b].double()).transpose(0, 1).reshape(n, D)
-    return out
-
-
 @pytest.mark.parametrize("heads", [1, 7, 71])
 def test_mqa_attention_vs_float64(cuda, heads):
     """Packed ragged lengths 1 .. 2048 (unaligned sequence starts), a row pitch wider than (heads + 1) * 64."""
@@ -84,9 +72,9 @@ def test_mqa_attention_vs_float64(cuda, heads):
     ctx = torch.full((qkv.shape[0], heads * HD), float("nan"), dtype=torch.float16, device=cuda)
     _mqa(qkv, ld, vt, ctx, cu, max(lens), heads)
     assert bool(torch.isfinite(ctx).all())
-    err = _rel(ctx, _mqa_reference(qkv, v, cu, heads))
-    print(f"multi-query causal attention, {heads} heads: max-rel {err:.2e}")
-    assert err < 2e-3, err  # fp16 P and the fp16 output rounding
+    err = R.tc_bound_ratio(ctx, qkv, cu.tolist(), heads, "f16", causal=True, v=v, mqa=True)
+    print(f"multi-query causal attention, {heads} heads: max |err| / bound {err:.2f}")
+    assert err <= 1.0, err  # attention_tc_bound: fp16 P, fp32 sums, the fp16 output rounding
 
 
 @pytest.mark.parametrize("heads", [1, 7, 71])
@@ -120,7 +108,7 @@ def test_mqa_attention_future_and_foreign_nan_do_not_leak(cuda):
     qkv[:, D + HD:] = float("nan")
     ref = _mqa(qkv, ld, vt, torch.empty(T, D, dtype=torch.float16, device=cuda), cu, 300, heads)
     assert bool(torch.isfinite(ref).all())
-    assert _rel(ref, _mqa_reference(qkv, v, cu, heads)) < 2e-3
+    assert R.tc_bound_ratio(ref, qkv, cu.tolist(), heads, "f16", causal=True, v=v, mqa=True) <= 1.0
     a, b = 37 + i + 1, 37 + 300
     qkv2, vt2 = qkv.clone(), vt.clone()
     qkv2[a:b, D:D + HD] = float("nan")

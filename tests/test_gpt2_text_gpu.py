@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 import torch
 
+import _kernel_refs as R
 from mertools_b200 import _lib as L
 from mertools_b200 import synthetic as S
 from mertools_b200.extract import ln_decoder_text as LD
@@ -50,20 +51,6 @@ def _att_operands(lens, heads, hd, cuda, seed=23, pad=0, pad_value=0.0):
     return qkv, vt, cu
 
 
-def _reference(qkv, cu, heads, hd):
-    """float64 causal softmax(Q K^T / sqrt(hd)) V on the device."""
-    D = heads * hd
-    x = qkv.double()
-    out = torch.zeros(qkv.shape[0], D, dtype=torch.float64, device=qkv.device)
-    for a, b in zip(cu.tolist()[:-1], cu.tolist()[1:]):
-        n = b - a
-        q, k, v = (x[a:b, i * D:(i + 1) * D].view(n, heads, hd).transpose(0, 1) for i in range(3))
-        s = (q @ k.transpose(1, 2)) / hd ** 0.5
-        s = s.masked_fill(torch.ones(n, n, dtype=torch.bool, device=qkv.device).triu(1), float("-inf"))
-        out[a:b] = (torch.softmax(s, -1) @ v).transpose(0, 1).reshape(n, D)
-    return out
-
-
 def _rel(a, b):
     a, b = torch.as_tensor(a).double().cpu(), torch.as_tensor(b).double().cpu()
     return float((a - b).abs().max() / b.abs().max())
@@ -82,9 +69,9 @@ def test_causal_attention_vs_float64(cuda, hd, heads):
     ctx = torch.full((qkv.shape[0], heads * hd), float("nan"), dtype=torch.float16, device=cuda)
     _att_hd(qkv, vt, ctx, cu, max(lens), heads, hd)
     assert bool(torch.isfinite(ctx).all())
-    err = _rel(ctx, _reference(qkv, cu, heads, hd))
-    print(f"causal attention head_dim {hd}, {heads} heads: max-rel {err:.2e}")
-    assert err < 2e-3, err  # fp16 P and the fp16 output rounding
+    err = R.tc_bound_ratio(ctx, qkv, cu.tolist(), heads, "f16", hd=hd, scale=hd ** -0.5, causal=True)
+    print(f"causal attention head_dim {hd}, {heads} heads: max |err| / bound {err:.2f}")
+    assert err <= 1.0, err  # attention_tc_bound: fp16 P, fp32 sums, the fp16 output rounding
 
 
 @pytest.mark.parametrize("hd", [64, 96])
@@ -108,10 +95,11 @@ def test_causal_attention_nan_padding_does_not_leak(cuda, hd):
     """NaN in the V^T columns past `tokens` and in the (unread) V columns of qkv."""
     lens, heads = [5, 197, 65, 17, 131], 4
     qkv, vt, cu = _att_operands(lens, heads, hd, cuda, pad=64, pad_value=float("nan"))
-    ref = _reference(qkv, cu, heads, hd)
+    clean = qkv.clone()
     qkv[:, 2 * heads * hd:] = float("nan")
     ctx = _att_hd(qkv, vt, torch.empty(sum(lens), heads * hd, dtype=torch.float16, device=cuda), cu, 197, heads, hd)
-    assert bool(torch.isfinite(ctx).all()) and _rel(ctx, ref) < 2e-3
+    assert bool(torch.isfinite(ctx).all())
+    assert R.tc_bound_ratio(ctx, clean, cu.tolist(), heads, "f16", hd=hd, scale=hd ** -0.5, causal=True) <= 1.0
 
 
 def test_head_dim_128_is_the_llama_kernel(cuda):

@@ -522,3 +522,151 @@ def test_cnn_plan_mirrors_the_executor_on_the_extractor_tables():
                      En.manet_tables(S.manet_state_dict(3), pack), En.emonet_tables(S.emonet_state_dict(3), pack)):
         for n in (1, 3):
             assert R.cnn_plan(m, n)[0]["total"] == dll.mer_cnn_workspace_bytes(C.byref(m), n)
+
+
+# ---- tensor-core attention: reference, bound and faults (tests/test_attention_tc_gpu.py) -------------------------------
+def _sdpa_packed(qkv, cu, heads, hd, scale, causal=False, slopes=None, mqa=False, v=None, offset=0):
+    """torch's float64 scaled_dot_product_attention per sequence: is_causal, ALiBi as an additive attn_mask
+    (slope * (j + offset)), multi-query with K / V expanded to every head."""
+    D = heads * hd
+    x = qkv.double()
+    out = torch.zeros(x.shape[0], D, dtype=torch.float64)
+    for a, b in zip(cu, cu[1:]):
+        n = b - a
+        if n <= 0:
+            continue
+        q = x[a:b, :D].reshape(n, heads, hd).transpose(0, 1)
+        if mqa:
+            k = x[a:b, D:D + hd].reshape(1, n, hd).expand(heads, n, hd)
+            vv = v[a:b].double().reshape(1, n, hd).expand(heads, n, hd)
+        else:
+            k = x[a:b, D:2 * D].reshape(n, heads, hd).transpose(0, 1)
+            vv = (x[a:b, 2 * D:3 * D] if v is None else v[a:b].double()).reshape(n, heads, hd).transpose(0, 1)
+        if slopes is None:
+            o = F.scaled_dot_product_attention(q, k, vv, is_causal=causal, scale=scale)
+        else:
+            j = torch.arange(n, dtype=torch.float64)
+            mask = slopes.double()[:, None, None] * (j + offset)[None, None, :]
+            if causal:
+                mask = mask.masked_fill(j[None, :] > j[:, None], float("-inf"))
+            o = F.scaled_dot_product_attention(q, k, vv, attn_mask=mask, scale=scale)
+        out[a:b] = o.transpose(0, 1).reshape(n, D)
+    return out
+
+
+def test_attention_packed_default_form_is_unchanged():
+    """The generalised reference gives the callers of its first form (head_dim 64, / 8, Q | K | V) the same bits."""
+    heads = 3
+    cu = [0, 5, 5, 22, 87]
+    qkv = (torch.randn(87, 3 * heads * 64, generator=_g(9)) * 1.5).half().float()
+    got, mag, amp = R.attention_packed(qkv, cu, heads)
+    x = qkv.double()
+    D = heads * 64
+    for a, b in zip(cu, cu[1:]):
+        if b <= a:
+            continue
+        q, k, v = (x[a:b, i * D:(i + 1) * D].view(b - a, heads, 64).transpose(0, 1) for i in range(3))
+        p = torch.softmax(q @ k.transpose(1, 2) / 8.0, dim=-1)
+        assert torch.equal(got[a:b], (p @ v).transpose(0, 1).reshape(b - a, D))
+        assert torch.equal(mag[a:b], (p @ v.abs()).transpose(0, 1).reshape(b - a, D))
+        top = (q.abs() @ k.abs().transpose(1, 2) / 8.0).amax(-1)
+        assert torch.equal(amp[a:b], top.T[:, :, None].expand(-1, -1, 64).reshape(b - a, D))
+
+
+@pytest.mark.parametrize("hd", [32, 64, 96, 128])
+def test_attention_packed_is_sdpa_in_every_form(hd):
+    heads = 3
+    cu = [0, 7, 7, 30, 31, 95]
+    T = cu[-1]
+    scale = 1.0 / math.sqrt(hd - 6)
+    qkv = (torch.randn(T, 3 * heads * hd, generator=_g(hd)) * 2).half().float()
+    slopes = torch.tensor([0.5, 0.125, 0.03125])
+    for causal in (False, True):
+        got = R.attention_packed(qkv, cu, heads, hd, scale, causal=causal)[0]
+        assert float((got - _sdpa_packed(qkv, cu, heads, hd, scale, causal)).abs().max()) < 1e-12, causal
+        got = R.attention_packed(qkv, cu, heads, hd, scale, causal=causal, slopes=slopes)[0]
+        want = _sdpa_packed(qkv, cu, heads, hd, scale, causal, slopes)
+        assert float((got - want).abs().max()) < 1e-12, causal
+        # ALiBi on packed positions (slope * (start + j)) adds a constant per row: the softmax cancels it
+        packed = torch.zeros_like(want)
+        for a, b in zip(cu, cu[1:]):
+            packed[a:b] = _sdpa_packed(qkv[a:b], [0, b - a], heads, hd, scale, causal, slopes, offset=a)
+        assert float((packed - want).abs().max()) < 1e-12
+    v = (torch.randn(T, hd, generator=_g(1)) * 2).half().float()
+    for causal in (False, True):
+        got = R.attention_packed(qkv, cu, heads, hd, scale, causal=causal, v=v, mqa=True)[0]
+        want = _sdpa_packed(qkv, cu, heads, hd, scale, causal, mqa=True, v=v)
+        assert float((got - want).abs().max()) < 1e-12, causal
+    # the stats: tiny keys and key counts against a direct evaluation of one row
+    ref, mag, amp, st = R.attention_packed(qkv * 4, cu, heads, hd, scale, causal=True, stats=True)
+    a, b = cu[4], cu[5]
+    assert torch.equal(st["keys"][a:b, 0], torch.arange(1, b - a + 1, dtype=torch.float64))
+    x = (qkv * 4).double()
+    q, k, vv = (x[a:b, i * heads * hd + hd:i * heads * hd + 2 * hd] for i in range(3))       # head 1
+    s = (q @ k.T * scale).masked_fill(torch.ones(b - a, b - a, dtype=torch.bool).triu(1), float("-inf"))
+    pt = torch.exp(s - s.amax(-1, keepdim=True))
+    want = ((pt < 2.0 ** -13) & (pt > 0)).double() @ vv.abs() / pt.sum(-1, keepdim=True)
+    assert float(want.max()) > 0 and float((st["tiny"][a:b, hd:2 * hd] - want).abs().max()) < 1e-15
+
+
+_TC_CACHE = {}
+
+
+def _tc_case(name, amp):
+    """(case, operands, reference, bound-ingredients) of an operand set of tests/test_attention_tc_gpu.py, cached."""
+    if (name, amp) not in _TC_CACHE:
+        c = R.att_tc_case(name)
+        ops = R.att_tc_operands(c, amp)
+        _TC_CACHE[(name, amp)] = (c, ops) + tuple(R.att_tc_reference(c, ops))
+    return _TC_CACHE[(name, amp)]
+
+
+def _tc_ratio(name, amp, fault=None, fmts=None):
+    c, ops, ref, mag, amp_, st = _tc_case(name, amp)
+    x = R.attention_tc_emulated(ops["qkv"], ops["cu"], c["heads"], c["hd"], c["scale"], c["causal"], ops["slopes"],
+                                ops["v"], c["mqa"], p_fmt=c["fmt"], fault=fault)
+    worst = 0.0
+    for fmt in fmts or (("f16",) if c["causal"] else ("fp32", "f16", "tf32", "split")):
+        got = R.ctx_format(x, fmt).double()
+        worst = max(worst, float(R.bound_ratio(got, ref, R.attention_tc_bound(mag, amp_, st, ref, fmt)).max()))
+    return worst
+
+
+@pytest.mark.parametrize("amp", [1.5, 4.0])
+def test_attention_emulation_fits_under_the_bound(amp):
+    """The kernels' arithmetic (fp16 / tf32 P, fp32 sums, every ctx format), emulated in fp32, stays at or below 0.85
+    of attention_tc_bound on every operand set of the GPU test.  The bound is a worst case that short rows nearly
+    attain: with a few dominant keys the fp16 rounding of P (2^-11 each, the bound's 2^-11 P |V|) can fall the same
+    way on every key, and such rows reach 0.7 .. 0.8 of the bound; rows of hundreds of keys stay near 0.5."""
+    worst = {name: _tc_ratio(name, amp) for name in R.ATT_TC_CASES}
+    print("emulation / bound: " + ", ".join(f"{k} {v:.2f}" for k, v in worst.items()))
+    assert all(v <= 0.85 for v in worst.values()), worst
+
+
+# the operand sets each fault is restated on (where the fault can act at all)
+_FAULT_CASES = {
+    "bf16_p": ("short", "tile_f16_505", "tile_tf32", "hd32_26_f16", "causal64", "causal128", "mqa7"),
+    "acc16": ("short", "tile_f16_505", "hd64_f16", "causal64", "causal128", "mqa7"),
+    "vt_shift": ("short", "tile_f16_505", "tile_tf32", "causal64"),
+    "causal_diag": ("causal64", "causal96", "alibi4", "mqa7"),
+    "alibi_tile": ("alibi4", "alibi40"),
+    "mqa_head_k": ("mqa7", "mqa71"),
+    "hd96_scale": ("causal96",),
+    "foreign_keys": ("short", "tile_f16", "tile_tf32", "hd32_26_f16", "causal64", "mqa7"),
+}
+
+
+def test_attention_bound_rejects_the_faults():
+    """Each restated kernel fault of ATT_TC_FAULTS leaves attention_tc_bound by more than 1.5x on some element of an
+    operand set the GPU test runs (at operand scale 1.5 or 4); the worst ratio per fault is printed.  A fault whose
+    restatement makes a row NaN (a causal row left with no key) counts as infinitely far out."""
+    assert set(_FAULT_CASES) == set(R.ATT_TC_FAULTS)
+    worst = {}
+    for fault, names in _FAULT_CASES.items():
+        for name in names:
+            for amp in (1.5, 4.0):
+                r = _tc_ratio(name, amp, fault=fault)
+                if r > worst.get(fault, ("", 0.0))[1]:
+                    worst[fault] = (f"{name} x{amp}", r)
+    print("fault / bound: " + ", ".join(f"{k} {v[1]:.2f} ({v[0]})" for k, v in worst.items()))
+    assert all(worst[f][1] > 1.5 for f in R.ATT_TC_FAULTS), worst

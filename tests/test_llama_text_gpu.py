@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import _kernel_refs as R
 from mertools_b200 import _lib as L
 from mertools_b200 import synthetic as S
 from mertools_b200.extract import llama_text as LT
@@ -48,21 +49,6 @@ def _att_operands(lens, heads, cuda, seed=23, pad=0, pad_value=0.0):
     return qkv, vt, cu
 
 
-def _att_reference(qkv, cu, heads):
-    """float64 causal softmax(Q K^T / sqrt(128)) V on the device."""
-    D = heads * HD
-    x = qkv.double()
-    out = torch.zeros(qkv.shape[0], D, dtype=torch.float64, device=qkv.device)
-    cu = cu.tolist()
-    for a, b in zip(cu[:-1], cu[1:]):
-        n = b - a
-        q, k, v = (x[a:b, i * D:(i + 1) * D].view(n, heads, HD).transpose(0, 1) for i in range(3))
-        s = (q @ k.transpose(1, 2)) / HD ** 0.5
-        s = s.masked_fill(torch.ones(n, n, dtype=torch.bool, device=qkv.device).triu(1), float("-inf"))
-        out[a:b] = (torch.softmax(s, -1) @ v).transpose(0, 1).reshape(n, D)
-    return out
-
-
 def _rel(a, b):
     a, b = torch.as_tensor(a).double().cpu(), torch.as_tensor(b).double().cpu()
     return float((a - b).abs().max() / b.abs().max())
@@ -75,9 +61,9 @@ def test_causal_attention_vs_float64(cuda, heads):
     ctx = torch.full((qkv.shape[0], heads * HD), float("nan"), dtype=torch.float16, device=cuda)
     _att(qkv, vt, ctx, cu, max(lens), heads)
     assert bool(torch.isfinite(ctx).all())
-    err = _rel(ctx, _att_reference(qkv, cu, heads))
-    print(f"causal attention, {heads} heads: max-rel {err:.2e}")
-    assert err < 2e-3, err  # fp16 P and the fp16 output rounding
+    err = R.tc_bound_ratio(ctx, qkv, cu.tolist(), heads, "f16", hd=HD, scale=HD ** -0.5, causal=True)
+    print(f"causal attention, {heads} heads: max |err| / bound {err:.2f}")
+    assert err <= 1.0, err  # attention_tc_bound: fp16 P, fp32 sums, the fp16 output rounding
 
 
 def test_causal_attention_ignores_future_keys(cuda):
@@ -99,10 +85,11 @@ def test_causal_attention_nan_padding_does_not_leak(cuda):
     """NaN in the V^T columns past `tokens` and in the (unread) V columns of qkv."""
     lens, heads = [5, 197, 65, 17, 131], 4
     qkv, vt, cu = _att_operands(lens, heads, cuda, pad=64, pad_value=float("nan"))
-    ref = _att_reference(qkv, cu, heads)
+    clean = qkv.clone()
     qkv[:, 2 * heads * HD:] = float("nan")
     ctx = _att(qkv, vt, torch.empty(sum(lens), heads * HD, dtype=torch.float16, device=cuda), cu, 197, heads)
-    assert bool(torch.isfinite(ctx).all()) and _rel(ctx, ref) < 2e-3
+    assert bool(torch.isfinite(ctx).all())
+    assert R.tc_bound_ratio(ctx, clean, cu.tolist(), heads, "f16", hd=HD, scale=HD ** -0.5, causal=True) <= 1.0
 
 
 @pytest.mark.parametrize("dim", [512, 4096, 5120])
