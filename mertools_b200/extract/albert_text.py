@@ -35,6 +35,7 @@ import numpy as np
 import torch
 
 from .deberta_text import activation_bytes_per_token
+from .packed_text import DeviceOps, PackedTextEncoder
 from .text import TextExtractor
 
 KERNEL_HEAD_DIM = {26: 32, 32: 32, 64: 64}   # ALBERT head_dim -> the attention kernel's head_dim (26: zero-padded)
@@ -262,56 +263,23 @@ class TorchOps:
         return torch.nn.functional.gelu(y @ w.T + b, approximate="tanh" if act == "gelu_new" else "none")
 
 
-class CudaOps:
+class CudaOps(DeviceOps):
     """Product backend.  precision "f16": fp16 weights, GEMM operands and q | k | V^T (MER_GEMM_F16, MER_ATT_QKV_F16);
     "bf16x3": split-bf16 weights and operands (MER_GEMM_BF16X3), tf32-rounded q | k | V^T, ctx written as split rows.
     fp32 biases, residual stream and readout.  LayerNorm: ``mer_layernorm`` at its widths (MER_LN_PAD for a padded
     row), ``mer_layernorm_f16`` at multiples of 256 beyond them (xxlarge's 4096; on bf16x3 followed by mer_split_bf16).
-    ``timing``: None, or a list that collects (kernel class, start, end) CUDA events per launch."""
+    ``timing``: see DeviceOps."""
 
     def __init__(self, precision, device="cuda"):
         import ctypes as C
-
-        from .. import _lib as L
-        L.check(L.lib().mer_check_device())
-        assert precision in ("f16", "bf16x3"), precision
-        self.L, self.f16, self.device, self.timing = L, precision == "f16", torch.device(device), None
-        self.mode = L.MER_GEMM_F16 if self.f16 else L.MER_GEMM_BF16X3
-        self.op_dtype = torch.float16 if self.f16 else torch.float32
+        super().__init__(precision, device)
+        L = self.L
         vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_longlong, C.c_float
         self._att = L.declare("mer_attention_hd", [vp, vp, i64, vp, vp, i32, i64, i32, i32, i32, f32, i32, vp])
         self._ln16 = L.declare("mer_layernorm_f16", [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp])
 
-    def _run(self, klass, fn):
-        if self.timing is None:
-            return fn()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = fn()
-        b.record()
-        self.timing.append((klass, a, b))
-        return r
-
-    def weight(self, t):
-        """fp32 rows -> GEMM operand: fp16, or split bf16 rows."""
-        t = torch.as_tensor(t).to(self.device, torch.float32).contiguous()
-        return t.half() if self.f16 else self.L.split_bf16(t)
-
-    def vector(self, t):
-        return torch.as_tensor(t).to(self.device, torch.float32).contiguous()
-
-    embedding = vector
-
     def embed(self, word, ids, pos_type, pos):
         return word[torch.as_tensor(ids, device=self.device)] + pos_type[torch.as_tensor(pos, device=self.device)]
-
-    def zeros_like(self, x):
-        return torch.zeros_like(x)
-
-    def batch(self, lens):
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
-        return dict(cu=torch.from_numpy(cu.astype(np.int32)).to(self.device), n=len(lens), max_len=int(max(lens)))
 
     def layernorm(self, x, g, b, eps, valid, acc=None, want_y=True):
         """(y fp32 or None, y as the next GEMM operand); acc += y when given.  valid: the unpadded width."""
@@ -360,39 +328,19 @@ class CudaOps:
             d.scale, flags, L.stream_ptr())))
         return ctx
 
-    def linear_res(self, a, w, bias, x):
-        self._run("gemm", lambda: self.L.gemm(a, w, x, bias=bias, res=x, mode=self.mode))
-        return x
-
-    def ffn_up(self, y, w, bias, act):
-        h = torch.empty(y.shape[0], w.shape[0], dtype=self.op_dtype, device=self.device)
-        if act == "gelu":
-            self._run("gemm", lambda: self.L.gemm(y, w, h, bias=bias, mode=self.mode, gelu=True, f16_out=self.f16,
-                                                  split_out=not self.f16))
-        elif self.f16:
-            self._run("gemm", lambda: self.L.gemm(y, w, h, bias=bias, mode=self.mode, gelu_tanh=True, f16_out=True))
-        else:   # mer_gemm's tanh-GELU epilogue writes fp32 or fp16 only: fp32, then split for the FC2 operand
-            f = torch.empty(y.shape[0], w.shape[0], dtype=torch.float32, device=self.device)
-            self._run("gemm", lambda: self.L.gemm(y, w, f, bias=bias, mode=self.mode, gelu_tanh=True))
-            self._run("split", lambda: self.L.check(self.L.lib().mer_split_bf16(
-                self.L.ptr(f), self.L.ptr(h), f.shape[0], f.shape[1], self.L.stream_ptr())))
-        return h
-
 
 def default_precision(hidden):
     """BertEncoder's rule, MER_TEXT_PRECISION overriding it: "f16" up to hidden 768, "bf16x3" above."""
     return os.environ.get("MER_TEXT_PRECISION", "f16" if hidden <= 768 else "bf16x3")
 
 
-class AlbertTextEncoder:
-    """``forward(id_lists, start, end, want_tokens)`` (the contract TextExtractor drives) over ``AlbertNet`` with the
-    CUDA backend.  ``sd``: {name: tensor}; ``cfg``: the checkpoint's AlbertConfig.  ``precision``: None =
-    default_precision(hidden)."""
+class AlbertTextEncoder(PackedTextEncoder):
+    """PackedTextEncoder over ``AlbertNet`` with the CUDA backend.  ``sd``: {name: tensor}; ``cfg``: the checkpoint's
+    AlbertConfig.  ``precision``: None = default_precision(hidden)."""
+
+    span = (0, -2)
 
     def __init__(self, sd, cfg, device="cuda", precision=None):
-        import ctypes as C
-
-        from .. import _lib as L
         check_albert_config(cfg)
         self.dims = d = AlbertDims(cfg)
         self.precision = precision or default_precision(d.hidden)
@@ -402,31 +350,6 @@ class AlbertTextEncoder:
         self.hidden, self.vocab_size = d.hidden, self.net.word.shape[0]
         self.max_pos = self.net.pos_type.shape[0]
         self.bytes_per_token = activation_bytes_per_token(d.hidden_pad, d.ffn_pad)
-        self._L = L
-        self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                                     C.c_void_p, C.c_void_p])
-
-    def forward(self, id_lists, start=0, end=-2, want_tokens=False):
-        """id_lists: non-empty token id sequences of at most max_position_embeddings tokens.  Returns (utt [n, hidden] =
-        mean over each sentence's kept range [start : len + end], tokens [sum len, hidden] | None), fp32."""
-        L, d = self._L, self.dims
-        lens = [len(x) for x in id_lists]
-        assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
-        assert max(lens) <= self.max_pos, f"a sentence of {max(lens)} tokens (max_position_embeddings {self.max_pos})"
-        ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
-        assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
-        acc = self.net.forward(ids, lens)
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
-        seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)
-        seg = torch.from_numpy(np.maximum(seg, seg[:1])).to(self.device)   # empty kept range -> zeros (caller skips it)
-        utt = torch.empty(len(lens), d.hidden_pad, dtype=torch.float32, device=self.device)
-        L.check(self._seg(L.ptr(acc), L.ptr(seg[0]), L.ptr(seg[1]), len(lens), d.hidden_pad, 1, L.ptr(utt),
-                          L.stream_ptr()))
-        if d.hidden_pad != d.hidden:   # the pad columns are zero: slice them off
-            utt = utt[:, :d.hidden].contiguous()
-            acc = acc[:, :d.hidden].contiguous() if want_tokens else acc
-        return utt, (acc if want_tokens else None)
 
 
 def albert_tokenizer(model_name, model_dir):

@@ -1,6 +1,7 @@
 """Shared host-side pieces of the extractors: checkpoint loading and the .npy feature contract."""
 from __future__ import annotations
 
+import json
 import os
 
 import numpy as np
@@ -41,7 +42,6 @@ def load_hf_state_dict(model_dir):
     """HF checkpoint directory -> {name: numpy fp32} without instantiating the HF model (only the tensors are
     needed here).  Single-file checkpoints (``model.safetensors`` / ``pytorch_model.bin``) and sharded ones
     (``model.safetensors.index.json`` / ``pytorch_model.bin.index.json`` with their ``weight_map``)."""
-    import json
     for single in ("model.safetensors", "pytorch_model.bin"):
         path = os.path.join(model_dir, single)
         if os.path.exists(path):
@@ -57,11 +57,54 @@ def load_hf_state_dict(model_dir):
     raise AssertionError(f"no model.safetensors / pytorch_model.bin (or their .index.json) under {model_dir}")
 
 
+def _checkpoint_files(model_dir, prefer_bin=False):
+    kinds = [("pytorch_model.bin", "pytorch_model.bin.index.json"), ("model.safetensors", "model.safetensors.index.json")]
+    if not prefer_bin:
+        kinds.reverse()
+    for single, index in kinds:
+        if os.path.exists(os.path.join(model_dir, single)):
+            return [os.path.join(model_dir, single)]
+        if os.path.exists(os.path.join(model_dir, index)):
+            shards = sorted(set(json.load(open(os.path.join(model_dir, index)))["weight_map"].values()))
+            return [os.path.join(model_dir, s) for s in shards]
+    raise FileNotFoundError(f"no model.safetensors / pytorch_model.bin (or their .index.json) under {model_dir}")
+
+
+def _iter_tensors(path):
+    if path.endswith(".safetensors"):
+        from safetensors import safe_open
+        with safe_open(path, framework="pt", device="cpu") as f:
+            for k in f.keys():
+                yield k, f.get_tensor(k)
+    else:
+        import torch
+        sd = torch.load(path, map_location="cpu", mmap=True, weights_only=True)
+        for k in list(sd):
+            yield k, sd.pop(k)
+
+
+def stream_fp16_weights(model_dir, device, rename, prefer_bin=False):
+    """Yield (name, fp16 tensor on ``device``) for every tensor of a checkpoint, read one at a time (safetensors through
+    ``safe_open``, ``.bin`` through an mmap'ed ``torch.load``) from fp32 / fp16 / bf16 shards, so that a large
+    checkpoint never exists as fp32 in host memory.  Safetensors are read when both formats exist, ``.bin`` with
+    ``prefer_bin``.  ``rename(key)``: the name to yield, or None to skip the tensor.  A value that is not finite
+    in fp16 is refused."""
+    import torch
+    for path in _checkpoint_files(model_dir, prefer_bin):
+        for k, v in _iter_tensors(path):
+            k = rename(k)
+            if k is None:
+                continue
+            t = v.to(device).to(torch.float16)
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError(f"{path}: {k} is not finite in fp16")
+            yield k, t
+
+
 def read_do_normalize(model_dir, default=True):
     """``do_normalize`` of the checkpoint's ``preprocessor_config.json``: the reference builds
     ``Wav2Vec2FeatureExtractor.from_pretrained(model_file)`` (extract_audio_huggingface.py:60-64), which applies the
     zero-mean / unit-variance step only when the checkpoint says so (hubert-base-ls960 and wavlm-base ship false)."""
-    import json
     path = os.path.join(model_dir, "preprocessor_config.json")
     if not os.path.exists(path):
         return default

@@ -31,6 +31,7 @@ import numpy as np
 import torch
 
 from .ln_decoder_text import deinterleave_qkv
+from .packed_text import DeviceOps, PackedTextEncoder
 
 HEAD_DIM = 64
 LN_DIMS = (512, 768, 1024, 1280, 1536)  # mer_layernorm's row widths
@@ -286,68 +287,28 @@ class TorchOps:
         return torch.nn.functional.gelu(torch.cat(out))
 
 
-class CudaOps:
+class CudaOps(DeviceOps):
     """Product backend.  precision "f16": fp16 weights, GEMM operands, q | k | V^T and PK | PQ (MER_GEMM_F16,
     MER_ATT_QKV_F16); "bf16x3": split-bf16 weights and operands (MER_GEMM_BF16X3), tf32-rounded q | k | V^T and PK | PQ,
     ctx written as split rows.  fp32 biases, residual stream and readout; ``mer_layernorm`` writes the fp32 row, the
-    next operand and the readout term in one pass.  ``timing``: None, or a list that collects (kernel class, start,
-    end) CUDA events per launch."""
+    next operand and the readout term in one pass.  ``timing``: see DeviceOps."""
 
     def __init__(self, precision, device="cuda"):
         import ctypes as C
-
-        from .. import _lib as L
-        L.check(L.lib().mer_check_device())
-        assert precision in ("f16", "bf16x3"), precision
-        self.L, self.f16, self.device, self.timing = L, precision == "f16", torch.device(device), None
+        super().__init__(precision, device)
         vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_longlong, C.c_float
-        self._att = L.declare("mer_disentangled_attention", [vp, vp, i64, vp, vp, i64, i32, vp, f32, vp, vp, i32, i64,
-                                                             i32, i32, i32, vp])
-        self.mode = L.MER_GEMM_F16 if self.f16 else L.MER_GEMM_BF16X3
-        self.op_dtype = torch.float16 if self.f16 else torch.float32
-
-    def _run(self, klass, fn):
-        if self.timing is None:
-            return fn()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = fn()
-        b.record()
-        self.timing.append((klass, a, b))
-        return r
-
-    def weight(self, t):
-        t = torch.as_tensor(t).to(self.device, torch.float32).contiguous()
-        return t.half() if self.f16 else self.L.split_bf16(t)
-
-    operand = weight
-
-    def vector(self, t):
-        return torch.as_tensor(t).to(self.device, torch.float32).contiguous()
-
-    embedding = vector
-
-    def embed(self, table, ids):
-        return table[torch.as_tensor(ids, device=self.device)]
-
-    def zeros_like(self, x):
-        return torch.zeros_like(x)
+        self._att = self.L.declare("mer_disentangled_attention", [vp, vp, i64, vp, vp, i64, i32, vp, f32, vp, vp, i32,
+                                                                  i64, i32, i32, i32, vp])
 
     def batch(self, lens, rows):
+        """DeviceOps.batch, with the distance -> table row map and the conv operand rows of each token.  The rows are
+        built before the first host-to-device copy, which waits for the previous pass: host work after it idles the
+        GPU."""
         cu = np.zeros(len(lens) + 1, np.int64)
         cu[1:] = np.cumsum(lens)
         pad = np.concatenate([cu[s] + 2 * s + 1 + np.arange(m) for s, m in enumerate(lens)])  # conv operand rows
-        return dict(cu=torch.from_numpy(cu.astype(np.int32)).to(self.device), n=len(lens), max_len=int(max(lens)),
-                    rows=torch.from_numpy(rows).to(self.device), pad=torch.from_numpy(pad).to(self.device))
-
-    def layernorm(self, x, g, b, eps, acc=None):
-        """(y fp32, y as the next GEMM operand); acc += y when given."""
-        L = self.L
-        y = torch.empty_like(x)
-        op = torch.empty(x.shape, dtype=self.op_dtype, device=self.device)
-        flags = (L.MER_LN_SPLIT_F16 if self.f16 else 0) | (L.MER_LN_ACC_ADD if acc is not None else 0)
-        self._run("layernorm", lambda: L.layernorm(x, g, b, y, eps=eps, y_split=op, acc=acc, flags=flags))
-        return y, op
+        return dict(super().batch(lens), rows=torch.from_numpy(rows).to(self.device),
+                    pad=torch.from_numpy(pad).to(self.device))
 
     def pos_proj(self, rel, w, b):
         out = torch.empty(rel.shape[0], w.shape[0], dtype=self.op_dtype, device=self.device)
@@ -368,16 +329,6 @@ class CudaOps:
             scale, L.ptr(ctx), L.ptr(b["cu"]), b["n"], T, b["max_len"], heads, flags, L.stream_ptr())))
         return ctx
 
-    def linear_res(self, a, w, bias, x):
-        self._run("gemm", lambda: self.L.gemm(a, w, x, bias=bias, res=x, mode=self.mode))
-        return x
-
-    def ffn_up(self, y, w, bias):
-        h = torch.empty(y.shape[0], w.shape[0], dtype=self.op_dtype, device=self.device)
-        self._run("gemm", lambda: self.L.gemm(y, w, h, bias=bias, mode=self.mode, gelu=True, f16_out=self.f16,
-                                              split_out=not self.f16))
-        return h
-
     def conv(self, y0, w, bias, b):
         """gelu(conv1d_k3(h[0]) + bias) per token: one 3-tap GEMM over the operand rows laid out with a zero row before
         and after every sentence, so that no tap reads a neighbouring sentence."""
@@ -397,15 +348,14 @@ def activation_bytes_per_token(hidden, ffn):
     return hidden * 4 * 11 + ffn * 4
 
 
-class DebertaTextEncoder:
-    """``forward(id_lists, start, end, want_tokens)`` (the contract TextExtractor drives) over ``DebertaNet`` with the
-    CUDA backend.  ``sd``: {name: tensor}; ``cfg``: the checkpoint's DebertaConfig / DebertaV2Config.  ``precision``:
-    None = MER_TEXT_PRECISION, else BertEncoder's rule ("f16" at hidden 768, "bf16x3" above)."""
+class DebertaTextEncoder(PackedTextEncoder):
+    """PackedTextEncoder over ``DebertaNet`` with the CUDA backend.  ``sd``: {name: tensor}; ``cfg``: the checkpoint's
+    DebertaConfig / DebertaV2Config.  ``precision``: None = MER_TEXT_PRECISION, else BertEncoder's rule ("f16" at
+    hidden 768, "bf16x3" above)."""
+
+    span = (1, -1)
 
     def __init__(self, sd, cfg, device="cuda", precision=None):
-        import ctypes as C
-
-        from .. import _lib as L
         check_deberta_config(cfg)
         self.dims = d = DebertaDims(cfg)
         if d.hidden not in LN_DIMS:
@@ -416,24 +366,3 @@ class DebertaTextEncoder:
         self.net = DebertaNet(sd, self.ops, d)
         self.hidden, self.vocab_size = d.hidden, self.net.word.shape[0]
         self.bytes_per_token = activation_bytes_per_token(d.hidden, d.ffn)
-        self._L = L
-        self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                                     C.c_void_p, C.c_void_p])
-
-    def forward(self, id_lists, start=1, end=-1, want_tokens=False):
-        """id_lists: non-empty token id sequences.  Returns (utt [n, hidden] = mean over each sentence's kept range
-        [start : len + end], tokens [sum len, hidden] | None), fp32."""
-        L = self._L
-        lens = [len(x) for x in id_lists]
-        assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
-        ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
-        assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
-        acc = self.net.forward(ids, lens)
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
-        seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)
-        seg = torch.from_numpy(np.maximum(seg, seg[:1])).to(self.device)   # empty kept range -> zeros (caller skips it)
-        utt = torch.empty(len(lens), self.hidden, dtype=torch.float32, device=self.device)
-        L.check(self._seg(L.ptr(acc), L.ptr(seg[0]), L.ptr(seg[1]), len(lens), self.hidden, 1, L.ptr(utt),
-                          L.stream_ptr()))
-        return utt, (acc if want_tokens else None)

@@ -13,11 +13,10 @@ pass covers many of them.  Weights are read shard by shard, tensor by tensor, an
 """
 from __future__ import annotations
 
-import json
-import os
-
-import numpy as np
 import torch
+
+from .common import stream_fp16_weights
+from .packed_text import DeviceOps, PackedTextEncoder
 
 HEAD_DIM = 128
 
@@ -57,49 +56,16 @@ def rope_tables(max_pos, theta, head_dim=HEAD_DIM):
 
 
 # ---- streaming checkpoint loader ------------------------------------------------------------------------------------
-def _checkpoint_files(model_dir, prefer_bin=False):
-    kinds = [("pytorch_model.bin", "pytorch_model.bin.index.json"), ("model.safetensors", "model.safetensors.index.json")]
-    if not prefer_bin:
-        kinds.reverse()
-    for single, index in kinds:
-        if os.path.exists(os.path.join(model_dir, single)):
-            return [os.path.join(model_dir, single)]
-        if os.path.exists(os.path.join(model_dir, index)):
-            shards = sorted(set(json.load(open(os.path.join(model_dir, index)))["weight_map"].values()))
-            return [os.path.join(model_dir, s) for s in shards]
-    raise FileNotFoundError(f"no model.safetensors / pytorch_model.bin (or their .index.json) under {model_dir}")
-
-
-def _iter_tensors(path):
-    if path.endswith(".safetensors"):
-        from safetensors import safe_open
-        with safe_open(path, framework="pt", device="cpu") as f:
-            for k in f.keys():
-                yield k, f.get_tensor(k)
-    else:
-        sd = torch.load(path, map_location="cpu", mmap=True, weights_only=True)
-        for k in list(sd):
-            yield k, sd.pop(k)
-
-
 def load_llama_weights(model_dir, device, prefer_bin=False):
     """{LlamaModel parameter name: fp16 tensor on ``device``}, read one tensor at a time (safetensors through
     ``safe_open``, ``.bin`` through an mmap'ed ``torch.load``) from fp32 / fp16 / bf16 checkpoints.  Accepts the
     ``model.`` prefix of ``LlamaForCausalLM`` checkpoints and drops ``lm_head.weight`` and the rotary ``inv_freq``
     buffers some older checkpoints carry.  ``prefer_bin``: read ``pytorch_model.bin*`` when both formats exist (the
     reference loads Llama-2-13b-hf with ``use_safetensors=False``)."""
-    out = {}
-    for path in _checkpoint_files(model_dir, prefer_bin):
-        for k, v in _iter_tensors(path):
-            if k.startswith("model."):
-                k = k[len("model."):]
-            if k == "lm_head.weight" or k.endswith("rotary_emb.inv_freq"):
-                continue
-            t = v.to(device).to(torch.float16)
-            if not bool(torch.isfinite(t).all()):
-                raise ValueError(f"{path}: {k} is not finite in fp16")
-            out[k] = t
-    return out
+    def rename(k):
+        k = k[len("model."):] if k.startswith("model.") else k
+        return None if k == "lm_head.weight" or k.endswith("rotary_emb.inv_freq") else k
+    return dict(stream_fp16_weights(model_dir, device, rename, prefer_bin))
 
 
 # ---- layer orchestration --------------------------------------------------------------------------------------------
@@ -144,9 +110,9 @@ class LlamaNet:
                 ops.add_(acc, x)
             y = ops.rmsnorm(x, L["ln1"], self.eps)
             ctx = ops.attention(y, L["qkv"], b, self.heads, self.cos, self.sin)
-            x = ops.linear_res(ctx, L["o"], x)
+            x = ops.linear_res(ctx, L["o"], None, x)
             y = ops.rmsnorm(x, L["ln2"], self.eps)
-            x = ops.linear_res(ops.mlp(y, L["gate_up"]), L["down"], x)
+            x = ops.linear_res(ops.mlp(y, L["gate_up"]), L["down"], None, x)
             if i >= n - 3 and i < n - 1:
                 ops.add_(acc, x)
             if return_hidden and i < n - 1:
@@ -210,7 +176,7 @@ class TorchOps:
             o += n
         return ctx
 
-    def linear_res(self, a, w, x):
+    def linear_res(self, a, w, b, x):   # LLaMA has no biases: b is None
         return x + a @ w.T
 
     def mlp(self, y, w_gu):
@@ -219,54 +185,21 @@ class TorchOps:
         return torch.nn.functional.silu(gu[:, :h]) * gu[:, h:]
 
 
-class CudaOps:
+class CudaOps(DeviceOps):
     """Product backend: fp16 weights and GEMM operands (MER_GEMM_F16), fp32 residual stream; every op is one or two
-    libmer_b200.so launches.  With ``timing`` set to a list, each launch is bracketed by CUDA events and recorded as
-    (kernel class, start, end) for the benchmark's time shares."""
+    libmer_b200.so launches.  ``timing``: see DeviceOps."""
+
+    embedding = DeviceOps.weight
 
     def __init__(self, device="cuda"):
         import ctypes as C
-
-        from .. import _lib as L
-        L.check(L.lib().mer_check_device())
-        self.L, self.device, self.timing = L, torch.device(device), None
+        super().__init__("f16", device)
+        L = self.L
         vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_longlong, C.c_float
         self._rms = L.declare("mer_rmsnorm", [vp, vp, vp, vp, i64, i32, f32, vp])
         self._rope = L.declare("mer_rope_f16", [vp, i64, i64, i32, vp, i32, vp, vp, vp, i32, vp])
         self._att = L.declare("mer_causal_attention_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, vp])
         self._swiglu = L.declare("mer_swiglu_f16", [vp, vp, i64, i32, vp])
-
-    def _run(self, klass, fn):
-        if self.timing is None:
-            return fn()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = fn()
-        b.record()
-        self.timing.append((klass, a, b))
-        return r
-
-    def weight(self, t):
-        return t.to(self.device, torch.float16).contiguous()
-
-    embedding = weight
-
-    def vector(self, t):
-        return t.to(self.device, torch.float32).contiguous()
-
-    def embed(self, table, ids):
-        return table[torch.as_tensor(ids, device=self.device)].float()
-
-    def zeros_like(self, x):
-        return torch.zeros_like(x)
-
-    def add_(self, acc, x):
-        acc += x
-
-    def batch(self, lens):
-        cu = np.zeros(len(lens) + 1, np.int32)
-        cu[1:] = np.cumsum(lens)
-        return dict(cu=torch.from_numpy(cu).to(self.device), n=len(lens), max_len=int(max(lens)))
 
     def rmsnorm(self, x, w, eps, acc=None):
         L = self.L
@@ -287,10 +220,6 @@ class CudaOps:
                                                          b["n"], T, b["max_len"], heads, L.stream_ptr())))
         return ctx
 
-    def linear_res(self, a, w, x):
-        self._run("gemm", lambda: self.L.gemm(a, w, x, res=x, mode=self.L.MER_GEMM_F16))
-        return x
-
     def mlp(self, y, w_gu):
         L, T, two_i = self.L, y.shape[0], w_gu.shape[0]
         gu = torch.empty(T, two_i, dtype=torch.float32, device=self.device)
@@ -306,14 +235,13 @@ def activation_bytes_per_token(hidden, intermediate):
     return hidden * (4 + 4 + 2 + 3 * 2 + 2 + 2) + intermediate * (2 * 4 + 2)
 
 
-class LlamaTextEncoder:
-    """``forward(id_lists, start, end, want_tokens)`` (the contract TextExtractor drives) over ``LlamaNet`` with the CUDA
-    backend.  ``cfg``: the checkpoint's LlamaConfig; ``sd``: {name: tensor} (load_llama_weights)."""
+class LlamaTextEncoder(PackedTextEncoder):
+    """PackedTextEncoder over ``LlamaNet`` with the CUDA backend.  ``cfg``: the checkpoint's LlamaConfig; ``sd``:
+    {name: tensor} (load_llama_weights)."""
+
+    span = (1, None)
 
     def __init__(self, sd, cfg, device="cuda"):
-        import ctypes as C
-
-        from .. import _lib as L
         check_llama_config(cfg)
         self.ops = CudaOps(device)
         self.device = self.ops.device
@@ -322,26 +250,3 @@ class LlamaTextEncoder:
                             rope_theta(cfg), self.max_pos)
         self.hidden, self.vocab_size = self.net.hidden, self.net.embed.shape[0]
         self.bytes_per_token = activation_bytes_per_token(self.hidden, cfg.intermediate_size)
-        self._L = L
-        self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                                     C.c_void_p, C.c_void_p])
-
-    def forward(self, id_lists, start=1, end=None, want_tokens=False):
-        """id_lists: non-empty token id sequences.  Returns (utt [n, hidden] = mean over each sentence's kept range
-        [start : len + end], tokens [sum len, hidden] | None), fp32."""
-        L = self._L
-        lens = [len(x) for x in id_lists]
-        assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
-        if max(lens) > self.max_pos:
-            raise ValueError(f"a sentence of {max(lens)} tokens exceeds max_position_embeddings {self.max_pos}")
-        ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
-        assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
-        acc = self.net.forward(ids, lens)
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
-        seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)
-        seg = torch.from_numpy(np.maximum(seg, seg[:1])).to(self.device)   # empty kept range -> zeros (caller skips it)
-        utt = torch.empty(len(lens), self.hidden, dtype=torch.float32, device=self.device)
-        L.check(self._seg(L.ptr(acc), L.ptr(seg[0]), L.ptr(seg[1]), len(lens), self.hidden, 1, L.ptr(utt),
-                          L.stream_ptr()))
-        return utt, (acc if want_tokens else None)

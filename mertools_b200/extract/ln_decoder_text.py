@@ -35,7 +35,9 @@ import re
 import numpy as np
 import torch
 
-from .llama_text import HEAD_DIM, _checkpoint_files, _iter_tensors, rope_tables, rope_theta
+from .common import stream_fp16_weights
+from .llama_text import HEAD_DIM, rope_tables, rope_theta
+from .packed_text import DeviceOps, PackedTextEncoder
 
 OPT_POS_OFFSET = 2  # OPTLearnedPositionalEmbedding: position p reads row p + 2
 GPT2_HEAD_DIMS = (64, 96, 128)  # the instances of mer_causal_attention_hd_f16
@@ -174,17 +176,8 @@ def load_ln_decoder_weights(model_dir, device, family):
     prefixes; ``lm_head`` and GPT-2's mask buffers are dropped.  GPT-2's Conv1D weights (GPT2_CONV1D, stored [in, out])
     are transposed to the [out, in] of the other families.  A value that is not finite in fp16 is refused."""
     out = {}
-    for path in _checkpoint_files(model_dir):
-        for k, v in _iter_tensors(path):
-            k = _strip(k, family)
-            if k is None:
-                continue
-            if family == "gpt2" and k.endswith(GPT2_CONV1D):
-                v = v.t()
-            t = v.to(device).to(torch.float16).contiguous()
-            if not bool(torch.isfinite(t).all()):
-                raise ValueError(f"{path}: {k} is not finite in fp16")
-            out[k] = t
+    for k, t in stream_fp16_weights(model_dir, device, lambda k: _strip(k, family)):
+        out[k] = t.t().contiguous() if family == "gpt2" and k.endswith(GPT2_CONV1D) else t
     return out
 
 
@@ -419,16 +412,16 @@ class TorchOps:
         return h * 0.5 * (1.0 + torch.tanh(0.79788456 * h * (1 + 0.044715 * h * h)))
 
 
-class CudaOps:
+class CudaOps(DeviceOps):
     """Product backend: fp16 weights and GEMM operands (MER_GEMM_F16) with fp32 biases, fp32 residual stream; every op
-    is one or two libmer_b200.so launches.  ``timing``: as llama_text.CudaOps (kernel class, start, end events)."""
+    is one or two libmer_b200.so launches.  ``timing``: see DeviceOps."""
+
+    embedding = DeviceOps.weight
 
     def __init__(self, device="cuda"):
         import ctypes as C
-
-        from .. import _lib as L
-        L.check(L.lib().mer_check_device())
-        self.L, self.device, self.timing = L, torch.device(device), None
+        super().__init__("f16", device)
+        L = self.L
         vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_longlong, C.c_float
         self._ln = L.declare("mer_layernorm_f16", [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp])
         self._att = L.declare("mer_causal_attention_hd_f16", [vp, vp, i64, vp, vp, i32, i64, i32, i32, i32, vp])
@@ -436,38 +429,6 @@ class CudaOps:
         self._ln_ld = L.declare("mer_layernorm_ld_f16", [vp, i64, vp, vp, vp, vp, vp, i64, i32, f32, vp])
         self._rope = L.declare("mer_rope_hd_f16", [vp, i64, i64, i32, i32, vp, i32, vp, vp, vp, i32, vp])
         self._att_mqa = L.declare("mer_causal_mqa_attention_f16", [vp, i64, vp, i64, vp, vp, i32, i64, i32, i32, vp])
-
-    def _run(self, klass, fn):
-        if self.timing is None:
-            return fn()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = fn()
-        b.record()
-        self.timing.append((klass, a, b))
-        return r
-
-    def weight(self, t):
-        return t.to(self.device, torch.float16).contiguous()
-
-    embedding = weight
-
-    def vector(self, t):
-        return t.to(self.device, torch.float32).contiguous()
-
-    def embed(self, table, ids):
-        return table[torch.as_tensor(ids, device=self.device)].float()
-
-    def zeros_like(self, x):
-        return torch.zeros_like(x)
-
-    def add_(self, acc, x):
-        acc += x
-
-    def batch(self, lens):
-        cu = np.zeros(len(lens) + 1, np.int32)
-        cu[1:] = np.cumsum(lens)
-        return dict(cu=torch.from_numpy(cu).to(self.device), n=len(lens), max_len=int(max(lens)))
 
     # ---- Falcon: hidden-wide rows padded to a multiple of 128 columns (mer_gemm's N), pad columns zero ----
     def falcon_embedding(self, t):
@@ -547,10 +508,6 @@ class CudaOps:
             self._run("attention", lambda: L.check(self._att(*args, D // heads, L.stream_ptr())))
         return ctx
 
-    def linear_res(self, a, w, bias, x):
-        self._run("gemm", lambda: self.L.gemm(a, w, x, bias=bias, res=x, mode=self.L.MER_GEMM_F16))
-        return x
-
     def mlp(self, y, w, bias, act):
         """act "gelu" (Falcon, erf form, no bias): y may be padded rows, the GEMM reads their first w.shape[1]
         columns."""
@@ -590,15 +547,13 @@ def net_dims(cfg):
             int(cfg.max_position_embeddings))
 
 
-class LnDecoderTextEncoder:
-    """``forward(id_lists, start, end, want_tokens)`` (the contract TextExtractor drives) over ``LnDecoderNet`` with
-    the CUDA backend.  ``cfg``: the checkpoint's BloomConfig / OPTConfig / GPT2Config / FalconConfig; ``sd``: {name:
-    tensor} (load_ln_decoder_weights)."""
+class LnDecoderTextEncoder(PackedTextEncoder):
+    """PackedTextEncoder over ``LnDecoderNet`` with the CUDA backend; token types are GPT-2's.  ``cfg``: the
+    checkpoint's BloomConfig / OPTConfig / GPT2Config / FalconConfig; ``sd``: {name: tensor} (load_ln_decoder_weights)."""
+
+    takes_token_types = True
 
     def __init__(self, sd, cfg, device="cuda"):
-        import ctypes as C
-
-        from .. import _lib as L
         check_ln_decoder_config(cfg)
         family, layers, heads, hidden, ffn, eps, self.max_pos = net_dims(cfg)
         self.ops = CudaOps(device)
@@ -607,33 +562,3 @@ class LnDecoderTextEncoder:
         self.net = LnDecoderNet(sd, self.ops, family, layers, heads, eps, self.max_pos, theta=theta)
         self.hidden, self.vocab_size = self.net.hidden, self.net.embed.shape[0]
         self.bytes_per_token = activation_bytes_per_token(hidden, ffn, family)
-        self._L = L
-        self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                                     C.c_void_p, C.c_void_p])
-
-    def forward(self, id_lists, start=0, end=None, want_tokens=False, token_types=None):
-        """id_lists: non-empty token id sequences; token_types: None, or one int sequence per sentence (GPT-2).  When
-        None, the ``token_types`` attribute TokenTypeTextExtractor attaches to each id list is used if present.  Returns
-        (utt [n, hidden] = mean over each sentence's kept range [start : len + end], tokens [sum len, hidden] | None),
-        fp32."""
-        from .text import packed_token_types
-        L = self._L
-        lens = [len(x) for x in id_lists]
-        assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
-        tt = packed_token_types(id_lists, token_types)
-        if self.max_pos is not None and max(lens) > self.max_pos:
-            raise ValueError(f"a sentence of {max(lens)} tokens exceeds max_position_embeddings {self.max_pos}")
-        ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
-        assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
-        assert tt is None or (tt.min() >= 0 and tt.max() < self.vocab_size), "token type outside the vocabulary"
-        acc = self.net.forward(ids, lens, token_types=tt)
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
-        seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)
-        seg = torch.from_numpy(np.maximum(seg, seg[:1])).to(self.device)   # empty kept range -> zeros (caller skips it)
-        width = acc.shape[1]   # hidden, or Falcon's padded row width
-        utt = torch.empty(len(lens), width, dtype=torch.float32, device=self.device)
-        L.check(self._seg(L.ptr(acc), L.ptr(seg[0]), L.ptr(seg[1]), len(lens), width, 1, L.ptr(utt), L.stream_ptr()))
-        if width != self.hidden:
-            utt, acc = utt[:, :self.hidden], acc[:, :self.hidden]
-        return utt, (acc if want_tokens else None)

@@ -21,6 +21,7 @@ import numpy as np
 
 from ..encoders import BertEncoder
 from . import common
+from .packed_text import packed_token_types  # noqa: F401  (re-exported)
 
 
 def find_start_end_pos(tokenizer):
@@ -115,23 +116,17 @@ class TokenTypeTextExtractor(TextExtractor):
         return ids
 
 
-def packed_token_types(id_lists, token_types=None):
-    """int64 [sum len] of the token types of packed id lists, or None: ``token_types`` (one sequence per id list) when
-    given, else the ``token_types`` TokenTypeTextExtractor attached to every id list (all or none of them)."""
-    if token_types is None:
-        found = [getattr(x, "token_types", None) for x in id_lists]
-        assert all(t is None for t in found) or all(t is not None for t in found), "token types for some only"
-        token_types = None if found[0] is None else found
-    if token_types is None:
-        return None
-    assert [len(t) for t in token_types] == [len(x) for x in id_lists], "one token type per token"
-    return np.concatenate([np.asarray(t, dtype=np.int64) for t in token_types])
+def _tokens_per_launch(enc, row_len):
+    """Tokens per launch of a packed text encoder: what half of the device memory left after its weights holds at its
+    ``bytes_per_token``, at least one sentence of ``row_len`` tokens and at most 16384."""
+    import torch
+    free, _ = torch.cuda.mem_get_info(enc.device)
+    return int(min(16384, max(row_len, free // 2 // enc.bytes_per_token)))
 
 
 def _llama_extractor(model_name, model_dir, cfg, device):
     """The reference's LLM branch (:170-175, 193-196): LlamaModel + AutoTokenizer(use_fast=False), fp16 features.
-    Tokens per launch: what half of the device memory left after the weights holds at the model's activation size."""
-    import torch
+    Tokens per launch: _tokens_per_launch with a row of max_position_embeddings."""
     from transformers import AutoTokenizer
 
     from .llama_text import LlamaTextEncoder, check_llama_config, load_llama_weights
@@ -139,23 +134,20 @@ def _llama_extractor(model_name, model_dir, cfg, device):
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = LlamaTextEncoder(load_llama_weights(model_dir, device, prefer_bin=(model_name == "Llama-2-13b-hf")), cfg,
                            device=device)
-    free, _ = torch.cuda.mem_get_info(enc.device)
-    tokens = int(min(16384, max(cfg.max_position_embeddings, free // 2 // enc.bytes_per_token)))
+    tokens = _tokens_per_launch(enc, cfg.max_position_embeddings)
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
 
 
 def _ln_decoder_extractor(model_dir, cfg, device):
     """The same LLM branch for BLOOM / OPT (:170-172, 193-196) and Falcon (:188-190, 193-196): BloomModel / OPTModel /
     FalconModel + AutoTokenizer(use_fast=False), fp16 features; tokens per launch as in _llama_extractor."""
-    import torch
     from transformers import AutoTokenizer
 
     from .ln_decoder_text import LnDecoderTextEncoder, check_ln_decoder_config, load_ln_decoder_weights
     check_ln_decoder_config(cfg)  # before any weight is read
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = LnDecoderTextEncoder(load_ln_decoder_weights(model_dir, device, cfg.model_type), cfg, device=device)
-    free, _ = torch.cuda.mem_get_info(enc.device)
-    tokens = int(min(16384, max(enc.max_pos or 2048, free // 2 // enc.bytes_per_token)))
+    tokens = _tokens_per_launch(enc, enc.max_pos or 2048)
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens, out_dtype=np.float16)
 
 
@@ -164,14 +156,11 @@ def _gpt2_extractor(model_name, model_dir, cfg, device):
     gpt2-chinese-cluecorpussmall through the AutoModel + AutoTokenizer(use_fast=False) branch (:188-190).  Neither is
     halved there, so the features are fp32.  The extractor forwards the tokenizer's token_type_ids when it returns them
     (gpt2-chinese's BertTokenizer does), as model(**inputs) does.  Tokens per launch as in _ln_decoder_extractor."""
-    import torch
-
     from .ln_decoder_text import LnDecoderTextEncoder, check_ln_decoder_config, load_ln_decoder_weights
     check_ln_decoder_config(cfg)  # before any weight is read
     tokenizer = _gpt2_tokenizer(model_name, model_dir)
     enc = LnDecoderTextEncoder(load_ln_decoder_weights(model_dir, device, "gpt2"), cfg, device=device)
-    free, _ = torch.cuda.mem_get_info(enc.device)
-    tokens = int(min(16384, max(enc.max_pos, free // 2 // enc.bytes_per_token)))
+    tokens = _tokens_per_launch(enc, enc.max_pos)
     return TokenTypeTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
@@ -187,7 +176,6 @@ def _deberta_extractor(model_name, model_dir, cfg, device):
     """The reference's DeBERTa models (:164-166 and the AutoModel branch), fp32 features.  Tokenizer by model name as
     the reference loads it: BertTokenizer for deberta-chinese-large, AutoTokenizer(use_fast=False) otherwise.  Tokens per
     launch as in _llama_extractor."""
-    import torch
     from transformers import AutoTokenizer, BertTokenizer
 
     from .deberta_text import DebertaTextEncoder, check_deberta_config
@@ -197,8 +185,7 @@ def _deberta_extractor(model_name, model_dir, cfg, device):
     else:
         tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = DebertaTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
-    free, _ = torch.cuda.mem_get_info(enc.device)
-    tokens = int(min(16384, max(cfg.max_position_embeddings, free // 2 // enc.bytes_per_token)))
+    tokens = _tokens_per_launch(enc, cfg.max_position_embeddings)
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
@@ -206,15 +193,13 @@ def _xlnet_extractor(model_dir, cfg, device):
     """The reference's XLNet models (the AutoModel + AutoTokenizer(use_fast=False) branch), fp32 features.  The
     extractor forwards the tokenizer's token_type_ids when it returns them, as model(**inputs) does.  Tokens per launch
     as in _deberta_extractor, with MAX_LEN (512) for the max_position_embeddings XLNet does not have."""
-    import torch
     from transformers import AutoTokenizer
 
     from .xlnet_text import MAX_LEN, XlnetTextEncoder, check_xlnet_config
     check_xlnet_config(cfg)  # before any weight is read
     tokenizer = AutoTokenizer.from_pretrained(model_dir, use_fast=False)
     enc = XlnetTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
-    free, _ = torch.cuda.mem_get_info(enc.device)
-    tokens = int(min(16384, max(MAX_LEN, free // 2 // enc.bytes_per_token)))
+    tokens = _tokens_per_launch(enc, MAX_LEN)
     return TokenTypeTextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 
@@ -222,14 +207,11 @@ def _albert_extractor(model_name, model_dir, cfg, device):
     """The reference's ALBERT models, fp32 features: albert_chinese_tiny / _small with BertTokenizer (:164-166), the
     English v2 models through the AutoModel + AutoTokenizer(use_fast=False) branch.  Tokens per launch as in
     _xlnet_extractor, with max_position_embeddings for the row length."""
-    import torch
-
     from .albert_text import AlbertTextEncoder, albert_tokenizer, check_albert_config
     check_albert_config(cfg)  # before any weight is read
     tokenizer = albert_tokenizer(model_name, model_dir)
     enc = AlbertTextEncoder(common.load_hf_state_dict(model_dir), cfg, device=device)
-    free, _ = torch.cuda.mem_get_info(enc.device)
-    tokens = int(min(16384, max(cfg.max_position_embeddings, free // 2 // enc.bytes_per_token)))
+    tokens = _tokens_per_launch(enc, cfg.max_position_embeddings)
     return TextExtractor(None, tokenizer, encoder=enc, max_tokens_per_launch=tokens)
 
 

@@ -31,7 +31,8 @@ import numpy as np
 import torch
 
 from .deberta_text import LN_DIMS, activation_bytes_per_token
-from .text import TokenIds, TokenTypeTextExtractor, packed_token_types  # noqa: F401  (TokenIds: re-exported)
+from .packed_text import DeviceOps, PackedTextEncoder
+from .text import TokenIds, TokenTypeTextExtractor  # noqa: F401  (TokenIds: re-exported)
 
 HEAD_DIM = 64
 MAX_LEN = 512   # tokens per sentence the launch sizing assumes (XLNet has no max_position_embeddings)
@@ -217,64 +218,16 @@ class TorchOps:
         return torch.relu(h) if act == "relu" else torch.nn.functional.gelu(h)
 
 
-class CudaOps:
+class CudaOps(DeviceOps):
     """Product backend.  precision "f16": fp16 weights, GEMM operands, q | k | V^T and R (MER_GEMM_F16,
     MER_ATT_QKV_F16); "bf16x3": split-bf16 weights and operands (MER_GEMM_BF16X3), tf32-rounded q | k | V^T and R,
     ctx written as split rows.  fp32 biases, residual stream and readout; ``mer_layernorm`` writes the fp32 row, the
-    next operand and the readout term in one pass.  ``timing``: None, or a list that collects (kernel class, start,
-    end) CUDA events per launch."""
-
-    def __init__(self, precision, device="cuda"):
-        from .. import _lib as L
-        L.check(L.lib().mer_check_device())
-        assert precision in ("f16", "bf16x3"), precision
-        self.L, self.f16, self.device, self.timing = L, precision == "f16", torch.device(device), None
-        self.mode = L.MER_GEMM_F16 if self.f16 else L.MER_GEMM_BF16X3
-        self.op_dtype = torch.float16 if self.f16 else torch.float32
-
-    def _run(self, klass, fn):
-        if self.timing is None:
-            return fn()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = fn()
-        b.record()
-        self.timing.append((klass, a, b))
-        return r
-
-    def weight(self, t):
-        """fp32 rows -> GEMM operand: fp16, or split bf16 rows."""
-        t = torch.as_tensor(t).to(self.device, torch.float32).contiguous()
-        return t.half() if self.f16 else self.L.split_bf16(t)
-
-    operand = weight
-
-    def vector(self, t):
-        return torch.as_tensor(t).to(self.device, torch.float32).contiguous()
-
-    embedding = vector
-
-    def embed(self, table, ids):
-        return table[torch.as_tensor(ids, device=self.device)]
-
-    def zeros_like(self, x):
-        return torch.zeros_like(x)
+    next operand and the readout term in one pass.  ``timing``: see DeviceOps."""
 
     def batch(self, lens, rows, token_types):
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
+        """DeviceOps.batch, with the distance -> table row map and the int32 token types (None: no segment term)."""
         tt = None if token_types is None else torch.as_tensor(np.asarray(token_types, np.int32), device=self.device)
-        return dict(cu=torch.from_numpy(cu.astype(np.int32)).to(self.device), n=len(lens), max_len=int(max(lens)),
-                    rows=torch.from_numpy(rows).to(self.device), types=tt)
-
-    def layernorm(self, x, g, b, eps, acc=None):
-        """(y fp32, y as the next GEMM operand); acc += y when given."""
-        L = self.L
-        y = torch.empty_like(x)
-        op = torch.empty(x.shape, dtype=self.op_dtype, device=self.device)
-        flags = (L.MER_LN_SPLIT_F16 if self.f16 else 0) | (L.MER_LN_ACC_ADD if acc is not None else 0)
-        self._run("layernorm", lambda: L.layernorm(x, g, b, y, eps=eps, y_split=op, acc=acc, flags=flags))
-        return y, op
+        return dict(super().batch(lens), rows=torch.from_numpy(rows).to(self.device), types=tt)
 
     def rel_proj(self, table, w_r, layers):
         """Every layer's R = pos_emb @ r in one GEMM: [rows, layers heads*64] in the attention's operand format; layer
@@ -300,34 +253,16 @@ class CudaOps:
             heads, flags, L.stream_ptr())))
         return ctx
 
-    def linear_res(self, a, w, bias, x):
-        self._run("gemm", lambda: self.L.gemm(a, w, x, bias=bias, res=x, mode=self.mode))
-        return x
 
-    def ffn_up(self, y, w, bias, act):
-        h = torch.empty(y.shape[0], w.shape[0], dtype=self.op_dtype, device=self.device)
-        if act == "gelu":
-            self._run("gemm", lambda: self.L.gemm(y, w, h, bias=bias, mode=self.mode, gelu=True, f16_out=self.f16,
-                                                  split_out=not self.f16))
-        elif self.f16:
-            self._run("gemm", lambda: self.L.gemm(y, w, h, bias=bias, mode=self.mode, relu=True, f16_out=True))
-        else:   # mer_gemm's ReLU epilogue writes fp32 or fp16 only: fp32, then split for the FC2 operand
-            f = torch.empty(y.shape[0], w.shape[0], dtype=torch.float32, device=self.device)
-            self._run("gemm", lambda: self.L.gemm(y, w, f, bias=bias, mode=self.mode, relu=True))
-            self._run("gemm", lambda: self.L.check(self.L.lib().mer_split_bf16(
-                self.L.ptr(f), self.L.ptr(h), f.shape[0], f.shape[1], self.L.stream_ptr())))
-        return h
+class XlnetTextEncoder(PackedTextEncoder):
+    """PackedTextEncoder over ``XlnetNet`` with the CUDA backend; token types give the segment term.  ``sd``: {name:
+    tensor}; ``cfg``: the checkpoint's XLNetConfig.  ``precision``: None = MER_TEXT_PRECISION, else BertEncoder's rule
+    ("f16" at hidden 768, "bf16x3" above)."""
 
-
-class XlnetTextEncoder:
-    """``forward(id_lists, start, end, want_tokens, token_types)`` (the contract TextExtractor drives) over
-    ``XlnetNet`` with the CUDA backend.  ``sd``: {name: tensor}; ``cfg``: the checkpoint's XLNetConfig.
-    ``precision``: None = MER_TEXT_PRECISION, else BertEncoder's rule ("f16" at hidden 768, "bf16x3" above)."""
+    span = (0, -2)
+    takes_token_types = True
 
     def __init__(self, sd, cfg, device="cuda", precision=None):
-        import ctypes as C
-
-        from .. import _lib as L
         check_xlnet_config(cfg)
         self.dims = d = XlnetDims(cfg)
         self.precision = precision or os.environ.get("MER_TEXT_PRECISION", "f16" if d.hidden == 768 else "bf16x3")
@@ -336,30 +271,6 @@ class XlnetTextEncoder:
         self.net = XlnetNet(sd, self.ops, d)
         self.hidden, self.vocab_size = d.hidden, self.net.word.shape[0]
         self.bytes_per_token = activation_bytes_per_token(d.hidden, d.ffn)
-        self._L = L
-        self._seg = L.declare("mer_segment_reduce", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                                     C.c_void_p, C.c_void_p])
-
-    def forward(self, id_lists, start=0, end=-2, want_tokens=False, token_types=None):
-        """id_lists: non-empty token id sequences; token_types: None, or one int sequence per sentence (then the
-        segment term is applied).  When None, the ``token_types`` attribute XlnetTextExtractor attaches to each id
-        list is used if present.  Returns (utt [n, hidden] = mean over each sentence's kept range [start : len + end],
-        tokens [sum len, hidden] | None), fp32."""
-        L = self._L
-        lens = [len(x) for x in id_lists]
-        assert all(n > 0 for n in lens), "empty sentences are handled by the caller (zeros)"
-        tt = packed_token_types(id_lists, token_types)
-        ids = np.concatenate([np.asarray(x, dtype=np.int64) for x in id_lists])
-        assert ids.min() >= 0 and ids.max() < self.vocab_size, "token id outside the vocabulary"
-        acc = self.net.forward(ids, lens, tt)
-        cu = np.zeros(len(lens) + 1, np.int64)
-        cu[1:] = np.cumsum(lens)
-        seg = np.stack([cu[:-1] + (start or 0), cu[1:] + (end or 0)]).astype(np.int32)
-        seg = torch.from_numpy(np.maximum(seg, seg[:1])).to(self.device)   # empty kept range -> zeros (caller skips it)
-        utt = torch.empty(len(lens), self.hidden, dtype=torch.float32, device=self.device)
-        L.check(self._seg(L.ptr(acc), L.ptr(seg[0]), L.ptr(seg[1]), len(lens), self.hidden, 1, L.ptr(utt),
-                          L.stream_ptr()))
-        return utt, (acc if want_tokens else None)
 
 
 XlnetTextExtractor = TokenTypeTextExtractor   # the token-type hook, under its XLNet name
