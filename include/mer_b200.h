@@ -581,6 +581,41 @@ MER_API int mer_logmel(const float* wave, int batch, int n_samples, long long ld
 MER_API int mer_videomae_patchify(const uint8_t* frames_bgr, int n_clips, const float* mean, const float* std,
                                   float* out, void* stream);
 
+/* ---- VideoMAE face-clip encoder of MER2024 / MER2026 (feature_extraction/visual/extract_sun_videomae.py:216-359 over
+ * the vendored videomae/modeling_finetune.py VisionTransformer, attn_type 'joint', use_mean_pooling=False). ---- */
+typedef struct MerVideoMaeModel {
+  int n_layers;          /* 12 (base) / 24 (large) */
+  int dim, heads, ffn;   /* 768 / 12 / 3072 or 1024 / 16 / 4096; heads * 64 == dim */
+  int img;               /* S: 160 (vit_base_patch16_160) or 224; tokens per view 8 (S / 16)^2 = 800 or 1568 */
+  float ln_eps;          /* 1e-6 */
+  const void* patch_w;   /* fp16 [dim, 1536]: patch_embed.proj (Conv3d (2, 16, 16)) flattened (c, dt, dy, dx) */
+  const float* patch_b;  /* [dim] */
+  const float* pos;      /* [tokens per view, dim]: get_sinusoid_encoding_table, fp32 */
+  const MerLayerWeights* layers; /* fp16 GEMM weights (MER_GEMM_F16); b_qkv = q_bias | 0 | v_bias */
+  const float* norm_g;   /* final norm */
+  const float* norm_b;
+} MerVideoMaeModel;
+
+/* The tubelet patch operand of n_views clips: frames uint8 [n_frames, S, S, 3] RGB (already resized to S x S; no
+ * channel swap, the reference reads them through Image.convert('RGB')), view_rows a DEVICE int32 [n_views, 16] table
+ * of frame rows -> out [n_views * 8 (S / 16)^2, 1536], row = (view, tubelet, patch row, patch column), columns in the
+ * Conv3d weight's (c, dt, dy, dx) order, value (float(p) / 255 - mean[c]) / std[c] in IEEE fp32 with the ImageNet
+ * mean / std (ClipToTensor + Normalize, bit for bit).  out_f32 != 0: fp32; 0: fp16 (round-to-nearest; the patch GEMM's
+ * operand).  S is 160 or 224.  A row outside [0, n_frames) is not read: the entries it would feed are NaN. */
+MER_API int mer_videomae_clips(const uint8_t* frames, int n_frames, int S, const int32_t* view_rows, int n_views,
+                               void* out, int out_f32, void* stream);
+/* bytes of workspace for n_views views; -1 for a model mer_videomae_forward refuses (mer_last_error) */
+MER_API long long mer_videomae_workspace_bytes(const MerVideoMaeModel* model, int n_views);
+/* model(videos, save_feature=True)[1] of the reference (engine_for_finetuning.py:final_test) for n_views views:
+ * mer_videomae_clips (fp16), the patch GEMM (+ bias + pos), the pre-LN stack on fp16 operands (erf-GELU, eps ln_eps,
+ * the fp16 V^T attention kernel for the 800 / 1568-token rows), the final norm and the mean over each view's tokens.
+ * view_rows is a HOST int32 [n_views, 16] table of rows of frames (uint8 [n_frames, img, img, 3] RGB); out: [n_views,
+ * dim].  Refused before any launch: a NULL operand, heads * 64 != dim, img other than 160 / 224 (tokens per view
+ * outside 254 .. MER_ATT_LONG_MAX), a workspace below mer_videomae_workspace_bytes, a view row outside [0, n_frames). */
+MER_API int mer_videomae_forward(const MerVideoMaeModel* model, const uint8_t* frames, int n_frames,
+                                 const int32_t* view_rows, int n_views, void* workspace, long long workspace_bytes,
+                                 float* out, void* stream);
+
 /* SwiGLU gate of HF Dinov2SwiGLUFFN (dinov2-giant, extract_vision_huggingface.py:135-145): in fp32 [rows, 2 * hidden]
  * = weights_in(x); out [rows, hidden] = silu(in[:, :hidden]) * in[:, hidden:], TF32-rounded when round_tf32_out. */
 MER_API int mer_swiglu(const float* in, float* out, long long rows, int hidden, int round_tf32_out, void* stream);
