@@ -245,6 +245,11 @@ typedef struct MerLayerWeights {
   const float* w_fc2; /* [768, 3072] */
   const float* b_fc2;
 } MerLayerWeights;
+/* gamma / beta of one LayerNorm (device pointers); the per-layer FFN norms of the EVA02 tower */
+typedef struct MerNormWeights {
+  const float* g;
+  const float* b;
+} MerNormWeights;
 
 /* ---- frame resize (visual preprocessing) ------------------------------------------------------- */
 /* PIL.Image.resize((OW, OH), BILINEAR) on uint8 [n, H, W, 3] frames, bit-exact: the resize step of HF
@@ -316,11 +321,41 @@ typedef struct MerClipVisionModel {
   /* MER_VISION_EMBED_ONLY (2): stop after the embeddings; out_embeds [n_frames * tokens, hidden] = class row
    * (cls_pos0) + patch rows (patch conv + pos_rest) = hidden_states[0] of a model whose layers the host orchestrates
    * (data2vec-vision: relative position bias in attention, extract/data2vec_vision.py); layers / n_layers unused. */
+  /* MER_VISION_EVA02 (3): timm Eva (eva02_base_patch14_224, the EVACLIP_VIT branch of the visual extractor) on the same
+   * tower: no pre_layrnorm (pre_ln_g NULL), the patch-conv bias folded into pos_rest, q_bias | 0 | v_bias as b_qkv; in
+   * every layer the 2D rotary embedding below on the q | k of the patch rows (the class row is not rotated), and the
+   * FFN x + fc2(LN(silu(fc1_g h) * fc1_x h)) with w_fc1 / b_fc1 = rows fc1_g | fc1_x ([2 ffn, hidden]), w_fc2 [hidden,
+   * ffn] and the LN of ffn_norms (eps ln_eps).  out_embeds [n_frames, hidden] = post_ln (fc_norm) of the mean over the
+   * patch rows of the last layer's output; proj_w unused, proj_dim = hidden.  Refused before any launch: a NULL table or
+   * norm array, NULL post_ln_*, rope_rows other than (image / patch)^2, ffn > 3 hidden, gemm_mode MER_GEMM_BF16X3.
+   * Attention at 257 tokens runs on fp16 q | k | V^T in both operand formats, so the rotation is always on fp16. */
   int variant;
+  const float* rope_cos;  /* MER_VISION_EVA02: [rope_rows, 32] fp32 cos of the pair angles of each patch row */
+  const float* rope_sin;  /* (see mer_rope2d_f16); 16-byte aligned */
+  int rope_rows;
+  const MerNormWeights* ffn_norms; /* MER_VISION_EVA02: host array of n_layers entries (mlp.norm) */
 } MerClipVisionModel;
 #define MER_VISION_CLIP 0
 #define MER_VISION_DINOV2 1
 #define MER_VISION_EMBED_ONLY 2
+#define MER_VISION_EVA02 3
+
+/* ---- the EVA02 kernels (csrc/eva02.cu), run by the MER_VISION_EVA02 tower ---- */
+/* timm RotaryEmbeddingCat / apply_rot_embed_cat, in place on the q | k columns [0, 2 * heads * 64) of fp16 rows qkv16
+ * [tokens, ld]: tokens are whole frames of tokens_per_frame rows whose first `prefix` rows are left alone; row j >=
+ * prefix of a frame uses table row p = j - prefix, and for every q / k head and pair i < 32,
+ * (x[2i], x[2i+1]) -> (x[2i] c - x[2i+1] s, x[2i+1] c + x[2i] s), c / s = cos_t / sin_t[p * 32 + i] (fp32, built on the
+ * host), computed in fp32 and rounded once.  Columns from 2 * heads * 64 on (V) are not touched.  Refused before any
+ * launch: a NULL operand, head_dim other than 64, ld < 2 * heads * 64 or not a multiple of 4, a misaligned operand,
+ * tokens not a multiple of tokens_per_frame, table_rows != tokens_per_frame - prefix. */
+MER_API int mer_rope2d_f16(void* qkv16, long long ld, long long tokens, int tokens_per_frame, int prefix, int heads,
+                           int head_dim, const float* cos_t, const float* sin_t, int table_rows, void* stream);
+/* timm SwiGLU with its norm (Eva's scale_mlp): in fp32 [rows, 2 * hidden] = rows fc1_g | fc1_x of the FC1 output;
+ * out [rows, hidden] = LayerNorm(silu(g) * x) * gamma + beta, mean and centred variance in fp32 over the product kept on
+ * chip; out fp16 (out_f16, the MER_GEMM_F16 operand of fc2) or tf32-rounded fp32.  Refused before any launch: hidden
+ * not a multiple of 128 or above 4096, a NULL operand, out == in, rows outside 1 .. 2^31 - 1. */
+MER_API int mer_swiglu_ln(const float* in, const float* gamma, const float* beta, float eps, void* out, long long rows,
+                          int hidden, int out_f16, void* stream);
 
 MER_API long long mer_clip_vision_workspace_bytes(const MerClipVisionModel* model, int n_frames);
 

@@ -82,6 +82,20 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
   MER_REQUIRE(HEADS * 64 == D, "mer_run_stack: heads %d x 64 != hidden %d", HEADS, D);
   const int ACT = a.quick_gelu ? MER_EPI_QUICK_GELU : MER_EPI_GELU;  // FC1 activation
   const size_t hs_bytes = (size_t)M * D * sizeof(float);
+  // EVA02: the rotation needs fp16 q | k, which the pre-LN stacks write exactly when attention takes the fp16 V^T kernel
+  const bool rope = a.rope_cos != nullptr;
+  if (rope || a.ffn_norms) {
+    const bool f16_qk = a.vt && (mer_attention_f16_supported(a.max_seqlen) ||
+                                 (a.long_rows && mer_attention_f16_long_supported(a.max_seqlen))) &&
+                        (a.mode == MER_GEMM_F16 || !mer_attention_uses_tc(a.max_seqlen));
+    MER_REQUIRE(a.pre_ln && (a.mode == MER_GEMM_F16 || a.mode == MER_GEMM_TF32),
+                "mer_run_stack: rotary / FFN-norm layers need a pre-LN F16 or TF32 stack");
+    MER_REQUIRE(!rope || (a.rope_sin && f16_qk && a.max_seqlen - a.rope_prefix == a.rope_rows &&
+                          M % a.max_seqlen == 0),
+                "mer_run_stack: rotary table of %d rows for rows of %d tokens (prefix %d) on fp16 q | k", a.rope_rows,
+                a.max_seqlen, a.rope_prefix);
+    MER_REQUIRE(!a.ffn_norms || DFF <= 3 * D, "mer_run_stack: FFN-norm width %d > 3 x hidden %d", DFF, D);
+  }
   if (a.opt_hidden && !a.hidden0_done) MER_CUDA_CHECK(cudaMemcpyAsync(a.opt_hidden, a.x, hs_bytes, cudaMemcpyDeviceToDevice, stream));
   for (int l = 0; l < a.n_layers; ++l) {
     const MerLayerWeights& w = a.layers[l];
@@ -112,6 +126,9 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
       if (f16_att) {
         MER_TRY(linear(a.mode, xn16, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, MER_EPI_OUT_F16, stream,
                        vt, a.vt_ld, 2 * D));
+        if (rope)
+          MER_TRY(mer_rope2d_f16(a.qkv, DQKV, M, a.max_seqlen, a.rope_prefix, HEADS, 64, a.rope_cos, a.rope_sin,
+                                 a.rope_rows, stream));
         MER_TRY(attend(f16_long, a.qkv, vt, a.vt_ld, xn16, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
                        MER_EPI_OUT_F16 | MER_ATT_QKV_F16, stream));
         MER_TRY(linear(a.mode, xn16, w.w_o, w.b_o, a.x, a.x, M, D, D, 0, stream));
@@ -127,22 +144,37 @@ int mer_run_stack(const MerStackArgs& a, cudaStream_t stream) {
       }
       MER_TRY(mer_layernorm_launch(a.x, w.ln2_g, w.ln2_b, xn16, nullptr, nullptr, M, D, a.eps, MER_LN_OUT_F16,
                                    stream));
-      MER_TRY(linear(a.mode, xn16, w.w_fc1, w.b_fc1, nullptr, h16, M, DFF, D, ACT | MER_EPI_OUT_F16,
-                     stream));
-      MER_TRY(linear(a.mode, h16, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
+      if (a.ffn_norms) {  // EVA02: x += fc2(LN(silu(fc1_g h) * fc1_x h)), the normed product in the dead qkv buffer
+        MER_TRY(linear(a.mode, xn16, w.w_fc1, w.b_fc1, nullptr, a.h, M, 2 * DFF, D, 0, stream));
+        MER_TRY(mer_swiglu_ln(a.h, a.ffn_norms[l].g, a.ffn_norms[l].b, a.eps, a.qkv, M, DFF, 1, stream));
+        MER_TRY(linear(a.mode, a.qkv, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
+      } else {
+        MER_TRY(linear(a.mode, xn16, w.w_fc1, w.b_fc1, nullptr, h16, M, DFF, D, ACT | MER_EPI_OUT_F16,
+                       stream));
+        MER_TRY(linear(a.mode, h16, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
+      }
     } else if (a.pre_ln) {
       // x = x + Wo * Attn(LN1(x));  x = x + W2 * GELU(W1 * LN2(x))
       MER_TRY(mer_layernorm_launch(a.x, w.ln1_g, w.ln1_b, split ? nullptr : a.xn, split ? a.xn : nullptr,
                                    nullptr, M, D, a.eps, MER_LN_ROUND_TF32, stream));
       MER_TRY(linear(a.mode, a.xn, w.w_qkv, w.b_qkv, nullptr, a.qkv, M, DQKV, D, qkv_fl, stream,
                      vt, a.vt_ld, 2 * D));
+      if (rope)
+        MER_TRY(mer_rope2d_f16(a.qkv, DQKV, M, a.max_seqlen, a.rope_prefix, HEADS, 64, a.rope_cos, a.rope_sin,
+                               a.rope_rows, stream));
       MER_TRY(attend(f16_long, a.qkv, vt, a.vt_ld, a.xn, a.cu_seqlens, a.n_seq, M, a.max_seqlen, HEADS,
                      opnd | att_in, stream));
       MER_TRY(linear(a.mode, a.xn, w.w_o, w.b_o, a.x, a.x, M, D, D, 0, stream));
       MER_TRY(mer_layernorm_launch(a.x, w.ln2_g, w.ln2_b, split ? nullptr : a.xn, split ? a.xn : nullptr,
                                    nullptr, M, D, a.eps, MER_LN_ROUND_TF32, stream));
-      MER_TRY(linear(a.mode, a.xn, w.w_fc1, w.b_fc1, nullptr, a.h, M, DFF, D, ACT | opnd, stream));
-      MER_TRY(linear(a.mode, a.h, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
+      if (a.ffn_norms) {  // EVA02 (TF32 stack): the normed product tf32-rounded in the dead qkv buffer
+        MER_TRY(linear(a.mode, a.xn, w.w_fc1, w.b_fc1, nullptr, a.h, M, 2 * DFF, D, 0, stream));
+        MER_TRY(mer_swiglu_ln(a.h, a.ffn_norms[l].g, a.ffn_norms[l].b, a.eps, a.qkv, M, DFF, 0, stream));
+        MER_TRY(linear(a.mode, a.qkv, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
+      } else {
+        MER_TRY(linear(a.mode, a.xn, w.w_fc1, w.b_fc1, nullptr, a.h, M, DFF, D, ACT | opnd, stream));
+        MER_TRY(linear(a.mode, a.h, w.w_fc2, w.b_fc2, a.x, a.x, M, D, DFF, 0, stream));
+      }
     } else if (a.mode == MER_GEMM_F16) {
       // post-LN on fp16 operands (scripts/precision_table.py): x stays the exact fp32 LayerNorm output
       // (residual stream, hidden state), xs carries its fp16 copy (GEMM operand, written by the same LayerNorm
@@ -316,7 +348,9 @@ static ClipPlan clip_plan(const MerClipVisionModel* m, int n_frames) {
   p.off_x = o;   o += al(p.M * D * 4);
   p.off_xn = o;  o += al(p.M * D * 4);
   p.off_qkv = o; o += al(p.M * 3 * D * 4);
-  long long hb = p.M * (long long)m->ffn * 4, pb = (long long)n_frames * p.P * m->kpad * 4;
+  // EVA02's FC1 writes the gate and value halves side by side: 2 ffn fp32 columns
+  const long long hcols = m->variant == MER_VISION_EVA02 ? 2ll * m->ffn : m->ffn;
+  long long hb = p.M * hcols * 4, pb = (long long)n_frames * p.P * m->kpad * 4;
   p.off_h = o;   o += al(hb > pb ? hb : pb);   // FFN buffer; the patch operand lives here first
   p.off_vt = o;  o += al(D * p.vt_ld * 4);
   p.off_cu = o;  o += al(((long long)n_frames + 1) * 4);
@@ -345,6 +379,24 @@ int mer_clip_vision_forward(const MerClipVisionModel* m, const uint8_t* frames_b
   MER_REQUIRE(workspace_bytes >= p.total, "mer_clip_vision_forward: workspace %lld B < required %lld B",
               workspace_bytes, p.total);
   MER_REQUIRE(p.M < (1ll << 31) / 4, "mer_clip_vision_forward: too many frames");
+  const bool dinov2 = m->variant == MER_VISION_DINOV2, eva02 = m->variant == MER_VISION_EVA02;
+  MER_REQUIRE(m->variant >= MER_VISION_CLIP && m->variant <= MER_VISION_EVA02, "mer_clip_vision_forward: variant %d",
+              m->variant);
+  MER_REQUIRE(m->variant != MER_VISION_CLIP ? (m->pre_ln_g == nullptr && m->proj_dim == D)
+                                            : (m->pre_ln_g && m->post_ln_g && m->proj_w),
+              "mer_clip_vision_forward: variant %d operands", m->variant);
+  if (eva02) {
+    MER_REQUIRE(m->rope_cos && m->rope_sin && m->ffn_norms && m->post_ln_g && m->post_ln_b,
+                "mer_clip_vision_forward: EVA02 needs rope tables, FFN norms and fc_norm");
+    MER_REQUIRE(m->rope_rows == p.P, "mer_clip_vision_forward: EVA02 rope table of %d rows for %d patches",
+                m->rope_rows, p.P);
+    MER_REQUIRE(m->ffn <= 3 * D && m->ffn <= 4096, "mer_clip_vision_forward: EVA02 FFN width %d (up to min(3 x %d, 4096))",
+                m->ffn, D);
+    MER_REQUIRE(mer_attention_f16_supported(p.tokens),
+                "mer_clip_vision_forward: EVA02 needs the fp16 attention rows (%d tokens)", p.tokens);
+    for (int l = 0; l < m->n_layers; ++l)
+      MER_REQUIRE(m->ffn_norms[l].g && m->ffn_norms[l].b, "mer_clip_vision_forward: EVA02 FFN norm %d is NULL", l);
+  }
   char* ws = static_cast<char*>(workspace);
   float* x = reinterpret_cast<float*>(ws + p.off_x);
   float* xn = reinterpret_cast<float*>(ws + p.off_xn);
@@ -382,17 +434,11 @@ int mer_clip_vision_forward(const MerClipVisionModel* m, const uint8_t* frames_b
     g.mode = MER_GEMM_TF32;
     MER_TRY(mer_gemm_launch(&g, stream));
   }
-  const bool dinov2 = m->variant == MER_VISION_DINOV2;
-  MER_REQUIRE(m->variant >= MER_VISION_CLIP && m->variant <= MER_VISION_EMBED_ONLY, "mer_clip_vision_forward: variant %d",
-              m->variant);
-  MER_REQUIRE(m->variant != MER_VISION_CLIP ? (m->pre_ln_g == nullptr && m->proj_dim == D)
-                                            : (m->pre_ln_g && m->post_ln_g && m->proj_w),
-              "mer_clip_vision_forward: variant %d operands", m->variant);
   if (m->variant == MER_VISION_EMBED_ONLY) {  // the embedding output (hidden_states[0]) for a host-orchestrated stack
     MER_CUDA_CHECK(cudaMemcpyAsync(out_embeds, x, (size_t)p.M * D * 4, cudaMemcpyDeviceToDevice, stream));
     return 0;
   }
-  if (!dinov2)
+  if (m->variant == MER_VISION_CLIP)
     MER_TRY(mer_layernorm_launch(x, m->pre_ln_g, m->pre_ln_b, x, nullptr, nullptr, p.M, D, m->ln_eps, 0, stream));
   MerStackArgs a;
   memset(&a, 0, sizeof(a));
@@ -416,9 +462,25 @@ int mer_clip_vision_forward(const MerClipVisionModel* m, const uint8_t* frames_b
   a.vt = vt;
   a.vt_ld = p.vt_ld;
   a.opt_hidden = opt_hidden;
+  if (eva02) {
+    a.rope_cos = m->rope_cos;
+    a.rope_sin = m->rope_sin;
+    a.rope_rows = m->rope_rows;
+    a.rope_prefix = 1;
+    a.ffn_norms = m->ffn_norms;
+  }
   MER_TRY(mer_run_stack(a, stream));
   if (dinov2)  // hidden_states[-1].sum(dim=1): every token of the last layer's output, per frame
     return mer_segment_reduce_launch(x, offsets, offsets + 1, n_frames, D, MER_SEG_SUM, out_embeds, stream);
+  if (eva02) {  // timm forward_head, global_pool 'avg': mean over the patch rows, then fc_norm
+    int* begins = reinterpret_cast<int*>(qkv);  // the QKV buffer is dead now
+    int* ends = begins + n_frames;
+    float* pooled = reinterpret_cast<float*>(ws + p.off_vt);
+    MER_TRY(mer_frame_spans_launch(begins, ends, n_frames, p.tokens, 1, stream));
+    MER_TRY(mer_segment_reduce_launch(x, begins, ends, n_frames, D, MER_SEG_MEAN, pooled, stream));
+    return mer_layernorm_launch(pooled, m->post_ln_g, m->post_ln_b, out_embeds, nullptr, nullptr, n_frames, D,
+                                m->ln_eps, 0, stream);
+  }
   // class-token rows -> post_layernorm (tf32-rounded: GEMM operand) -> visual_projection
   float* cls = qkv;                        // [n_frames, D]   (the QKV buffer is dead now)
   float* pooled = qkv + (long long)n_frames * D;

@@ -118,5 +118,15 @@ struct MerStackArgs {
   int hidden0_done;          // caller already wrote opt_hidden[0] (post-LN: the un-rounded LN)
   int long_rows;             // 1 (HuBERT / wav2vec2): rows of 506 .. MER_ATT_LONG_MAX tokens take the fp16 V^T kernel
                              // like the 254 .. 505-token rows; 0: they take the kernel of attention.cu
+  // EVA02 (pre-LN F16 / TF32 stacks; zero = absent).  rope_cos / rope_sin [rope_rows, 32]: mer_rope2d_f16 on the fp16
+  // q | k after the QKV GEMM, every sequence max_seqlen tokens of which the first rope_prefix are not rotated.
+  const float* rope_cos;
+  const float* rope_sin;
+  int rope_rows, rope_prefix;
+  // per-layer mlp.norm: FC1 writes fp32 [tokens, 2 * ffn] (gate | x) to h without activation, mer_swiglu_ln writes the
+  // FC2 operand [tokens, ffn] (fp16 or tf32) into the dead qkv buffer (3 * dim >= ffn), FC2 runs at K = ffn
+  const MerNormWeights* ffn_norms;
 };
 int mer_run_stack(const MerStackArgs& a, cudaStream_t stream);
+// eva02.cu: begins[i] = i * step + skip, ends[i] = (i + 1) * step for i < n (device int32)
+int mer_frame_spans_launch(int* begins, int* ends, int n, int step, int skip, cudaStream_t stream);

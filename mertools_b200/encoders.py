@@ -8,6 +8,7 @@ reference spells as ``model(x, output_hidden_states=True).hidden_states`` follow
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -138,13 +139,22 @@ class VitEncoder:
 VIT_PROBE = "encoder.layer.{i}.layernorm_before.weight"
 
 
+class MerNormWeights(C.Structure):
+    _fields_ = [("g", C.c_void_p), ("b", C.c_void_p)]
+
+
 class MerClipVisionModel(C.Structure):
     _fields_ = [("n_layers", C.c_int), ("ln_eps", C.c_float), ("hidden", C.c_int), ("ffn", C.c_int),
                 ("heads", C.c_int), ("patch", C.c_int), ("image", C.c_int), ("proj_dim", C.c_int),
                 ("kpad", C.c_int), ("gemm_mode", C.c_int), ("mean", C.c_float * 3), ("std", C.c_float * 3),
                 ("patch_w", C.c_void_p), ("cls_pos0", C.c_void_p), ("pos_rest", C.c_void_p),
                 ("pre_ln_g", C.c_void_p), ("pre_ln_b", C.c_void_p), ("post_ln_g", C.c_void_p),
-                ("post_ln_b", C.c_void_p), ("proj_w", C.c_void_p), ("layers", C.POINTER(W.MerLayerWeights)), ("variant", C.c_int)]
+                ("post_ln_b", C.c_void_p), ("proj_w", C.c_void_p), ("layers", C.POINTER(W.MerLayerWeights)), ("variant", C.c_int),
+                ("rope_cos", C.c_void_p), ("rope_sin", C.c_void_p), ("rope_rows", C.c_int),
+                ("ffn_norms", C.POINTER(MerNormWeights))]
+
+
+MER_VISION_EVA02 = 3
 
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
@@ -196,7 +206,7 @@ class ClipVisionEncoder:
         self.tokens = (image // p) ** 2 + 1
         self.variant, self.resize = int(variant), int(resize or image)
         self.proj_dim = int(sd["visual_projection.weight"].shape[0]) if variant == 0 else int(D)
-        ffn = int(sd[v + "encoder.layers.0.mlp.fc1.weight"].shape[0])
+        ffn = int(sd[v + "encoder.layers.0.mlp.fc2.weight"].shape[1])
         kpad = (3 * p * p + 31) // 32 * 32
         wflat = np.zeros((D, kpad), np.float32)
         wflat[:, :3 * p * p] = pw.reshape(D, 3 * p * p)
@@ -223,6 +233,18 @@ class ClipVisionEncoder:
             m.post_ln_g = pk.keep(sd[v + "post_layernorm.weight"]).data_ptr()
             m.post_ln_b = pk.keep(sd[v + "post_layernorm.bias"]).data_ptr()
             m.proj_w = pk.keep(sd["visual_projection.weight"], tf32=True).data_ptr()
+        elif self.variant == MER_VISION_EVA02:
+            m.post_ln_g = pk.keep(sd[v + "post_layernorm.weight"]).data_ptr()
+            m.post_ln_b = pk.keep(sd[v + "post_layernorm.bias"]).data_ptr()
+            self.ffn_norms = (MerNormWeights * self.n_layers)()
+            for i in range(self.n_layers):
+                n_ = f"{v}encoder.layers.{i}.mlp.norm."
+                self.ffn_norms[i].g = pk.keep(sd[n_ + "weight"]).data_ptr()
+                self.ffn_norms[i].b = pk.keep(sd[n_ + "bias"]).data_ptr()
+            m.ffn_norms = self.ffn_norms
+            cos, sin = eva02_rope_tables(image // p)
+            m.rope_cos, m.rope_sin = pk.keep(cos).data_ptr(), pk.keep(sin).data_ptr()
+            m.rope_rows = cos.shape[0]
         m.layers = self.layers
         self.model = m
         self.ws, self.ws_resize = _Workspace(self.device), _Workspace(self.device)
@@ -239,7 +261,7 @@ class ClipVisionEncoder:
 
     def preprocess_geometry(self, h, w):
         """(new_h, new_w, crop_y0, crop_x0) of CLIPImageProcessor: shorter edge -> image, center crop
-        (Dinov2Encoder: shorter edge -> 256, then the 224 crop)."""
+        (Dinov2Encoder: shorter edge -> 256, then the 224 crop; Eva02Encoder overrides the crop rule)."""
         nh, nw, _, _ = clip_preprocess_geometry(h, w, self.resize)
         return nh, nw, (nh - self.image) // 2, (nw - self.image) // 2
 
@@ -328,6 +350,100 @@ class Dinov2Encoder(ClipVisionEncoder):
                  mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225)):
         super().__init__(dinov2_to_clip_layout(state_dict, image), device=device, ln_eps=ln_eps, image=image,
                          precision=precision, variant=1, mean=mean, std=std, resize=resize)
+
+
+def eva02_rope_tables(grid, head_dim=64, temperature=10000.0):
+    """(cos, sin) float32 [grid * grid, head_dim / 2] of timm ``RotaryEmbeddingCat(head_dim, in_pixels=False,
+    feat_shape=(grid, grid), ref_feat_shape=(grid, grid))``, one entry per rotated pair (timm repeats each twice):
+    bands[j] = 1 / temperature^(j / nb) (nb = head_dim / 4), patch (r, c) in row-major order, pairs [0, nb) at angle
+    r * bands, pairs [nb, 2 nb) at c * bands.  Built with torch in float32 in timm's order of operations, so the tables
+    are the ones the reference's model holds."""
+    nb = head_dim // 4
+    bands = 1.0 / (temperature ** (torch.arange(0, nb, 1, dtype=torch.int64).to(torch.float32) / nb))
+    t = [torch.arange(grid, dtype=torch.int64).to(torch.float32) / grid * grid for _ in range(2)]
+    pos = torch.stack(torch.meshgrid(*t, indexing="ij"), dim=-1).unsqueeze(-1) * bands   # [g, g, 2, nb]
+    return pos.cos().reshape(grid * grid, 2 * nb).numpy(), pos.sin().reshape(grid * grid, 2 * nb).numpy()
+
+
+EVA02_BLOCK_KEYS = ("norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.q_bias", "attn.v_bias", "attn.proj.weight",
+                    "attn.proj.bias", "norm2.weight", "norm2.bias", "mlp.fc1_g.weight", "mlp.fc1_g.bias",
+                    "mlp.fc1_x.weight", "mlp.fc1_x.bias", "mlp.norm.weight", "mlp.norm.bias", "mlp.fc2.weight",
+                    "mlp.fc2.bias")
+EVA02_TOP_KEYS = ("cls_token", "pos_embed", "patch_embed.proj.weight", "patch_embed.proj.bias", "fc_norm.weight",
+                  "fc_norm.bias")
+
+
+def eva02_to_clip_layout(state_dict):
+    """timm ``Eva`` tensors (eva02_base_patch14_224) re-expressed in the layout of the CLIP tower, for the
+    MER_VISION_EVA02 variant of mer_clip_vision_forward: the fused qkv weight split into q / k / v with the bias
+    q_bias | 0 | v_bias (Eva's k_bias is a zero buffer), the patch-conv bias folded into the patch rows of the position
+    table, fc1 = rows fc1_g | fc1_x, mlp.norm and fc_norm carried as ``mlp.norm.*`` / ``post_layernorm.*``.  Widths come
+    from the tensor shapes.  Keys the model does not use (other than ``head.*``) and missing keys are refused by name."""
+    sd = W._np(state_dict)
+    n = 0
+    while f"blocks.{n}.norm1.weight" in sd:
+        n += 1
+    want = set(EVA02_TOP_KEYS) | {f"blocks.{i}.{k}" for i in range(n) for k in EVA02_BLOCK_KEYS}
+    missing = sorted(want - set(sd))
+    extra = sorted(k for k in set(sd) - want if not k.startswith("head."))
+    if missing or extra or n == 0:
+        raise ValueError(f"not an eva02 state_dict: missing {missing[:8]}{' ...' if len(missing) > 8 else ''}, "
+                         f"unexpected {extra[:8]}{' ...' if len(extra) > 8 else ''}, {n} blocks")
+    f32 = lambda k: np.asarray(sd[k], np.float32)  # noqa: E731
+    pw = f32("patch_embed.proj.weight")
+    D = pw.shape[0]
+    pos = f32("pos_embed").reshape(-1, D).copy()
+    pos[1:] += f32("patch_embed.proj.bias")
+    v = "vision_model."
+    out = {v + "embeddings.patch_embedding.weight": pw, v + "embeddings.class_embedding": f32("cls_token").reshape(D),
+           v + "embeddings.position_embedding.weight": pos,
+           v + "post_layernorm.weight": f32("fc_norm.weight"), v + "post_layernorm.bias": f32("fc_norm.bias")}
+    for i in range(n):
+        s_, d_ = f"blocks.{i}.", f"{v}encoder.layers.{i}."
+        q, k, vv = np.split(f32(s_ + "attn.qkv.weight"), 3, axis=0)
+        for name, w_, b_ in (("q_proj", q, f32(s_ + "attn.q_bias")), ("k_proj", k, np.zeros(D, np.float32)),
+                             ("v_proj", vv, f32(s_ + "attn.v_bias"))):
+            out[d_ + f"self_attn.{name}.weight"], out[d_ + f"self_attn.{name}.bias"] = w_, b_
+        for a, b in (("norm1", "layer_norm1"), ("norm2", "layer_norm2"), ("attn.proj", "self_attn.out_proj"),
+                     ("mlp.norm", "mlp.norm"), ("mlp.fc2", "mlp.fc2")):
+            out[d_ + b + ".weight"], out[d_ + b + ".bias"] = f32(s_ + a + ".weight"), f32(s_ + a + ".bias")
+        out[d_ + "mlp.fc1.weight"] = np.concatenate([f32(s_ + "mlp.fc1_g.weight"), f32(s_ + "mlp.fc1_x.weight")], 0)
+        out[d_ + "mlp.fc1.bias"] = np.concatenate([f32(s_ + "mlp.fc1_g.bias"), f32(s_ + "mlp.fc1_x.bias")], 0)
+    return out
+
+
+EVA02_MEAN = CLIP_MEAN   # OPENAI_CLIP_MEAN / _STD: the registry values of eva02_base_patch14_224.mim_in22k
+EVA02_STD = CLIP_STD
+
+
+def eva02_preprocess_geometry(h, w, size=224, crop_pct=0.9):
+    """(new_h, new_w, crop_y0, crop_x0) of timm's eval transform: torchvision Resize(floor(size / crop_pct)) of the
+    shorter edge (the longer one int(scale * long / short)), then CenterCrop(size) at int(round((new - size) / 2.0))
+    (Python's round-half-even, not the floor of HF's processors)."""
+    scale = int(math.floor(size / crop_pct))
+    nh, nw, _, _ = clip_preprocess_geometry(h, w, scale)
+    return nh, nw, int(round((nh - size) / 2.0)), int(round((nw - size) / 2.0))
+
+
+class Eva02Encoder(ClipVisionEncoder):
+    """timm ``Eva`` (eva02_base_patch14_224.mim_in22k: 12 blocks, hidden 768, patch 14, 257 tokens) with the
+    reference's ``model(batch)`` readout (num_classes=0: mean over the patch rows, then fc_norm) per frame, on the CLIP
+    tower kernels (MER_VISION_EVA02): timm's eval transform on the device (shorter edge -> 248 bicubic, centre crop 224
+    at torchvision's offset, rescale, OPENAI CLIP normalise).  ``frame_features`` returns [N, hidden].
+
+    precision: "f16" (default) or "tf32" operands of the linear layers; attention takes fp16 q | k | V^T in both
+    (profiles/eva02_precision_table.json).  eva02 large / giant (FFN width 2730) are refused by shape.
+
+    Reference: MER2024/feature_extraction/visual/extract_vision_huggingface.py:127-131, 202-210."""
+
+    def __init__(self, state_dict, device="cuda", ln_eps=1e-6, image=224, precision="f16"):
+        assert precision in ("f16", "tf32"), precision
+        super().__init__(eva02_to_clip_layout(state_dict), device=device, ln_eps=ln_eps, image=image,
+                         precision=precision, variant=MER_VISION_EVA02, mean=EVA02_MEAN, std=EVA02_STD,
+                         resize=int(math.floor(image / 0.9)))
+
+    def preprocess_geometry(self, h, w):
+        return eva02_preprocess_geometry(h, w, self.image)
 
 
 class MerResnetConv(C.Structure):

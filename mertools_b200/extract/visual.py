@@ -24,6 +24,7 @@ DINO2_GIANT = "dinov2-giant"
 DATA2VEC_VISUAL = "data2vec-vision-base-ft1k"
 VIDEOMAE_BASE = "videomae-base"
 VIDEOMAE_LARGE = "videomae-large"
+EVACLIP_VIT = "eva02_base_patch14_224.mim_in22k"
 
 
 def func_read_frames(face_dir, vid):
@@ -120,6 +121,10 @@ class VisualExtractor:
             from .dinov2_giant import Dinov2GiantEncoder
             self.enc = Dinov2GiantEncoder(state_dict, device=device)
             self.feature_dim = self.enc.hidden
+        elif "blocks.0.mlp.fc1_g.weight" in state_dict:  # timm Eva (eva02_base_patch14_224; :127-131, 202-210)
+            from ..encoders import Eva02Encoder
+            self.enc = Eva02Encoder(state_dict, device=device)
+            self.feature_dim = self.enc.hidden
         elif "encoder.layer.0.layer_scale1.lambda1" in state_dict:  # HF Dinov2Model (dinov2-large; :135-145)
             from ..encoders import Dinov2Encoder
             self.enc = Dinov2Encoder(state_dict, device=device)
@@ -207,6 +212,9 @@ def main(params, config=None, clips_per_launch=32):
     if params.model_name in (VIDEOMAE_BASE, VIDEOMAE_LARGE):                    # :147-159: 16 frames -> 8 tubelet rows
         from .videomae import VideoMaeExtractor
         ext = VideoMaeExtractor.from_pretrained(model_dir, device=f"cuda:{params.gpu}")
+    elif params.model_name == EVACLIP_VIT:
+        ext = VisualExtractor(load_timm_state_dict(timm_checkpoint_path(config, params.model_name)),
+                              device=f"cuda:{params.gpu}")
     else:
         ext = VisualExtractor(common.load_hf_state_dict(model_dir), device=f"cuda:{params.gpu}")
         if params.model_name == DATA2VEC_VISUAL:   # processor settings from the checkpoint's preprocessor_config.json
@@ -225,6 +233,16 @@ def main(params, config=None, clips_per_launch=32):
         files = [os.path.join(save_dir, f"{vid}.npy") for vid in chunk]
         ext.extract_clips(clips, params.feature_level, nframe=nframe, save_files=files)
         print(f"Processed {min(s + clips_per_launch, len(vids))}/{len(vids)} videos")
+
+
+def timm_checkpoint_path(config, model_name):
+    """The reference's timm weights file (:128): PATH_TO_PRETRAINED_MODELS/timm/<model_name>/model.safetensors."""
+    return os.path.join(config.PATH_TO_PRETRAINED_MODELS, f"timm/{model_name}/model.safetensors")
+
+
+def load_timm_state_dict(path):
+    from safetensors.torch import load_file
+    return load_file(path)
 
 
 def build_parser():

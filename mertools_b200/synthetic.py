@@ -953,3 +953,31 @@ def electra_state_dict(cfg, seed=51, scale=1.0, pretraining=False):
     g.linear("discriminator_predictions.dense", d, d, 0.02)
     g.linear("discriminator_predictions.dense_prediction", 1, d, 0.02)
     return g.sd
+
+
+def eva02_state_dict(seed=27, layers=12, scale=1.0, hidden=768, patch=14, image=224):
+    """Keys of timm ``Eva`` as ``create_model('eva02_base_patch14_224', num_classes=0)`` holds them (hidden 768, 12
+    heads, patch 14, 257 tokens, SwiGLU hidden int(768 * 4 * 2 / 3) = 2048 with its LayerNorm, fc_norm; the zero
+    k_bias and the rotary table are non-persistent buffers, so not keys).  ``scale`` multiplies every block matrix
+    (stress checkpoints)."""
+    g = _Gen(seed)
+    d, hf = hidden, int(hidden * 4 * 2 / 3)
+    g.normal("cls_token", (1, 1, d), 0.02)
+    g.normal("pos_embed", (1, (image // patch) ** 2 + 1, d), 0.02)
+    g.normal("patch_embed.proj.weight", (d, 3, patch, patch), 0.02)
+    g.normal("patch_embed.proj.bias", (d,), 0.02)
+    std = 0.02 * scale
+    for i in range(layers):
+        p = f"blocks.{i}."
+        g.ln(p + "norm1", d)
+        g.normal(p + "attn.qkv.weight", (3 * d, d), std)
+        g.normal(p + "attn.q_bias", (d,), 0.02)
+        g.normal(p + "attn.v_bias", (d,), 0.02)
+        g.linear(p + "attn.proj", d, d, std)
+        g.ln(p + "norm2", d)
+        g.linear(p + "mlp.fc1_g", hf, d, std)
+        g.linear(p + "mlp.fc1_x", hf, d, std)
+        g.ln(p + "mlp.norm", hf)
+        g.linear(p + "mlp.fc2", d, hf, std)
+    g.ln("fc_norm", d)
+    return g.sd
