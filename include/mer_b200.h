@@ -856,8 +856,12 @@ typedef struct MerFusionDims {
   int audio_dim, text_dim, video_dim; /* 768 each for the base encoders */
   int hidden;                         /* a multiple of 4, <= 256 */
   int out1;                           /* emotion classes (6) */
-  int out2;                           /* valence outputs (1) */
+  int out2;                           /* valence outputs (1), or 0: see below */
 } MerFusionDims;
+/* Emotion-only heads (out2 == 0: the MER2024 / MER2025 / MER2026 dataloaders, nn.Linear(hidden, 0) as fc_out_2).
+ * Accepted by every fusion entry point, utterance, frame-level and top-N alike.  fc_out_2.weight / .bias are two
+ * empty segments at the end of the flat layout (still the state_dict order), the loss is CE alone (loss_out[1] = 0,
+ * loss_out[2] = the CE term), and vals, vals_out and d_vals may be NULL -- only when out2 == 0. */
 
 MER_API long long mer_fusion_param_count(const MerFusionDims* dims);
 MER_API long long mer_fusion_workspace_bytes(const MerFusionDims* dims, int max_batch);

@@ -269,7 +269,7 @@ fus_dropout_mask_kernel(float* mask, long long n, float p, unsigned long long se
 
 int check_dims(const MerFusionDims* d, int B) {
   MER_REQUIRE(d && d->hidden > 0 && d->hidden <= 256 && d->out1 > 0 && d->out1 <= 16 &&
-                  d->out2 > 0 && d->out2 <= 4 && d->audio_dim > 0 && d->text_dim > 0 &&
+                  d->out2 >= 0 && d->out2 <= 4 && d->audio_dim > 0 && d->text_dim > 0 &&
                   d->video_dim > 0,
               "mer_fusion: unsupported dims (hidden <= 256, out1 <= 16, out2 <= 4)");
   MER_REQUIRE(B > 0 && B <= 65535, "mer_fusion: batch %d out of range", B);
@@ -651,7 +651,7 @@ TopnScratch topn_carve(const MerFusionTopnDims& d, int B, float* base) {
 
 int topn_check(const MerFusionTopnDims* d, int B) {
   MER_REQUIRE(d && d->n_feats >= 1 && d->n_feats <= TOPN_MAX && d->hidden > 0 && d->hidden <= 256 && d->out1 > 0 &&
-                  d->out1 <= 16 && d->out2 > 0 && d->out2 <= 4,
+                  d->out1 <= 16 && d->out2 >= 0 && d->out2 <= 4,
               "mer_fusion_topn: unsupported dims (1..18 features, hidden <= 256, out1 <= 16, out2 <= 4)");
   for (int m = 0; m < d->n_feats; ++m) MER_REQUIRE(d->feat_dims[m] > 0, "mer_fusion_topn: feature %d has no width", m);
   MER_REQUIRE(B > 0 && B <= 65535, "mer_fusion_topn: batch %d out of range", B);
@@ -737,7 +737,7 @@ int mer_fusion_frm_forward(const MerFusionDims* d, const float* params, const fl
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int T[3] = {seq_a, seq_t, seq_v};
   if (int rc = frm_check(d, B, T)) return rc;
-  MER_REQUIRE(params && audios && texts && videos && workspace && features && emos_out && vals_out,
+  MER_REQUIRE(params && audios && texts && videos && workspace && features && emos_out && (vals_out || d->out2 == 0),
               "mer_fusion_frm_forward: null operand");
   MER_REQUIRE(workspace_bytes >= frm_scratch_floats(*d, B, T) * 4, "mer_fusion_frm_forward: workspace too small");
   const FrmLayout L = make_frm_layout(*d);
@@ -767,8 +767,8 @@ int mer_fusion_frm_fwd_bwd(const MerFusionDims* d, const float* params, float* g
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int T[3] = {seq_a, seq_t, seq_v};
   if (int rc = frm_check(d, B, T)) return rc;
-  MER_REQUIRE(params && grads && audios && texts && videos && emos && vals && workspace && loss_out &&
-                  features && emos_out && vals_out && step_counter,
+  MER_REQUIRE(params && grads && audios && texts && videos && emos && (vals || d->out2 == 0) && workspace && loss_out &&
+                  features && emos_out && (vals_out || d->out2 == 0) && step_counter,
               "mer_fusion_frm_fwd_bwd: null operand");
   MER_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "mer_fusion_frm_fwd_bwd: dropout %f", dropout_p);
   MER_REQUIRE(workspace_bytes >= frm_scratch_floats(*d, B, T) * 4, "mer_fusion_frm_fwd_bwd: workspace too small");
@@ -879,9 +879,10 @@ int mer_fusion_topn_step(const MerFusionTopnDims* d, const float* params, float*
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (int rc = topn_check(d, B)) return rc;
   const bool train = emos != nullptr;
-  MER_REQUIRE(params && feats && workspace && features && emos_out && vals_out, "mer_fusion_topn_step: null operand");
-  MER_REQUIRE(!train || (grads && vals && loss_out && step_counter), "mer_fusion_topn_step: training needs grads, "
-                                                                     "vals, loss_out and step_counter");
+  MER_REQUIRE(params && feats && workspace && features && emos_out && (vals_out || d->out2 == 0),
+              "mer_fusion_topn_step: null operand");
+  MER_REQUIRE(!train || (grads && (vals || d->out2 == 0) && loss_out && step_counter),
+              "mer_fusion_topn_step: training needs grads, vals, loss_out and step_counter");
   MER_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "mer_fusion_topn_step: dropout %f", dropout_p);
   MER_REQUIRE(workspace_bytes >= topn_scratch_floats(*d, B) * 4, "mer_fusion_topn_step: workspace too small");
   const int N = d->n_feats, H = d->hidden;

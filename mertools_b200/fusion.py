@@ -100,9 +100,39 @@ def param_shapes(audio_dim, text_dim, video_dim, hidden, out1, out2, feat_type="
     return shapes
 
 
-class FusionNet:
+class _Replicated:
+    """Data-parallel bookkeeping shared by FusionNet and TopnFusionNet: both keep params / exp_avg / exp_avg_sq /
+    step_counter as device tensors, and the gradient with the three loss scalars behind it as ``_grads_loss``."""
+
+    def broadcast_from(self, src=0):
+        """Make every rank a replica of rank ``src`` (parameters, Adam moments, step counter): SURVEY.md §8e
+        'identical initial weights (broadcast once)'."""
+        import torch.distributed as dist
+        for buf in (self.params, self.exp_avg, self.exp_avg_sq, self.step_counter):
+            dist.broadcast(buf, src)
+        self._replicas_checked = False
+        return self
+
+    def check_replicas(self, world):
+        """Once per model: the ranks must hold identical parameters, or the all-reduced gradient trains W
+        different models.  One small all-reduce of (sum, sum of squares) min against max."""
+        if getattr(self, "_replicas_checked", False):
+            return
+        import torch.distributed as dist
+        sig = torch.stack([self.params.double().sum(), (self.params.double() ** 2).sum()])
+        lo, hi = sig.clone(), sig.clone()
+        dist.all_reduce(lo, op=dist.ReduceOp.MIN)
+        dist.all_reduce(hi, op=dist.ReduceOp.MAX)
+        if not torch.equal(lo, hi):
+            raise RuntimeError(f"{type(self).__name__}: the data-parallel ranks hold different parameters "
+                               "(call broadcast_from(0) after construction / load_state_dict)")
+        self._replicas_checked = True
+
+
+class FusionNet(_Replicated):
     """Device-resident Attention fusion model.  feat_type 'utt': MLP encoders on [B, D] features;
-    'frm_align' / 'frm_unalign': LSTM encoders on [B, T, D] sequences (attention.py:25-33)."""
+    'frm_align' / 'frm_unalign': LSTM encoders on [B, T, D] sequences (attention.py:25-33).  output_dim2 = 0 is the
+    emotion-only head of the MER2024 / 25 / 26 dataloaders: vals_out is [B, 0] and the loss is CE alone."""
 
     def __init__(self, audio_dim=768, text_dim=768, video_dim=768, hidden_dim=128, output_dim1=6,
                  output_dim2=1, dropout=0.0, grad_clip=-1.0, device="cuda", max_batch=4096, seed=0,
@@ -334,31 +364,6 @@ class FusionNet:
         return self.loss, st["emos"], st["vals"]
 
 
-    # ---- data parallelism ------------------------------------------------------------------------
-    def broadcast_from(self, src=0):
-        """Make every rank a replica of rank ``src`` (parameters, Adam moments, step counter): SURVEY.md §8e
-        'identical initial weights (broadcast once)'."""
-        import torch.distributed as dist
-        for buf in (self.params, self.exp_avg, self.exp_avg_sq, self.step_counter):
-            dist.broadcast(buf, src)
-        self._replicas_checked = False
-        return self
-
-    def check_replicas(self, world):
-        """Once per model: the ranks must hold identical parameters, or the all-reduced gradient trains W
-        different models.  One small all-reduce of (sum, sum of squares) min against max."""
-        if getattr(self, "_replicas_checked", False):
-            return
-        import torch.distributed as dist
-        sig = torch.stack([self.params.double().sum(), (self.params.double() ** 2).sum()])
-        lo, hi = sig.clone(), sig.clone()
-        dist.all_reduce(lo, op=dist.ReduceOp.MIN)
-        dist.all_reduce(hi, op=dist.ReduceOp.MAX)
-        if not torch.equal(lo, hi):
-            raise RuntimeError("FusionNet: the data-parallel ranks hold different parameters "
-                               "(call broadcast_from(0) after construction / load_state_dict)")
-        self._replicas_checked = True
-
     # ---- the two halves of the autograd node (utterance-level net) -----------------------------------
     def forward_train(self, a, t, v, ext_masks=None):
         """Train-mode forward (dropout from (seed, step_counter) or ext_masks) -> (features, emos_out, vals_out)."""
@@ -390,9 +395,9 @@ class MerFusionTopnDims(C.Structure):
                 ("out2", C.c_int)]
 
 
-class TopnFusionNet:
+class TopnFusionNet(_Replicated):
     """Attention_TOPN (MER2026_Track1/toolkit/models/attention_topn.py): the utterance-level fusion net over
-    N <= 18 features ``batch['feat0'] .. batch['feat{N-1}']`` ([B, feat_dims[i]] each)."""
+    N <= 18 features ``batch['feat0'] .. batch['feat{N-1}']`` ([B, feat_dims[i]] each).  output_dim2 may be 0."""
 
     def __init__(self, feat_dims, hidden_dim=128, output_dim1=6, output_dim2=1, dropout=0.0, grad_clip=-1.0,
                  device="cuda", seed=0):
@@ -425,9 +430,12 @@ class TopnFusionNet:
             self.shapes[f"{l}.weight"], self.shapes[f"{l}.bias"] = (o, H), (o,)
         assert sum(int(np.prod(s)) for s in self.shapes.values()) == self.n_params
         z = lambda: torch.zeros(self.n_params, dtype=torch.float32, device=self.device)  # noqa: E731
-        self.params, self.grads, self.exp_avg, self.exp_avg_sq = z(), z(), z(), z()
+        self.params, self.exp_avg, self.exp_avg_sq = z(), z(), z()
+        # as in FusionNet: the gradient and the three loss scalars are ONE all-reduce under data parallelism
+        self._grads_loss = torch.zeros(self.n_params + 4, dtype=torch.float32, device=self.device)
+        self.grads = self._grads_loss[:self.n_params]
+        self.loss = self._grads_loss[self.n_params:self.n_params + 3]
         self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self.loss = torch.zeros(3, dtype=torch.float32, device=self.device)
         self.ws = torch.empty(0, dtype=torch.uint8, device=self.device)
         self.training = True
 
@@ -437,6 +445,9 @@ class TopnFusionNet:
 
     def eval(self):
         return self.train(False)
+
+    def parameters(self):
+        return [self.params]
 
     def named_views(self, flat=None):
         flat = self.params if flat is None else flat
@@ -458,7 +469,7 @@ class TopnFusionNet:
             dst.copy_(src.to(self.device, torch.float32))
         return self
 
-    def _run(self, feats, emo, val, ext_masks, world):
+    def _run(self, feats, emo, val, ext_masks, world, global_batch=None):
         B = feats[0].shape[0]
         need = int(L.lib().mer_fusion_topn_workspace_bytes(C.byref(self.dims), B))
         if self.ws.numel() < need:
@@ -471,7 +482,8 @@ class TopnFusionNet:
         d = self.dims
         out = [torch.empty(B, n, dtype=torch.float32, device=self.device) for n in (d.hidden, d.out1, d.out2)]
         L.check(self._step(C.byref(d), L.ptr(self.params), L.ptr(self.grads), C.cast(fp, C.c_void_p), L.ptr(emo),
-                           L.ptr(val), B, 1.0 / (B * world), self.dropout if emo is not None else 0.0,
+                           L.ptr(val), B, 1.0 / (global_batch if global_batch is not None else B * world),
+                           self.dropout if emo is not None else 0.0,
                            _dist_seed(self.seed, world),
                            L.ptr(self.step_counter), C.cast(mp, C.c_void_p) if mp is not None else None,
                            L.ptr(self.ws), self.ws.numel(), L.ptr(self.loss), L.ptr(out[0]), L.ptr(out[1]),
@@ -487,13 +499,17 @@ class TopnFusionNet:
     __call__ = forward
 
     def train_step(self, feats, emo, val, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, world_size=1,
-                   ext_masks=None):
-        """One optimisation step (forward, CE + MSE, backward, optional all-reduce, Adam)."""
+                   ext_masks=None, global_batch=None):
+        """One optimisation step (forward, CE + MSE, backward, optional all-reduce, Adam).  world_size > 1: this rank's
+        slice of a data-parallel batch of ``global_batch`` rows (default: batch * world_size); the gradient and the
+        loss returned are the global ones."""
         assert emo.dtype == torch.int64 and val.dtype == torch.float32
-        _, eo, vo = self._run(feats, emo.contiguous(), val.contiguous(), ext_masks, world_size)
+        if world_size > 1:
+            self.check_replicas(world_size)
+        _, eo, vo = self._run(feats, emo.contiguous(), val.contiguous(), ext_masks, world_size, global_batch)
         if world_size > 1:
             import torch.distributed as dist
-            dist.all_reduce(self.grads)
+            dist.all_reduce(self._grads_loss)  # SUM: gradient and loss terms already carry 1 / global_batch
         L.check(self._adam(L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg), L.ptr(self.exp_avg_sq),
                            self.n_params, lr, betas[0], betas[1], eps, weight_decay, 1.0,
                            self.grad_clip if self.grad_clip != -1 else 0.0, L.ptr(self.step_counter), L.stream_ptr()))
@@ -522,6 +538,22 @@ def reference_init(feat_type, audio_dim, text_dim, video_dim, hidden, out1, out2
                 take(f"{e}.{l}", nn.Linear(k, hidden))
     for l, o in (("fc_att", 3), ("fc_out_1", out1), ("fc_out_2", out2)):
         take(l, nn.Linear(hidden, o))
+    return sd
+
+
+def reference_init_topn(feat_dims, hidden, out1, out2):
+    """reference_init for Attention_TOPN: torch's own nn.Linear constructors on the CPU in the order
+    Attention_TOPN.__init__ builds them (attention_topn.py:27-50): encoder0 .. encoder{N-1} (MLPEncoder: linear_1..3),
+    attention_mlp, fc_att, fc_out_1, fc_out_2 -- nn.Linear(hidden, 0) when out2 == 0, an empty weight and bias."""
+    nn = torch.nn
+    sd = {}
+    for e, d in [(f"encoder{i}", d) for i, d in enumerate(feat_dims)] + [("attention_mlp", hidden * len(feat_dims))]:
+        for l, k in (("linear_1", d), ("linear_2", hidden), ("linear_3", hidden)):
+            for n, v in nn.Linear(k, hidden).state_dict().items():
+                sd[f"{e}.{l}.{n}"] = v
+    for l, o in (("fc_att", len(feat_dims)), ("fc_out_1", out1), ("fc_out_2", out2)):
+        for n, v in nn.Linear(hidden, o).state_dict().items():
+            sd[f"{l}.{n}"] = v
     return sd
 
 
@@ -619,7 +651,11 @@ class get_models(torch.nn.Module):  # noqa: N801 -- the reference's name (toolki
         if args.model == "attention_topn":  # MER2026 toolkit: args.audio_dim holds the list of feature widths
             net = TopnFusionNet(args.audio_dim, args.hidden_dim, args.output_dim1, args.output_dim2,
                                 dropout=args.dropout, grad_clip=args.grad_clip,
-                                device=getattr(args, "device", "cuda"))
+                                device=getattr(args, "device", "cuda"), seed=getattr(args, "seed", 0))
+            # the reference's initial weights, drawn here and not in TopnFusionNet.__init__: callers that construct
+            # the net directly and load their own state dict draw nothing from torch's generator
+            net.load_state_dict(reference_init_topn(args.audio_dim, args.hidden_dim, args.output_dim1,
+                                                    args.output_dim2))
             object.__setattr__(self, "model", net)
             return
         assert args.model == "attention", "only the Attention / Attention_TOPN fusion nets are on the H100 path"
@@ -670,14 +706,27 @@ def mer2023_calculate_results(emo_probs=(), emo_labels=(), val_preds=(), val_lab
     return res, f"f1:{f1:.4f}_acc:{acc:.4f}_val:{mse:.4f}"
 
 
+def mer2026_calculate_results(emo_probs=(), emo_labels=(), val_preds=(), val_labels=()):
+    """MER2026_Track1/toolkit/dataloader/mer2026.py:132-145 (MER2024 / MER2025 have the same rule): emotion metrics
+    only, the valence arguments are ignored."""
+    from sklearn.metrics import accuracy_score, f1_score
+    emo_preds = np.argmax(emo_probs, 1)
+    acc = accuracy_score(emo_labels, emo_preds)
+    f1 = f1_score(emo_labels, emo_preds, average="weighted")
+    return dict(emoprobs=emo_probs, emolabels=emo_labels, emoacc=acc, emofscore=f1), f"f1:{f1:.4f}_acc:{acc:.4f}"
+
+
 def train_or_eval_model(args, model, reg_loss, cls_loss, dataloader, epoch, optimizer=None, train=False,
                         calculate_results=None, world_size=1):
     """main-release.py:17-87: same arguments, same ``save_results`` dict (names, loss, then the keys of
-    ``dataloader_class.calculate_results``; default: the MER2023 rule).  With a ``torch.optim`` optimizer this IS the
+    ``dataloader_class.calculate_results``; default: the MER2023 rule).  The regression loss and the valence
+    predictions enter only when ``args.output_dim2 != 0`` (MER2026_Track1/main-release.py:49-57); pass
+    ``mer2026_calculate_results`` for the MER2024 / 25 / 26 corpora.  With a ``torch.optim`` optimizer this IS the
     reference loop (zero_grad, forward, ``cls_loss + reg_loss``, backward, clip_grad_value_, step) running on the
     autograd node; with this module's ``Adam`` holder each training batch is one fused FusionNet.train_step."""
     vidnames, val_preds, val_labels, emo_probs, emo_labels, losses = [], [], [], [], [], []
     assert not train or optimizer is not None
+    has_val = getattr(args, "output_dim2", 1) != 0
     fused = train and isinstance(optimizer, Adam)
     net = getattr(model, "net", None) or getattr(getattr(model, "model", None), "net", None) or \
         getattr(model, "model", model)
@@ -691,18 +740,25 @@ def train_or_eval_model(args, model, reg_loss, cls_loss, dataloader, epoch, opti
             batch[key] = batch[key].cuda()
         emos, vals = emos.cuda(), vals.cuda()
         if fused:
-            loss3, emos_out, vals_out = net.train_step(
-                batch["audios"], batch["texts"], batch["videos"], emos.long(), vals.float().view(-1, 1),
-                lr=optimizer.lr, betas=optimizer.betas, eps=optimizer.eps,
-                weight_decay=optimizer.weight_decay, world_size=world_size)
+            kw = dict(lr=optimizer.lr, betas=optimizer.betas, eps=optimizer.eps, weight_decay=optimizer.weight_decay,
+                      world_size=world_size)
+            if isinstance(net, TopnFusionNet):
+                feats = [batch[f"feat{i}"] for i in range(len(net.feat_dims))]
+                loss3, emos_out, vals_out = net.train_step(feats, emos.long(), vals.float().view(-1, 1), **kw)
+            else:
+                loss3, emos_out, vals_out = net.train_step(
+                    batch["audios"], batch["texts"], batch["videos"], emos.long(), vals.float().view(-1, 1), **kw)
             loss = loss3[2]
         else:
             _, emos_out, vals_out, interloss = model(batch)
-            loss = interloss + cls_loss(emos_out, emos) + reg_loss(vals_out, vals)
+            loss = interloss + cls_loss(emos_out, emos)
+            if has_val:
+                loss = loss + reg_loss(vals_out, vals)
         emo_probs.append(emos_out.data.cpu().numpy())
         emo_labels.append(emos.data.cpu().numpy())
-        val_preds.append(vals_out.data.cpu().numpy())
-        val_labels.append(vals.data.cpu().numpy())
+        if has_val:
+            val_preds.append(vals_out.data.cpu().numpy())
+            val_labels.append(vals.data.cpu().numpy())
         losses.append(loss.data.cpu().numpy())
         if train and not fused:
             loss.backward()
@@ -711,7 +767,8 @@ def train_or_eval_model(args, model, reg_loss, cls_loss, dataloader, epoch, opti
                 torch.nn.utils.clip_grad_value_([p for p in model.parameters() if p.requires_grad], clip)
             optimizer.step()
     emo_probs, emo_labels = np.concatenate(emo_probs), np.concatenate(emo_labels)
-    val_preds, val_labels = np.concatenate(val_preds), np.concatenate(val_labels)
+    if has_val:
+        val_preds, val_labels = np.concatenate(val_preds), np.concatenate(val_labels)
     results, _ = (calculate_results or mer2023_calculate_results)(emo_probs, emo_labels, val_preds, val_labels)
     return dict(names=vidnames, loss=np.mean(losses), **results)
 

@@ -1,6 +1,10 @@
 """Attention-fusion training CLI — H100 mirror of MERBench/main-release.py for
 ``--model attention --feat_type utt --dataset MER2023`` (the configuration of SURVEY.md §8 rows
-a9-a12).  Same flags (:93-124), same hyper-parameter handling (model-tune.yaml ``attention`` grid or
+a9-a12), and of the Track 1 trainers of the three later challenges (MER2024/main-release.py,
+MER2025/MER2025_Track1/main-release.py, MER2026/MER2026_Track1/main-release.py: one script up to an unused import) for
+``--dataset MER2024 | MER2025 | MER2026`` with ``--model attention`` or ``--model attention_topn --fusion_topn n
+--fusion_modality AVT | AV | AT | VT``.  Those corpora train an emotion-only head (output_dim2 = 0, metric 'emo',
+toolkit/dataloader/mer2026.py:26-28) and have one test set, test1.  Same flags (:93-124), same hyper-parameter handling (model-tune.yaml ``attention`` grid or
 ``--hyper_path``, :159-165), same label / feature file formats (toolkit/dataloader/mer2023.py:82-104,
 toolkit/utils/read_data.py:15-41,92-97), same 5-fold protocol (mer2023.py:108-134), metrics
 (toolkit/utils/metric.py) and result files ``cv_*.npz`` / ``test{j}_*.npz`` (:256-272).
@@ -27,23 +31,100 @@ import numpy as np
 import torch
 
 from . import shard
-from .fusion import Adam, get_models, mer2023_calculate_results
+from .fusion import Adam, get_models, mer2023_calculate_results, mer2026_calculate_results
 
 EMOS_MER = ["neutral", "angry", "happy", "sad", "worried", "surprise"]      # toolkit/globals.py:2
 EMO2IDX = {e: i for i, e in enumerate(EMOS_MER)}
 ATTENTION_GRID = dict(hidden_dim=[64, 128, 256], dropout=[0.2, 0.3, 0.4, 0.5], grad_clip=[-1.0],
                       lr=[1e-3, 1e-4])                                       # toolkit/model-tune.yaml:76-80
+# the attention_topn entry of model-tune.yaml:108-112 in the MER2024, MER2025_Track1 and MER2026_Track1 trees
+TOPN_GRID = dict(hidden_dim=[64, 128, 256], dropout=[0.2, 0.3, 0.4, 0.5], grad_clip=[-1.0], lr=[1e-3, 1e-4])
+
+# Corpora whose dataloaders (toolkit/dataloader/mer2024.py, mer2025.py, mer2026.py; identical up to the name) read
+# train_corpus / test1_corpus, label every clip {'emo': idx, 'val': -10} and set output_dim1 = 6, output_dim2 = 0,
+# metric_name = 'emo'.
+EMO_CORPORA = ("MER2024", "MER2025", "MER2026")
+
+# Feature rankings, weakest first, that Data_Feat_TOPN takes the top n of (toolkit/globals.py of each tree):
+#   MER2024/toolkit/globals.py:218-231, MER2025/MER2025_Track1/toolkit/globals.py:218-242,
+#   MER2026/MER2026_Track1/toolkit/globals.py:218-240.
+RANK_LISTS = {
+    "MER2024": dict(
+        audio=["eGeMAPS", "VGGish", "Whisper-base", "emotion2vec", "Whisper-large", "wav2vec 2.0-base",
+               "wav2vec 2.0-large", "HUBERT-base", "HUBERT-large"],
+        text=["XLNet-base", "ELECTRA-large", "MOSS-7B", "PERT-large", "PERT-base", "LERT-large", "ELECTRA-base",
+              "LERT-base", "RoBERTa-base", "MacBERT-base", "RoBERTa-large", "ChatGLM2-6B", "MacBERT-large", "BLOOM-7B",
+              "Baichuan-13B"],
+        image=["VideoMAE-base", "EmoNet", "VideoMAE-large", "DINOv2-large", "SENet-FER2013", "ResNet-FER2013",
+               "MANet-RAFDB", "EVA-02-base", "CLIP-base", "VideoMAE-base (VoxCeleb2)", "VideoMAE-base (MER2023)",
+               "CLIP-large"]),
+    "MER2025": dict(
+        audio=["WavLM-base", "wav2vec 2.0-large", "wav2vec 2.0-base", "Whisper-large", "HUBERT-base", "HUBERT-large"],
+        text=["MacBERT-base", "MacBERT-large", "BLOOM-7B", "RoBERTa-large", "RoBERTa-base"],
+        image=["ResNet-FER2013", "DINOv2-large", "SENet-FER2013", "MANet-RAFDB", "CLIP-base", "CLIP-large"]),
+    "MER2026": dict(
+        audio=["WavLM-base", "wav2vec 2.0-base", "wav2vec 2.0-large", "HUBERT-large", "HUBERT-base"],
+        text=["RoBERTa-base", "RoBERTa-large", "MacBERT-base", "MacBERT-large"],
+        image=["VideoMAE-large", "ResNet-FER2013", "EmoNet", "SENet-FER2013", "CLIP-base", "CLIP-large"]),
+}
+# The display name -> feature directory entries of featname_mapping (toolkit/globals.py:145-203, the same in the
+# three trees) that the rank lists above use.
+FEATNAME_DIRS = {
+    "BLOOM-7B": "bloom-7b1", "Baichuan-13B": "Baichuan-13B-Base", "CLIP-base": "clip-vit-base-patch32",
+    "CLIP-large": "clip-vit-large-patch14", "ChatGLM2-6B": "chatglm2-6b", "DINOv2-large": "dinov2-large",
+    "ELECTRA-base": "chinese-electra-180g-base", "ELECTRA-large": "chinese-electra-180g-large",
+    "EVA-02-base": "eva02_base_patch14_224", "EmoNet": "emonet", "HUBERT-base": "chinese-hubert-base",
+    "HUBERT-large": "chinese-hubert-large", "LERT-base": "chinese-lert-base", "LERT-large": "chinese-lert-large",
+    "MANet-RAFDB": "manet", "MOSS-7B": "moss-base-7b", "MacBERT-base": "chinese-macbert-base",
+    "MacBERT-large": "chinese-macbert-large", "PERT-base": "chinese-pert-base", "PERT-large": "chinese-pert-large",
+    "ResNet-FER2013": "resnet50face", "RoBERTa-base": "chinese-roberta-wwm-ext",
+    "RoBERTa-large": "chinese-roberta-wwm-ext-large", "SENet-FER2013": "senet50face", "VGGish": "vggish",
+    "VideoMAE-base": "videomae-base", "VideoMAE-base (MER2023)": "videomae-base-K400-mer2023-299",
+    "VideoMAE-base (VoxCeleb2)": "videomae-base-VoxCeleb2-99", "VideoMAE-large": "videomae-large",
+    "WavLM-base": "wavlm-base", "Whisper-base": "whisper-base", "Whisper-large": "whisper-large-v2",
+    "XLNet-base": "chinese-xlnet-base", "eGeMAPS": "eGeMAPS", "emotion2vec": "emotion2vec",
+    "wav2vec 2.0-base": "chinese-wav2vec2-base", "wav2vec 2.0-large": "chinese-wav2vec2-large",
+}
+# Data_Feat_TOPN's RANK_LIST per --fusion_modality (toolkit/data/feat_data_topn.py:16-24): three lists, not one per
+# modality -- AT takes the text ranking twice, AV the image ranking twice, VT text twice then image.
+FUSION_MODALITIES = {"AVT": ("audio", "text", "image"), "AT": ("audio", "text", "text"),
+                     "AV": ("audio", "image", "image"), "VT": ("text", "text", "image")}
+
+
+def func_name_conversion(display_name, feature_root, suffix="UTT"):
+    """toolkit/utils/functions.py:329-336 (MER2025 / MER2026): ``<dir>_UTT`` when that directory exists under the
+    corpus' feature root, otherwise ``<dir>-UTT``.  MER2024's copy (functions.py:246-253) looks under
+    config.PATH_TO_FEATURES['SIMS'] whatever the corpus; here every corpus looks under its own feature root, which is
+    what the MER2025 / MER2026 copies do and the only root that holds MER2024's features."""
+    d = FEATNAME_DIRS[display_name]
+    return f"{d}_{suffix}" if os.path.exists(os.path.join(feature_root, f"{d}_{suffix}")) else f"{d}-{suffix}"
+
+
+def topn_feature_names(dataset, fusion_topn, fusion_modality, feature_root):
+    """Data_Feat_TOPN (toolkit/data/feat_data_topn.py:16-31): the last ``fusion_topn`` names of each of the three
+    rank lists, in list order, resolved to feature directories -> 3 * fusion_topn names (repeats included)."""
+    assert fusion_topn is not None and fusion_modality in FUSION_MODALITIES, (fusion_topn, fusion_modality)
+    assert 1 <= fusion_topn, fusion_topn
+    names = []
+    for which in FUSION_MODALITIES[fusion_modality]:
+        names.extend(RANK_LISTS[dataset][which][-fusion_topn:])
+    assert len(names) == 3 * fusion_topn, f"a rank list of {dataset} is shorter than --fusion_topn {fusion_topn}"
+    return [func_name_conversion(n, feature_root) for n in names]
 
 
 # ---- data (host side, same file formats as the reference) ---------------------------------------
-def read_names_labels(label_path, data_type, debug=False):
-    """mer2023.py:82-104."""
-    assert data_type in ("train", "test1", "test2", "test3")
+def read_names_labels(label_path, data_type, debug=False, dataset="MER2023"):
+    """mer2023.py:82-104; for MER2024 / 25 / 26 mer2026.py:83-99 (train / test1 only, the valence is always -10)."""
+    emo_only = dataset in EMO_CORPORA
+    assert data_type in (("train", "test1") if emo_only else ("train", "test1", "test2", "test3"))
     corpus = np.load(label_path, allow_pickle=True)[f"{data_type}_corpus"].tolist()
     names, labels = [], []
     for name, label in corpus.items():
         names.append(name)
-        val = label["val"] if ("val" in label and label["val"] != "") else -10
+        if emo_only:
+            val = -10
+        else:
+            val = label["val"] if ("val" in label and label["val"] != "") else -10
         labels.append({"emo": EMO2IDX[label["emo"]], "val": val})
     if debug:
         names, labels = names[:100], labels[:100]
@@ -95,12 +176,18 @@ def random_split_indexes(whole_num, num_folder):
 
 class DeviceSplit:
     """One corpus split resident on the GPU: A/T/V fp32 -- [N, D] for feat_type 'utt', [N, T_m, D] for the
-    frame-level types (shaped exactly as Data_Feat does, feat_data.py:33-44) -- emo int64, val fp32."""
+    frame-level types (shaped exactly as Data_Feat does, feat_data.py:33-44) -- emo int64, val fp32.  For
+    attention_topn: the 3 * fusion_topn utterance-level features ``args.topn_features`` (Data_Feat_TOPN: the mean over
+    time of each clip), as ``feats``."""
 
     def __init__(self, args, names, labels, config, device):
         root = config.PATH_TO_FEATURES[args.dataset]
         feats = []
-        if args.feat_type == "utt":
+        if args.model == "attention_topn":
+            for fname in args.topn_features:
+                fr = os.path.join(root, fname)
+                feats.append(np.stack([read_utt_feature(fr, n) for n in names]).astype(np.float32))
+        elif args.feat_type == "utt":
             for fname in (args.audio_feature, args.text_feature, args.video_feature):
                 fr = os.path.join(root, fname)
                 feats.append(np.stack([read_utt_feature(fr, n) for n in names]).astype(np.float32))
@@ -111,7 +198,9 @@ class DeviceSplit:
             shaped = FF.shape_split(raw[0], raw[1], raw[2], args.feat_type, args.feat_scale)
             feats = [np.array(x).astype(np.float32) for x in shaped]  # torch.FloatTensor(np.array(...)) in the collater
         self.names = names
-        self.a, self.t, self.v = (torch.from_numpy(f).to(device) for f in feats)
+        self.feats = [torch.from_numpy(f).to(device) for f in feats]
+        if args.model != "attention_topn":
+            self.a, self.t, self.v = self.feats
         self.emo = torch.tensor([l["emo"] for l in labels], dtype=torch.int64, device=device)
         self.val = torch.tensor([l["val"] for l in labels], dtype=torch.float32, device=device).view(-1, 1)
         self.dims = tuple(int(f.shape[-1]) for f in feats)
@@ -151,6 +240,21 @@ def get_loaders(n_train, folds, n_tests, batch_size, num_workers=0):
 calculate_results = mer2023_calculate_results  # mer2023.py:137-155
 
 
+def corpus_calculate_results(dataset):
+    """dataloader_class.calculate_results: mer2023.py:137-155, or mer2026.py:132-145 for MER2024 / 25 / 26."""
+    return mer2026_calculate_results if dataset in EMO_CORPORA else mer2023_calculate_results
+
+
+def gain_cv_results(folder_save):
+    """toolkit/utils/metric.py:35-54: the means over the folds' best epochs of the eval metrics that are present."""
+    keys = folder_save[0].keys()
+    out = []
+    for key, label in (("eval_emofscore", "f1"), ("eval_emoacc", "acc"), ("eval_valmse", "val")):
+        if key in keys:
+            out.append(f"{label}:{np.mean([e[key] for e in folder_save]):.4f}")
+    return "_".join(out)
+
+
 def gain_metric_from_results(res, metric_name="emoval"):
     """toolkit/utils/metric.py:15-32."""
     if metric_name == "emoval":
@@ -179,8 +283,12 @@ def _gather_strided(local, n_global, rank, world):
 # ---- one pass over a split (main-release.py:17-87) ------------------------------------------------
 def run_split(args, net, split, loader, optimizer=None, train=False, rank=0, world_size=1):
     """``loader`` yields batches of sample indices in the reference's order.  Training: one fused step per batch
-    (under data parallelism on rows ``rank::world_size`` of it); evaluation: eval forward + the two losses."""
-    dev = split.a.device
+    (under data parallelism on rows ``rank::world_size`` of it); evaluation: eval forward + the losses.  The
+    regression loss and the valence predictions enter only when ``args.output_dim2 != 0`` (MER2026_Track1/
+    main-release.py:49-57)."""
+    dev = split.emo.device
+    topn = args.model == "attention_topn"
+    has_val = args.output_dim2 != 0
     names, emo_probs, val_preds, losses, order = [], [], [], [], []
     net.train(train)
     for b in loader:
@@ -188,34 +296,43 @@ def run_split(args, net, split, loader, optimizer=None, train=False, rank=0, wor
         b = b.to(dev)
         order.append(b)
         mine = b[rank::world_size] if (train and world_size > 1) else b
-        a, t, v = split.a.index_select(0, mine), split.t.index_select(0, mine), split.v.index_select(0, mine)
+        xs = [f.index_select(0, mine) for f in split.feats]
         emo, val = split.emo.index_select(0, mine), split.val.index_select(0, mine)
         if train:
-            loss3, eo, vo = net.train_step(a, t, v, emo, val, lr=optimizer.lr, betas=optimizer.betas,
-                                           eps=optimizer.eps, weight_decay=optimizer.weight_decay,
-                                           world_size=world_size, global_batch=len(b))
+            kw = dict(lr=optimizer.lr, betas=optimizer.betas, eps=optimizer.eps, weight_decay=optimizer.weight_decay,
+                      world_size=world_size, global_batch=len(b))
+            loss3, eo, vo = net.train_step(xs, emo, val, **kw) if topn else net.train_step(*xs, emo, val, **kw)
             losses.append(loss3[2:3].clone())
             if world_size > 1:
-                eo, vo = (_gather_strided(x, len(b), rank, world_size) for x in (eo, vo))
+                eo = _gather_strided(eo, len(b), rank, world_size)
+                if has_val:
+                    vo = _gather_strided(vo, len(b), rank, world_size)
         else:
-            _, eo, vo, _ = net({"audios": a, "texts": t, "videos": v})
-            ce = torch.nn.functional.cross_entropy(eo, emo, reduction="sum") / len(eo)
-            mse = torch.nn.functional.mse_loss(vo, val, reduction="sum") / len(vo)
-            losses.append((ce + mse).view(1))
+            batch = {f"feat{i}": x for i, x in enumerate(xs)} if topn else dict(zip(("audios", "texts", "videos"), xs))
+            _, eo, vo, _ = net(batch)
+            loss = torch.nn.functional.cross_entropy(eo, emo, reduction="sum") / len(eo)
+            if has_val:
+                loss = loss + torch.nn.functional.mse_loss(vo, val, reduction="sum") / len(vo)
+            losses.append(loss.view(1))
         emo_probs.append(eo.clone())
-        val_preds.append(vo.clone())
+        if has_val:
+            val_preds.append(vo.clone())
     order = torch.cat(order)
     emo_probs = torch.cat(emo_probs).cpu().numpy()
-    val_preds = torch.cat(val_preds).cpu().numpy()
     emo_labels = split.emo.index_select(0, order).cpu().numpy()
-    val_labels = split.val.index_select(0, order).cpu().numpy()
-    res, _ = calculate_results(emo_probs, emo_labels, val_preds, val_labels)
+    val_labels = []
+    if has_val:
+        val_preds = torch.cat(val_preds).cpu().numpy()
+        val_labels = split.val.index_select(0, order).cpu().numpy()
+    res, _ = corpus_calculate_results(args.dataset)(emo_probs, emo_labels, val_preds, val_labels)
     return dict(names=names, loss=np.mean(torch.cat(losses).cpu().numpy()), **res)
 
 
 def build_parser():
     p = argparse.ArgumentParser()
     p.add_argument("--dataset", type=str, default="MER2023")
+    p.add_argument("--fusion_topn", type=int, default=None)
+    p.add_argument("--fusion_modality", type=str, default="AVT")
     p.add_argument("--save_root", type=str, default="./saved")
     p.add_argument("--debug", action="store_true", default=False)
     p.add_argument("--audio_feature", type=str, default=None)
@@ -258,13 +375,18 @@ def main(args, config=None, log=None):
     what tests/golden/main_release_golden.npz holds for the unmodified script."""
     if config is None:
         from . import config as config  # noqa: PLW0127
-    assert args.model == "attention" and args.dataset == "MER2023", \
-        "the H100 path covers --model attention --dataset MER2023 (SURVEY.md §8)"
+    assert args.dataset in ("MER2023",) + EMO_CORPORA, \
+        f"the H100 path covers --dataset MER2023 / {' / '.join(EMO_CORPORA)}, not {args.dataset}"
+    assert args.model == "attention" or (args.model == "attention_topn" and args.dataset in EMO_CORPORA), \
+        "the H100 path covers --model attention, and attention_topn on the corpora with feature rankings"
+    topn = args.model == "attention_topn"
     rank, world = _init_distributed(args)
     torch.cuda.set_device(args.gpu)
     device = torch.device("cuda", args.gpu)
     say = print if rank == 0 else (lambda *a, **k: None)
     # pre-compression of the frame-level types (main-release.py:131-142)
+    if topn:
+        assert args.feat_type == "utt", "attention_topn reads utterance-level features (feat_data_topn.py:36-39)"
     if args.feat_type == "utt":
         args.feat_scale = 1
     else:
@@ -272,17 +394,23 @@ def main(args, config=None, log=None):
         for f in (args.audio_feature, args.text_feature, args.video_feature):
             assert f.endswith("FRA"), f"feat_type {args.feat_type} needs frame-level features, got {f}"
         args.feat_scale = 6 if args.feat_type == "frm_align" else 12
+    if args.fusion_topn is not None:
+        args.save_root = f"{args.save_root}-multitop"
     feats = [f for f in (args.audio_feature, args.text_feature, args.video_feature) if f is not None]
     args.save_root = f"{args.save_root}-" + {0: "others", 1: "unimodal", 2: "bimodal", 3: "trimodal"}[len(set(feats))]
     if args.hyper_path is None:
-        cfg = {k: v[random.randint(0, len(v) - 1)] for k, v in ATTENTION_GRID.items()}   # func_random_select
+        grid = TOPN_GRID if topn else ATTENTION_GRID
+        cfg = {k: v[random.randint(0, len(v) - 1)] for k, v in grid.items()}              # func_random_select
     else:
         import yaml
         cfg = yaml.safe_load(open(args.hyper_path))[args.model]
     for k, v in cfg.items():                                                               # merge_args_config
         if getattr(args, k, None) is None:
             setattr(args, k, v)
-    args.output_dim1, args.output_dim2, args.metric_name = 6, 1, "emoval"
+    if args.dataset in EMO_CORPORA:
+        args.output_dim1, args.output_dim2, args.metric_name = 6, 0, "emo"
+    else:
+        args.output_dim1, args.output_dim2, args.metric_name = 6, 1, "emoval"
     say("args: ", args)
     save_resroot = os.path.join(args.save_root, "result")
     if rank == 0:
@@ -290,21 +418,30 @@ def main(args, config=None, log=None):
         os.makedirs(os.path.join(args.save_root, "model"), exist_ok=True)
     feature_name = "+".join(sorted(set(feats)))
     prefix_name = f"features:{feature_name}_dataset:{args.dataset}_model:{args.model}+{args.feat_type}+{args.e2e_name}"
+    if args.fusion_topn is not None:
+        prefix_name += f"_fusiontopn:{args.fusion_topn}_modality:{args.fusion_modality}"
 
     say("====== Reading Data =======")
     label_path = config.PATH_TO_LABEL[args.dataset]
-    names, labels = read_names_labels(label_path, "train", args.debug)
+    if topn:
+        args.topn_features = topn_feature_names(args.dataset, args.fusion_topn, args.fusion_modality,
+                                                config.PATH_TO_FEATURES[args.dataset])
+        say(f"feature number: {len(args.topn_features)}")
+    names, labels = read_names_labels(label_path, "train", args.debug, args.dataset)
     say(f"train: sample number {len(names)}")
     train_split = DeviceSplit(args, names, labels, config, device)
     folds = random_split_indexes(len(names), 5)
     tests = []
-    for dt in ("test1", "test2", "test3"):
-        n, l = read_names_labels(label_path, dt, args.debug)
+    for dt in ("test1",) if args.dataset in EMO_CORPORA else ("test1", "test2", "test3"):
+        n, l = read_names_labels(label_path, dt, args.debug, args.dataset)
         say(f"{dt}: sample number {len(n)}")
         tests.append(DeviceSplit(args, n, l, config, device))
     train_loaders, eval_loaders, test_loaders = get_loaders(len(names), folds, [len(ts) for ts in tests],
                                                             args.batch_size, args.num_workers)
-    args.audio_dim, args.text_dim, args.video_dim = train_split.dims
+    if topn:  # Data_Feat_TOPN.get_featdim: the list of widths, three times
+        args.audio_dim = args.text_dim = args.video_dim = list(train_split.dims)
+    else:
+        args.audio_dim, args.text_dim, args.video_dim = train_split.dims
 
     say("====== Training and Evaluation =======")
     folder_save, folder_duration = [], []
@@ -314,7 +451,7 @@ def main(args, config=None, log=None):
         start_time = name_time = time.time()
         args.seed = random.randint(0, 2 ** 31 - 1)        # dropout-mask stream of this fold's model
         model = get_models(args).cuda()                   # default init from torch's generator, as the reference
-        net = model.net
+        net = model.model if topn else model.net
         if world > 1:
             net.broadcast_from(0)
         optimizer = Adam(lr=args.lr, weight_decay=args.l2)
@@ -336,7 +473,8 @@ def main(args, config=None, log=None):
             if log is not None:
                 log.setdefault("train_loss", []).append(float(train_res["loss"]))
                 log.setdefault("eval_loss", []).append(float(eval_res["loss"]))
-                log.setdefault("test_loss", []).append([float(epoch_store[f"test{j}_loss"]) for j in (1, 2, 3)])
+                log.setdefault("test_loss", []).append([float(epoch_store[f"test{j + 1}_loss"])
+                                                        for j in range(len(tests))])
                 log.setdefault("train_names", []).append(train_res["names"])
                 log.setdefault("eval_names", []).append(eval_res["names"])
         best_index = int(np.argmax(np.array(whole_metrics)))
@@ -352,23 +490,25 @@ def main(args, config=None, log=None):
     if log is not None:
         log["folder_save"] = folder_save
     args.duration = float(np.sum(folder_duration))
-    f1 = np.mean([e["eval_emofscore"] for e in folder_save])
-    acc = np.mean([e["eval_emoacc"] for e in folder_save])
-    mse = np.mean([e["eval_valmse"] for e in folder_save])
-    cv_result = f"f1:{f1:.4f}_acc:{acc:.4f}_val:{mse:.4f}"
-    saved = []
+    cv_result = gain_cv_results(folder_save)
+    saved, contents = [], []
     path = f"{save_resroot}/cv_{prefix_name}_{cv_result}_{name_time}.npz"
     saved.append(path)
+    contents.append({})
     for jj in range(len(tests)):
         emo_labels = folder_save[0][f"test{jj + 1}_emolabels"]
         emo_probs = np.mean(np.array([f[f"test{jj + 1}_emoprobs"] for f in folder_save]), axis=0)
-        val_labels = folder_save[0][f"test{jj + 1}_vallabels"]
-        val_preds = np.mean(np.array([f[f"test{jj + 1}_valpreds"] for f in folder_save]), axis=0)
-        _, test_result = calculate_results(emo_probs, emo_labels, val_preds, val_labels)
+        val_labels, val_preds = [], []
+        if args.output_dim2 != 0:
+            val_labels = folder_save[0][f"test{jj + 1}_vallabels"]
+            val_preds = np.mean(np.array([f[f"test{jj + 1}_valpreds"] for f in folder_save]), axis=0)
+        _, test_result = corpus_calculate_results(args.dataset)(emo_probs, emo_labels, val_preds, val_labels)
         saved.append(f"{save_resroot}/test{jj + 1}_{prefix_name}_{test_result}_{name_time}.npz")
+        # MER2024 / 25 / 26 keep the fold-averaged emotion scores (MER2026_Track1/main-release.py:286-288)
+        contents.append(dict(emo_probs=emo_probs) if args.dataset in EMO_CORPORA else {})
     if rank == 0:
-        for p in saved:
-            np.savez_compressed(p, args=np.array(args, dtype=object))
+        for p, extra in zip(saved, contents):
+            np.savez_compressed(p, **extra, args=np.array(args, dtype=object))
             print(f"save results in {p}")
     return saved
 

@@ -899,6 +899,41 @@ def write_mer2023_corpus(root, n_train=32, n_test=8, dim=768, seed=0, frame_leve
     return label_path, feats
 
 
+# Feature directories of a synthetic MER2026 corpus: every entry of MER2026's three rank lists
+# (main_release.RANK_LISTS), named the way func_name_conversion resolves them -- the face extractors as `<dir>_UTT`,
+# the rest as `<dir>-UTT` -- with a few different widths; videomae-large keeps 2..4 rows per clip (mean over time).
+MER2026_FEATURE_DIRS = {
+    "wavlm-base-UTT": 96, "chinese-wav2vec2-base-UTT": 96, "chinese-wav2vec2-large-UTT": 128,
+    "chinese-hubert-large-UTT": 128, "chinese-hubert-base-UTT": 96,
+    "chinese-roberta-wwm-ext-UTT": 96, "chinese-roberta-wwm-ext-large-UTT": 128, "chinese-macbert-base-UTT": 96,
+    "chinese-macbert-large-UTT": 128,
+    "videomae-large-UTT": 128, "resnet50face_UTT": 64, "emonet_UTT": 40, "senet50face_UTT": 64,
+    "clip-vit-base-patch32-UTT": 64, "clip-vit-large-patch14-UTT": 100,
+}
+
+
+def write_mer2026_corpus(root, n_train=80, n_test=20, seed=0, dims=None):
+    """A MER2024 / 25 / 26-format corpus under ``root``: ``track1_label_6way.npz`` with the ``train_corpus`` /
+    ``test1_corpus`` dicts of toolkit/dataloader/mer2026.py:83-99 (emotion labels only) and N(0,1) float32 ``.npy``
+    utterance features under ``features/<dir>/`` for every directory of ``dims`` (default MER2026_FEATURE_DIRS:
+    name -> width).  Returns (label_path, feature_root)."""
+    import os
+    dims = MER2026_FEATURE_DIRS if dims is None else dims
+    rng = np.random.default_rng(seed)
+    corp = {f"{split}_corpus": {f"{split}_{i:04d}": {"emo": EMOS_MER[int(rng.integers(0, 6))]} for i in range(n)}
+            for split, n in (("train", n_train), ("test1", n_test))}
+    label_path = os.path.join(root, "track1_label_6way.npz")
+    np.savez(label_path, **corp)
+    feats = os.path.join(root, "features")
+    for fname, dim in dims.items():
+        os.makedirs(os.path.join(feats, fname), exist_ok=True)
+        for split in corp.values():
+            for name in split:
+                shape = (int(rng.integers(2, 5)), dim) if fname.startswith("videomae") else (dim,)
+                np.save(os.path.join(feats, fname, name + ".npy"), rng.standard_normal(shape).astype(np.float32))
+    return label_path, feats
+
+
 # ELECTRA (ElectraConfig keywords).  Goldens: ``small`` (the factorised 128-wide embedding + embeddings_project into
 # hidden 256, 4 heads of 64, FFN 1024), ``base`` (embedding_size == hidden_size: BERT's graph) and ``lert_small`` (a
 # hidden-256 BertModel, as chinese-lert-small).  PUBLISHED: the checkpoints' shapes (seeded weights; vocab as given).
