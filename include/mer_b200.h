@@ -855,13 +855,18 @@ MER_API int mer_bert_forward_projected(const MerBertModel* model, const MerBertE
 typedef struct MerFusionDims {
   int audio_dim, text_dim, video_dim; /* 768 each for the base encoders */
   int hidden;                         /* a multiple of 4, <= 256 */
-  int out1;                           /* emotion classes (6) */
+  int out1;                           /* emotion classes (6), or 0: see below */
   int out2;                           /* valence outputs (1), or 0: see below */
 } MerFusionDims;
 /* Emotion-only heads (out2 == 0: the MER2024 / MER2025 / MER2026 dataloaders, nn.Linear(hidden, 0) as fc_out_2).
  * Accepted by every fusion entry point, utterance, frame-level and top-N alike.  fc_out_2.weight / .bias are two
  * empty segments at the end of the flat layout (still the state_dict order), the loss is CE alone (loss_out[1] = 0,
  * loss_out[2] = the CE term), and vals, vals_out and d_vals may be NULL -- only when out2 == 0. */
+/* Regression-only heads (out1 == 0: the CMU-MOSI / MOSEI, SIMS / SIMSv2 and cross-corpus sentiment dataloaders,
+ * nn.Linear(hidden, 0) as fc_out_1).  Accepted by the utterance-level and frame-level entry points when out2 >= 1;
+ * the top-N net refuses it, and out1 == out2 == 0 is refused everywhere.  fc_out_1.weight / .bias are two empty
+ * segments of the flat layout (between fc_att and fc_out_2), the loss is MSE alone (loss_out[0] = 0, loss_out[2] = the
+ * MSE term: emo is never read), and emos, emos_out and d_emos may be NULL -- only when out1 == 0. */
 
 MER_API long long mer_fusion_param_count(const MerFusionDims* dims);
 MER_API long long mer_fusion_workspace_bytes(const MerFusionDims* dims, int max_batch);

@@ -19,6 +19,8 @@ PATH_TO_RAW_AUDIO = {ds: os.path.join(_root(ds), "audio") for ds in DATASETS}
 PATH_TO_RAW_FACE = {ds: os.path.join(_root(ds), "openface_face") for ds in DATASETS}
 PATH_TO_TRANSCRIPTIONS = {ds: os.path.join(_root(ds), "transcription-engchi-polish.csv") for ds in DATASETS}
 PATH_TO_FEATURES = {ds: os.path.join(_root(ds), "features") for ds in DATASETS}
-PATH_TO_LABEL = {ds: os.path.join(_root(ds), "label-6way.npz" if ds == "MER2023" else "label.npz")
-                 for ds in DATASETS}
+# MERBench/config.py:64-73: IEMOCAP's two label sets are label_4way.npz / label_6way.npz (iemocap.py of the
+# preprocessing writes both); here each has its own corpus root, where the reference shares one
+_LABEL_FILES = {"MER2023": "label-6way.npz", "IEMOCAPFour": "label_4way.npz", "IEMOCAPSix": "label_6way.npz"}
+PATH_TO_LABEL = {ds: os.path.join(_root(ds), _LABEL_FILES.get(ds, "label.npz")) for ds in DATASETS}
 PATH_TO_PRETRAINED_MODELS = os.environ.get("MER_PRETRAINED_ROOT", "./tools")

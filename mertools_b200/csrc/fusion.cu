@@ -140,6 +140,7 @@ struct HeadArgs {
   float* loss_terms;   // [B,2]
   float* d_emos; float* d_vals; float* d_att; float* d_cat; float* d_a3;
   int H, O1, O2;
+  int train;           // losses and backward follow the forward (emo may be null when O1 == 0)
   float inv_batch;     // 1 / (batch the loss is averaged over)
 };
 
@@ -178,21 +179,26 @@ fus_head_kernel(const HeadArgs a) {
     if (tid == 0) { dval[c] = s + a.b_o2[c]; a.vals_out[(long long)b * a.O2 + c] = dval[c]; }
   }
   __syncthreads();
-  if (!a.emo) return;  // eval: forward only
+  if (!a.train) return;  // eval: forward only
   if (tid == 0) {
-    // CELoss: NLL(log_softmax) summed / N ; MSELoss: squared error summed / N  (loss.py:11-28)
-    float mx = logits[0];
-    for (int c = 1; c < a.O1; ++c) mx = fmaxf(mx, logits[c]);
-    float se = 0.f;
-    for (int c = 0; c < a.O1; ++c) se += expf(logits[c] - mx);
-    const float lse = mx + logf(se);
-    const int tgt = (int)a.emo[b];
-    a.loss_terms[2 * b + 0] = lse - logits[tgt];
-    for (int c = 0; c < a.O1; ++c) {
-      const float sm = expf(logits[c] - lse);
-      dlog[c] = (sm - (c == tgt ? 1.f : 0.f)) * a.inv_batch;
-      a.d_emos[(long long)b * a.O1 + c] = dlog[c];
+    // CELoss: NLL(log_softmax) summed / N ; MSELoss: squared error summed / N  (loss.py:11-28).  A regression-only
+    // head (O1 == 0) has no CE term: emo is not read and the term is 0.
+    float ce = 0.f;
+    if (a.O1 > 0) {
+      float mx = logits[0];
+      for (int c = 1; c < a.O1; ++c) mx = fmaxf(mx, logits[c]);
+      float se = 0.f;
+      for (int c = 0; c < a.O1; ++c) se += expf(logits[c] - mx);
+      const float lse = mx + logf(se);
+      const int tgt = (int)a.emo[b];
+      ce = lse - logits[tgt];
+      for (int c = 0; c < a.O1; ++c) {
+        const float sm = expf(logits[c] - lse);
+        dlog[c] = (sm - (c == tgt ? 1.f : 0.f)) * a.inv_batch;
+        a.d_emos[(long long)b * a.O1 + c] = dlog[c];
+      }
     }
+    a.loss_terms[2 * b + 0] = ce;
     float mse = 0.f;
     for (int c = 0; c < a.O2; ++c) {
       const float d = dval[c] - a.val[(long long)b * a.O2 + c];
@@ -268,10 +274,10 @@ fus_dropout_mask_kernel(float* mask, long long n, float p, unsigned long long se
 }
 
 int check_dims(const MerFusionDims* d, int B) {
-  MER_REQUIRE(d && d->hidden > 0 && d->hidden <= 256 && d->out1 > 0 && d->out1 <= 16 &&
-                  d->out2 >= 0 && d->out2 <= 4 && d->audio_dim > 0 && d->text_dim > 0 &&
+  MER_REQUIRE(d && d->hidden > 0 && d->hidden <= 256 && d->out1 >= 0 && d->out1 <= 16 &&
+                  d->out2 >= 0 && d->out2 <= 4 && d->out1 + d->out2 > 0 && d->audio_dim > 0 && d->text_dim > 0 &&
                   d->video_dim > 0,
-              "mer_fusion: unsupported dims (hidden <= 256, out1 <= 16, out2 <= 4)");
+              "mer_fusion: unsupported dims (hidden <= 256, out1 <= 16, out2 <= 4, at least one output head)");
   MER_REQUIRE(B > 0 && B <= 65535, "mer_fusion: batch %d out of range", B);
   return 0;
 }
@@ -652,7 +658,7 @@ TopnScratch topn_carve(const MerFusionTopnDims& d, int B, float* base) {
 int topn_check(const MerFusionTopnDims* d, int B) {
   MER_REQUIRE(d && d->n_feats >= 1 && d->n_feats <= TOPN_MAX && d->hidden > 0 && d->hidden <= 256 && d->out1 > 0 &&
                   d->out1 <= 16 && d->out2 >= 0 && d->out2 <= 4,
-              "mer_fusion_topn: unsupported dims (1..18 features, hidden <= 256, out1 <= 16, out2 <= 4)");
+              "mer_fusion_topn: unsupported dims (1..18 features, hidden <= 256, 1 <= out1 <= 16, out2 <= 4)");
   for (int m = 0; m < d->n_feats; ++m) MER_REQUIRE(d->feat_dims[m] > 0, "mer_fusion_topn: feature %d has no width", m);
   MER_REQUIRE(B > 0 && B <= 65535, "mer_fusion_topn: batch %d out of range", B);
   return 0;
@@ -737,7 +743,8 @@ int mer_fusion_frm_forward(const MerFusionDims* d, const float* params, const fl
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int T[3] = {seq_a, seq_t, seq_v};
   if (int rc = frm_check(d, B, T)) return rc;
-  MER_REQUIRE(params && audios && texts && videos && workspace && features && emos_out && (vals_out || d->out2 == 0),
+  MER_REQUIRE(params && audios && texts && videos && workspace && features && (emos_out || d->out1 == 0) &&
+                  (vals_out || d->out2 == 0),
               "mer_fusion_frm_forward: null operand");
   MER_REQUIRE(workspace_bytes >= frm_scratch_floats(*d, B, T) * 4, "mer_fusion_frm_forward: workspace too small");
   const FrmLayout L = make_frm_layout(*d);
@@ -767,8 +774,9 @@ int mer_fusion_frm_fwd_bwd(const MerFusionDims* d, const float* params, float* g
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int T[3] = {seq_a, seq_t, seq_v};
   if (int rc = frm_check(d, B, T)) return rc;
-  MER_REQUIRE(params && grads && audios && texts && videos && emos && (vals || d->out2 == 0) && workspace && loss_out &&
-                  features && emos_out && (vals_out || d->out2 == 0) && step_counter,
+  MER_REQUIRE(params && grads && audios && texts && videos && (emos || d->out1 == 0) && (vals || d->out2 == 0) &&
+                  workspace && loss_out && features && (emos_out || d->out1 == 0) && (vals_out || d->out2 == 0) &&
+                  step_counter,
               "mer_fusion_frm_fwd_bwd: null operand");
   MER_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "mer_fusion_frm_fwd_bwd: dropout %f", dropout_p);
   MER_REQUIRE(workspace_bytes >= frm_scratch_floats(*d, B, T) * 4, "mer_fusion_frm_fwd_bwd: workspace too small");
@@ -802,7 +810,7 @@ int mer_fusion_frm_fwd_bwd(const MerFusionDims* d, const float* params, float* g
   h.features = features; h.emos_out = emos_out; h.vals_out = vals_out;
   h.loss_terms = s.loss_terms; h.d_emos = s.d_emos; h.d_vals = s.d_vals; h.d_att = s.d_att;
   h.d_cat = s.d_cat; h.d_a3 = s.d_a3;
-  h.H = H; h.O1 = d->out1; h.O2 = d->out2; h.inv_batch = loss_inv_batch;
+  h.H = H; h.O1 = d->out1; h.O2 = d->out2; h.train = 1; h.inv_batch = loss_inv_batch;
   fus_head_kernel<<<B, 128, 0, st>>>(h);
   fus_loss_reduce_kernel<<<1, 32, 0, st>>>(s.loss_terms, B, loss_inv_batch, loss_out);
   mer_count_launches(2);

@@ -329,25 +329,29 @@ __device__ __forceinline__ void head_rows(const RowArgs& a, int rank, int row0, 
     for (int c = 0; c < 4; ++c) dval[c] = 0.f;
     if (a.mode == MODE_LOSS) {
       // CELoss: NLL(log_softmax) summed / N; MSELoss: squared error summed / N  (loss.py:11-28)
-      const int tgt = live ? (int)a.emo[row] : 0;   // (issued first: the loads fly while the softmax is evaluated)
+      // (the labels are issued first: the loads fly while the softmax is evaluated).  A regression-only head (O1 == 0)
+      // has no CE term: emo is not read (it may be null) and ce stays 0.
+      const int tgt = (live && O1 > 0) ? (int)a.emo[row] : 0;
       float tval[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) tval[c] = (live && c < O2) ? a.val[(long long)row * O2 + c] : 0.f;
-      float mx = logit[0];
-#pragma unroll
-      for (int c = 1; c < MO1; ++c)
-        if (c < O1) mx = fmaxf(mx, logit[c]);
-      float se = 0.f;
-#pragma unroll
-      for (int c = 0; c < MO1; ++c)
-        if (c < O1) se += expf(logit[c] - mx);
-      const float lse = mx + logf(se);
       float ce = 0.f, mse = 0.f;
+      if (O1 > 0) {
+        float mx = logit[0];
 #pragma unroll
-      for (int c = 0; c < MO1; ++c) {
-        if (c < O1) {
-          if (c == tgt) ce = lse - logit[c];
-          dlog[c] = live ? (expf(logit[c] - lse) - (c == tgt ? 1.f : 0.f)) * a.inv_batch : 0.f;
+        for (int c = 1; c < MO1; ++c)
+          if (c < O1) mx = fmaxf(mx, logit[c]);
+        float se = 0.f;
+#pragma unroll
+        for (int c = 0; c < MO1; ++c)
+          if (c < O1) se += expf(logit[c] - mx);
+        const float lse = mx + logf(se);
+#pragma unroll
+        for (int c = 0; c < MO1; ++c) {
+          if (c < O1) {
+            if (c == tgt) ce = lse - logit[c];
+            dlog[c] = live ? (expf(logit[c] - lse) - (c == tgt ? 1.f : 0.f)) * a.inv_batch : 0.f;
+          }
         }
       }
 #pragma unroll
@@ -1160,9 +1164,11 @@ __global__ void __launch_bounds__(NT) fus_wgrad_kernel(const __grid_constant__ W
 }
 
 int check_dims(const MerFusionDims* d, int B) {
-  MER_REQUIRE(d && d->hidden >= 4 && d->hidden <= 256 && d->hidden % 4 == 0 && d->out1 > 0 && d->out1 <= 16 &&
-                  d->out2 >= 0 && d->out2 <= 4 && d->audio_dim > 0 && d->text_dim > 0 && d->video_dim > 0,
-              "mer_fusion: unsupported dims (hidden a multiple of 4 up to 256, out1 <= 16, out2 <= 4)");
+  MER_REQUIRE(d && d->hidden >= 4 && d->hidden <= 256 && d->hidden % 4 == 0 && d->out1 >= 0 && d->out1 <= 16 &&
+                  d->out2 >= 0 && d->out2 <= 4 && d->out1 + d->out2 > 0 && d->audio_dim > 0 && d->text_dim > 0 &&
+                  d->video_dim > 0,
+              "mer_fusion: unsupported dims (hidden a multiple of 4 up to 256, out1 <= 16, out2 <= 4, at least one "
+              "output head)");
   MER_REQUIRE(B > 0 && B <= 65535, "mer_fusion: batch %d out of range", B);
   return 0;
 }
@@ -1263,8 +1269,9 @@ int launch_wgrad(const MerFusionDims& d, const ULayout& L, const GWs& ws, const 
   static const bool no_vec = getenv("MER_FUSION_WGRAD_SCALAR") != nullptr;  // A/B and bit-equality tests
   if (no_vec) vec = false;
   const int per_block = NT * (vec ? 4 : 1);
-  // an empty tensor (fc_out_2 of an emotion-only head, out2 == 0) takes no block: its blk0 equals the next problem's (or
-  // nblocks), and the block -> problem search below picks the last problem whose blk0 is <= blockIdx.x
+  // an empty tensor (fc_out_1 of a regression-only head, out1 == 0, or fc_out_2 of an emotion-only head, out2 == 0)
+  // takes no block: its blk0 equals the next problem's (or nblocks), and the block -> problem search below picks the
+  // last problem whose blk0 is <= blockIdx.x
   auto add = [&](const float* dy, int lddy, const float* xin, int ldx, int N, int K, long long w_off, long long b_off) {
     w.p[np] = WProb{dy, lddy, xin, ldx, N, K, w_off, b_off, blk};
     blk += (int)(((long long)N * K + per_block - 1) / per_block);
@@ -1307,7 +1314,8 @@ int fill_rows(RowArgs& a, const MerFusionDims* d, const float* params, const flo
               const float* const* ext_masks, void* workspace, long long workspace_bytes, float* features,
               float* emos_out, float* vals_out) {
   if (int rc = check_dims(d, B)) return rc;
-  MER_REQUIRE(params && audios && texts && videos && workspace && features && emos_out && (vals_out || d->out2 == 0),
+  MER_REQUIRE(params && audios && texts && videos && workspace && features && (emos_out || d->out1 == 0) &&
+                  (vals_out || d->out2 == 0),
               "mer_fusion: null operand");
   MER_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "mer_fusion: dropout %f", dropout_p);
   MER_REQUIRE(dropout_p == 0.f || step, "mer_fusion: dropout needs the step counter");
@@ -1366,7 +1374,8 @@ int mer_fusion_fwd_bwd(const MerFusionDims* d, const float* params, float* grads
   if (int rc = fill_rows(a, d, params, audios, texts, videos, B, dropout_p, seed, step_counter, ext_masks, workspace,
                          workspace_bytes, features, emos_out, vals_out))
     return rc;
-  MER_REQUIRE(grads && emos && (vals || d->out2 == 0) && loss_out && step_counter, "mer_fusion_fwd_bwd: null operand");
+  MER_REQUIRE(grads && (emos || d->out1 == 0) && (vals || d->out2 == 0) && loss_out && step_counter,
+              "mer_fusion_fwd_bwd: null operand");
   a.mode = MODE_LOSS;
   a.emo = reinterpret_cast<const long long*>(emos);
   a.val = vals;
@@ -1387,7 +1396,8 @@ int mer_fusion_step(const MerFusionDims* d, float* params, float* grads, float* 
   if (int rc = fill_rows(a, d, params, audios, texts, videos, B, dropout_p, seed, step_counter, ext_masks, workspace,
                          workspace_bytes, features, emos_out, vals_out))
     return rc;
-  MER_REQUIRE(grads && exp_avg && exp_avg_sq && emos && (vals || d->out2 == 0) && loss_out && step_counter && adam,
+  MER_REQUIRE(grads && exp_avg && exp_avg_sq && (emos || d->out1 == 0) && (vals || d->out2 == 0) && loss_out &&
+                  step_counter && adam,
               "mer_fusion_step: null operand");
   a.mode = MODE_LOSS;
   a.emo = reinterpret_cast<const long long*>(emos);

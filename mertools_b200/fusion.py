@@ -132,7 +132,9 @@ class _Replicated:
 class FusionNet(_Replicated):
     """Device-resident Attention fusion model.  feat_type 'utt': MLP encoders on [B, D] features;
     'frm_align' / 'frm_unalign': LSTM encoders on [B, T, D] sequences (attention.py:25-33).  output_dim2 = 0 is the
-    emotion-only head of the MER2024 / 25 / 26 dataloaders: vals_out is [B, 0] and the loss is CE alone."""
+    emotion-only head of the MER2024 / 25 / 26 dataloaders: vals_out is [B, 0] and the loss is CE alone.
+    output_dim1 = 0 is the regression-only head of the sentiment dataloaders (CMU-MOSI / MOSEI, SIMS / SIMSv2,
+    cmudata.py:20-23): emos_out is [B, 0], the loss is MSE alone and the emotion labels are never read."""
 
     def __init__(self, audio_dim=768, text_dim=768, video_dim=768, hidden_dim=128, output_dim1=6,
                  output_dim2=1, dropout=0.0, grad_clip=-1.0, device="cuda", max_batch=4096, seed=0,
@@ -716,16 +718,29 @@ def mer2026_calculate_results(emo_probs=(), emo_labels=(), val_preds=(), val_lab
     return dict(emoprobs=emo_probs, emolabels=emo_labels, emoacc=acc, emofscore=f1), f"f1:{f1:.4f}_acc:{acc:.4f}"
 
 
+def sentiment_calculate_results(emo_probs=(), emo_labels=(), val_preds=(), val_labels=()):
+    """cmudata.py:69-84 (sims.py, simsv2.py and crossdim.py have the same rule): acc-2 and weighted F1 of the sign of
+    the valence over the clips whose label is not 0; the emotion arguments are ignored."""
+    from sklearn.metrics import accuracy_score, f1_score
+    labels, preds = np.asarray(val_labels).reshape(-1), np.asarray(val_preds).reshape(-1)
+    keep = labels != 0
+    acc = accuracy_score(labels[keep] > 0, preds[keep] > 0)
+    f1 = f1_score(labels[keep] > 0, preds[keep] > 0, average="weighted")
+    return dict(valpreds=val_preds, vallabels=val_labels, emoacc=acc, emofscore=f1), f"f1:{f1:.4f}_acc:{acc:.4f}"
+
+
 def train_or_eval_model(args, model, reg_loss, cls_loss, dataloader, epoch, optimizer=None, train=False,
                         calculate_results=None, world_size=1):
     """main-release.py:17-87: same arguments, same ``save_results`` dict (names, loss, then the keys of
-    ``dataloader_class.calculate_results``; default: the MER2023 rule).  The regression loss and the valence
-    predictions enter only when ``args.output_dim2 != 0`` (MER2026_Track1/main-release.py:49-57); pass
-    ``mer2026_calculate_results`` for the MER2024 / 25 / 26 corpora.  With a ``torch.optim`` optimizer this IS the
+    ``dataloader_class.calculate_results``; default: the MER2023 rule).  The CE loss and the emotion scores enter only
+    when ``args.output_dim1 != 0``, the regression loss and the valence predictions only when ``args.output_dim2 != 0``
+    (main-release.py:51-58); pass ``mer2026_calculate_results`` for the MER2024 / 25 / 26 corpora and
+    ``sentiment_calculate_results`` for the sentiment corpora.  With a ``torch.optim`` optimizer this IS the
     reference loop (zero_grad, forward, ``cls_loss + reg_loss``, backward, clip_grad_value_, step) running on the
     autograd node; with this module's ``Adam`` holder each training batch is one fused FusionNet.train_step."""
     vidnames, val_preds, val_labels, emo_probs, emo_labels, losses = [], [], [], [], [], []
     assert not train or optimizer is not None
+    has_emo = getattr(args, "output_dim1", 6) != 0
     has_val = getattr(args, "output_dim2", 1) != 0
     fused = train and isinstance(optimizer, Adam)
     net = getattr(model, "net", None) or getattr(getattr(model, "model", None), "net", None) or \
@@ -751,11 +766,14 @@ def train_or_eval_model(args, model, reg_loss, cls_loss, dataloader, epoch, opti
             loss = loss3[2]
         else:
             _, emos_out, vals_out, interloss = model(batch)
-            loss = interloss + cls_loss(emos_out, emos)
+            loss = interloss
+            if has_emo:
+                loss = loss + cls_loss(emos_out, emos)
             if has_val:
                 loss = loss + reg_loss(vals_out, vals)
-        emo_probs.append(emos_out.data.cpu().numpy())
-        emo_labels.append(emos.data.cpu().numpy())
+        if has_emo:
+            emo_probs.append(emos_out.data.cpu().numpy())
+            emo_labels.append(emos.data.cpu().numpy())
         if has_val:
             val_preds.append(vals_out.data.cpu().numpy())
             val_labels.append(vals.data.cpu().numpy())
@@ -766,7 +784,8 @@ def train_or_eval_model(args, model, reg_loss, cls_loss, dataloader, epoch, opti
             if clip != -1:
                 torch.nn.utils.clip_grad_value_([p for p in model.parameters() if p.requires_grad], clip)
             optimizer.step()
-    emo_probs, emo_labels = np.concatenate(emo_probs), np.concatenate(emo_labels)
+    if has_emo:
+        emo_probs, emo_labels = np.concatenate(emo_probs), np.concatenate(emo_labels)
     if has_val:
         val_preds, val_labels = np.concatenate(val_preds), np.concatenate(val_labels)
     results, _ = (calculate_results or mer2023_calculate_results)(emo_probs, emo_labels, val_preds, val_labels)

@@ -15,6 +15,13 @@ torch's generator are the reference's by construction), batches are index-select
 training step is one fused FusionNet.train_step (forward + CE/MSE + backward + Adam in two kernels).  The golden of
 the unmodified script (tests/golden/make_golden_main_release.py) is reproduced fold for fold, epoch for epoch.
 
+The other MERBench corpora follow their own dataloaders (toolkit/dataloader/*.py of MERBench):
+``--dataset CMUMOSI | CMUMOSEI | SIMS | SIMSv2`` train a regression-only head (output_dim1 = 0) on train / val / test
+and report acc-2 / weighted F1 of the valence sign; ``--dataset MELD`` a 7-class emotion head on train / val / test;
+``--dataset IEMOCAPFour | IEMOCAPSix`` a 4- / 6-class head with leave-one-session-out folds and no test set.  The
+cross-corpus runs ``--train_dataset X --test_dataset Y`` are crossdim.py (sentiment corpora) and crossdis.py (the four
+shared emotions of IEMOCAP, MER2023 and MELD).
+
 Under ``python -m torch.distributed.run --nproc-per-node W -m mertools_b200.main_release ...`` the trainer is
 data-parallel (SURVEY.md §8e): rank 0's seed and initial weights are broadcast once, every rank draws the same
 permutation, takes the rank-strided slice ``batch[rank::W]`` of each reference batch, and the flat gradient (with
@@ -31,7 +38,7 @@ import numpy as np
 import torch
 
 from . import shard
-from .fusion import Adam, get_models, mer2023_calculate_results, mer2026_calculate_results
+from .fusion import Adam, get_models, mer2023_calculate_results, mer2026_calculate_results, sentiment_calculate_results
 
 EMOS_MER = ["neutral", "angry", "happy", "sad", "worried", "surprise"]      # toolkit/globals.py:2
 EMO2IDX = {e: i for i, e in enumerate(EMOS_MER)}
@@ -44,6 +51,25 @@ TOPN_GRID = dict(hidden_dim=[64, 128, 256], dropout=[0.2, 0.3, 0.4, 0.5], grad_c
 # train_corpus / test1_corpus, label every clip {'emo': idx, 'val': -10} and set output_dim1 = 6, output_dim2 = 0,
 # metric_name = 'emo'.
 EMO_CORPORA = ("MER2024", "MER2025", "MER2026")
+# The sentiment corpora (DIM_DATASET, toolkit/dataloader/__init__.py:10): cmudata.py:20-23, sims.py:21-23, simsv2.py:21-24
+# and crossdim.py:19-21 set output_dim1 = 0, output_dim2 = 1, metric_name = 'emo' and read train / val / test.
+SENTIMENT_CORPORA = ("CMUMOSI", "CMUMOSEI", "SIMS", "SIMSv2")
+# The corpora crossdis.py trains and tests across (DIS_DATASET, toolkit/dataloader/__init__.py:11).
+CROSSDIS_CORPORA = ("IEMOCAPFour", "IEMOCAPSix", "MER2023", "MELD")
+IEMOCAP_CORPORA = ("IEMOCAPFour", "IEMOCAPSix")
+# (output_dim1, output_dim2, metric_name) per --dataset: mer2023.py, mer2026.py:26-28, iemocap.py:25-33, meld.py:20-22
+# and the sentiment loaders above.
+HEADS = {"MER2023": (6, 1, "emoval"), **{d: (6, 0, "emo") for d in EMO_CORPORA},
+         **{d: (0, 1, "emo") for d in SENTIMENT_CORPORA}, "IEMOCAPFour": (4, 0, "emo"), "IEMOCAPSix": (6, 0, "emo"),
+         "MELD": (7, 0, "emo")}
+# crossdis.py:9-16: the four shared emotions and each corpus' label -> emotion map (samples outside it are dropped)
+CROSSDIS_EMO2IDX = {"happy": 0, "sad": 1, "neutral": 2, "angry": 3}
+CROSSDIS_MAP = {
+    "IEMOCAPFour": {0: "happy", 1: "sad", 2: "neutral", 3: "angry"},
+    "IEMOCAPSix": {0: "happy", 1: "sad", 2: "neutral", 3: "angry"},
+    "MELD": {0: "angry", 1: "happy", 2: "sad", 3: "neutral"},
+    "MER2023": {"neutral": "neutral", "angry": "angry", "happy": "happy", "sad": "sad"},
+}
 
 # Feature rankings, weakest first, that Data_Feat_TOPN takes the top n of (toolkit/globals.py of each tree):
 #   MER2024/toolkit/globals.py:218-231, MER2025/MER2025_Track1/toolkit/globals.py:218-242,
@@ -113,22 +139,74 @@ def topn_feature_names(dataset, fusion_topn, fusion_modality, feature_root):
 
 
 # ---- data (host side, same file formats as the reference) ---------------------------------------
+SPLITS = {"MER2023": ("train", "test1", "test2", "test3"), **{d: ("train", "test1") for d in EMO_CORPORA},
+          **{d: ("train", "val", "test") for d in SENTIMENT_CORPORA + ("MELD",)},
+          **{d: ("whole",) for d in IEMOCAP_CORPORA}}
+
+
 def read_names_labels(label_path, data_type, debug=False, dataset="MER2023"):
-    """mer2023.py:82-104; for MER2024 / 25 / 26 mer2026.py:83-99 (train / test1 only, the valence is always -10)."""
-    emo_only = dataset in EMO_CORPORA
-    assert data_type in (("train", "test1") if emo_only else ("train", "test1", "test2", "test3"))
+    """mer2023.py:82-104; for MER2024 / 25 / 26 mer2026.py:83-99 (train / test1 only, the valence is always -10); for
+    the sentiment corpora and MELD cmudata.py:58-70 / sims.py / simsv2.py / meld.py:56-68 (train / val / test), for
+    IEMOCAP iemocap.py:64-75 (whole): those labels are stored as the loaders use them (an integer emotion, a float
+    valence) and are passed through."""
+    assert data_type in SPLITS[dataset], (dataset, data_type)
     corpus = np.load(label_path, allow_pickle=True)[f"{data_type}_corpus"].tolist()
     names, labels = [], []
     for name, label in corpus.items():
         names.append(name)
-        if emo_only:
-            val = -10
-        else:
+        if dataset in EMO_CORPORA:
+            labels.append({"emo": EMO2IDX[label["emo"]], "val": -10})
+        elif dataset == "MER2023":
             val = label["val"] if ("val" in label and label["val"] != "") else -10
-        labels.append({"emo": EMO2IDX[label["emo"]], "val": val})
+            labels.append({"emo": EMO2IDX[label["emo"]], "val": val})
+        else:
+            labels.append({"emo": int(label["emo"]), "val": label["val"]})
     if debug:
         names, labels = names[:100], labels[:100]
     return names, labels
+
+
+def read_crossdim_labels(label_path, dataset, data_type, debug=False):
+    """crossdim.py:66-83: a sentiment corpus' split with the SIMS / SIMSv2 valences (in [-1, 1]) scaled by 3 to the CMU
+    range [-3, 3]."""
+    assert dataset in SENTIMENT_CORPORA, dataset
+    names, labels = read_names_labels(label_path, data_type, False, dataset)
+    if dataset in ("SIMS", "SIMSv2"):
+        for l in labels:
+            l["val"] = l["val"] * 3
+    if debug:
+        names, labels = names[:100], labels[:100]
+    return names, labels
+
+
+def read_crossdis_labels(label_path, dataset, data_type, debug=False):
+    """crossdis.py:162-188: a split mapped onto the four shared emotions (CROSSDIS_MAP then CROSSDIS_EMO2IDX), the
+    samples whose emotion is outside the map dropped; the valence is passed through (-10 where the corpus has none)."""
+    assert dataset in CROSSDIS_CORPORA, dataset
+    assert data_type in {"MER2023": ("train", "test1"), "MELD": ("train", "val", "test")}.get(dataset, ("whole",)), \
+        (dataset, data_type)
+    corpus = np.load(label_path, allow_pickle=True)[f"{data_type}_corpus"].tolist()
+    mapping = CROSSDIS_MAP[dataset]
+    names, labels = [], []
+    for name, label in corpus.items():
+        if label["emo"] in mapping:
+            names.append(name)
+            val = label.get("val", -10)
+            labels.append({"emo": CROSSDIS_EMO2IDX[mapping[label["emo"]]], "val": -10 if val == "" else val})
+    if debug:
+        names, labels = names[:100], labels[:100]
+    return names, labels
+
+
+def session_split_indexes(names, num_folder=5):
+    """iemocap.py:78-96 / crossdis.py:191-203: leave-one-session-out -- fold i evaluates session i + 1
+    (``int(name[4]) - 1``: ``Ses0N...``) and trains on the other four, each in corpus order."""
+    session_to_idx = {}
+    for idx, vid in enumerate(names):
+        session_to_idx.setdefault(int(vid[4]) - 1, []).append(idx)
+    assert len(session_to_idx) == num_folder, "Must split into five folder"
+    return [[[i for j in range(num_folder) if j != k for i in session_to_idx[j]], list(session_to_idx[k])]
+            for k in range(num_folder)]
 
 
 def read_utt_feature(feature_root, name):
@@ -180,8 +258,8 @@ class DeviceSplit:
     attention_topn: the 3 * fusion_topn utterance-level features ``args.topn_features`` (Data_Feat_TOPN: the mean over
     time of each clip), as ``feats``."""
 
-    def __init__(self, args, names, labels, config, device):
-        root = config.PATH_TO_FEATURES[args.dataset]
+    def __init__(self, args, names, labels, config, device, dataset=None):
+        root = config.PATH_TO_FEATURES[dataset or args.dataset]     # each corpus' own features (feat_data.py:12)
         feats = []
         if args.model == "attention_topn":
             for fname in args.topn_features:
@@ -237,12 +315,27 @@ def get_loaders(n_train, folds, n_tests, batch_size, num_workers=0):
     return train_loaders, eval_loaders, test_loaders
 
 
+def sequential_loader(n, batch_size, num_workers=0):
+    """The train, val and test loaders of cmudata.py:29-52 (and sims.py, simsv2.py, meld.py, crossdim.py, crossdis.py's
+    MELD branch): no shuffle, no sampler -- the split in corpus order.  Iterating it still draws the loader's base seed
+    from torch's generator, as the reference's does."""
+    from torch.utils.data import DataLoader
+    return DataLoader(_Indices(n), batch_size=batch_size, num_workers=num_workers, shuffle=False)
+
+
 calculate_results = mer2023_calculate_results  # mer2023.py:137-155
 
 
-def corpus_calculate_results(dataset):
-    """dataloader_class.calculate_results: mer2023.py:137-155, or mer2026.py:132-145 for MER2024 / 25 / 26."""
-    return mer2026_calculate_results if dataset in EMO_CORPORA else mer2023_calculate_results
+def corpus_calculate_results(dataset, train_dataset=None):
+    """dataloader_class.calculate_results: mer2023.py:137-155; the argmax f1 / acc rule of mer2026.py:132-145 for
+    MER2024 / 25 / 26, which is also iemocap.py:99-115, meld.py:72-87 and crossdis.py:228-243; acc-2 of the valence
+    sign (cmudata.py:69-84, crossdim.py:87-102) for the sentiment corpora.  A cross-corpus run takes the rule of its
+    protocol, chosen by the train corpus (toolkit/dataloader/__init__.py:32-37)."""
+    if train_dataset is not None:
+        return sentiment_calculate_results if train_dataset in SENTIMENT_CORPORA else mer2026_calculate_results
+    if dataset in SENTIMENT_CORPORA:
+        return sentiment_calculate_results
+    return mer2023_calculate_results if dataset == "MER2023" else mer2026_calculate_results
 
 
 def gain_cv_results(folder_save):
@@ -280,15 +373,91 @@ def _gather_strided(local, n_global, rank, world):
     return out
 
 
+def load_protocol(args, config, device, say=print):
+    """The splits and loader objects of the corpus' dataloader class (toolkit/dataloader/__init__.py:14-37), in the order
+    the reference builds them.  Returns (folds, tests, train_loaders, eval_loaders, test_loaders): ``folds[i]`` is the
+    (train, eval) pair of DeviceSplits fold i's loaders index into, ``tests`` the test DeviceSplits."""
+    bs, nw = args.batch_size, args.num_workers
+    mk = lambda names, labels, ds: DeviceSplit(args, names, labels, config, device, ds)  # noqa: E731
+    seq = lambda split: sequential_loader(len(split), bs, nw)  # noqa: E731
+    if args.train_dataset is not None:
+        return _load_cross(args, config, mk, seq, say)
+    ds = args.dataset
+    lp = config.PATH_TO_LABEL[ds]
+    if ds in IEMOCAP_CORPORA:                     # iemocap.py:35-61: five session folds over whole_corpus, no test set
+        names, labels = read_names_labels(lp, "whole", args.debug, ds)
+        folds = session_split_indexes(names)
+        say(f"sample number {len(names)}")
+        whole = mk(names, labels, ds)
+        trl, evl, _ = get_loaders(len(names), folds, [], bs, nw)
+        return [(whole, whole)] * len(folds), [], trl, evl, []
+    if ds in SENTIMENT_CORPORA or ds == "MELD":   # cmudata.py:26-55 / sims.py / simsv2.py / meld.py: one fold
+        splits = []
+        for dt in ("train", "val", "test"):
+            names, labels = read_names_labels(lp, dt, args.debug, ds)
+            say(f"{dt}: sample number {len(names)}")
+            splits.append(mk(names, labels, ds))
+        return [(splits[0], splits[1])], [splits[2]], [seq(splits[0])], [seq(splits[1])], [seq(splits[2])]
+    # MER2023 (mer2023.py:31-79), MER2024 / 25 / 26 (mer2026.py:31-80): five random folds of train, then the test sets
+    names, labels = read_names_labels(lp, "train", args.debug, ds)
+    say(f"train: sample number {len(names)}")
+    train_split = mk(names, labels, ds)
+    folds = random_split_indexes(len(names), 5)
+    tests = []
+    for dt in SPLITS[ds][1:]:
+        n, l = read_names_labels(lp, dt, args.debug, ds)
+        say(f"{dt}: sample number {len(n)}")
+        tests.append(mk(n, l, ds))
+    trl, evl, tel = get_loaders(len(names), folds, [len(ts) for ts in tests], bs, nw)
+    return [(train_split, train_split)] * len(folds), tests, trl, evl, tel
+
+
+def _load_cross(args, config, mk, seq, say):
+    """crossdim.py:23-56 (sentiment corpora: train / val of the train corpus, test of the test corpus, one fold) and
+    crossdis.py:33-139 (IEMOCAP: session folds of whole; MER2023: five random folds of train; MELD: train / val; then
+    the test split of the test corpus: whole, test1 or test).  Each split reads its own corpus' features."""
+    tr, te = args.train_dataset, args.test_dataset
+    assert te is not None, "--train_dataset needs --test_dataset"
+    if tr in SENTIMENT_CORPORA:
+        assert te in SENTIMENT_CORPORA, f"crossdim tests on {SENTIMENT_CORPORA}, not {te}"
+        s = []
+        for ds, dt in ((tr, "train"), (tr, "val"), (te, "test")):
+            names, labels = read_crossdim_labels(config.PATH_TO_LABEL[ds], ds, dt, args.debug)
+            say(f"{dt}: sample number {len(names)}")
+            s.append(mk(names, labels, ds))
+        return [(s[0], s[1])], [s[2]], [seq(s[0])], [seq(s[1])], [seq(s[2])]
+    assert tr in CROSSDIS_CORPORA and te in CROSSDIS_CORPORA, \
+        f"cross-corpus runs pair {SENTIMENT_CORPORA} or {CROSSDIS_CORPORA}, not {tr} -> {te}"
+    rd = lambda ds, dt: read_crossdis_labels(config.PATH_TO_LABEL[ds], ds, dt, args.debug)  # noqa: E731
+    if tr in IEMOCAP_CORPORA:
+        names, labels = rd(tr, "whole")
+        folds = session_split_indexes(names)
+        whole = mk(names, labels, tr)
+        pairs = [(whole, whole)] * len(folds)
+        trl, evl, _ = get_loaders(len(names), folds, [], args.batch_size, args.num_workers)
+    elif tr == "MER2023":
+        names, labels = rd(tr, "train")
+        whole = mk(names, labels, tr)
+        folds = random_split_indexes(len(names), 5)
+        pairs = [(whole, whole)] * len(folds)
+        trl, evl, _ = get_loaders(len(names), folds, [], args.batch_size, args.num_workers)
+    else:
+        train, val = mk(*rd(tr, "train"), tr), mk(*rd(tr, "val"), tr)
+        pairs, trl, evl = [(train, val)], [seq(train)], [seq(val)]
+    test = mk(*rd(te, {"MER2023": "test1", "MELD": "test"}.get(te, "whole")), te)
+    say(f"test: sample number {len(test)}")
+    return pairs, [test], trl, evl, [seq(test)]
+
+
 # ---- one pass over a split (main-release.py:17-87) ------------------------------------------------
 def run_split(args, net, split, loader, optimizer=None, train=False, rank=0, world_size=1):
     """``loader`` yields batches of sample indices in the reference's order.  Training: one fused step per batch
-    (under data parallelism on rows ``rank::world_size`` of it); evaluation: eval forward + the losses.  The
-    regression loss and the valence predictions enter only when ``args.output_dim2 != 0`` (MER2026_Track1/
-    main-release.py:49-57)."""
+    (under data parallelism on rows ``rank::world_size`` of it); evaluation: eval forward + the losses.  The CE loss
+    and the emotion scores enter only when ``args.output_dim1 != 0``, the regression loss and the valence predictions
+    only when ``args.output_dim2 != 0`` (main-release.py:51-58)."""
     dev = split.emo.device
     topn = args.model == "attention_topn"
-    has_val = args.output_dim2 != 0
+    has_emo, has_val = args.output_dim1 != 0, args.output_dim2 != 0
     names, emo_probs, val_preds, losses, order = [], [], [], [], []
     net.train(train)
     for b in loader:
@@ -304,33 +473,41 @@ def run_split(args, net, split, loader, optimizer=None, train=False, rank=0, wor
             loss3, eo, vo = net.train_step(xs, emo, val, **kw) if topn else net.train_step(*xs, emo, val, **kw)
             losses.append(loss3[2:3].clone())
             if world_size > 1:
-                eo = _gather_strided(eo, len(b), rank, world_size)
+                if has_emo:
+                    eo = _gather_strided(eo, len(b), rank, world_size)
                 if has_val:
                     vo = _gather_strided(vo, len(b), rank, world_size)
         else:
             batch = {f"feat{i}": x for i, x in enumerate(xs)} if topn else dict(zip(("audios", "texts", "videos"), xs))
             _, eo, vo, _ = net(batch)
-            loss = torch.nn.functional.cross_entropy(eo, emo, reduction="sum") / len(eo)
+            loss = torch.zeros(1, device=dev)
+            if has_emo:
+                loss = loss + torch.nn.functional.cross_entropy(eo, emo, reduction="sum") / len(eo)
             if has_val:
                 loss = loss + torch.nn.functional.mse_loss(vo, val, reduction="sum") / len(vo)
             losses.append(loss.view(1))
-        emo_probs.append(eo.clone())
+        if has_emo:
+            emo_probs.append(eo.clone())
         if has_val:
             val_preds.append(vo.clone())
     order = torch.cat(order)
-    emo_probs = torch.cat(emo_probs).cpu().numpy()
-    emo_labels = split.emo.index_select(0, order).cpu().numpy()
-    val_labels = []
+    emo_labels, val_labels = [], []
+    if has_emo:
+        emo_probs = torch.cat(emo_probs).cpu().numpy()
+        emo_labels = split.emo.index_select(0, order).cpu().numpy()
     if has_val:
         val_preds = torch.cat(val_preds).cpu().numpy()
         val_labels = split.val.index_select(0, order).cpu().numpy()
-    res, _ = corpus_calculate_results(args.dataset)(emo_probs, emo_labels, val_preds, val_labels)
+    res, _ = corpus_calculate_results(args.dataset, getattr(args, "train_dataset", None))(
+        emo_probs, emo_labels, val_preds, val_labels)
     return dict(names=names, loss=np.mean(torch.cat(losses).cpu().numpy()), **res)
 
 
 def build_parser():
     p = argparse.ArgumentParser()
-    p.add_argument("--dataset", type=str, default="MER2023")
+    p.add_argument("--dataset", type=str, default=None)          # MER2023 unless a cross-corpus run
+    p.add_argument("--train_dataset", type=str, default=None)    # cross-corpus runs (main-release.py:96-97)
+    p.add_argument("--test_dataset", type=str, default=None)
     p.add_argument("--fusion_topn", type=int, default=None)
     p.add_argument("--fusion_modality", type=str, default="AVT")
     p.add_argument("--save_root", type=str, default="./saved")
@@ -351,6 +528,20 @@ def build_parser():
     p.add_argument("--print_iters", type=int, default=1e8)
     p.add_argument("--gpu", default=0, type=int)
     return p
+
+
+def result_prefix(args):
+    """prefix_name of the result files (main-release.py:170-179).  The reference builds it before its loaders run, so
+    the dataset: field is --dataset as given -- None in a cross-corpus run that passes only --train_dataset /
+    --test_dataset."""
+    feats = [f for f in (args.audio_feature, args.text_feature, args.video_feature) if f is not None]
+    prefix = (f"features:{'+'.join(sorted(set(feats)))}_dataset:{args.dataset}_model:{args.model}+{args.feat_type}+"
+              f"{args.e2e_name}")
+    if args.fusion_topn is not None:
+        prefix += f"_fusiontopn:{args.fusion_topn}_modality:{args.fusion_modality}"
+    if getattr(args, "train_dataset", None) is not None:
+        prefix += f"_train:{args.train_dataset}_test:{args.test_dataset}"
+    return prefix
 
 
 def _init_distributed(args):
@@ -375,9 +566,13 @@ def main(args, config=None, log=None):
     what tests/golden/main_release_golden.npz holds for the unmodified script."""
     if config is None:
         from . import config as config  # noqa: PLW0127
-    assert args.dataset in ("MER2023",) + EMO_CORPORA, \
-        f"the H100 path covers --dataset MER2023 / {' / '.join(EMO_CORPORA)}, not {args.dataset}"
-    assert args.model == "attention" or (args.model == "attention_topn" and args.dataset in EMO_CORPORA), \
+    cross = getattr(args, "train_dataset", None) is not None
+    if not cross:
+        args.train_dataset = args.test_dataset = None
+        if args.dataset is None:
+            args.dataset = "MER2023"
+        assert args.dataset in HEADS, f"the H100 path covers --dataset {' / '.join(HEADS)}, not {args.dataset}"
+    assert args.model == "attention" or (args.model == "attention_topn" and args.dataset in EMO_CORPORA and not cross), \
         "the H100 path covers --model attention, and attention_topn on the corpora with feature rankings"
     topn = args.model == "attention_topn"
     rank, world = _init_distributed(args)
@@ -396,6 +591,8 @@ def main(args, config=None, log=None):
         args.feat_scale = 6 if args.feat_type == "frm_align" else 12
     if args.fusion_topn is not None:
         args.save_root = f"{args.save_root}-multitop"
+    if cross:
+        args.save_root = f"{args.save_root}-cross"
     feats = [f for f in (args.audio_feature, args.text_feature, args.video_feature) if f is not None]
     args.save_root = f"{args.save_root}-" + {0: "others", 1: "unimodal", 2: "bimodal", 3: "trimodal"}[len(set(feats))]
     if args.hyper_path is None:
@@ -407,41 +604,31 @@ def main(args, config=None, log=None):
     for k, v in cfg.items():                                                               # merge_args_config
         if getattr(args, k, None) is None:
             setattr(args, k, v)
-    if args.dataset in EMO_CORPORA:
-        args.output_dim1, args.output_dim2, args.metric_name = 6, 0, "emo"
+    if cross:   # crossdim.py:19-21 / crossdis.py:29-31
+        args.output_dim1, args.output_dim2, args.metric_name = (0, 1, "emo") if args.train_dataset in SENTIMENT_CORPORA \
+            else (4, 0, "emo")
     else:
-        args.output_dim1, args.output_dim2, args.metric_name = 6, 1, "emoval"
+        args.output_dim1, args.output_dim2, args.metric_name = HEADS[args.dataset]
     say("args: ", args)
     save_resroot = os.path.join(args.save_root, "result")
     if rank == 0:
         os.makedirs(save_resroot, exist_ok=True)
         os.makedirs(os.path.join(args.save_root, "model"), exist_ok=True)
-    feature_name = "+".join(sorted(set(feats)))
-    prefix_name = f"features:{feature_name}_dataset:{args.dataset}_model:{args.model}+{args.feat_type}+{args.e2e_name}"
-    if args.fusion_topn is not None:
-        prefix_name += f"_fusiontopn:{args.fusion_topn}_modality:{args.fusion_modality}"
+    prefix_name = result_prefix(args)
 
     say("====== Reading Data =======")
-    label_path = config.PATH_TO_LABEL[args.dataset]
     if topn:
         args.topn_features = topn_feature_names(args.dataset, args.fusion_topn, args.fusion_modality,
                                                 config.PATH_TO_FEATURES[args.dataset])
         say(f"feature number: {len(args.topn_features)}")
-    names, labels = read_names_labels(label_path, "train", args.debug, args.dataset)
-    say(f"train: sample number {len(names)}")
-    train_split = DeviceSplit(args, names, labels, config, device)
-    folds = random_split_indexes(len(names), 5)
-    tests = []
-    for dt in ("test1",) if args.dataset in EMO_CORPORA else ("test1", "test2", "test3"):
-        n, l = read_names_labels(label_path, dt, args.debug, args.dataset)
-        say(f"{dt}: sample number {len(n)}")
-        tests.append(DeviceSplit(args, n, l, config, device))
-    train_loaders, eval_loaders, test_loaders = get_loaders(len(names), folds, [len(ts) for ts in tests],
-                                                            args.batch_size, args.num_workers)
+    folds, tests, train_loaders, eval_loaders, test_loaders = load_protocol(args, config, device, say)
+    if cross:   # the cross-corpus loaders leave args.dataset at the test corpus (crossdim.py:36, crossdis.py:122)
+        args.dataset = args.test_dataset
+    say(f"train&val folder:{len(train_loaders)}; test sets:{len(test_loaders)}")
     if topn:  # Data_Feat_TOPN.get_featdim: the list of widths, three times
-        args.audio_dim = args.text_dim = args.video_dim = list(train_split.dims)
+        args.audio_dim = args.text_dim = args.video_dim = list(folds[0][0].dims)
     else:
-        args.audio_dim, args.text_dim, args.video_dim = train_split.dims
+        args.audio_dim, args.text_dim, args.video_dim = folds[0][0].dims
 
     say("====== Training and Evaluation =======")
     folder_save, folder_duration = [], []
@@ -458,8 +645,8 @@ def main(args, config=None, log=None):
         whole_store, whole_metrics = [], []
         for epoch in range(args.epochs):
             epoch_store = {}
-            train_res = run_split(args, net, train_split, train_loaders[ii], optimizer, True, rank, world)
-            eval_res = run_split(args, net, train_split, eval_loaders[ii])
+            train_res = run_split(args, net, folds[ii][0], train_loaders[ii], optimizer, True, rank, world)
+            eval_res = run_split(args, net, folds[ii][1], eval_loaders[ii])
             for k, v in eval_res.items():
                 epoch_store[f"eval_{k}"] = v
             tm, em = (gain_metric_from_results(r, args.metric_name) for r in (train_res, eval_res))
@@ -495,14 +682,16 @@ def main(args, config=None, log=None):
     path = f"{save_resroot}/cv_{prefix_name}_{cv_result}_{name_time}.npz"
     saved.append(path)
     contents.append({})
-    for jj in range(len(tests)):
-        emo_labels = folder_save[0][f"test{jj + 1}_emolabels"]
-        emo_probs = np.mean(np.array([f[f"test{jj + 1}_emoprobs"] for f in folder_save]), axis=0)
-        val_labels, val_preds = [], []
+    for jj in range(len(tests)):   # average_folder_for_emos / _vals (metric.py:57-100): [] when the head is absent
+        emo_labels, emo_probs, val_labels, val_preds = [], [], [], []
+        if args.output_dim1 != 0:
+            emo_labels = folder_save[0][f"test{jj + 1}_emolabels"]
+            emo_probs = np.mean(np.array([f[f"test{jj + 1}_emoprobs"] for f in folder_save]), axis=0)
         if args.output_dim2 != 0:
             val_labels = folder_save[0][f"test{jj + 1}_vallabels"]
             val_preds = np.mean(np.array([f[f"test{jj + 1}_valpreds"] for f in folder_save]), axis=0)
-        _, test_result = corpus_calculate_results(args.dataset)(emo_probs, emo_labels, val_preds, val_labels)
+        _, test_result = corpus_calculate_results(args.dataset, args.train_dataset)(emo_probs, emo_labels, val_preds,
+                                                                                    val_labels)
         saved.append(f"{save_resroot}/test{jj + 1}_{prefix_name}_{test_result}_{name_time}.npz")
         # MER2024 / 25 / 26 keep the fold-averaged emotion scores (MER2026_Track1/main-release.py:286-288)
         contents.append(dict(emo_probs=emo_probs) if args.dataset in EMO_CORPORA else {})

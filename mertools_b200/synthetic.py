@@ -899,6 +899,64 @@ def write_mer2023_corpus(root, n_train=32, n_test=8, dim=768, seed=0, frame_leve
     return label_path, feats
 
 
+# The label files of the MERBench corpora other than MER2023, in the formats their preprocessing scripts write
+# (MERBench/toolkit/preprocess/cmumosi.py:70-86, cmumosei.py:130-142, sims.py:83-101, simsv2.py:67-77,
+# iemocap.py:101-106, meld.py:57-80): (file name, splits, number of emotion classes or 0 for a sentiment corpus, valence
+# range).  Every sentiment split holds some valences of exactly 0, which the acc-2 rule drops.
+MERBENCH_LABELS = {
+    "CMUMOSI": ("label.npz", ("train", "val", "test"), 0, 3.0),
+    "CMUMOSEI": ("label.npz", ("train", "val", "test"), 0, 3.0),
+    "SIMS": ("label.npz", ("train", "val", "test"), 0, 1.0),
+    "SIMSv2": ("label.npz", ("train", "val", "test"), 0, 1.0),
+    "IEMOCAPFour": ("label_4way.npz", ("whole",), 4, None),
+    "IEMOCAPSix": ("label_6way.npz", ("whole",), 6, None),
+    "MELD": ("label.npz", ("train", "val", "test"), 7, None),
+}
+MERBENCH_DIMS = (48, 64, 40)   # synA / synT / synV widths (the same in every corpus: cross-corpus runs share them)
+
+
+def write_merbench_corpus(root, dataset, n=(40, 12, 12), seed=0, frame_level=False):
+    """A ``dataset``-format corpus (a key of MERBENCH_LABELS) under ``root``: its label file with the
+    ``{split}_corpus`` dicts the preprocessors write -- sentiment corpora ``{'emo': 0, 'val': v}`` with v on the
+    corpus' label grid (CMU: steps of 1/3 in [-3, 3], SIMS: steps of 0.2 in [-1, 1]); IEMOCAP ``whole_corpus``
+    ``{'emo': idx, 'val': -10}`` named ``Ses0{s}{F|M}_...`` with the five sessions interleaved, n[0] clips in all;
+    MELD ``{'emo': idx, 'val': -10}`` -- and N(0,1) float32 ``.npy`` features under ``features/{synA,synT,synV}-UTT/``
+    (and ``-FRA`` with 2..39 / 2..5 / 2..5 rows per clip when ``frame_level``).  ``n`` = clips per split, in the order
+    of the corpus' splits.  Returns (label_path, feature_root)."""
+    import os
+    fname, splits, n_emo, vmax = MERBENCH_LABELS[dataset]
+    rng = np.random.default_rng(seed)
+    corp = {}
+    for si, split in enumerate(splits):
+        c = {}
+        for i in range(n[si]):
+            if split == "whole":
+                sess = int(rng.integers(1, 6)) if i >= 5 else i + 1        # every session present
+                name = f"Ses0{sess}{'FM'[i % 2]}_impro{i % 7:02d}_{'FM'[(i // 2) % 2]}{i:03d}"
+            else:
+                name = f"{split}_{dataset.lower()}_{i:04d}"
+            if n_emo:
+                c[name] = {"emo": int(rng.integers(0, n_emo)), "val": -10}
+            else:
+                steps = 9 if vmax == 3.0 else 5
+                c[name] = {"emo": 0, "val": 0.0 if i % 5 == 0 else float(rng.integers(-steps, steps + 1)) * vmax / steps}
+        corp[f"{split}_corpus"] = c
+    os.makedirs(root, exist_ok=True)
+    label_path = os.path.join(root, fname)
+    np.savez(label_path, **corp)
+    feats = os.path.join(root, "features")
+    sets = [(f"syn{m}-UTT", 0, d) for m, d in zip("ATV", MERBENCH_DIMS)]
+    if frame_level:
+        sets += [(f"syn{m}-FRA", hi, d) for m, hi, d in zip("ATV", (40, 6, 6), MERBENCH_DIMS)]
+    for fdir, hi, dim in sets:
+        os.makedirs(os.path.join(feats, fdir), exist_ok=True)
+        for split in corp.values():
+            for name in split:
+                shape = (int(rng.integers(2, hi)), dim) if hi else (dim,)
+                np.save(os.path.join(feats, fdir, name + ".npy"), rng.standard_normal(shape).astype(np.float32))
+    return label_path, feats
+
+
 # Feature directories of a synthetic MER2026 corpus: every entry of MER2026's three rank lists
 # (main_release.RANK_LISTS), named the way func_name_conversion resolves them -- the face extractors as `<dir>_UTT`,
 # the rest as `<dir>-UTT` -- with a few different widths; videomae-large keeps 2..4 rows per clip (mean over time).
