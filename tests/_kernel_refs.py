@@ -353,15 +353,18 @@ def hubert_hidden0(sd, wave, conv_f16=False, ln_eps=1e-5):
     return x, ex
 
 
-def attention_packed(qkv, cu, heads, hd=64, scale=0.125, causal=False, slopes=None, v=None, mqa=False, stats=False):
+def attention_packed(qkv, cu, heads, hd=64, scale=0.125, causal=False, slopes=None, v=None, mqa=False, stats=False,
+                     rel=None):
     """softmax(scale Q K^T (+ ALiBi)) V per (sequence, head) of packed rows.  qkv [tokens, >= 3 * heads * hd]: Q | K | V
     column blocks; with `mqa` Q is columns [0, heads * hd) and the one K head the next hd columns (the rest of the row is
     not read).  v (optional): V as its own [tokens, heads * hd] ([tokens, hd] with mqa) tensor instead of qkv's V block.
     causal: query i sees keys 0 .. i of its sequence.  slopes [heads]: HF's ALiBi, + slope_h * j with j counted from the
-    sequence start.  Empty sequences in cu are skipped.
+    sequence start.  rel: a relative-position score term (deberta_rel, xlnet_rel), rel(a, q, k, j) -> (t, |t|), added
+    to Q K^T before the scale, its sum of absolute products to A.  Empty sequences in cu are skipped.
     Returns (ctx, P |V|, A) [tokens, heads * hd]: P |V| is the scale of the error a perturbed probability leaves, A the
-    row's score amplitude max_j scale sum_d |q_d k_jd| (+ max |slope_h (j - i)| over the keys whose probability is not
-    negligible, the bias the kernel adds in fp32), the scale of the error of a score summed in fp32.  stats: a fourth
+    row's score amplitude max_j scale sum_d |q_d k_jd| (+ the absolute products of the rel term; + max |slope_h (j - i)|
+    over the keys whose probability is not negligible, the bias the kernel adds in fp32), the scale of the error of a
+    score summed in fp32.  stats: a fourth
     item, dict(tiny = sum_{j: p~_j < 2^-13} |v_j| / sum_j p~_j with p~ = exp(s - max s) (the keys whose probability is an
     fp16 subnormal or in the lowest normal binade), keys = the number of keys each row sees)."""
     D = heads * hd
@@ -382,6 +385,10 @@ def attention_packed(qkv, cu, heads, hd=64, scale=0.125, causal=False, slopes=No
         sc = q @ k.transpose(1, 2) * scale
         top = q.abs() @ k.abs().transpose(1, 2) * scale                            # [heads, n, n]
         ii = torch.arange(n, device=x.device)
+        if rel is not None:
+            t, ta = rel(a, q, k, ii)
+            sc = sc + t * scale
+            top = top + ta * scale
         if slopes is not None:
             sl = slopes.double().to(x.device)[:, None, None]
             sc = sc + sl * ii[None, None, :]
@@ -420,7 +427,7 @@ def ctx_rounding(v, fmt):
     return torch.zeros_like(v)
 
 
-def attention_tc_bound(mag, amp, st, ref, fmt):
+def attention_tc_bound(mag, amp, st, ref, fmt, score=18):
     """Elementwise bound of the fp16 / tf32 tensor-core attention kernels against attention_packed(stats=True)'s
     (ref, mag = P |V|, amp = A, st), u = 2^-24, n = st["keys"].  A = max_j scale sum_d |q_d k_jd| (+ the largest
     ALiBi bias |slope (j - i)| over the keys that keep a probability), so every scaled score s_j and the row maximum m
@@ -452,9 +459,20 @@ def attention_tc_bound(mag, amp, st, ref, fmt):
     The P, O, normaliser and finish terms act on the perturbed probabilities, whose P |V| is at most e^{2D} P |V|, and
     the P rounding acts on values already off by those fp32 errors: factor (1 + 2^-10).  Total
       (e^{2D} - 1) P |V| + e^{2D} ((1 + 2^-10) (2^-11 + (11 n / 64 + 52) u) P |V| + 2^-25 tiny)
-    plus ctx_rounding of |ref| plus that (the ctx store).  A worst case: no constant is fitted to observed errors."""
+    plus ctx_rounding of |ref| plus that (the ctx store).  A worst case: no constant is fitted to observed errors.
+
+    `score` is the score term's coefficient (18 above), so D = (score + 11) u A.  The relative-position kernels share
+    everything but the score, with A the scaled sum of the absolute products of every term (attention_packed's rel):
+      attention_rel.cu   S = Q K^T, C1 = Q PKwin^T, C2 = K PQwin^T: three mma.sync sums as above, each <= 16 u of its
+                         own absolute products, together <= 16 u A; s + C1 + C2, two fp32 adds of partials <= A: 2 u A.
+                         score = 18.
+      attention_xl.cu    S and C1 = Q Rwin^T on mma.sync: <= 16 u of their absolute products.  kb = r_w . k_j,
+                         rb = r_r . Rwin[w] and the segment scalars (q_i + r_s) . seg[0 | 1] are warp-reduced fp32 dots:
+                         a per-lane product and fma (2 u), then 5 shuffle adds (5 u), <= 7 u of their absolute products;
+                         the segment dot reads q + r_s rounded once in fp32 (u): 8 u.  All <= 16 u of their own
+                         products, together <= 16 u A; s + kb + C1 + rb + segment, four fp32 adds: 4 u A.  score = 20."""
     n = st["keys"]
-    d2 = 2 * (29 * U32 * amp + (n / 16 + 12) * U32)
+    d2 = 2 * ((score + 11) * U32 * amp + (n / 16 + 12) * U32)
     grow = torch.exp(d2)
     own = torch.expm1(d2) * mag + grow * ((1 + 2.0 ** -10) * (2.0 ** -11 + (11 * n / 64 + 52) * U32) * mag +
                                          2.0 ** -25 * st["tiny"])
@@ -506,10 +524,11 @@ ATT_TC_FAULTS = ("bf16_p", "acc16", "vt_shift", "causal_diag", "alibi_tile", "mq
 
 
 def attention_tc_emulated(qkv, cu, heads, hd=64, scale=0.125, causal=False, slopes=None, v=None, mqa=False,
-                          p_fmt="f16", fault=None):
+                          p_fmt="f16", fault=None, rel=None):
     """An fp32 evaluation with the kernels' arithmetic (fp32 scores, p~ = exp(s - max) in fp32, P rounded to p_fmt
     ("f16", "tf32") for P V, the normaliser summed from the unrounded p~, fp32 O), before the ctx store (ctx_format).
-    Same arguments as attention_packed; `fault` (ATT_TC_FAULTS) restates a wrong kernel."""
+    Same arguments as attention_packed (rel: evaluated in fp32 on the same pieces, with its own fault); `fault`
+    (ATT_TC_FAULTS) restates a wrong kernel."""
     D = heads * hd
     x = qkv.float()
     T = x.shape[0]
@@ -537,9 +556,12 @@ def attention_tc_emulated(qkv, cu, heads, hd=64, scale=0.125, causal=False, slop
             moved = vv[src, :kh * hd] * (a + j + 1 < T)[:, None]
             vs = torch.where((j + (a & 7) >= 64)[:, None], moved, vs)
         vs = vs.reshape(nk, kh, hd).transpose(0, 1)
-        sc = (q @ k.transpose(1, 2)) * scale
+        sc = q @ k.transpose(1, 2)
         i = torch.arange(n, device=x.device)[:, None] + (a - ka)                # query index on the key axis
         jj = torch.arange(nk, device=x.device)[None, :]
+        if rel is not None:
+            sc = sc + rel(a, q, k, jj[0] - (a - ka))[0]
+        sc = sc * scale
         if slopes is not None:
             pos = jj % 64 if fault == "alibi_tile" else jj
             sc = sc + slopes.float().to(x.device)[:, None, None] * (pos - i).float()
@@ -670,6 +692,192 @@ def att_tc_reference(case, ops, device="cpu"):
     return attention_packed(ops["qkv"].to(device), ops["cu"], case["heads"], case["hd"], case["scale"],
                             causal=case["causal"], slopes=None if ops["slopes"] is None else ops["slopes"].to(device),
                             v=ops["v"].to(device), mqa=case["mqa"], stats=True)
+
+
+# ---- relative-position tensor-core attention: attention_rel.cu (DeBERTa), attention_xl.cu (XLNet) ------------------------
+# The two kernels are attention_f16.cu's tiled kernel with extra score terms, each read from a 127-row window of a
+# gathered table, so attention_packed takes their terms as `rel` and attention_tc_bound covers them with a larger score
+# coefficient (ATT_REL_SCORE).  Restated faults (tests/test_kernel_refs.py: each must leave the bound), besides
+# ATT_TC_FAULTS' bf16_p and foreign_keys:
+#   window_off_by_one  window column w = i - j + 64: every table term read at distance i - j + 1
+#   p2c_untransposed   DeBERTa's PQ term read at row(j - i)
+#   shift_dropped      distances counted on the 8-aligned key axis: off by start % 8
+#   origin_len         rel_row indexed from the sentence's length instead of max_seqlen
+#   seg_swapped        XLNet's segment embedding taken as seg[type_i == type_j]
+#   seg_row_type       every query of a 16-row slice takes the token type of the slice's first row
+#   rb_dropped         XLNet's r_r_bias . R term missing
+#   bias_in_operand    q + r_w_bias and q + r_r_bias rounded to the operand format before their dots, which the kernel
+#                      never does (2^-11 relative on every product: the bound resolves it at scale 1.5 already)
+ATT_REL_FAULTS = ("window_off_by_one", "p2c_untransposed", "shift_dropped", "origin_len", "seg_swapped", "seg_row_type",
+                  "rb_dropped", "bias_in_operand", "bf16_p", "foreign_keys")
+ATT_REL_SCORE = {"deberta": 18, "xlnet": 20}   # attention_tc_bound's score coefficient (derived in its docstring)
+
+
+def _rel_index(d, a, n, rows, max_seqlen, fault):
+    """rel_row's entries for the distances d of a sentence that starts at token a and has n tokens (the kernels' index
+    d + max_seqlen - 1, clamped to the map), as a fault restates it."""
+    if fault == "window_off_by_one":
+        d = d + 1
+    elif fault == "shift_dropped":
+        d = d - a % 8
+    origin = n if fault == "origin_len" else max_seqlen
+    return rows[(d + origin - 1).clamp(0, 2 * max_seqlen - 2)]
+
+
+def deberta_rel(pk, pq, rel_row, max_seqlen, span, fault=None):
+    """attention_rel.cu's score term for attention_packed / attention_tc_emulated: q_i . PK[row(i - j)] +
+    k_j . PQ[row(i - j)] with row(d) = rel_row[d + max_seqlen - 1] clamped to [0, 2 span), as the kernel documents.
+    pk, pq [2 span, >= heads * hd] (columns past heads * hd are not read).  Computed in q's dtype on q's device;
+    fault: one of ATT_REL_FAULTS."""
+    def term(a, q, k, j):
+        H, n, hd = q.shape
+        dev, dt = q.device, q.dtype
+        rows = torch.as_tensor(rel_row, device=dev).long().clamp(0, 2 * span - 1)
+        PK, PQ = (t[:, :H * hd].to(dev, dt).reshape(-1, H, hd).transpose(0, 1) for t in (pk, pq))
+        d = torch.arange(n, device=dev)[:, None] - j.to(dev)[None, :]
+        r1 = _rel_index(d, a, n, rows, max_seqlen, fault).expand(H, -1, -1)
+        r2 = _rel_index(-d if fault == "p2c_untransposed" else d, a, n, rows, max_seqlen, fault).transpose(0, 1)
+        r2 = r2.expand(H, -1, -1)
+
+        def c(x, y):
+            return (torch.gather(x[0] @ y[0].transpose(1, 2), -1, r1) +
+                    torch.gather(x[1] @ y[1].transpose(1, 2), -1, r2).transpose(1, 2))
+        return c((q, k), (PK, PQ)), c((q.abs(), k.abs()), (PK.abs(), PQ.abs()))
+    return term
+
+
+def xlnet_rel(r, rel_row, max_seqlen, r_w, r_r, r_s, seg, types=None, fault=None, op=None):
+    """attention_xl.cu's score term beyond q_i . k_j, for attention_packed / attention_tc_emulated:
+    r_w . k_j + (q_i + r_r) . R[row(i - j)] (+ (q_i + r_s) . seg[type_i != type_j] with token types), row(d) =
+    rel_row[d + max_seqlen - 1].  r [rows, >= heads * hd]; r_w, r_r, r_s [heads, hd] and seg [2, heads, hd], HF's
+    parameter shapes; types: one int per packed token.  Computed in q's dtype on q's device; fault: one of
+    ATT_REL_FAULTS or bias_in_operand, which rounds to the operand format `op` ("f16", "tf32")."""
+    def term(a, q, k, j):
+        H, n, hd = q.shape
+        dev, dt = q.device, q.dtype
+        rows = torch.as_tensor(rel_row, device=dev).long()
+        R = r[:, :H * hd].to(dev, dt).reshape(-1, H, hd).transpose(0, 1)
+        bw, br, bs = (b.to(dev, dt)[:, None, :] for b in (r_w, r_r, r_s))
+        sg = seg.to(dev, dt)
+        j = j.to(dev)
+        d = torch.arange(n, device=dev)[:, None] - j[None, :]
+        ix = _rel_index(d, a, n, rows, max_seqlen, fault)
+        win = lambda x: torch.gather(x @ R.transpose(1, 2), -1, ix.expand(H, -1, -1))      # noqa: E731
+        absw = lambda x: torch.gather(x @ R.abs().transpose(1, 2), -1, ix.expand(H, -1, -1))  # noqa: E731
+        if fault == "bias_in_operand":
+            rnd = (lambda x: x.half().to(dt)) if op == "f16" else (lambda x: round_tf32_ties_away(x.float()).to(dt))
+            t = rnd(q + bw) @ k.transpose(1, 2) - q @ k.transpose(1, 2) + win(rnd(q + br))
+        else:
+            t = bw @ k.transpose(1, 2) + win(q)
+            if fault != "rb_dropped":
+                t = t + (br @ R.transpose(1, 2))[:, 0][:, ix]
+        ta = bw.abs() @ k.abs().transpose(1, 2) + absw(q.abs()) + (br.abs() @ R.abs().transpose(1, 2))[:, 0][:, ix]
+        if types is not None:
+            tt = torch.as_tensor(types, device=dev).long()
+            ti = tt[a + torch.arange(n, device=dev) // 16 * 16] if fault == "seg_row_type" else tt[a:a + n]
+            s = (ti[:, None] == tt[a + j][None, :]) if fault == "seg_swapped" else (ti[:, None] != tt[a + j][None, :])
+            s = s.long().expand(H, -1, -1)
+            t = t + torch.gather(torch.einsum("hid,shd->his", q + bs, sg), -1, s)
+            ta = ta + torch.gather(torch.einsum("hid,shd->his", (q + bs).abs(), sg.abs()), -1, s)
+        return t, ta
+    return term
+
+
+# The operand sets of tests/test_attention_rel_gpu.py; tests/test_kernel_refs.py runs the emulation and the faults on the
+# same sets.  Lengths: 1 .. 9, 15 .. 17 and every 64-token tile edge +-1 through 257, an odd length first so that most
+# starts are not multiples of 8, an empty sequence inside cu_seqlens; one case per kernel with ~1100 tokens (17 key
+# tiles, 18 query blocks).  extra: max_seqlen passed as the longest sentence + extra, rel_row built for that origin.
+ATT_REL_EDGES = [9, 1, 2, 3, 4, 5, 6, 7, 8, 15, 16, 17, 63, 64, 65, 127, 128, 129, 255, 256, 257]
+
+
+def _rel_lens(*more):
+    ls = ATT_REL_EDGES + list(more)
+    ls.insert(3, 0)
+    return ls
+
+
+_ATT_REL_SHAPES = {
+    # DeBERTa v1 (max_relative_positions 512): sentences over 513 tokens clamp distances at both ends
+    "deb_v1": dict(entry="deberta", rmap="v1", heads=3, lens=_rel_lens(600, 1100)),
+    "deb_v1_h16": dict(entry="deberta", rmap="v1", heads=16, lens=_rel_lens(), extra=37),
+    # DeBERTa-v2 (position_buckets 256, max_relative_positions 512): log buckets from |d| 128 through 512 and past it
+    "deb_v2": dict(entry="deberta", rmap="v2", heads=1, lens=_rel_lens(300, 450, 513, 600), extra=37),
+    "deb_v2_h24": dict(entry="deberta", rmap="v2", heads=24, lens=_rel_lens(200)),
+    # XLNet: clamp_len unset and 20; token types of two segments inside each sentence and the CLS type 2
+    "xl": dict(entry="xlnet", clamp=-1, types=True, heads=3, lens=_rel_lens(600, 1100), extra=37),
+    "xl_clamp20_h12": dict(entry="xlnet", clamp=20, types=True, heads=12, lens=_rel_lens(300)),
+    "xl_h16": dict(entry="xlnet", clamp=-1, types=True, heads=16, lens=_rel_lens()),
+    "xl_notypes_h1": dict(entry="xlnet", clamp=-1, types=False, heads=1, lens=_rel_lens(400), extra=37),
+}
+ATT_REL_CASES = {f"{name}_{fmt}": dict(c, fmt=fmt) for name, c in _ATT_REL_SHAPES.items() for fmt in ("f16", "tf32")}
+
+
+def att_rel_case(name):
+    """ATT_REL_CASES[name] with its defaults: extra, the kernel's name, the score scale (fp32) and coefficient."""
+    c = dict(ATT_REL_CASES[name])
+    c.setdefault("extra", 0)
+    c["kernel"] = ("disentangled" if c["entry"] == "deberta" else "xlnet") + \
+        f"_attention_kernel<{'true' if c['fmt'] == 'f16' else 'false'}>"
+    c["scale"] = float(np.float32(1.0 / math.sqrt(3 * 64) if c["entry"] == "deberta" else 0.125))
+    c["score"] = ATT_REL_SCORE[c["entry"]]
+    return c
+
+
+def _token_types(lens):
+    """XLNet's token types per sentence: a first segment (1) of a third of the tokens, the second (0), CLS (2) last."""
+    out = []
+    for n in lens:
+        t = np.zeros(n, np.int32)
+        t[:n // 3] = 1
+        t[n - 1:] = 2
+        out.append(t)
+    return np.concatenate(out)
+
+
+def att_rel_operands(case, amp, seed=0):
+    """Host operands of a case at operand scale amp (randn * amp on q, k, v, the tables and XLNet's biases; the kernel
+    operands rounded to fp16 or tf32, the biases fp32): dict(qkv, v, cu, max_seqlen, rows, and pk, pq, span or r, r_w,
+    r_r, r_s, seg, types)."""
+    g = torch.Generator().manual_seed(seed)
+    lens, H = case["lens"], case["heads"]
+    D, T = H * 64, sum(lens)
+    cu = [0]
+    for n in lens:
+        cu.append(cu[-1] + n)
+    ms = max(lens) + case["extra"]
+    rnd = (lambda x: x.half().float()) if case["fmt"] == "f16" else round_tf32_ties_away
+    qkv = rnd(torch.randn(T, 3 * D, generator=g) * amp)
+    ops = dict(qkv=qkv, v=qkv[:, 2 * D:].clone(), cu=cu, max_seqlen=ms)
+    if case["entry"] == "deberta":
+        import types
+        from mertools_b200.extract import deberta_text as DT
+        v2 = case["rmap"] == "v2"
+        dims = types.SimpleNamespace(v2=v2, buckets=256 if v2 else -1, max_rel=512, span=256 if v2 else 512)
+        ops.update(rows=DT.rel_rows(dims, ms), span=dims.span,
+                   pk=rnd(torch.randn(2 * dims.span, D, generator=g) * amp),
+                   pq=rnd(torch.randn(2 * dims.span, D, generator=g) * amp))
+    else:
+        from mertools_b200.extract import xlnet_text as XT
+        _, rows = XT.rel_table(D, ms, case["clamp"])
+        ops.update(rows=rows, r=rnd(torch.randn(int(rows.max()) + 1, D, generator=g) * amp),
+                   r_w=torch.randn(H, 64, generator=g) * amp, r_r=torch.randn(H, 64, generator=g) * amp,
+                   r_s=torch.randn(H, 64, generator=g) * amp, seg=torch.randn(2, H, 64, generator=g) * amp,
+                   types=torch.from_numpy(_token_types(lens)) if case["types"] else None)
+    return ops
+
+
+def att_rel_term(case, ops, fault=None):
+    """The case's rel term (deberta_rel / xlnet_rel) on its operands."""
+    if case["entry"] == "deberta":
+        return deberta_rel(ops["pk"], ops["pq"], ops["rows"], ops["max_seqlen"], ops["span"], fault)
+    return xlnet_rel(ops["r"], ops["rows"], ops["max_seqlen"], ops["r_w"], ops["r_r"], ops["r_s"], ops["seg"],
+                     ops["types"], fault, case["fmt"])
+
+
+def att_rel_reference(case, ops, device="cpu"):
+    """(ref, mag, amp, st) of attention_packed(stats=True, rel=...) on a case's operands, in float64 on `device`."""
+    return attention_packed(ops["qkv"].to(device), ops["cu"], case["heads"], 64, case["scale"], v=ops["v"].to(device),
+                            stats=True, rel=att_rel_term(case, ops))
 
 
 def attention_kernels(fn):

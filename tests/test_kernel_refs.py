@@ -670,3 +670,152 @@ def test_attention_bound_rejects_the_faults():
                     worst[fault] = (f"{name} x{amp}", r)
     print("fault / bound: " + ", ".join(f"{k} {v[1]:.2f} ({v[0]})" for k, v in worst.items()))
     assert all(worst[f][1] > 1.5 for f in R.ATT_TC_FAULTS), worst
+
+
+# ---- relative-position attention: attention_rel.cu (DeBERTa), attention_xl.cu (XLNet) ----------------------------------
+def _rand_params(module, g, scale):
+    with torch.no_grad():
+        for p in module.parameters():
+            p.copy_(torch.randn(p.shape, generator=g, dtype=torch.float64) * scale)
+
+
+@pytest.mark.parametrize("v2,max_rel,buckets", [(False, 16, -1), (False, 512, -1), (True, 32, 8), (True, 512, 256)])
+def test_deberta_rel_reference_is_hf_disentangled_attention(v2, max_rel, buckets):
+    """attention_packed with deberta_rel and DT.rel_rows is HF's DisentangledSelfAttention (deberta / deberta-v2, c2p |
+    p2c), run per sentence in float64 on the same projections: sentences longer than the span in both directions, log
+    buckets through max_position, and the map built for an origin (max_seqlen) beyond the longest sentence."""
+    import types
+
+    import transformers as tf
+    from transformers.models.deberta import modeling_deberta as M1
+    from transformers.models.deberta_v2 import modeling_deberta_v2 as M2
+
+    from mertools_b200.extract import deberta_text as DT
+    heads, D, lens = 2, 128, [5, 40, 0, 70]
+    kw = dict(vocab_size=10, hidden_size=D, num_attention_heads=heads, intermediate_size=8, num_hidden_layers=1,
+              max_position_embeddings=512, relative_attention=True, pos_att_type=["c2p", "p2c"],
+              max_relative_positions=max_rel, hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0)
+    if v2:
+        kw.update(position_buckets=buckets)
+    att = (M2 if v2 else M1).DisentangledSelfAttention((tf.DebertaV2Config if v2 else tf.DebertaConfig)(**kw))
+    att = att.double().eval()
+    g = _g(max_rel + buckets)
+    _rand_params(att, g, 0.05)
+    span = buckets if v2 else max_rel
+    E = torch.randn(2 * span, D, generator=g, dtype=torch.float64)
+    X = torch.randn(sum(lens), D, generator=g, dtype=torch.float64)
+    lin = lambda m, x: x @ m.weight.T + (0 if m.bias is None else m.bias)       # noqa: E731
+    if v2:
+        q, k, v = (lin(m, X) for m in (att.query_proj, att.key_proj, att.value_proj))
+        pk, pq = lin(att.pos_key_proj, E), lin(att.pos_query_proj, E)
+    else:
+        q, k, v = (X @ att.in_proj.weight.T).view(-1, heads, 3, 64).unbind(2)     # per head q | k | v
+        q, v = q + att.q_bias.view(heads, 64), v + att.v_bias.view(heads, 64)
+        pk, pq = lin(att.pos_proj, E), lin(att.pos_q_proj, E)
+    qkv = torch.cat([t.reshape(-1, D) for t in (q, k, v)], 1)
+    cu = np.concatenate([[0], np.cumsum(lens)]).tolist()
+    ms = max(lens) + 5
+    scale = 1.0 / float(torch.sqrt(torch.tensor(3 * 64.0)))      # HF's scaled_size_sqrt, a float32 square root
+    rows = DT.rel_rows(types.SimpleNamespace(v2=v2, buckets=buckets if v2 else -1, max_rel=max_rel, span=span), ms)
+    got = R.attention_packed(qkv, cu, heads, 64, scale, rel=R.deberta_rel(pk, pq, rows, ms, span))[0]
+    plain = R.attention_packed(qkv, cu, heads, 64, scale)[0]
+    with torch.no_grad():
+        for a, b in zip(cu, cu[1:]):
+            if b <= a:
+                continue
+            x = X[a:b][None]
+            if v2:
+                rp = M2.build_relative_position(x[0], x[0], bucket_size=buckets, max_position=max_rel)
+            else:
+                rp = M1.build_relative_position(x[0], x[0])
+            want = att(x, torch.ones(1, 1, b - a, b - a, dtype=torch.bool), relative_pos=rp, rel_embeddings=E)[0][0]
+            assert float((got[a:b] - want).abs().max()) < 1e-12, (a, b)
+            assert b - a == 5 or float((plain[a:b] - want).abs().max()) > 1e-3
+
+
+@pytest.mark.parametrize("with_types,clamp_len", [(False, -1), (True, -1), (True, 7)])
+def test_xlnet_rel_reference_is_hf_rel_attn_core(with_types, clamp_len):
+    """attention_packed with xlnet_rel and XT.rel_table is HF's XLNetRelativeAttention.rel_attn_core, run per sentence
+    in float64 on the same heads, biases and projected relative positions (relative_positional_encoding, clamp_len
+    included), with and without token types; the map built for an origin beyond the longest sentence."""
+    import transformers as tf
+
+    from mertools_b200.extract import xlnet_text as XT
+    heads, D, lens = 2, 128, [5, 40, 0, 23]
+    m = tf.XLNetModel(tf.XLNetConfig(vocab_size=8, d_model=D, n_head=heads, d_inner=8, n_layer=1, clamp_len=clamp_len,
+                                     dropout=0.0)).double().eval()
+    att = m.layer[0].rel_attn
+    g = _g(11 + clamp_len)
+    _rand_params(att, g, 0.3)
+    T = sum(lens)
+    qkv = torch.randn(T, 3 * D, generator=g, dtype=torch.float64) * 0.3
+    w_r = torch.randn(D, heads, 64, generator=g, dtype=torch.float64) * 0.05
+    tt = torch.from_numpy(R._token_types(lens))
+    cu = np.concatenate([[0], np.cumsum(lens)]).tolist()
+    ms = max(lens) + 5
+    table, rows = XT.rel_table(D, ms, clamp_len)
+    rel = R.xlnet_rel(table.double() @ w_r.reshape(D, -1), rows, ms, att.r_w_bias, att.r_r_bias, att.r_s_bias,
+                      att.seg_embed, tt if with_types else None)
+    got = R.attention_packed(qkv, cu, heads, 64, 0.125, rel=rel)[0]
+    with torch.no_grad():
+        for a, b in zip(cu, cu[1:]):
+            n = b - a
+            if n <= 0:
+                continue
+            q, k, v = (qkv[a:b, i * D:(i + 1) * D].view(n, 1, heads, 64) for i in range(3))
+            kr = torch.einsum("ibh,hnd->ibnd", m.relative_positional_encoding(n, n, bsz=1).double(), w_r)
+            seg = None
+            if with_types:
+                seg = F.one_hot((tt[a:b][:, None] != tt[a:b][None, :]).long(), 2).double()[:, :, None]
+            want = att.rel_attn_core(q, k, v, kr, seg_mat=seg).reshape(n, D)
+            assert float((got[a:b] - want).abs().max()) < 1e-12, (a, b)
+
+
+_REL_CACHE = {}
+
+
+def _rel_ratio(name, amp, fault=None):
+    """Worst ratio of the fp32 emulation of a relative-position case (ATT_REL_CASES) over every ctx format."""
+    if (name, amp) not in _REL_CACHE:
+        c = R.att_rel_case(name)
+        ops = R.att_rel_operands(c, amp)
+        _REL_CACHE[(name, amp)] = (c, ops) + tuple(R.att_rel_reference(c, ops))
+    c, ops, ref, mag, amp_, st = _REL_CACHE[(name, amp)]
+    tc_fault = fault if fault in R.ATT_TC_FAULTS else None
+    x = R.attention_tc_emulated(ops["qkv"], ops["cu"], c["heads"], 64, c["scale"], v=ops["v"], p_fmt=c["fmt"],
+                                fault=tc_fault, rel=R.att_rel_term(c, ops, None if tc_fault else fault))
+    worst = 0.0
+    for fmt in ("fp32", "f16", "tf32", "split"):
+        bound = R.attention_tc_bound(mag, amp_, st, ref, fmt, c["score"])
+        worst = max(worst, float(R.bound_ratio(R.ctx_format(x, fmt).double(), ref, bound).max()))
+    return worst
+
+
+@pytest.mark.parametrize("amp", [1.5, 4.0])
+def test_rel_attention_emulation_fits_under_the_bound(amp):
+    """The relative-position kernels' arithmetic (fp32 score pieces, fp16 / tf32 P, every ctx format), emulated in
+    fp32, stays at or below 0.85 of attention_tc_bound (score coefficient ATT_REL_SCORE) on every operand set of
+    tests/test_attention_rel_gpu.py, as the tensor-core routes do."""
+    worst = {name: _rel_ratio(name, amp) for name in R.ATT_REL_CASES}
+    print("emulation / bound: " + ", ".join(f"{k} {v:.2f}" for k, v in worst.items()))
+    assert all(v <= 0.85 for v in worst.values()), worst
+
+
+def test_rel_attention_bound_rejects_the_faults():
+    """Each restated fault of ATT_REL_FAULTS leaves attention_tc_bound by more than 1.5x on some element of an operand
+    set the GPU test runs (at operand scale 1.5 or 4); the worst ratio per fault is printed.  XLNet's segment and bias
+    faults act on its cases only, p2c_untransposed on DeBERTa's."""
+    xl = [n for n in R.ATT_REL_CASES if n.startswith("xl") and "notypes" not in n]
+    deb = [n for n in R.ATT_REL_CASES if n.startswith("deb")]
+    cases = {f: (xl if f in ("seg_swapped", "seg_row_type", "rb_dropped", "bias_in_operand") else
+                 deb if f == "p2c_untransposed" else ["deb_v1_h16_f16", "deb_v2_tf32", "xl_tf32", "xl_notypes_h1_f16"])
+             for f in R.ATT_REL_FAULTS}
+    worst = {}
+    for fault, names in cases.items():
+        for name in names:
+            for amp in (1.5, 4.0):
+                r = _rel_ratio(name, amp, fault=fault)
+                if r > worst.get(fault, ("", 0.0))[1]:
+                    worst[fault] = (f"{name} x{amp}", r)
+    print("fault / bound: " + ", ".join(f"{k} {v[1]:.3g} ({v[0]})" for k, v in worst.items()))
+    assert all(worst[f][1] > 1.5 for f in R.ATT_REL_FAULTS), worst
