@@ -981,6 +981,51 @@ MER_API int mer_fusion_adam(float* params, const float* grads, float* exp_avg, f
                             float weight_decay, float grad_scale, float grad_clip, int* step_counter,
                             void* stream);
 
+/* ---- MER2023 baseline nets: MLP and Attention over a free --layers list (MER2023/main-release.py) -------------
+ * MLP (:226-245): one chain of Linear -> ReLU -> Dropout per entry of `layers` over the concat A | T | V, then
+ * fc_out_1 / fc_out_2 on the chain's output (the features).  Attention (:248-290): such a chain per modality (audio,
+ * text, video), attention_mlp (the same chain) over the concat of their outputs, fc_att (layers[last] -> 3, no
+ * softmax), the weighted sum of the three outputs (the features), then the two heads.  Parameters, gradients and Adam
+ * moments are flat fp32 buffers in state_dict order: module.{0,3,..}.weight/.bias, fc_out_1.*, fc_out_2.* (MLP);
+ * audio_mlp.*, text_mlp.*, video_mlp.*, attention_mlp.*, fc_att.*, fc_out_1.*, fc_out_2.* (Attention).
+ * Dropout mask t (t = chain * n_layers + layer, chains in the reference's forward order; the MLP has one chain) acts on
+ * that layer's [batch, layers[layer]] output.  Limits: 1..8 layers of width 1..1024, input widths 1..65536 (any
+ * value: IS10's 1582 and eGeMAPS's 88 included), 1..16 emotion classes, 1..4 valence outputs.  The Attention net
+ * refuses a batch of one row: the reference squeezes its [1, L] fused features to a vector and fails. */
+#define MER_MLP_KIND_MLP 0
+#define MER_MLP_KIND_ATTENTION 1
+#define MER_MLP_MAX_LAYERS 8
+#define MER_MLP_MAX_WIDTH 1024
+#define MER_MLP_MAX_INPUT 65536
+#define MER_MLP_MAX_OUT1 16
+#define MER_MLP_MAX_OUT2 4
+typedef struct MerMlpDims {
+  int kind;                            /* MER_MLP_KIND_MLP | MER_MLP_KIND_ATTENTION */
+  int audio_dim, text_dim, video_dim;  /* input widths */
+  int n_layers;                        /* entries of --layers */
+  int layers[MER_MLP_MAX_LAYERS];      /* widths, layers[0 .. n_layers - 1] */
+  int out1, out2;                      /* 6 emotion classes, 1 valence */
+} MerMlpDims;
+/* -1 (mer_last_error says why) for dims or a batch the kernels refuse */
+MER_API long long mer_mlp_param_count(const MerMlpDims* dims);
+MER_API long long mer_mlp_workspace_bytes(const MerMlpDims* dims, int max_batch);
+/* eval-mode forward: features [B, layers[last]], emos_out [B, out1], vals_out [B, out2] */
+MER_API int mer_mlp_forward(const MerMlpDims* dims, const float* params, const float* audios, const float* texts,
+                            const float* videos, int batch, void* workspace, long long workspace_bytes,
+                            float* features, float* emos_out, float* vals_out, void* stream);
+/* One training step of main-release.py:334-369: train-mode forward (dropout_p on every layer's output, keep-masks from
+ * the counter hash of (seed, *step_counter, mask, element) unless ext_masks -- a HOST array of (1 or 4) * n_layers
+ * device keep-masks (0/1), entries may be NULL -- supplies them), CE + MSE averaged over the batch, backward, and with
+ * adam != NULL torch.optim.Adam (coupled L2; grad_clip <= 0: none) through mer_fusion_adam, which advances
+ * *step_counter.  adam == NULL: grads only, no update, the step counter untouched.  grads receives d(loss)/d(params),
+ * loss_out (device float[3]) {CE, MSE, CE + MSE}, features / emos_out / vals_out the train-mode outputs. */
+MER_API int mer_mlp_train_step(const MerMlpDims* dims, float* params, float* grads, float* exp_avg,
+                               float* exp_avg_sq, const float* audios, const float* texts, const float* videos,
+                               const int64_t* emos, const float* vals, int batch, float dropout_p,
+                               unsigned long long seed, int* step_counter, const float* const* ext_masks,
+                               const MerAdamHyper* adam, void* workspace, long long workspace_bytes,
+                               float* loss_out, float* features, float* emos_out, float* vals_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

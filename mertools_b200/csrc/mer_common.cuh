@@ -394,6 +394,20 @@ __device__ __forceinline__ float adam_param(float pi, float grad, float& m, floa
   return __fsub_rn(pi, __fmul_rn(__fdiv_rn(lr, bc1), __fdiv_rn(m, denom)));
 }
 
+// The fusion nets' dropout keep-mask: element i of mask tensor m at step counter `step`, 1 (keep) with probability
+// 1 - p.  A splitmix64 counter hash, the draw of fusion.cu:fus_dropout_mask_kernel with the tensor's 0x1000 (m + 1)
+// folded into the seed; used by fusion_fused.cu and fusion_mlp.cu.
+__device__ __forceinline__ float keep_hash(unsigned long long seed, int m, int step, long long i, float p) {
+  unsigned long long z = seed + 0x1000ull * (unsigned long long)(m + 1) +
+                         0x9E3779B97F4A7C15ull * (unsigned long long)(step + 1) +
+                         0xD1B54A32D192ED03ull * (unsigned long long)(i + 1);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z ^= z >> 31;
+  const float u = (float)(z >> 40) * (1.0f / 16777216.0f);
+  return u >= p ? 1.f : 0.f;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

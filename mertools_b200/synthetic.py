@@ -871,15 +871,25 @@ def synth_fusion_features(n, dim=768, seed=0):
 EMOS_MER = ("neutral", "angry", "happy", "sad", "worried", "surprise")  # toolkit/globals.py:2
 
 
-def write_mer2023_corpus(root, n_train=32, n_test=8, dim=768, seed=0, frame_level=False):
+def write_mer2023_corpus(root, n_train=32, n_test=8, dim=768, seed=0, frame_level=False, dims=None,
+                         numeric_val=False):
     """A MER2023-format corpus under ``root`` (SURVEY.md §8d, config C1): ``label-6way.npz`` with the
     ``{split}_corpus`` dict-of-dicts of toolkit/dataloader/mer2023.py:82-104 (every 7th valence left '' = missing)
     and N(0,1) float32 ``.npy`` features under ``features/{synA,synT,synV}-UTT/`` (and ``-FRA`` with 2..39 / 2..5
-    rows per clip when ``frame_level``).  Returns (label_path, feature_root)."""
+    rows per clip when ``frame_level``).  ``dims``: (audio, text, video) widths instead of ``dim`` for all three.
+    ``numeric_val``: every valence a number, test3's the -10 placeholder of the released label file -- what
+    MER2023/main-release.py reads (its loader turns the valences into a float tensor).  Returns (label_path,
+    feature_root)."""
     import os
     rng = np.random.default_rng(seed)
     corp = {}
     for split, n in (("train", n_train), ("test1", n_test), ("test2", n_test), ("test3", n_test)):
+        if numeric_val:
+            corp[f"{split}_corpus"] = {
+                f"{split}_{i:04d}": {"emo": EMOS_MER[int(rng.integers(0, 6))],
+                                     "val": -10.0 if split == "test3" else float(rng.uniform(-3, 3))}
+                for i in range(n)}
+            continue
         corp[f"{split}_corpus"] = {
             f"{split}_{i:04d}": {"emo": EMOS_MER[int(rng.integers(0, 6))],
                                  "val": float(rng.uniform(-3, 3)) if i % 7 else ""}
@@ -890,11 +900,12 @@ def write_mer2023_corpus(root, n_train=32, n_test=8, dim=768, seed=0, frame_leve
     sets = [("synA-UTT", 0), ("synT-UTT", 0), ("synV-UTT", 0)]
     if frame_level:
         sets += [("synA-FRA", 40), ("synT-FRA", 6), ("synV-FRA", 6)]
-    for fname, hi in sets:
+    for si, (fname, hi) in enumerate(sets):
+        width = dim if dims is None else dims[si % 3]
         os.makedirs(os.path.join(feats, fname), exist_ok=True)
         for split in corp.values():
             for name in split:
-                shape = (int(rng.integers(2, hi)), dim) if hi else (dim,)
+                shape = (int(rng.integers(2, hi)), width) if hi else (width,)
                 np.save(os.path.join(feats, fname, name + ".npy"), rng.standard_normal(shape).astype(np.float32))
     return label_path, feats
 

@@ -154,7 +154,23 @@ def fusion():
     print("fusion ok")
 
 
+def fusion_mlp():
+    """The MER2023 baseline nets: both kinds, an input chunked through the staging buffer, a ragged last cluster."""
+    from mertools_b200.fusion_mlp import MlpFusionNet, reference_init
+    for kind, layers, dims, B in (("mlp", "256,128", (1582, 88, 1500), 33), ("attention", "130,3", (10, 12, 7), 6)):
+        net = MlpFusionNet(kind, *dims, layers, device=dev, max_batch=64, seed=1)
+        net.load_state_dict(reference_init(kind, *dims, layers))
+        g = torch.Generator().manual_seed(5)
+        x = [torch.randn(B, d, generator=g).to(dev) for d in dims]
+        emo, val = torch.randint(0, 6, (B,), generator=g).to(dev), torch.randn(B, 1, generator=g).to(dev)
+        for _ in range(2):
+            net.train_step(*x, emo, val, use_graph=False)
+        net(*x)
+    torch.cuda.synchronize()
+    print("fusion_mlp ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["gemms", "attention", "llama", "ln_decoders", "encoders", "fusion"]
+    which = sys.argv[1:] or ["gemms", "attention", "llama", "ln_decoders", "encoders", "fusion", "fusion_mlp"]
     for w in which:
         globals()[w]()
