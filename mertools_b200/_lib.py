@@ -95,10 +95,10 @@ def _declare(l):
     # optional (later-added) entry points are declared by the modules that use them
 
 
-def declare(name, args):
+def declare(name, args, restype=C.c_int):
     fn = getattr(lib(), name)
     fn.argtypes = args
-    fn.restype = C.c_int
+    fn.restype = restype
     return fn
 
 

@@ -1165,29 +1165,10 @@ size_t rows_smem_bytes(int H, int RB) { return sizeof(float) * (size_t)RB * (XCH
 
 template <int RB>
 int launch_rows_t(const RowArgs& a, cudaStream_t st) {
-  static MerPerDevice once;
   const size_t smem = rows_smem_bytes(a.d.hidden, RB);
-  if (once.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(fus_rows_kernel<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    once.mark();
-  }
   MER_REQUIRE(smem <= 200 * 1024, "mer_fusion: shared-memory plan of %zu bytes", smem);
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)(CL * ((a.B + RB - 1) / RB)));
-  cfg.blockDim = dim3(NT);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  MER_CUDA_CHECK(cudaLaunchKernelEx(&cfg, fus_rows_kernel<RB>, a));
-  mer_count_launches(1);
-  return 0;
+  return mer_launch_cluster<fus_rows_kernel<RB>>(dim3((unsigned)(CL * ((a.B + RB - 1) / RB))), dim3(NT), smem, CL,
+                                                 200 * 1024, st, a);
 }
 
 // fast path: hidden <= 128 (a multiple of 4), feature widths multiples of 4, everything within 227 KB of shared memory
@@ -1206,27 +1187,8 @@ bool fast_plan_for(const MerFusionDims& d, FastPlan* out) {
 }
 
 int launch_rows_fast(const RowArgs& a, const FastPlan& pl, cudaStream_t st) {
-  static MerPerDevice once;
-  if (once.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(fus_rows_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    once.mark();
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)(CL * ((a.B + FRB - 1) / FRB)));
-  cfg.blockDim = dim3(NT);
-  cfg.dynamicSmemBytes = (size_t)pl.total * 4;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  MER_CUDA_CHECK(cudaLaunchKernelEx(&cfg, fus_rows_fast_kernel, a, pl, g_fus_trace));
-  mer_count_launches(1);
-  return 0;
+  return mer_launch_cluster<fus_rows_fast_kernel>(dim3((unsigned)(CL * ((a.B + FRB - 1) / FRB))), dim3(NT),
+                                                  (size_t)pl.total * 4, CL, 227 * 1024, st, a, pl, g_fus_trace);
 }
 
 int launch_rows(const RowArgs& a, cudaStream_t st) {

@@ -611,30 +611,11 @@ int fill(MlpArgs& a, const MerMlpDims* d, const float* params, const float* audi
 }
 
 int launch_rows(const MlpArgs& a, cudaStream_t st) {
-  static MerPerDevice once;
   const Plan pl = make_plan(a);
   const size_t smem = (size_t)pl.total * 4;
   MER_REQUIRE(smem <= 227 * 1024, "mer_mlp: shared-memory plan of %zu bytes", smem);
-  if (once.needs_setup()) {
-    MER_CUDA_CHECK(cudaFuncSetAttribute(mlp_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    once.mark();
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)(CL * ((a.B + RB - 1) / RB)));
-  cfg.blockDim = dim3(NT);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  MER_CUDA_CHECK(cudaLaunchKernelEx(&cfg, mlp_rows_kernel, a, pl));
-  mer_count_launches(1);
-  return 0;
+  return mer_launch_cluster<mlp_rows_kernel>(dim3((unsigned)(CL * ((a.B + RB - 1) / RB))), dim3(NT), smem, CL,
+                                             227 * 1024, st, a, pl);
 }
 
 int launch_wgrad(const MlpArgs& a, const Layout& L, float* grads, float* loss_out, cudaStream_t st) {

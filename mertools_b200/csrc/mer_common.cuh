@@ -42,6 +42,47 @@ int mer_make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, int rank, const v
 int mer_num_sms();
 void mer_count_launches(int n);  // cumulative count of kernels launched by this library
 
+// One-shot per-device state (cudaFuncSetAttribute, the SM count): keyed by the current device so that a process
+// driving several GPUs does not reuse the first device's setup.  Not a lock: the C ABI is single-threaded per
+// device (mer_b200.h), a repeated cudaFuncSetAttribute is harmless.
+struct MerPerDevice {
+  bool done[64] = {};
+  static int current() {
+    int d = 0;
+    return (cudaGetDevice(&d) == cudaSuccess && d >= 0 && d < 64) ? d : 0;
+  }
+  bool needs_setup() const { return !done[current()]; }
+  void mark() { done[current()] = true; }
+};
+
+// Launch Kernel over `grid` as clusters of `cluster` CTAs along x, with `smem` bytes of dynamic shared memory; the
+// first launch on each device opts the kernel in to `smem_optin` bytes.  Counted by mer_count_launches.
+template <auto Kernel, typename... Args>
+int mer_launch_cluster(dim3 grid, dim3 block, size_t smem, int cluster, int smem_optin, cudaStream_t stream,
+                       const Args&... args) {
+  static MerPerDevice once;
+  if (once.needs_setup()) {
+    MER_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+    once.mark();
+  }
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  MER_CUDA_CHECK(cudaLaunchKernelEx(&cfg, Kernel, args...));
+  mer_count_launches(1);
+  return 0;
+}
+
 // --------------------------------------------------------------------------------------------
 // device-side helpers
 // --------------------------------------------------------------------------------------------

@@ -15,19 +15,6 @@ void mer_prof_pause(int on);  // nest: launches of a composite op (timed as a wh
 int mer_cast_f16_launch(const float* in, void* out, long long n, cudaStream_t stream);  // rowwise.cu
 int mer_accumulate_launch(const float* x, float* acc, long long n, int init, cudaStream_t stream);  // acc (+)= x
 
-// One-shot per-device state (cudaFuncSetAttribute, the SM count): keyed by the current device so that a process
-// driving several GPUs does not reuse the first device's setup.  Not a lock: the C ABI is single-threaded per
-// device (mer_b200.h), a repeated cudaFuncSetAttribute is harmless.
-struct MerPerDevice {
-  bool done[64] = {};
-  static int current() {
-    int d = 0;
-    return (cudaGetDevice(&d) == cudaSuccess && d >= 0 && d < 64) ? d : 0;
-  }
-  bool needs_setup() const { return !done[current()]; }
-  void mark() { done[current()] = true; }
-};
-
 // gemm.cu
 int mer_gemm_launch(const MerGemmDesc* g, cudaStream_t stream);
 

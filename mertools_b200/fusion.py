@@ -1,11 +1,11 @@
 """Attention-fusion training on the device — mirror of MERBench ``toolkit/models`` (get_models,
 Attention), ``toolkit/utils/loss.py`` and the step of ``main-release.py:train_or_eval_model``.
 
-``FusionNet`` owns flat fp32 parameter / gradient / Adam-moment buffers (reference state_dict order)
-and drives libmer_b200.so: eval forward, or one fused training step = forward + CELoss + MSELoss +
-backward + Adam in two kernels (csrc/fusion_fused.cu), replayed as a CUDA graph; under data parallelism the
-gradient (with the three loss scalars riding behind it) takes one NCCL all-reduce between the backward and the
-Adam kernel.
+``FusionNet`` owns flat fp32 parameter / gradient / Adam-moment buffers (reference state_dict order; the
+``_DeviceNet`` base it shares with ``TopnFusionNet`` and ``fusion_mlp.MlpFusionNet``) and drives libmer_b200.so: eval
+forward, or one fused training step = forward + CELoss + MSELoss + backward + Adam in two kernels
+(csrc/fusion_fused.cu), replayed as a CUDA graph; under data parallelism the gradient (with the three loss scalars
+riding behind it) takes one NCCL all-reduce between the backward and the Adam kernel.
 
 ``get_models(args)`` is the reference's object (toolkit/models/__init__.py:18-46): a ``torch.nn.Module`` whose
 ``.model`` is the Attention net, whose ``parameters()`` are ``nn.Parameter`` views of the flat buffer under the
@@ -17,6 +17,8 @@ loop; handed this module's ``Adam`` holder instead of ``torch.optim.Adam`` it ta
 from __future__ import annotations
 
 import ctypes as C
+import functools
+import types
 
 import numpy as np
 import torch
@@ -33,10 +35,6 @@ class MerFusionDims(C.Structure):
 
 class MerAdamHyper(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("lr", "beta1", "beta2", "eps", "weight_decay", "grad_clip")]
-
-
-LSTM_PARAMS = ("rnn.weight_ih_l0", "rnn.weight_hh_l0", "rnn.bias_ih_l0", "rnn.bias_hh_l0",
-               "linear_1.weight", "linear_1.bias")
 
 
 _M64 = (1 << 64) - 1
@@ -63,20 +61,9 @@ def _dist_seed(seed, world):
     return rank_dropout_seed(seed, dist.get_rank(), world)
 
 
-def param_names(feat_type="utt"):
-    names = []
-    for e in ENC:
-        if feat_type != "utt" and e != "attention_mlp":  # LSTMEncoder (encoder.py:45-72)
-            names += [f"{e}.{n}" for n in LSTM_PARAMS]
-            continue
-        for l in ("linear_1", "linear_2", "linear_3"):
-            names += [f"{e}.{l}.weight", f"{e}.{l}.bias"]
-    for l in ("fc_att", "fc_out_1", "fc_out_2"):
-        names += [f"{l}.weight", f"{l}.bias"]
-    return names
-
-
 def param_shapes(audio_dim, text_dim, video_dim, hidden, out1, out2, feat_type="utt"):
+    """{name: shape} of the Attention net in state_dict order: the three encoders (MLPEncoder: linear_1..3; LSTMEncoder,
+    encoder.py:45-72: rnn then linear_1), attention_mlp, fc_att, fc_out_1, fc_out_2."""
     ins = dict(audio_encoder=audio_dim, text_encoder=text_dim, video_encoder=video_dim,
                attention_mlp=3 * hidden)
     shapes = {}
@@ -100,10 +87,195 @@ def param_shapes(audio_dim, text_dim, video_dim, hidden, out1, out2, feat_type="
     return shapes
 
 
-class _Replicated:
-    """Data-parallel bookkeeping shared by FusionNet and TopnFusionNet: both keep params / exp_avg / exp_avg_sq /
-    step_counter as device tensors, and the gradient with the three loss scalars behind it as ``_grads_loss``."""
+def param_names(feat_type="utt"):
+    """The Attention net's state_dict names, in order (they do not depend on the widths)."""
+    return list(param_shapes(1, 1, 1, 1, 1, 1, feat_type))
 
+
+def topn_param_shapes(feat_dims, hidden, out1, out2):
+    """{name: shape} of Attention_TOPN in state_dict order (attention_topn.py:27-50): encoder0 .. encoder{N-1} and
+    attention_mlp (MLPEncoder: linear_1..3), fc_att, fc_out_1, fc_out_2."""
+    N, shapes = len(feat_dims), {}
+    for i, d in enumerate(list(feat_dims) + [hidden * N]):
+        e = f"encoder{i}" if i < N else "attention_mlp"
+        for l, k in (("linear_1", d), ("linear_2", hidden), ("linear_3", hidden)):
+            shapes[f"{e}.{l}.weight"], shapes[f"{e}.{l}.bias"] = (hidden, k), (hidden,)
+    for l, o in (("fc_att", N), ("fc_out_1", out1), ("fc_out_2", out2)):
+        shapes[f"{l}.weight"], shapes[f"{l}.bias"] = (o, hidden), (o,)
+    return shapes
+
+
+def _torch_init(shapes):
+    """The initial state_dict of the reference net laid out as ``shapes``: torch's own constructors on the CPU, one per
+    parameter group in dict order -- ``nn.Linear`` for each ``.weight``, ``nn.LSTM`` for each ``.rnn.weight_ih_l0``.
+    When ``shapes`` follows the order in which the reference's __init__ builds its sub-modules, the values AND the
+    consumption of torch's global generator are the reference's by construction."""
+    sd = {}
+    for name, shape in shapes.items():
+        if name.endswith(".rnn.weight_ih_l0"):
+            prefix, mod = name[:-len("weight_ih_l0")], torch.nn.LSTM(shape[1], shape[0] // 4, batch_first=True)
+        elif name.endswith(".weight"):
+            prefix, mod = name[:-len("weight")], torch.nn.Linear(shape[1], shape[0])
+        else:
+            continue
+        sd.update((prefix + k, v) for k, v in mod.state_dict().items())
+    return {k: sd[k] for k in shapes}
+
+
+@functools.cache
+def _api():
+    """ctypes handles of the mer_fusion_* entry points, declared once, on first use; the nets bind the ones they call
+    as ``_fwd``, ``_fb``, ``_step``, ``_fwd_train``, ``_bwd``, ``_fwd_frm``, ``_fb_frm`` and ``_adam``."""
+    D, T = C.POINTER(MerFusionDims), C.POINTER(MerFusionTopnDims)
+    vp, i32, f32, i64, u64 = C.c_void_p, C.c_int, C.c_float, C.c_longlong, C.c_ulonglong
+    return types.SimpleNamespace(
+        param_count=L.declare("mer_fusion_param_count", [D], restype=i64),
+        workspace_bytes=L.declare("mer_fusion_workspace_bytes", [D, i32], restype=i64),
+        frm_param_count=L.declare("mer_fusion_frm_param_count", [D], restype=i64),
+        frm_workspace_bytes=L.declare("mer_fusion_frm_workspace_bytes", [D, i32, i32, i32, i32], restype=i64),
+        topn_param_count=L.declare("mer_fusion_topn_param_count", [T], restype=i64),
+        topn_workspace_bytes=L.declare("mer_fusion_topn_workspace_bytes", [T, i32], restype=i64),
+        forward=L.declare("mer_fusion_forward", [D, vp, vp, vp, vp, i32, vp, i64, vp, vp, vp, vp]),
+        fwd_bwd=L.declare("mer_fusion_fwd_bwd", [D, vp, vp, vp, vp, vp, vp, vp, i32, f32, f32, u64, vp, vp, vp, i64,
+                                                 vp, vp, vp, vp, vp]),
+        step=L.declare("mer_fusion_step", [D, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, f32, f32, u64, vp, vp,
+                                           C.POINTER(MerAdamHyper), vp, i64, vp, vp, vp, vp, vp]),
+        forward_train=L.declare("mer_fusion_forward_train", [D, vp, vp, vp, vp, i32, f32, u64, vp, vp, vp, i64, vp,
+                                                             vp, vp, vp]),
+        backward=L.declare("mer_fusion_backward", [D, vp, vp, vp, vp, vp, i32, vp, vp, vp, f32, u64, vp, vp, vp, i64,
+                                                   vp, vp, vp, vp]),
+        frm_forward=L.declare("mer_fusion_frm_forward", [D, vp, vp, vp, vp, i32, i32, i32, i32, vp, i64, vp, vp, vp,
+                                                         vp]),
+        frm_fwd_bwd=L.declare("mer_fusion_frm_fwd_bwd", [D, vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, i32, f32, f32,
+                                                         u64, vp, vp, vp, i64, vp, vp, vp, vp, vp]),
+        topn_step=L.declare("mer_fusion_topn_step", [T, vp, vp, vp, vp, vp, i32, f32, f32, u64, vp, vp, vp, i64, vp,
+                                                     vp, vp, vp, vp]),
+        adam=L.declare("mer_fusion_adam", [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, f32, vp, vp]))
+
+
+def _size(n):
+    """A parameter count or workspace size from the library; a negative one means it refused the dims or the batch."""
+    n = int(n)
+    if n < 0:
+        L.check(2)
+    return n
+
+
+class _DeviceNet:
+    """A device-resident fusion net: flat fp32 parameters, gradient and Adam moments in the reference's state_dict order
+    (``shapes``: {name: shape}), the step counter and a workspace, with the host side every such net shares -- views by
+    name, state dicts, data-parallel replicas, the Adam launch and CUDA-graph replay of a training step."""
+
+    def __init__(self, shapes, n_params, device):
+        L.check(L.lib().mer_check_device())
+        self.device = torch.device(device)
+        self.shapes, self.n_params = shapes, _size(n_params)
+        assert sum(int(np.prod(s)) for s in shapes.values()) == self.n_params
+        z = lambda: torch.zeros(self.n_params, dtype=torch.float32, device=self.device)  # noqa: E731
+        self.params, self.exp_avg, self.exp_avg_sq = z(), z(), z()
+        # the gradient and the three loss scalars share one allocation: ONE all-reduce under data parallelism
+        self._grads_loss = torch.zeros(self.n_params + 4, dtype=torch.float32, device=self.device)
+        self.grads = self._grads_loss[:self.n_params]
+        self.loss = self._grads_loss[self.n_params:self.n_params + 3]
+        self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.ws = torch.empty(0, dtype=torch.uint8, device=self.device)
+        self.training = True
+        self.graph_launches = 0  # kernels launched through CUDA-graph replays (not seen by the library counter)
+        self._graphs = {}
+        self._adam = _api().adam
+
+    # ---- nn.Module-flavoured surface used by the reference loop --------------------------------
+    def train(self, mode=True):
+        self.training = mode
+        return self
+
+    def eval(self):
+        return self.train(False)
+
+    def parameters(self):
+        return [self.params]
+
+    def named_views(self, flat=None):
+        flat = self.params if flat is None else flat
+        out, o = {}, 0
+        for name, shape in self.shapes.items():
+            k = int(np.prod(shape))
+            out[name] = flat[o:o + k].view(shape)
+            o += k
+        return out
+
+    def state_dict(self):
+        return {k: v.clone() for k, v in self.named_views().items()}
+
+    def load_state_dict(self, sd):
+        """Accepts the reference's names with or without the ``model.`` wrapper prefix
+        (toolkit/models/__init__.py wraps the net as ``.model``)."""
+        for n, dst in self.named_views().items():
+            src = sd[n] if n in sd else sd["model." + n]
+            if isinstance(src, np.ndarray):
+                src = torch.from_numpy(src)
+            dst.copy_(src.to(self.device, torch.float32))
+        self._graphs.clear()
+        return self
+
+    # ---- shared pieces of the steps --------------------------------------------------------------
+    def _workspace(self, nbytes):
+        """``self.ws``, grown to ``nbytes`` (a workspace query's answer).  Growing drops the captured graphs: they hold
+        the old buffer's address."""
+        nbytes = _size(nbytes)
+        if self.ws.numel() < nbytes:
+            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self._graphs.clear()
+        return self.ws
+
+    @staticmethod
+    def _mask_array(ext_masks, n):
+        """ext_masks (device keep-masks; a None entry takes the counter hash) as the host ``void*[]`` the library reads
+        ``n`` entries of, or None."""
+        if ext_masks is None:
+            return None
+        ptrs = [m.data_ptr() if m is not None else None for m in ext_masks]
+        return C.cast((C.c_void_p * max(n, len(ptrs)))(*ptrs), C.c_void_p)
+
+    def _adam_update(self, world, lr, betas, eps, weight_decay, grad_clip):
+        """mer_fusion_adam on ``grads`` (grad_clip 0 = off); with world > 1 the gradient and the loss terms behind it
+        are summed over the ranks first."""
+        if world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(self._grads_loss)  # SUM: gradient and loss terms already carry 1 / global_batch
+        L.check(self._adam(L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg), L.ptr(self.exp_avg_sq),
+                           self.n_params, lr, betas[0], betas[1], eps, weight_decay, 1.0, grad_clip,
+                           L.ptr(self.step_counter), L.stream_ptr()))
+
+    def _graph_step(self, key, inputs, make_outs, launch):
+        """One training step through the CUDA graph cached under ``key``: ``inputs`` are copied into the graph's static
+        buffers and the graph is replayed; returns its static outputs.  ``launch(*static_inputs, outs)`` enqueues the
+        step on the current stream, writing into ``outs = make_outs()``.  A new key is warmed up outside capture on a
+        side stream, with the state it advances restored afterwards, then captured."""
+        if key not in self._graphs:
+            st, outs = [x.clone() for x in inputs], make_outs()
+            state = (self.params, self.exp_avg, self.exp_avg_sq, self.step_counter)
+            saved = [x.clone() for x in state]
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                launch(*st, outs)
+            torch.cuda.current_stream().wait_stream(s)
+            for dst, src in zip(state, saved):
+                dst.copy_(src)
+            g = torch.cuda.CUDAGraph()
+            n0 = L.launch_count()
+            with torch.cuda.graph(g):
+                launch(*st, outs)
+            self._graphs[key] = (g, (st, outs), L.launch_count() - n0)
+        g, (st, outs), n_kernels = self._graphs[key]
+        for dst, src in zip(st, inputs):
+            dst.copy_(src, non_blocking=True)
+        g.replay()
+        self.graph_launches += n_kernels
+        return outs
+
+    # ---- data parallelism ----------------------------------------------------------------------
     def broadcast_from(self, src=0):
         """Make every rank a replica of rank ``src`` (parameters, Adam moments, step counter): SURVEY.md §8e
         'identical initial weights (broadcast once)'."""
@@ -129,7 +301,7 @@ class _Replicated:
         self._replicas_checked = True
 
 
-class FusionNet(_Replicated):
+class FusionNet(_DeviceNet):
     """Device-resident Attention fusion model.  feat_type 'utt': MLP encoders on [B, D] features;
     'frm_align' / 'frm_unalign': LSTM encoders on [B, T, D] sequences (attention.py:25-33).  output_dim2 = 0 is the
     emotion-only head of the MER2024 / 25 / 26 dataloaders: vals_out is [B, 0] and the loss is CE alone.
@@ -139,105 +311,23 @@ class FusionNet(_Replicated):
     def __init__(self, audio_dim=768, text_dim=768, video_dim=768, hidden_dim=128, output_dim1=6,
                  output_dim2=1, dropout=0.0, grad_clip=-1.0, device="cuda", max_batch=4096, seed=0,
                  feat_type="utt"):
-        L.check(L.lib().mer_check_device())
         assert feat_type in ("utt", "frm_align", "frm_unalign"), feat_type
         self.feat_type = feat_type
         self.frm = feat_type != "utt"
-        self.device = torch.device(device)
         self.dims = MerFusionDims(audio_dim, text_dim, video_dim, hidden_dim, output_dim1, output_dim2)
         self.dropout, self.grad_clip, self.seed = float(dropout), float(grad_clip), int(seed)
-        lib = L.lib()
-        lib.mer_fusion_param_count.restype = C.c_longlong
-        lib.mer_fusion_param_count.argtypes = [C.POINTER(MerFusionDims)]
-        lib.mer_fusion_workspace_bytes.restype = C.c_longlong
-        lib.mer_fusion_workspace_bytes.argtypes = [C.POINTER(MerFusionDims), C.c_int]
-        vp, i32, f32, i64 = C.c_void_p, C.c_int, C.c_float, C.c_longlong
-        self._fwd = L.declare("mer_fusion_forward", [C.POINTER(MerFusionDims), vp, vp, vp, vp, i32, vp,
-                                                     i64, vp, vp, vp, vp])
-        self._fb = L.declare("mer_fusion_fwd_bwd", [C.POINTER(MerFusionDims), vp, vp, vp, vp, vp, vp, vp,
-                                                    i32, f32, f32, C.c_ulonglong, vp, vp, vp, i64, vp,
-                                                    vp, vp, vp, vp])
-        self._adam = L.declare("mer_fusion_adam", [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32,
-                                                   f32, vp, vp])
-        self._step = L.declare("mer_fusion_step", [C.POINTER(MerFusionDims), vp, vp, vp, vp, vp, vp, vp, vp, vp,
-                                                   i32, f32, f32, C.c_ulonglong, vp, vp, C.POINTER(MerAdamHyper),
-                                                   vp, i64, vp, vp, vp, vp, vp])
-        self._fwd_train = L.declare("mer_fusion_forward_train", [C.POINTER(MerFusionDims), vp, vp, vp, vp, i32, f32,
-                                                                 C.c_ulonglong, vp, vp, vp, i64, vp, vp, vp, vp])
-        self._bwd = L.declare("mer_fusion_backward", [C.POINTER(MerFusionDims), vp, vp, vp, vp, vp, i32, vp, vp, vp,
-                                                      f32, C.c_ulonglong, vp, vp, vp, i64, vp, vp, vp, vp])
-        if self.frm:
-            lib.mer_fusion_frm_param_count.restype = C.c_longlong
-            lib.mer_fusion_frm_param_count.argtypes = [C.POINTER(MerFusionDims)]
-            lib.mer_fusion_frm_workspace_bytes.restype = C.c_longlong
-            lib.mer_fusion_frm_workspace_bytes.argtypes = [C.POINTER(MerFusionDims)] + [i32] * 4
-            self._fwd_frm = L.declare("mer_fusion_frm_forward", [C.POINTER(MerFusionDims), vp, vp, vp, vp, i32,
-                                                                 i32, i32, i32, vp, i64, vp, vp, vp, vp])
-            self._fb_frm = L.declare("mer_fusion_frm_fwd_bwd", [C.POINTER(MerFusionDims), vp, vp, vp, vp, vp,
-                                                                i32, i32, i32, vp, vp, i32, f32, f32,
-                                                                C.c_ulonglong, vp, vp, vp, i64, vp, vp, vp, vp,
-                                                                vp])
-        self.n_params = int((lib.mer_fusion_frm_param_count if self.frm else lib.mer_fusion_param_count)(
-            C.byref(self.dims)))
-        self.shapes = param_shapes(audio_dim, text_dim, video_dim, hidden_dim, output_dim1, output_dim2,
-                                   feat_type)
-        assert sum(int(np.prod(s)) for s in self.shapes.values()) == self.n_params
-        z = lambda: torch.zeros(self.n_params, dtype=torch.float32, device=self.device)  # noqa: E731
-        self.params, self.exp_avg, self.exp_avg_sq = z(), z(), z()
-        # the gradient and the three loss scalars share one allocation: ONE all-reduce under data parallelism
-        self._grads_loss = torch.zeros(self.n_params + 4, dtype=torch.float32, device=self.device)
-        self.grads = self._grads_loss[:self.n_params]
-        self.loss = self._grads_loss[self.n_params:self.n_params + 3]
-        self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.max_batch = max_batch
-        self.ws = torch.empty(int(lib.mer_fusion_workspace_bytes(C.byref(self.dims), max_batch)) if not self.frm
-                              else 0, dtype=torch.uint8, device=self.device)
-        self.training = True
-        self.graph_launches = 0  # kernels launched through CUDA-graph replays (not seen by the library counter)
-        lib.mer_launch_count.restype = C.c_longlong
-        self._graphs = {}
-        self._static = None
-
-    # ---- nn.Module-flavoured surface used by the reference loop --------------------------------
-    def train(self, mode=True):
-        self.training = mode
-        return self
-
-    def eval(self):
-        return self.train(False)
+        api = _api()
+        super().__init__(param_shapes(audio_dim, text_dim, video_dim, hidden_dim, output_dim1, output_dim2, feat_type),
+                         (api.frm_param_count if self.frm else api.param_count)(C.byref(self.dims)), device)
+        if not self.frm:  # one workspace for every batch up to max_batch; the frame-level one grows with the lengths
+            self._workspace(api.workspace_bytes(C.byref(self.dims), max_batch))
+        self._fwd, self._fb, self._step = api.forward, api.fwd_bwd, api.step
+        self._fwd_train, self._bwd = api.forward_train, api.backward
+        self._fwd_frm, self._fb_frm = api.frm_forward, api.frm_fwd_bwd
 
     def cuda(self):
         return self
-
-    def parameters(self):
-        return [self.params]
-
-    def named_views(self, flat=None):
-        flat = self.params if flat is None else flat
-        out, o = {}, 0
-        for n in param_names(self.feat_type):
-            k = int(np.prod(self.shapes[n]))
-            out[n] = flat[o:o + k].view(self.shapes[n])
-            o += k
-        return out
-
-    def state_dict(self):
-        return {k: v.clone() for k, v in self.named_views().items()}
-
-    def load_state_dict(self, sd):
-        """Accepts the reference's names with or without the ``model.`` wrapper prefix
-        (toolkit/models/__init__.py wraps the net as ``.model``)."""
-        views = self.named_views()
-        for n, dst in views.items():
-            src = sd[n] if n in sd else sd["model." + n]
-            if isinstance(src, np.ndarray):
-                src = torch.from_numpy(src)
-            dst.copy_(src.to(self.device, torch.float32))
-        self._invalidate()
-        return self
-
-    def _invalidate(self):
-        self._graphs.clear()
 
     # ---- forward / step --------------------------------------------------------------------------
     def _bufs(self, B):
@@ -268,26 +358,16 @@ class FusionNet(_Replicated):
     def _frm_ws(self, B, a, t, v):
         """Workspace of the frame-level variant: depends on the three padded sequence lengths."""
         assert a.dim() == t.dim() == v.dim() == 3, "frame-level features are [B, T, D] (read_data.py:118-125)"
-        need = int(L.lib().mer_fusion_frm_workspace_bytes(C.byref(self.dims), B, a.shape[1], t.shape[1],
-                                                          v.shape[1]))
-        if self.ws.numel() < need:
-            self.ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-            self._invalidate()
-        return self.ws
+        return self._workspace(_api().frm_workspace_bytes(C.byref(self.dims), B, a.shape[1], t.shape[1], v.shape[1]))
 
-    def _masks(self, ext_masks):
-        if ext_masks is None:
-            return None
-        arr = (C.c_void_p * 4)(*[m.data_ptr() if m is not None else None for m in ext_masks])
-        return C.cast(arr, C.c_void_p)
-
-    def _launch_step(self, a, t, v, emo, val, feats, emos_out, vals_out, lr, betas, eps, wd,
-                     world, ext_masks, global_batch=None, fused_adam=True):
+    def _launch_step(self, a, t, v, emo, val, outs, lr, betas, eps, wd, world, ext_masks, global_batch=None,
+                     fused_adam=True):
         B = a.shape[0]
         inv = 1.0 / (global_batch if global_batch is not None else B * world)
-        masks = self._masks(ext_masks)
+        masks = self._mask_array(ext_masks, 4)
         clip = self.grad_clip if self.grad_clip != -1 else 0.0
         seed = _dist_seed(self.seed, world)
+        feats, emos_out, vals_out = outs
         if not self.frm and world == 1 and fused_adam:  # the whole step in two kernels, Adam fused into the weight gradients
             hyper = MerAdamHyper(lr, betas[0], betas[1], eps, wd, clip)
             L.check(self._step(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg),
@@ -308,12 +388,7 @@ class FusionNet(_Replicated):
                              L.ptr(v), L.ptr(emo), L.ptr(val), B, inv, self.dropout,
                              seed, L.ptr(self.step_counter), masks, L.ptr(self.ws), self.ws.numel(),
                              L.ptr(self.loss), L.ptr(feats), L.ptr(emos_out), L.ptr(vals_out), L.stream_ptr()))
-        if world > 1:
-            import torch.distributed as dist
-            dist.all_reduce(self._grads_loss)  # SUM: gradient and loss terms already carry 1 / global_batch
-        L.check(self._adam(L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg),
-                           L.ptr(self.exp_avg_sq), self.n_params, lr, betas[0], betas[1], eps, wd, 1.0,
-                           clip, L.ptr(self.step_counter), L.stream_ptr()))
+        self._adam_update(world, lr, betas, eps, wd, clip)
 
     def train_step(self, a, t, v, emo, val, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
                    world_size=1, ext_masks=None, use_graph=True, global_batch=None, fused_adam=True):
@@ -327,44 +402,18 @@ class FusionNet(_Replicated):
             self.check_replicas(world_size)
         # under data parallelism the step is launched eagerly (4 launches around the NCCL all-reduce)
         if not use_graph or ext_masks is not None or world_size > 1 or not fused_adam:
-            feats, emos_out, vals_out = self._bufs(B)
-            self._launch_step(a.contiguous(), t.contiguous(), v.contiguous(), emo.contiguous(),
-                              val.contiguous(), feats, emos_out, vals_out, lr, betas, eps,
-                              weight_decay, world_size, ext_masks, global_batch, fused_adam)
-            return self.loss, emos_out, vals_out
+            outs = self._bufs(B)
+            self._launch_step(a.contiguous(), t.contiguous(), v.contiguous(), emo.contiguous(), val.contiguous(), outs,
+                              lr, betas, eps, weight_decay, world_size, ext_masks, global_batch, fused_adam)
+            return self.loss, outs[1], outs[2]
         if self.frm:
             self._frm_ws(B, a, t, v)  # sized (and graphs invalidated on growth) before any capture
         key = (B, tuple(a.shape[1:]), tuple(t.shape[1:]), tuple(v.shape[1:]), lr, betas, eps, weight_decay,
                world_size, self.dropout, self.grad_clip)
-        if key not in self._graphs:
-            st = dict(a=torch.empty_like(a), t=torch.empty_like(t), v=torch.empty_like(v),
-                      emo=torch.empty_like(emo), val=torch.empty_like(val))
-            st["feats"], st["emos"], st["vals"] = self._bufs(B)
-            for k, src in (("a", a), ("t", t), ("v", v), ("emo", emo), ("val", val)):
-                st[k].copy_(src)
-            # warm-up outside capture on a side stream, with state restored afterwards
-            saved = [x.clone() for x in (self.params, self.exp_avg, self.exp_avg_sq, self.step_counter)]
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._launch_step(st["a"], st["t"], st["v"], st["emo"], st["val"], st["feats"],
-                                  st["emos"], st["vals"], lr, betas, eps, weight_decay, world_size, None)
-            torch.cuda.current_stream().wait_stream(s)
-            for dst, src in zip((self.params, self.exp_avg, self.exp_avg_sq, self.step_counter), saved):
-                dst.copy_(src)
-            g = torch.cuda.CUDAGraph()
-            n0 = L.lib().mer_launch_count()
-            with torch.cuda.graph(g):
-                self._launch_step(st["a"], st["t"], st["v"], st["emo"], st["val"], st["feats"],
-                                  st["emos"], st["vals"], lr, betas, eps, weight_decay, world_size, None)
-            self._graphs[key] = (g, st, int(L.lib().mer_launch_count() - n0))
-        g, st, n_kernels = self._graphs[key]
-        for k, src in (("a", a), ("t", t), ("v", v), ("emo", emo), ("val", val)):
-            st[k].copy_(src, non_blocking=True)
-        g.replay()
-        self.graph_launches += n_kernels
-        return self.loss, st["emos"], st["vals"]
-
+        _, emos_out, vals_out = self._graph_step(
+            key, (a, t, v, emo, val), lambda: self._bufs(B),
+            lambda *x: self._launch_step(*x, lr, betas, eps, weight_decay, world_size, None))
+        return self.loss, emos_out, vals_out
 
     # ---- the two halves of the autograd node (utterance-level net) -----------------------------------
     def forward_train(self, a, t, v, ext_masks=None):
@@ -373,9 +422,10 @@ class FusionNet(_Replicated):
         B = a.shape[0]
         assert B <= self.max_batch
         feats, emos, vals = self._bufs(B)
-        L.check(self._fwd_train(C.byref(self.dims), L.ptr(self.params), L.ptr(a), L.ptr(t), L.ptr(v), B, self.dropout,
-                                self.seed, L.ptr(self.step_counter), self._masks(ext_masks), L.ptr(self.ws),
-                                self.ws.numel(), L.ptr(feats), L.ptr(emos), L.ptr(vals), L.stream_ptr()))
+        L.check(self._fwd_train(C.byref(self.dims), L.ptr(self.params), L.ptr(a), L.ptr(t), L.ptr(v), B,
+                                self.dropout, self.seed, L.ptr(self.step_counter), self._mask_array(ext_masks, 4),
+                                L.ptr(self.ws), self.ws.numel(), L.ptr(feats), L.ptr(emos), L.ptr(vals),
+                                L.stream_ptr()))
         return feats, emos, vals
 
     def backward(self, a, t, v, d_feats, d_emos, d_vals, ext_masks=None):
@@ -385,10 +435,10 @@ class FusionNet(_Replicated):
         feats, emos, vals = self._bufs(B)
         c = lambda g: None if g is None else g.contiguous().float()  # noqa: E731
         d_feats, d_emos, d_vals = c(d_feats), c(d_emos), c(d_vals)
-        L.check(self._bwd(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(a), L.ptr(t), L.ptr(v), B,
-                          L.ptr(d_feats), L.ptr(d_emos), L.ptr(d_vals), self.dropout, self.seed,
-                          L.ptr(self.step_counter), self._masks(ext_masks), L.ptr(self.ws), self.ws.numel(),
-                          L.ptr(feats), L.ptr(emos), L.ptr(vals), L.stream_ptr()))
+        L.check(self._bwd(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(a), L.ptr(t),
+                          L.ptr(v), B, L.ptr(d_feats), L.ptr(d_emos), L.ptr(d_vals), self.dropout, self.seed,
+                          L.ptr(self.step_counter), self._mask_array(ext_masks, 4), L.ptr(self.ws),
+                          self.ws.numel(), L.ptr(feats), L.ptr(emos), L.ptr(vals), L.stream_ptr()))
         return self.grads
 
 
@@ -397,98 +447,34 @@ class MerFusionTopnDims(C.Structure):
                 ("out2", C.c_int)]
 
 
-class TopnFusionNet(_Replicated):
+class TopnFusionNet(_DeviceNet):
     """Attention_TOPN (MER2026_Track1/toolkit/models/attention_topn.py): the utterance-level fusion net over
     N <= 18 features ``batch['feat0'] .. batch['feat{N-1}']`` ([B, feat_dims[i]] each).  output_dim2 may be 0."""
 
     def __init__(self, feat_dims, hidden_dim=128, output_dim1=6, output_dim2=1, dropout=0.0, grad_clip=-1.0,
                  device="cuda", seed=0):
-        L.check(L.lib().mer_check_device())
         assert 1 <= len(feat_dims) <= 18
-        self.device = torch.device(device)
         self.feat_dims = [int(d) for d in feat_dims]
         self.dims = MerFusionTopnDims(len(feat_dims), (C.c_int * 18)(*self.feat_dims), hidden_dim, output_dim1,
                                       output_dim2)
         self.dropout, self.grad_clip, self.seed = float(dropout), float(grad_clip), int(seed)
-        lib = L.lib()
-        lib.mer_fusion_topn_param_count.restype = C.c_longlong
-        lib.mer_fusion_topn_param_count.argtypes = [C.POINTER(MerFusionTopnDims)]
-        lib.mer_fusion_topn_workspace_bytes.restype = C.c_longlong
-        lib.mer_fusion_topn_workspace_bytes.argtypes = [C.POINTER(MerFusionTopnDims), C.c_int]
-        vp, i32, f32, i64 = C.c_void_p, C.c_int, C.c_float, C.c_longlong
-        self._step = L.declare("mer_fusion_topn_step", [C.POINTER(MerFusionTopnDims), vp, vp, vp, vp, vp, i32, f32, f32,
-                                                        C.c_ulonglong, vp, vp, vp, i64, vp, vp, vp, vp, vp])
-        self._adam = L.declare("mer_fusion_adam", [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, f32, vp, vp])
-        self.n_params = int(lib.mer_fusion_topn_param_count(C.byref(self.dims)))
-        self.names, self.shapes = [], {}
-        H = hidden_dim
-        for i, d in enumerate(self.feat_dims + [H * len(self.feat_dims)]):
-            e = f"encoder{i}" if i < len(self.feat_dims) else "attention_mlp"
-            for l, k in (("linear_1", d), ("linear_2", H), ("linear_3", H)):
-                self.names += [f"{e}.{l}.weight", f"{e}.{l}.bias"]
-                self.shapes[f"{e}.{l}.weight"], self.shapes[f"{e}.{l}.bias"] = (H, k), (H,)
-        for l, o in (("fc_att", len(self.feat_dims)), ("fc_out_1", output_dim1), ("fc_out_2", output_dim2)):
-            self.names += [f"{l}.weight", f"{l}.bias"]
-            self.shapes[f"{l}.weight"], self.shapes[f"{l}.bias"] = (o, H), (o,)
-        assert sum(int(np.prod(s)) for s in self.shapes.values()) == self.n_params
-        z = lambda: torch.zeros(self.n_params, dtype=torch.float32, device=self.device)  # noqa: E731
-        self.params, self.exp_avg, self.exp_avg_sq = z(), z(), z()
-        # as in FusionNet: the gradient and the three loss scalars are ONE all-reduce under data parallelism
-        self._grads_loss = torch.zeros(self.n_params + 4, dtype=torch.float32, device=self.device)
-        self.grads = self._grads_loss[:self.n_params]
-        self.loss = self._grads_loss[self.n_params:self.n_params + 3]
-        self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self.ws = torch.empty(0, dtype=torch.uint8, device=self.device)
-        self.training = True
-
-    def train(self, mode=True):
-        self.training = mode
-        return self
-
-    def eval(self):
-        return self.train(False)
-
-    def parameters(self):
-        return [self.params]
-
-    def named_views(self, flat=None):
-        flat = self.params if flat is None else flat
-        out, o = {}, 0
-        for n in self.names:
-            k = int(np.prod(self.shapes[n]))
-            out[n] = flat[o:o + k].view(self.shapes[n])
-            o += k
-        return out
-
-    def state_dict(self):
-        return {k: v.clone() for k, v in self.named_views().items()}
-
-    def load_state_dict(self, sd):
-        for n, dst in self.named_views().items():
-            src = sd[n] if n in sd else sd["model." + n]
-            if isinstance(src, np.ndarray):
-                src = torch.from_numpy(src)
-            dst.copy_(src.to(self.device, torch.float32))
-        return self
+        super().__init__(topn_param_shapes(self.feat_dims, hidden_dim, output_dim1, output_dim2),
+                         _api().topn_param_count(C.byref(self.dims)), device)
+        self._step = _api().topn_step
 
     def _run(self, feats, emo, val, ext_masks, world, global_batch=None):
         B = feats[0].shape[0]
-        need = int(L.lib().mer_fusion_topn_workspace_bytes(C.byref(self.dims), B))
-        if self.ws.numel() < need:
-            self.ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        ws = self._workspace(_api().topn_workspace_bytes(C.byref(self.dims), B))
         feats = [f.contiguous() for f in feats]
         fp = (C.c_void_p * len(feats))(*[f.data_ptr() for f in feats])
-        mp = None
-        if ext_masks is not None:
-            mp = (C.c_void_p * len(ext_masks))(*[m.data_ptr() if m is not None else None for m in ext_masks])
         d = self.dims
         out = [torch.empty(B, n, dtype=torch.float32, device=self.device) for n in (d.hidden, d.out1, d.out2)]
-        L.check(self._step(C.byref(d), L.ptr(self.params), L.ptr(self.grads), C.cast(fp, C.c_void_p), L.ptr(emo),
-                           L.ptr(val), B, 1.0 / (global_batch if global_batch is not None else B * world),
-                           self.dropout if emo is not None else 0.0,
-                           _dist_seed(self.seed, world),
-                           L.ptr(self.step_counter), C.cast(mp, C.c_void_p) if mp is not None else None,
-                           L.ptr(self.ws), self.ws.numel(), L.ptr(self.loss), L.ptr(out[0]), L.ptr(out[1]),
+        L.check(self._step(C.byref(d), L.ptr(self.params), L.ptr(self.grads), C.cast(fp, C.c_void_p),
+                           L.ptr(emo), L.ptr(val), B,
+                           1.0 / (global_batch if global_batch is not None else B * world),
+                           self.dropout if emo is not None else 0.0, _dist_seed(self.seed, world),
+                           L.ptr(self.step_counter), self._mask_array(ext_masks, d.n_feats + 1),
+                           L.ptr(ws), ws.numel(), L.ptr(self.loss), L.ptr(out[0]), L.ptr(out[1]),
                            L.ptr(out[2]), L.stream_ptr()))
         return out
 
@@ -509,12 +495,7 @@ class TopnFusionNet(_Replicated):
         if world_size > 1:
             self.check_replicas(world_size)
         _, eo, vo = self._run(feats, emo.contiguous(), val.contiguous(), ext_masks, world_size, global_batch)
-        if world_size > 1:
-            import torch.distributed as dist
-            dist.all_reduce(self._grads_loss)  # SUM: gradient and loss terms already carry 1 / global_batch
-        L.check(self._adam(L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg), L.ptr(self.exp_avg_sq),
-                           self.n_params, lr, betas[0], betas[1], eps, weight_decay, 1.0,
-                           self.grad_clip if self.grad_clip != -1 else 0.0, L.ptr(self.step_counter), L.stream_ptr()))
+        self._adam_update(world_size, lr, betas, eps, weight_decay, self.grad_clip if self.grad_clip != -1 else 0.0)
         return self.loss, eo, vo
 
 
@@ -523,40 +504,14 @@ def reference_init(feat_type, audio_dim, text_dim, video_dim, hidden, out1, out2
     constructors, called on the CPU in the order Attention.__init__ builds its sub-modules (attention.py:25-40;
     MLPEncoder: linear_1..3, encoder.py:25-27; LSTMEncoder: rnn then linear_1, encoder.py:59-61), so the values AND
     the consumption of torch's global generator are the reference's by construction."""
-    nn = torch.nn
-    sd = {}
-
-    def take(prefix, mod):
-        for k, v in mod.state_dict().items():
-            sd[f"{prefix}.{k}"] = v
-
-    for e, d in (("audio_encoder", audio_dim), ("text_encoder", text_dim), ("video_encoder", video_dim),
-                 ("attention_mlp", 3 * hidden)):
-        if feat_type != "utt" and e != "attention_mlp":
-            take(f"{e}.rnn", nn.LSTM(d, hidden, num_layers=1, dropout=0.0, bidirectional=False, batch_first=True))
-            take(f"{e}.linear_1", nn.Linear(hidden, hidden))
-        else:
-            for l, k in (("linear_1", d), ("linear_2", hidden), ("linear_3", hidden)):
-                take(f"{e}.{l}", nn.Linear(k, hidden))
-    for l, o in (("fc_att", 3), ("fc_out_1", out1), ("fc_out_2", out2)):
-        take(l, nn.Linear(hidden, o))
-    return sd
+    return _torch_init(param_shapes(audio_dim, text_dim, video_dim, hidden, out1, out2, feat_type))
 
 
 def reference_init_topn(feat_dims, hidden, out1, out2):
     """reference_init for Attention_TOPN: torch's own nn.Linear constructors on the CPU in the order
     Attention_TOPN.__init__ builds them (attention_topn.py:27-50): encoder0 .. encoder{N-1} (MLPEncoder: linear_1..3),
     attention_mlp, fc_att, fc_out_1, fc_out_2 -- nn.Linear(hidden, 0) when out2 == 0, an empty weight and bias."""
-    nn = torch.nn
-    sd = {}
-    for e, d in [(f"encoder{i}", d) for i, d in enumerate(feat_dims)] + [("attention_mlp", hidden * len(feat_dims))]:
-        for l, k in (("linear_1", d), ("linear_2", hidden), ("linear_3", hidden)):
-            for n, v in nn.Linear(k, hidden).state_dict().items():
-                sd[f"{e}.{l}.{n}"] = v
-    for l, o in (("fc_att", len(feat_dims)), ("fc_out_1", out1), ("fc_out_2", out2)):
-        for n, v in nn.Linear(hidden, o).state_dict().items():
-            sd[f"{l}.{n}"] = v
-    return sd
+    return _torch_init(topn_param_shapes(feat_dims, hidden, out1, out2))
 
 
 class _FusionFn(torch.autograd.Function):

@@ -10,12 +10,13 @@ their ``dropout`` argument (:601-612), so dropout is 0.3 whatever ``--dropout`` 
 from __future__ import annotations
 
 import ctypes as C
+import functools
+import types
 
-import numpy as np
 import torch
 
 from . import _lib as L
-from .fusion import MerAdamHyper
+from .fusion import MerAdamHyper, _DeviceNet, _torch_init
 
 KINDS = {"mlp": 0, "attention": 1}
 CHAINS = {"mlp": ("module",), "attention": ("audio_mlp", "text_mlp", "video_mlp", "attention_mlp")}
@@ -56,13 +57,7 @@ def reference_init(kind, audio_dim, text_dim, video_dim, layers, out1=6, out2=1)
     """The state_dict ``MLP(...)`` / ``Attention(...)`` of main-release.py:601-612 starts from: torch's own
     ``nn.Linear`` constructors on the CPU, in the order the reference's __init__ calls them (ReLU and Dropout draw
     nothing), so the values and the consumption of torch's global generator are the reference's by construction."""
-    shapes = param_shapes(kind, audio_dim, text_dim, video_dim, layers, out1, out2)
-    sd = {}
-    for name, shape in shapes.items():
-        if name.endswith(".weight"):
-            lin = torch.nn.Linear(shape[1], shape[0])
-            sd[name], sd[name[:-len("weight")] + "bias"] = lin.weight.detach(), lin.bias.detach()
-    return {k: sd[k] for k in shapes}
+    return _torch_init(param_shapes(kind, audio_dim, text_dim, video_dim, layers, out1, out2))
 
 
 def mask_shapes(kind, layers, batch):
@@ -80,67 +75,37 @@ def check_batch(kind, batch):
                          "leaves no batch of one row")
 
 
-class MlpFusionNet:
+@functools.cache
+def _api():
+    """ctypes handles of the mer_mlp_* entry points, declared once, on first use (bound as ``_fwd`` and ``_step``)."""
+    D = C.POINTER(MerMlpDims)
+    vp, i32, f32, i64 = C.c_void_p, C.c_int, C.c_float, C.c_longlong
+    return types.SimpleNamespace(
+        param_count=L.declare("mer_mlp_param_count", [D], restype=i64),
+        workspace_bytes=L.declare("mer_mlp_workspace_bytes", [D, i32], restype=i64),
+        forward=L.declare("mer_mlp_forward", [D, vp, vp, vp, vp, i32, vp, i64, vp, vp, vp, vp]),
+        train_step=L.declare("mer_mlp_train_step", [D, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, f32, C.c_ulonglong,
+                                                    vp, vp, C.POINTER(MerAdamHyper), vp, i64, vp, vp, vp, vp, vp]))
+
+
+class MlpFusionNet(_DeviceNet):
     """Device-resident MLP / Attention net of MER2023/main-release.py.  kind: 'mlp' | 'attention'; layers: the
     ``--layers`` string or list."""
 
     def __init__(self, kind, audio_dim, text_dim, video_dim, layers="256,128", output_dim1=6, output_dim2=1,
                  dropout=REFERENCE_DROPOUT, device="cuda", max_batch=1024, seed=0):
-        L.check(L.lib().mer_check_device())
         assert kind in KINDS, kind
         self.kind, self.layers = kind, parse_layers(layers)
         assert 1 <= len(self.layers) <= MAX_LAYERS, f"--layers takes 1..{MAX_LAYERS} entries, got {self.layers}"
-        self.device = torch.device(device)
         self.dropout, self.seed, self.max_batch = float(dropout), int(seed), int(max_batch)
         lay = (C.c_int * MAX_LAYERS)(*(self.layers + [0] * (MAX_LAYERS - len(self.layers))))
         self.dims = MerMlpDims(KINDS[kind], audio_dim, text_dim, video_dim, len(self.layers), lay, output_dim1,
                                output_dim2)
-        lib = L.lib()
-        lib.mer_mlp_param_count.restype = C.c_longlong
-        lib.mer_mlp_param_count.argtypes = [C.POINTER(MerMlpDims)]
-        lib.mer_mlp_workspace_bytes.restype = C.c_longlong
-        lib.mer_mlp_workspace_bytes.argtypes = [C.POINTER(MerMlpDims), C.c_int]
-        vp, i32, f32, i64 = C.c_void_p, C.c_int, C.c_float, C.c_longlong
-        self._fwd = L.declare("mer_mlp_forward", [C.POINTER(MerMlpDims), vp, vp, vp, vp, i32, vp, i64, vp, vp, vp, vp])
-        self._step = L.declare("mer_mlp_train_step", [C.POINTER(MerMlpDims), vp, vp, vp, vp, vp, vp, vp, vp, vp, i32,
-                                                      f32, C.c_ulonglong, vp, vp, C.POINTER(MerAdamHyper), vp, i64,
-                                                      vp, vp, vp, vp, vp])
-        n = int(lib.mer_mlp_param_count(C.byref(self.dims)))
-        if n < 0:
-            L.check(2)
-        self.n_params = n
-        self.shapes = param_shapes(kind, audio_dim, text_dim, video_dim, self.layers, output_dim1, output_dim2)
-        assert sum(int(np.prod(s)) for s in self.shapes.values()) == n
-        z = lambda: torch.zeros(n, dtype=torch.float32, device=self.device)  # noqa: E731
-        self.params, self.grads, self.exp_avg, self.exp_avg_sq = z(), z(), z(), z()
-        self.loss = torch.zeros(3, dtype=torch.float32, device=self.device)
-        self.step_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
-        ws = int(lib.mer_mlp_workspace_bytes(C.byref(self.dims), max(self.max_batch, 2)))
-        if ws < 0:
-            L.check(2)
-        self.ws = torch.empty(ws, dtype=torch.uint8, device=self.device)
-        self._graphs = {}
-
-    # ---- state ---------------------------------------------------------------------------------
-    def named_views(self, flat=None):
-        flat = self.params if flat is None else flat
-        out, o = {}, 0
-        for name, shape in self.shapes.items():
-            k = int(np.prod(shape))
-            out[name] = flat[o:o + k].view(shape)
-            o += k
-        return out
-
-    def state_dict(self):
-        return {k: v.clone() for k, v in self.named_views().items()}
-
-    def load_state_dict(self, sd):
-        for name, dst in self.named_views().items():
-            src = sd[name]
-            if isinstance(src, np.ndarray):
-                src = torch.from_numpy(src)
-            dst.copy_(src.to(self.device, torch.float32))
-        return self
+        api = _api()
+        super().__init__(param_shapes(kind, audio_dim, text_dim, video_dim, self.layers, output_dim1, output_dim2),
+                         api.param_count(C.byref(self.dims)), device)
+        self._workspace(api.workspace_bytes(C.byref(self.dims), max(self.max_batch, 2)))
+        self._fwd, self._step = api.forward, api.train_step
 
     # ---- forward / step --------------------------------------------------------------------------
     def _outs(self, B):
@@ -158,24 +123,22 @@ class MlpFusionNet:
         self._check(B)
         a, t, v = a.contiguous(), t.contiguous(), v.contiguous()
         feats, emos, vals = self._outs(B)
-        L.check(self._fwd(C.byref(self.dims), L.ptr(self.params), L.ptr(a), L.ptr(t), L.ptr(v), B, L.ptr(self.ws),
-                          self.ws.numel(), L.ptr(feats), L.ptr(emos), L.ptr(vals), L.stream_ptr()))
+        L.check(self._fwd(C.byref(self.dims), L.ptr(self.params), L.ptr(a), L.ptr(t), L.ptr(v), B,
+                          L.ptr(self.ws), self.ws.numel(), L.ptr(feats), L.ptr(emos), L.ptr(vals),
+                          L.stream_ptr()))
         return feats, emos, vals
 
     __call__ = forward
 
     def _launch(self, a, t, v, emo, val, outs, lr, betas, eps, weight_decay, ext_masks, update):
         B = a.shape[0]
-        masks = None
-        if ext_masks is not None:
-            arr = (C.c_void_p * len(ext_masks))(*[m.data_ptr() if m is not None else None for m in ext_masks])
-            masks = C.cast(arr, C.c_void_p)
+        masks = self._mask_array(ext_masks, len(CHAINS[self.kind]) * len(self.layers))
         hyper = MerAdamHyper(lr, betas[0], betas[1], eps, weight_decay, 0.0)
         L.check(self._step(C.byref(self.dims), L.ptr(self.params), L.ptr(self.grads), L.ptr(self.exp_avg),
                            L.ptr(self.exp_avg_sq), L.ptr(a), L.ptr(t), L.ptr(v), L.ptr(emo), L.ptr(val), B,
                            self.dropout, self.seed, L.ptr(self.step_counter), masks,
-                           C.byref(hyper) if update else None, L.ptr(self.ws), self.ws.numel(), L.ptr(self.loss),
-                           L.ptr(outs[0]), L.ptr(outs[1]), L.ptr(outs[2]), L.stream_ptr()))
+                           C.byref(hyper) if update else None, L.ptr(self.ws), self.ws.numel(),
+                           L.ptr(self.loss), L.ptr(outs[0]), L.ptr(outs[1]), L.ptr(outs[2]), L.stream_ptr()))
 
     def train_step(self, a, t, v, emo, val, lr=1e-4, weight_decay=1e-5, betas=(0.9, 0.999), eps=1e-8,
                    ext_masks=None, use_graph=True, update=True):
@@ -192,29 +155,6 @@ class MlpFusionNet:
             self._launch(a.contiguous(), t.contiguous(), v.contiguous(), emo.contiguous(), val.contiguous(), outs,
                          lr, betas, eps, weight_decay, ext_masks, update)
             return (self.loss, *outs)
-        key = (B, lr, betas, eps, weight_decay)
-        if key not in self._graphs:
-            st = dict(a=torch.empty_like(a), t=torch.empty_like(t), v=torch.empty_like(v), emo=torch.empty_like(emo),
-                      val=torch.empty_like(val), outs=self._outs(B))
-            for k, src in (("a", a), ("t", t), ("v", v), ("emo", emo), ("val", val)):
-                st[k].copy_(src)
-            # warm-up outside capture on a side stream, with the state restored afterwards
-            saved = [x.clone() for x in (self.params, self.exp_avg, self.exp_avg_sq, self.step_counter)]
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._launch(st["a"], st["t"], st["v"], st["emo"], st["val"], st["outs"], lr, betas, eps,
-                             weight_decay, None, True)
-            torch.cuda.current_stream().wait_stream(s)
-            for dst, src in zip((self.params, self.exp_avg, self.exp_avg_sq, self.step_counter), saved):
-                dst.copy_(src)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._launch(st["a"], st["t"], st["v"], st["emo"], st["val"], st["outs"], lr, betas, eps,
-                             weight_decay, None, True)
-            self._graphs[key] = (g, st)
-        g, st = self._graphs[key]
-        for k, src in (("a", a), ("t", t), ("v", v), ("emo", emo), ("val", val)):
-            st[k].copy_(src, non_blocking=True)
-        g.replay()
-        return (self.loss, *st["outs"])
+        outs = self._graph_step((B, lr, betas, eps, weight_decay), (a, t, v, emo, val), lambda: self._outs(B),
+                                lambda *x: self._launch(*x, lr, betas, eps, weight_decay, None, True))
+        return (self.loss, *outs)
